@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""bench.py -- LLaVA-MoD distillation step on B200 (BASELINE.json: distill samples/s at 1/2/4/8 GPUs; KL-kernel HBM GB/s vs peak;
-next to the reference CPU path).
+"""bench.py -- LLaVA-MoD distillation step on H100 (distill samples/s at 1/2/4/8 GPUs; KL-kernel HBM GB/s vs peak; next to the
+reference CPU path).
 
     python bench.py --gpus N --steps K --warmup W            # our path (one process per GPU; torchrun for N > 1)
+    python bench.py ... --dump-outputs DIR                   # + what the last timed step computed, as DIR/<name>.npy
     python bench.py --impl reference --gpus N --steps K ...  # the reference's own algorithm on the host cores (oracle)
 
 Headline (`value`, BASELINE config 2): a "step" = one optimizer step of the reference recipe on every GPU: 8 micro-batches of one
@@ -11,11 +12,15 @@ CLIP tower forward + frozen 7B teacher forward + 0.5B-4E sparse student forward/
 all-reduce (N > 1), global-norm clip and fused AdamW.  Synthetic inputs of the named shape (SURVEY.md section 8d): 336x336 image, 1473
 text ids with one <image> -> spliced length 2048, first 40% masked.
 
-`secondary` (same process, after the headline; BASELINE configs 3, 4 and 5 in front of the driver at every N):
+`secondary` (BASELINE configs 3, 4 and 5 in front of the driver at every N; 3 and 4 in the same process after the headline):
   config3  the same mimic step at GLOBAL batch 256 (256 / N micro-batches per GPU and optimizer step);
   config4  the preference (DPO) stage on the same 0.5B-4E <- 7B pair: chosen + rejected of T' = 2048, 2 reference + 2 policy forwards,
            2 policy backwards per pair (preference_distillation.sh:48-88), with the log-prob-gather kernel's roofline;
-  config5  1.8B-8E student <- 7B teacher at T' = 4096, mimic micro-batches and preference pairs in one step.
+  config5  1.8B-4E student <- 7B teacher at T' = 2048 (the recipe's model_max_length), mimic micro-batches and preference pairs in one
+           step (4 experts: with 8 the trainable state alone exceeds 80 GB).  It runs in a child process of its own, started before this
+           process builds its models, and eagerly: the CUDA-graph pools of its two stages (~17 GB) do not fit next to the 1.8B student's
+           optimizer state and the teacher in 80 GB.
+           The mimic stage alone at T' = 4096 runs as --workload mimic-1.8B-4E-from-7B-seq4096.
 """
 import argparse
 import json
@@ -36,14 +41,14 @@ WORKLOADS = {
     # name: kind, student arch, teacher arch, clip, spliced seq len, accumulation (micro-batches per optimizer step and GPU), experts
     "mimic-0.5B-4E-from-7B-seq2048": dict(kind="mimic", student="qwen1.5-0.5b", teacher="qwen1.5-7b", clip="clip-l-336", seq=2048, accum=8, experts=4),
     "preference-0.5B-4E-from-7B-seq2048": dict(kind="dpo", student="qwen1.5-0.5b", teacher="qwen1.5-7b", clip="clip-l-336", seq=2048, accum=8, experts=4),
-    "mimic-1.8B-8E-from-7B-seq4096": dict(kind="mimic", student="qwen1.5-1.8b", teacher="qwen1.5-7b", clip="clip-l-336", seq=4096, accum=8, experts=8),
-    "mimic+pref-1.8B-8E-from-7B-seq4096": dict(kind="mimic+dpo", student="qwen1.5-1.8b", teacher="qwen1.5-7b", clip="clip-l-336", seq=4096, accum=8, experts=8),
+    "mimic-1.8B-4E-from-7B-seq4096": dict(kind="mimic", student="qwen1.5-1.8b", teacher="qwen1.5-7b", clip="clip-l-336", seq=4096, accum=8, experts=4),
+    "mimic+pref-1.8B-4E-from-7B-seq2048": dict(kind="mimic+dpo", student="qwen1.5-1.8b", teacher="qwen1.5-7b", clip="clip-l-336", seq=2048, accum=8, experts=4),
     "tiny": dict(kind="mimic", student="tiny", teacher="tiny", clip="tiny", seq=64, accum=2, experts=4),
     "tiny-pref": dict(kind="dpo", student="tiny", teacher="tiny", clip="tiny", seq=64, accum=2, experts=4),
     "tiny-mimic+pref": dict(kind="mimic+dpo", student="tiny", teacher="tiny", clip="tiny", seq=64, accum=2, experts=4),
 }
 # nominal dense FLOP per unit (SURVEY.md 8d): mimic sample; preference pair = 2 teacher fwd + 2 student fwd/bwd + CLIP
-FLOP_PER_SAMPLE = {"mimic-0.5B-4E-from-7B-seq2048": 38.5e12, "mimic-1.8B-8E-from-7B-seq4096": 115.7e12,
+FLOP_PER_SAMPLE = {"mimic-0.5B-4E-from-7B-seq2048": 38.5e12, "mimic-1.8B-4E-from-7B-seq4096": 115.7e12,
                    "preference-0.5B-4E-from-7B-seq2048": (2 * 30.17 + 2 * 7.6 + 0.38) * 1e12}
 HEADLINE = "mimic-0.5B-4E-from-7B-seq2048"
 
@@ -54,7 +59,7 @@ def peaks():
             d = json.load(f)
         return d["hbm_gbs"], d.get("bf16_tflops_sustained", d["bf16_tflops"]), "measured"
     except Exception:
-        return 6650.0, 1400.0, "fallback"
+        return 3350.0, 989.0, "H100 SXM data sheet (HBM3 3.35 TB/s, dense BF16 989 TFLOP/s)"
 
 
 def synth_batch(wl, rank, idx, vocab, device=None, pinned=False):
@@ -93,7 +98,7 @@ def synth_pair(wl, rank, idx, vocab, pinned=False):
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
 
     def __init__(self, index):
         super().__init__(daemon=True)
@@ -275,7 +280,7 @@ def our_config(wl_name, accum, world, cuda_graphs=True, compact=True):
             "loss": {"mimic": "kd_lm (mimic KL + LM + aux)", "dpo": "sigmoid DPO + aux", "mimic+dpo": "kd_lm micro-batches + sigmoid-DPO pairs"}[wl["kind"]],
             "parallelism": "dp%d" % world,
             # timing rule: no explicit L2 flush between timed steps -- one step streams the 15.4 GB of frozen teacher weights, the student's
-            # weights / gradients / optimizer arenas and ~2 GB of activations and logits per micro-batch through a 126 MB L2
+            # weights / gradients / optimizer arenas and ~2 GB of activations and logits per micro-batch through a 50 MB L2
             "l2": "inputs larger than L2 (>= 17 GB touched per micro-batch); no flush"}
 
 
@@ -437,14 +442,7 @@ def kernel_rooflines(job, hbm_peak, src):
         ev = timers.get("kl_fwd_bwd", [])
         kl_ms = sum(a.elapsed_time(b) for a, b in ev) / max(1, len(ev))
         ach = bytes_launch / (kl_ms * 1e-3) / 1e9 if kl_ms > 0 else None
-        prof = {}
-        try:
-            with open(os.path.join(ROOT, "profiles", "kl_traffic_compact.json" if compact else "kl_traffic.json")) as f:
-                prof = json.load(f)
-        except Exception:
-            pass
-        # the ncu capture was taken at the headline workload's row count; another workload (config 5) has no capture of its own -> null
-        traffic = prof.get("traffic_bytes_per_launch") if abs(prof.get("rows", -10 ** 9) - active) <= 0.02 * max(1, active) else None
+        traffic = None                       # measured DRAM traffic: no hardware-counter capture is stored with the project
         out["kl"] = {"kernel": "kl_stream_kernel (lmod_kl_fwd_bwd_rows)" if compact else "kl_stream_kernel (lmod_kl_fwd_bwd)", "bound": "hbm",
                      "achieved": ach, "peak": hbm_peak, "unit": "GB/s",
                      "frac": (ach / hbm_peak) if ach else None, "peak_source": src, "traffic": traffic,
@@ -467,6 +465,29 @@ def kernel_rooflines(job, hbm_peak, src):
                        "note": "4V B/token for fwd+bwd of a policy forward (the backward re-reads the bf16 logits it overwrites: 6V B of real traffic), "
                                "2V B/token for the forward-only reference forwards"}
     return out
+
+
+DUMP_SAMPLE = 4 << 20          # trainable-parameter elements written by --dump-outputs (fixed, seeded positions; 16 MB as float32)
+
+
+def dump_outputs(out_dir, loss, student):
+    """What the timed path hands its caller after the last timed step: the step's loss and the updated trainable weights (a fixed,
+    seeded sample of them, in name order) -- float64 / float32 .npy files, so that two builds can be compared output for output."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    torch.cuda.synchronize()
+    np.save(os.path.join(out_dir, "loss.npy"), np.array([float(loss)], dtype=np.float64))
+    params = [p for _, p in sorted(student.named_parameters(), key=lambda kv: kv[0]) if p.requires_grad]
+    total = sum(p.numel() for p in params)
+    g = torch.Generator(device="cpu").manual_seed(0)
+    idx = torch.randint(0, total, (DUMP_SAMPLE,), generator=g).sort().values        # positions in the name-ordered concatenation
+    parts, off = [], 0
+    for p in params:
+        lo, hi = torch.searchsorted(idx, off), torch.searchsorted(idx, off + p.numel())
+        if hi > lo:
+            parts.append(p.detach().reshape(-1)[(idx[lo:hi] - off).to(p.device)].float().cpu())
+        off += p.numel()
+    np.save(os.path.join(out_dir, "trainable_params_sample.npy"), torch.cat(parts).numpy().astype(np.float32))
 
 
 def run_ours(args):
@@ -493,6 +514,8 @@ def run_ours(args):
             os.dup2(saved, 1)
             os.close(saved)
     dev = torch.device("cuda", local)
+    sec5 = config5_child(world, rank) if (args.workload == HEADLINE and not args.no_secondary) else None
+    torch.manual_seed(0)                               # host-side draws (router noise) repeat from run to run
     wl_name = args.workload
     wl = WORKLOADS[wl_name]
     accum = args.accum if args.accum else wl["accum"]
@@ -532,6 +555,8 @@ def run_ours(args):
     if os.environ.get("LMOD_PROFILE") == "1":          # ncu --profile-from-start off: capture only the timed region
         torch.cuda.cudart().cudaProfilerStart()
     ms, last = timed_steps(job, args.steps, barrier)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last, student)
     if os.environ.get("LMOD_PROFILE") == "1":
         torch.cuda.synchronize()
         torch.cuda.cudart().cudaProfilerStop()
@@ -557,8 +582,8 @@ def run_ours(args):
         "metric": "distill_samples_per_sec", "value": value, "unit": "samples/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
         "ms_per_step": ms / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "bf16", "data": "synthetic",
         "config": cfg,
-        "implementation": {"l2": "working set per micro-batch (15.4 GB of teacher weights) >> 126 MB L2; no explicit flush",
-                           "kernels": "hand-written tcgen05+TMA GEMM / grouped expert GEMM, tcgen05 flash-attention forward AND backward, router, "
+        "implementation": {"l2": "working set per micro-batch (15.4 GB of teacher weights) >> 50 MB L2; no explicit flush",
+                           "kernels": "hand-written wgmma+TMA GEMM / grouped expert GEMM, wgmma flash-attention forward AND backward, router, "
                                       "loss heads (liblmod_b200); no library GEMM or attention kernel on the path",
                            "cuda_graphs": all(bool(t.use_cuda_graphs) for t in job.trainers.values()),
                            "loss_head": ("supervised rows only (device-side row compaction, dynamic-extent GEMMs)"
@@ -572,12 +597,15 @@ def run_ours(args):
         "step_tensor_util": ({"tflops_per_gpu": FLOP_PER_SAMPLE[wl_name] * value / world / 1e12, "peak_tflops": tf_peak,
                               "frac": FLOP_PER_SAMPLE[wl_name] * value / world / 1e12 / tf_peak} if wl_name in FLOP_PER_SAMPLE else None),
         "final_loss": final_loss,
+        "peak_memory_gb": torch.cuda.max_memory_allocated() / 2 ** 30,
     }
     if "kl" in roofs and "logp" in roofs:
         line["roofline_logp"] = roofs["logp"]
-    # ---- secondary: BASELINE configs 3 / 4 / 5, same process, after the headline ----
+    # ---- secondary: BASELINE configs 3 / 4 in this process after the headline, config 5 from its own process (measured first) ----
     if wl_name == HEADLINE and not args.no_secondary:
-        line["secondary"] = secondary(args, job, teacher, student, rank, world, dev, barrier, reduce_max, hbm_peak, tf_peak, src)
+        sec = secondary(args, job, teacher, student, rank, world, dev, barrier, reduce_max, hbm_peak, tf_peak, src)
+        sec.update(sec5)
+        line["secondary"] = sec
     if rank != 0:
         if world > 1:
             dist.destroy_process_group()
@@ -593,10 +621,9 @@ def run_ours(args):
 
 
 def secondary(args, job, teacher, student, rank, world, dev, barrier, reduce_max, hbm_peak, tf_peak, src):
-    """BASELINE configs 3, 4, 5 measured with the same rules (CUDA events, barrier both sides, max over ranks).  Each entry is
+    """BASELINE configs 3 and 4 measured with the same rules (CUDA events, barrier both sides, max over ranks).  Each entry is
     independent: a failure is recorded in place and the headline line is still printed."""
     from llavamod import _C
-    from llavamod.model import synthetic as S
     out = {}
     # config 3: the headline workload at GLOBAL batch 256 (256 / N micro-batches per GPU per optimizer step); graphs are warm
     try:
@@ -637,38 +664,39 @@ def secondary(args, job, teacher, student, rank, world, dev, barrier, reduce_max
         del j4
     except Exception as e:          # noqa: BLE001
         out["config4_preference"] = {"error": "%s: %s" % (type(e).__name__, e)}
-    # config 5: 1.8B-8E student <- 7B teacher, T' 4096, mimic micro-batches + preference pairs.  The 0.5B student's graphs are released first.
-    try:
-        for t in job.trainers.values():
-            t._graphs.clear()
-            t._statics.clear()
-        torch.cuda.empty_cache()
-        name5 = "mimic+pref-1.8B-8E-from-7B-seq4096"
-        wl5 = WORKLOADS[name5]
-        s5 = S.make_student(wl5["student"], wl5["clip"], device=dev, seed=2,
-                            margs=S.moe_args(num_experts=wl5["experts"], train_modules=S.TRAIN_MODULES + ["deepspeed_experts"]), share_tower_with=teacher)
-        acc5 = 2
-        j5 = Job(name5, s5, teacher, acc5, rank, world, dev, n_batches=4)
-        j5.run(2)
-        _C.launch_count_reset(); j5.reset_counters()
-        steps5 = 2
-        ms5, last5 = timed_steps(j5, steps5, barrier)
-        l5 = _C.launch_count() + j5.replayed()
-        roofs5 = kernel_rooflines(j5, hbm_peak, src)
-        (ms5,) = reduce_max(ms5)
-        units5 = steps5 * j5.units_per_step * world
-        out["config5_mimic+pref_1.8B-8E_seq4096"] = {
-            "workload": name5, "config": our_config(name5, acc5, world), "steps": steps5, "warmup": 2, "ms_per_step": ms5 / steps5,
-            "value": units5 / (ms5 / 1e3), "unit": "samples/s (mimic samples + preference pairs)", "n_gpus": world, "gpu_launches": l5,
-            "final_loss": float(last5), "roofline_kl": roofs5.get("kl"), "roofline_logp": roofs5.get("logp"),
-            "peak_memory_gb": torch.cuda.max_memory_allocated() / 2 ** 30,
-            "note": "grad_accum 2 (a step = 2 mimic micro-batches + optimizer step + 2 preference pairs + optimizer step) to keep the bench short; "
-                    "per-sample cost does not depend on the accumulation count"}
-        del j5, s5
-        torch.cuda.empty_cache()
-    except Exception as e:          # noqa: BLE001
-        out["config5_mimic+pref_1.8B-8E_seq4096"] = {"error": "%s: %s" % (type(e).__name__, e)}
     return out
+
+
+CONFIG5 = "mimic+pref-1.8B-4E-from-7B-seq2048"
+
+
+def config5_child(world, rank):
+    """BASELINE config 5 measured by a child `bench.py --workload CONFIG5` (same rules: CUDA events, barrier both sides, max over ranks);
+    with N ranks every rank starts its own child and the children form their own process group.  Returns the `secondary` entry."""
+    key = "config5_mimic+pref_1.8B-4E_seq2048"
+    acc5, steps5 = 2, 2
+    cmd = [sys.executable, os.path.abspath(__file__), "--workload", CONFIG5, "--accum", str(acc5), "--steps", str(steps5), "--warmup", "2",
+           "--min-warmup", "2", "--no-secondary", "--no-cpu-baseline", "--no-e2e"]
+    env = dict(os.environ, LLAVAMOD_CUDA_GRAPHS="0")        # eager: see the module docstring
+    if world > 1:
+        env["MASTER_PORT"] = str(int(env.get("MASTER_PORT", "29500")) + 1)
+    try:
+        r = subprocess.run(cmd, env=env, capture_output=True, text=True, timeout=3600)
+    except subprocess.TimeoutExpired:
+        return {key: {"error": "config 5 child timed out"}}
+    lines = [ln for ln in r.stdout.splitlines() if ln.startswith("{")]
+    if r.returncode != 0 or (rank == 0 and not lines):
+        return {key: {"error": "config 5 child exited %d: %s" % (r.returncode, r.stderr[-3000:])}}
+    if not lines:
+        return {}
+    d = json.loads(lines[-1])
+    return {key: {"workload": CONFIG5, "config": d["config"], "steps": d["steps"], "warmup": d["warmup"], "ms_per_step": d["ms_per_step"],
+                  "value": d["value"], "unit": "samples/s (mimic samples + preference pairs)", "n_gpus": d["n_gpus"],
+                  "gpu_launches": d["gpu_launches"], "final_loss": d["final_loss"], "roofline_kl": d.get("roofline"),
+                  "roofline_logp": d.get("roofline_logp"), "peak_memory_gb": d.get("peak_memory_gb"), "process": "own",
+                  "cuda_graphs": d["implementation"]["cuda_graphs"],
+                  "note": "grad_accum 2 (a step = 2 mimic micro-batches + optimizer step + 2 preference pairs + optimizer step) to keep the "
+                          "bench short; per-sample cost does not depend on the accumulation count"}}
 
 
 def main():
@@ -684,6 +712,7 @@ def main():
     ap.add_argument("--accum", type=int, default=None, help="profiling aid: override gradient accumulation (micro-batches per step)")
     ap.add_argument("--min-warmup", type=int, default=3)
     ap.add_argument("--torch-profile", default=None, help="profiling aid: write a per-kernel device-time table of one step to this file")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write what the last timed step computed to DIR/<name>.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, args.min_warmup) if args.impl == "ours" else args.warmup
     if args.impl == "reference":

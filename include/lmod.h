@@ -1,4 +1,4 @@
-/* lmod.h -- C ABI of liblmod_b200.so: the B200 (sm_100a) kernels behind the LLaVA-MoD
+/* lmod.h -- C ABI of liblmod_b200.so: the H100 (sm_90a) kernels behind the LLaVA-MoD
  * distillation step.
  *
  * The reference (shufangxun/LLaVA-MoD) has NO plugin / FFI interface -- it is pure Python on
@@ -188,7 +188,7 @@ int lmod_adamw(float* master, float* m, float* v, const void* grad, int grad_is_
                const float* gnorm_sq /* optional */, float max_norm, float grad_scale, void* stream);
 
 /* ------------------------------------------------------------------------------------------
- * K5/K8/K9/K12/K14: hand-written tcgen05 + TMA GEMM  D[M,N] (+)= A[M,K] * B[N,K]^T, bf16 in, fp32 TMEM accumulate.
+ * K5/K8/K9/K12/K14: hand-written wgmma + TMA GEMM  D[M,N] (+)= A[M,K] * B[N,K]^T, bf16 in, fp32 register accumulate.
  * Replaces the nn.Linear call sites (modeling_qwen2.py:199-200,678-680,726,1176) and their autograd (dgrad / wgrad).
  *   a_mn_major / b_mn_major: 0 = operand stored K-major ([rows,K], "T"), 1 = stored MN-major ([K,rows], "N"), so that
  *   dgrad (B = W as stored) and wgrad (A = dY^T, B = X^T) need no transposed copies.
@@ -239,7 +239,7 @@ int lmod_grouped_gemm_bf16(const void* A, int64_t lda, const void* B, int64_t ld
                            int mode, int epilogue, void* stream);
 
 /* ------------------------------------------------------------------------------------------
- * K7: flash-attention FORWARD on tcgen05/TMEM/TMA (modeling_qwen2.py:713-721 causal; CLIP non-causal), reading the fused RoPE'd
+ * K7: flash-attention FORWARD on wgmma/TMA (modeling_qwen2.py:713-721 causal; CLIP non-causal), reading the fused RoPE'd
  * QKV buffer [batch*seq, (nh+2*nkv)*hd] in place (GQA by index).  hd in {64,128}.  out [batch*seq, nh*hd];
  * lse [batch, nh, seq] fp32 (natural-log LSE of the scaled scores, consumed by lmod_attn_bwd) or NULL.
  * Padded batches (the additive 4-D mask of modeling_qwen2.py:1035-1040; the varlen un-pad of :600-641): kv_lo / kv_hi are int32
@@ -248,11 +248,7 @@ int lmod_grouped_gemm_bf16(const void* A, int64_t lda, const void* B, int64_t ld
 int lmod_attn_fwd(const void* qkv, int64_t ld_qkv, int64_t batch, int64_t seq, int nh, int nkv, int hd, int causal,
                   float softmax_scale, void* out, int64_t ld_o, float* lse, const int32_t* kv_lo, const int32_t* kv_hi,
                   void* stream);
-/* Diagnostics only (profiles/attn_trace.py; no reference counterpart): the forward kernel compiled with clock64 stamps at the pipeline
- * hand-offs of head 0's CTAs.  trace: zero-filled int64 [ceil(seq/128)][64][16] device buffer, seq <= 4096; no padding arguments. */
-int lmod_attn_fwd_trace(const void* qkv, int64_t ld_qkv, int64_t batch, int64_t seq, int nh, int nkv, int hd, int causal,
-                        float softmax_scale, void* out, int64_t ld_o, float* lse, long long* trace, void* stream);
-/* flash-attention BACKWARD on tcgen05 (autograd of the call above): dqkv (fused dq|dk|dv, same layout as qkv) from qkv, out, dout, lse.
+/* flash-attention BACKWARD on wgmma/TMA (autograd of the call above): dqkv (fused dq|dk|dv, same layout as qkv) from qkv, out, dout, lse.
  * dq32_ws: fp32 [batch*seq, nh*hd] workspace (zeroed inside), dsum_ws: fp32 [batch, nh, seq] workspace; kv_lo / kv_hi as above. */
 int lmod_attn_bwd(const void* qkv, int64_t ld_qkv, const void* out, int64_t ld_o, const void* dout, int64_t ld_do,
                   const float* lse, int64_t batch, int64_t seq, int nh, int nkv, int hd, int causal, float softmax_scale,

@@ -1,29 +1,32 @@
-// attn.cu -- flash-attention FORWARD on tcgen05 / TMEM / TMA (sm_100a), bf16 in, fp32 softmax + accumulation.
+// attn.cu -- flash-attention FORWARD on wgmma / TMA (sm_90a), bf16 in, fp32 softmax + accumulation in registers.
 //
 // Replaces F.scaled_dot_product_attention of Qwen2SdpaAttention.forward (modeling_qwen2.py:713-721, causal, no padding) and the CLIP
 // tower's non-causal self-attention (transformers CLIPVisionModel via clip_encoder.py:54).  Operates directly on the fused, RoPE'd
 // QKV projection output [B*T, (nh + 2*nkv)*hd] -- no head transposes, GQA by index (repeat_kv :204-213 never materialises).
 //
-// One CTA = one (batch, head, 128-query block); two CTAs are co-resident per SM so one CTA's softmax overlaps the other's MMAs.
+// One CTA = one (batch, head, 128-query block), three warpgroups:
+//   warpgroup 0, thread 0 : TMA producer -- Q tile once, then K_j and V_j blocks (128B swizzle) into NST-stage rings with their own
+//                           full / empty barriers; gives its registers to the math warpgroups (setmaxnreg)
+//   warpgroups 1, 2       : 64 query rows each.  S_j = Q K_j^T (wgmma, both operands from shared memory, N = BKV) -> mask, online
+//                           softmax in registers (exp2, row max / sum across the 4 threads of a row) -> P_j as bf16 A fragments
+//                           (the S accumulator layout is the A-fragment layout) -> O += P_j V_j (wgmma, A from registers, V MN-major)
+//                           -> epilogue O / l -> bf16 -> global, LSE
 // Padded batches (right or left padding, per-row key range [kv_lo, kv_hi)) run on the same kernel: the CTA walks only the key blocks
 // its rows can see and masks per element; rows with no visible key are un-masked as in the reference's 4-D mask.
-//   warp 0 lane 0 : TMA producer -- Q tile once, then the K ring and the V ring (blocks of 64 keys, 128B swizzle; separate rings and
-//                                   barriers, so K runs NST blocks ahead of its use)
-//   warp 1 lane 0 : MMA issuer   -- S_j = Q K_j^T (SS, M=128 N=64 K=16 x hd/16) into one of two S buffers in TMEM;
-//                                   O += P_j V_j (TS: A = P_j read from TMEM, B = V_j MN-major from smem, N = hd)
-//   warps 2..9    : softmax      -- two threads per query row (TMEM lane = row; warps 2-5 take key columns 0-31 of each block, warps 6-9
-//                                   columns 32-63): tcgen05.ld half an S row -> mask, block max (halves exchanged through smem), exp2, row sum
-//                                   -> P (bf16x2) written back over S with tcgen05.st; each group rescales its half of O in TMEM when a
-//                                   running max moved (skipped warp-uniformly otherwise); epilogue O / l -> bf16 -> global, LSE
-// TMEM columns: S0 | S1 (64 each, P aliases its S) | O (hd).  All tensor-core work is issued by a single thread; tcgen05 executes MMAs in
-// issue order, which is what makes the S/P aliasing safe (S_{j+2} is issued after P_j V_j).
 #include <stdlib.h>
-#include "tc05.cuh"
+#include "sm90.cuh"
 
 namespace {
 
-constexpr int BQ = 128, BKV = 64;
-constexpr int ATT_THREADS = 320;          // TMA warp, MMA warp, 8 softmax warps (two threads per query row)
+constexpr int BQ = 128;
+constexpr int ATT_THREADS = 384;          // TMA warpgroup + two math warpgroups
+template <int HD> struct AttCfg {
+  static constexpr int BKV = (HD == 64) ? 128 : 64;   // keys per block: S (BKV/2) + O (HD/2) accumulator registers per thread
+  static constexpr int NST = 4;
+  static constexpr int KSUB = HD / 64;               // 64-column sub-tiles along the head dimension
+  static constexpr int Q_BYTES = BQ * HD * 2, KV_BYTES = BKV * HD * 2;
+  static constexpr int SMEM = Q_BYTES + 2 * NST * KV_BYTES + 1024;
+};
 
 struct AttnParams {
   __nv_bfloat16* out;
@@ -37,72 +40,37 @@ struct AttnParams {
   // _unmask_unattended: they attend to every key of the row, causal mask dropped.  NULL = no padding.
   const int32_t* kv_lo;
   const int32_t* kv_hi;
-  long long* trace;      // diagnostics build only (lmod_attn_fwd_trace): clock64 stamps of head 0's CTAs, [q block][key block][16]
 };
-#define ATT_TRACE(slot) do { if (TRACE && tr) tr[(size_t)j * 16 + (slot)] = clock64(); } while (0)
 
-// packed fp32x2 arithmetic (Blackwell FFMA2 / FADD2 / FMUL2): two lanes of a row per issue slot -- the softmax warps are issue-bound
-__device__ __forceinline__ void ffma2_bc(float& d0, float& d1, float a0, float a1, float b, float c) {     // d = a * b + c, b and c broadcast
-  asm("{ .reg .b64 ra, rb, rc, rd; mov.b64 ra, {%2,%3}; mov.b64 rb, {%4,%4}; mov.b64 rc, {%5,%5}; fma.rn.f32x2 rd, ra, rb, rc; mov.b64 {%0,%1}, rd; }"
-      : "=f"(d0), "=f"(d1) : "f"(a0), "f"(a1), "f"(b), "f"(c));
+template <int N, int TB>
+__device__ __forceinline__ void wgmma_ss_kmajor(float* d, uint64_t da, uint64_t db, uint32_t acc) {
+  if constexpr (N == 128) wgmma_ss_n128<0, TB>(d, da, db, acc);
+  else wgmma_ss_n64<0, TB>(d, da, db, acc);
 }
-__device__ __forceinline__ void fadd2_acc(float& d0, float& d1, float a0, float a1) {
-  asm("{ .reg .b64 ra, rd; mov.b64 ra, {%2,%3}; mov.b64 rd, {%0,%1}; add.rn.f32x2 rd, rd, ra; mov.b64 {%0,%1}, rd; }"
-      : "+f"(d0), "+f"(d1) : "f"(a0), "f"(a1));
-}
-__device__ __forceinline__ void fmul2_bc(float& d0, float& d1, float b) {
-  asm("{ .reg .b64 rb, rd; mov.b64 rd, {%0,%1}; mov.b64 rb, {%2,%2}; mul.rn.f32x2 rd, rd, rb; mov.b64 {%0,%1}, rd; }"
-      : "+f"(d0), "+f"(d1) : "f"(b));
-}
-constexpr float RESCALE_TAU = 8.0f;     // lazy rescale: the running max is only raised when a block max exceeds it by > 2^8 (log2 units)
-
-// instruction descriptor: F32 accumulate, BF16 inputs, M = 128, N = n ; b_mn selects the B major-ness
-__device__ __forceinline__ uint32_t attn_idesc(int n, bool b_mn) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((b_mn ? 1u : 0u) << 16) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(BQ >> 4) << 24);
+template <int N>
+__device__ __forceinline__ void wgmma_rs_mn(float* d, const uint32_t* a, uint64_t db, uint32_t acc) {
+  if constexpr (N == 128) wgmma_rs_n128<1>(d, a, db, acc);
+  else wgmma_rs_n64<1>(d, a, db, acc);
 }
 
-__device__ __forceinline__ void tmem_st16(uint32_t addr, const uint32_t* r) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-               :: "r"(addr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-                  "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]) : "memory");
-}
-
-// REGCAP: registers capped at 80 per thread (the compiler is told to plan for 384 threads).  Registers are handed out per SM sub-partition
-// and a 10-warp CTA is accounted as 12 warps, so two CTAs are only GUARANTEED to fit next to each other at <= 65536 / (24 * 32) = 85
-// registers; the compiler's own bound for (320 threads, 2 blocks) is 102.  Measured (profiles/attn_shapes_r2.txt): hd 64 fits in 80 without
-// spilling and gains 2-8 %; hd 128 spills (stack 80 -> 136 B) and loses 20 %, so it keeps 96.
-// Tried on this loop and dropped (same file): a truncating PRMT pack instead of F2FP plus a pairwise max exchange (no change: the softmax
-// warps are bound by dependent-issue latency, not by the XU pipe) and 6-8 of 16 exponential pairs on the FMA pipe (5-7 % slower).
-template <int HD, bool TRACE, bool SPLIT, bool REGCAP>
-__global__ void __launch_bounds__(REGCAP ? 384 : ATT_THREADS, 2)
+template <int HD>
+__global__ void __launch_bounds__(ATT_THREADS, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tma_q, const __grid_constant__ CUtensorMap tma_kv, const AttnParams p) {
-  constexpr int KSUB = HD / 64;                       // 64-column sub-tiles along the head dimension
-  constexpr int Q_BYTES = BQ * HD * 2;
-  constexpr int K_BYTES = BKV * HD * 2, V_BYTES = BKV * HD * 2;
-  constexpr int TMEM_COLS = (2 * BKV + HD <= 256) ? 256 : 512;
-  // K and V blocks ride in SEPARATE rings with their own full / empty barriers: a K slot is free again as soon as S = Q K^T of its block
-  // has been computed (long before the block's P V), so the K of block j+NST is in flight NST iterations ahead of its use and the
-  // L2 / HBM latency of the loads stays off the per-block critical path (with one K|V ring of two stages it was ON it: a block's loads
-  // could only be issued after the P V of block j-2, i.e. one softmax before they were needed).  hd 64: 4 stages; hd 128: 2 (shared memory)
-  constexpr int NST = (HD == 64) ? 4 : 2;
+  using C = AttCfg<HD>;
+  constexpr int BKV = C::BKV, NST = C::NST, KSUB = C::KSUB;
   extern __shared__ uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t q_full, k_full[NST], k_empty[NST], v_full[NST], v_empty[NST], s_full[2], p_full[2], pv_done;
-  __shared__ uint32_t tmem_slot;
-  __shared__ float xmax[2][2][BQ], xsum[2][BQ];        // row-max exchange (per S buffer, per column group) and final row-sum exchange
+  __shared__ __align__(8) uint64_t q_full, k_full[NST], k_empty[NST], v_full[NST], v_empty[NST];
 
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t* sQ = smem;
-  uint8_t* sK0 = smem + Q_BYTES;                      // K stage s at sK0 + s*K_BYTES
-  uint8_t* sV0 = sK0 + NST * K_BYTES;                 // V stage s at sV0 + s*V_BYTES
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  uint8_t* sK0 = smem + C::Q_BYTES;                   // K stage s at sK0 + s*KV_BYTES
+  uint8_t* sV0 = sK0 + NST * C::KV_BYTES;             // V stage s at sV0 + s*KV_BYTES
+  const int wg = threadIdx.x >> 7;
 
-  // Grid = (heads [x 2 halves], batch, query blocks): heads vary fastest and the heavy (late) causal query blocks of ALL heads are handed out
-  // first.  The round-1 order (query blocks fastest, head by head) left the last heads' 32-block CTAs to start when most SMs had already run
-  // dry: the clock stamps of profiles/attn_trace_r2.txt put the makespan at 1.6x the balanced one for 32 heads x 16 query blocks.
+  // Grid = (heads, batch, query blocks): heads vary fastest and the heavy (late) causal query blocks of ALL heads are handed out first
   const int nqb = (p.T + BQ - 1) / BQ;
   const int qb = p.causal ? (nqb - 1 - (int)blockIdx.z) : (int)blockIdx.z;
-  const int h = SPLIT ? (int)(blockIdx.x >> 1) : (int)blockIdx.x, b = blockIdx.y;
-  const int half = SPLIT ? (int)(blockIdx.x & 1) : 0;
+  const int h = (int)blockIdx.x, b = blockIdx.y;
   const int hk = h / (p.nh / p.nkv);
   const int q0 = qb * BQ;
   int lo = 0, hi = p.T;
@@ -111,342 +79,167 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tma_q, const __grid_constant
   // key blocks this query block walks: [jb, jb + nblk).  A block that holds an un-masked row (no visible key) walks every key.
   int kbeg = lo, kend = p.causal ? min(hi, q0 + BQ) : hi;
   if (all_pad || q0 < lo) { kbeg = 0; kend = p.T; }
-  int jb = kbeg / BKV;
-  int nblk = (kend + BKV - 1) / BKV - jb;
-  if (SPLIT) {
-    // SPLIT: a cluster of two CTAs shares one query block, each walks half of its key blocks (the second half holds the diagonal) and the
-    // partial (max, sum, O) of CTA 1 is merged into CTA 0 through distributed shared memory at the end (see attn_split_wanted).
-    const int n0 = nblk >> 1;
-    if (half == 0) nblk = n0; else { jb += n0; nblk -= n0; }
-  }
+  const int jb = kbeg / BKV;
+  const int nblk = (kend + BKV - 1) / BKV - jb;
   const int row_base = b * p.T;                       // row of token 0 of this batch in the fused buffer
   const int col_q = h * HD, col_k = (p.nh + hk) * HD, col_v = (p.nh + p.nkv + hk) * HD;
-  long long* tr = (TRACE && p.trace && h == 0 && b == 0) ? p.trace + (size_t)blockIdx.z * 64 * 16 : nullptr;
 
   if (threadIdx.x == 0) {
     mbar_init(&q_full, 1);
-    for (int s = 0; s < NST; ++s) { mbar_init(&k_full[s], 1); mbar_init(&k_empty[s], 1); mbar_init(&v_full[s], 1); mbar_init(&v_empty[s], 1); }
-    for (int s = 0; s < 2; ++s) { mbar_init(&s_full[s], 1); mbar_init(&p_full[s], 8); }
-    mbar_init(&pv_done, 1);
+    for (int s = 0; s < NST; ++s) { mbar_init(&k_full[s], 1); mbar_init(&k_empty[s], 2); mbar_init(&v_full[s], 1); mbar_init(&v_empty[s], 2); }
     mbar_fence_init();
     asm volatile("prefetch.tensormap [%0];" :: "l"(&tma_q) : "memory");
     asm volatile("prefetch.tensormap [%0];" :: "l"(&tma_kv) : "memory");
   }
-  if (warp == 1) tmem_alloc(&tmem_slot, TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = tmem_slot;
-  const uint32_t tS0 = tmem, tO = tmem + 2 * BKV;
 
-  float m_fin = -INFINITY, lt_fin = 0.f;               // softmax threads: final (stale) running max and total row sum of this CTA's key range
-  if (warp == 0 && lane == 0) {
-    // ===================== TMA producer: Q once, then the K ring and the V ring, whichever has a free slot (K first) =====================
-    if (nblk > 0) {
-      mbar_expect_tx(&q_full, Q_BYTES);
+  if (wg == 0) {
+    // ===================== TMA producer: Q once, then K_j and V_j =====================
+    regs_dealloc<40>();
+    if (threadIdx.x == 0 && nblk > 0) {
+      mbar_expect_tx(&q_full, C::Q_BYTES);
 #pragma unroll
       for (int i = 0; i < KSUB; ++i) tma_load_2d(sQ + i * (BQ * 128), &tma_q, col_q + 64 * i, row_base + q0, &q_full);
-    }
-    int jk = 0, jv = 0;
-    uint32_t spins = 0;
-    while (jk < nblk || jv < nblk) {
-      bool progressed = false;
-      if (jk < nblk) {
-        const int s = jk % NST;
-        if (jk < NST || mbar_try_wait(&k_empty[s], ((jk / NST) & 1) ^ 1)) {
-          uint8_t* sK = sK0 + s * K_BYTES;
-          mbar_expect_tx(&k_full[s], K_BYTES);
+      for (int j = 0; j < nblk; ++j) {
+        const int s = j % NST;
+        const uint32_t ph = ((j / NST) & 1) ^ 1;
+        mbar_wait_bounded(&k_empty[s], ph);
+        mbar_expect_tx(&k_full[s], C::KV_BYTES);
 #pragma unroll
-          for (int i = 0; i < KSUB; ++i) tma_load_2d(sK + i * (BKV * 128), &tma_kv, col_k + 64 * i, row_base + (jb + jk) * BKV, &k_full[s]);
-          ++jk; progressed = true;
+        for (int i = 0; i < KSUB; ++i) tma_load_2d(sK0 + s * C::KV_BYTES + i * (BKV * 128), &tma_kv, col_k + 64 * i, row_base + (jb + j) * BKV, &k_full[s]);
+        mbar_wait_bounded(&v_empty[s], ph);
+        mbar_expect_tx(&v_full[s], C::KV_BYTES);
+#pragma unroll
+        for (int i = 0; i < KSUB; ++i) tma_load_2d(sV0 + s * C::KV_BYTES + i * (BKV * 128), &tma_kv, col_v + 64 * i, row_base + (jb + j) * BKV, &v_full[s]);
+      }
+    }
+    return;
+  }
+
+  // ===================== math warpgroups =====================
+  regs_alloc<232>();
+  const int c = wg - 1;
+  const int w = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+  const bool wg_leader = (threadIdx.x & 127) == 0;
+  // fragment rows: r + 8h (h = 0, 1) of the 128-row block; columns 8i + cq + e
+  const int r = c * 64 + w * 16 + (lane >> 2);
+  const int cq = 2 * (lane & 3);
+  int klo[2], khi[2];
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    const int qrow = q0 + r + 8 * hh;
+    klo[hh] = lo; khi[hh] = p.causal ? min(hi, qrow + 1) : hi;
+    if (all_pad || qrow < lo) { klo[hh] = 0; khi[hh] = p.T; }
+  }
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+  float o[HD / 2];
+#pragma unroll
+  for (int i = 0; i < HD / 2; ++i) o[i] = 0.f;
+  const uint32_t aQ = smem_u32(sQ) + c * (64 * 128);
+  if (nblk > 0) mbar_wait(&q_full, 0);
+  for (int j = 0; j < nblk; ++j) {
+    const int s = j % NST;
+    const uint32_t ph = (j / NST) & 1;
+    float sacc[BKV / 2];
+    mbar_wait(&k_full[s], ph);
+    const uint32_t aK = smem_u32(sK0 + s * C::KV_BYTES);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < HD / 16; ++k)
+      wgmma_ss_kmajor<BKV, 0>(sacc, gmma_desc(aQ + (k / 4) * (BQ * 128) + (k % 4) * 32, 16, 1024),
+                              gmma_desc(aK + (k / 4) * (BKV * 128) + (k % 4) * 32, 16, 1024), k > 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence<BKV / 2>(sacc);
+    if (wg_leader) mbar_arrive(&k_empty[s]);
+
+    const int kv0 = (jb + j) * BKV;
+    if (kv0 < max(klo[0], klo[1]) || kv0 + BKV > min(khi[0], khi[1])) {
+#pragma unroll
+      for (int i = 0; i < BKV / 8; ++i)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int hh = e >> 1, kv = kv0 + 8 * i + cq + (e & 1);
+          if (kv < klo[hh] || kv >= khi[hh]) sacc[4 * i + e] = -INFINITY;
         }
-      }
-      if (jv < nblk && (jv < jk || jk == nblk)) {            // V never runs ahead of K: the K of a block is needed first
-        const int s = jv % NST;
-        if (jv < NST || mbar_try_wait(&v_empty[s], ((jv / NST) & 1) ^ 1)) {
-          uint8_t* sV = sV0 + s * V_BYTES;
-          mbar_expect_tx(&v_full[s], V_BYTES);
-#pragma unroll
-          for (int i = 0; i < KSUB; ++i) tma_load_2d(sV + i * (BKV * 128), &tma_kv, col_v + 64 * i, row_base + (jb + jv) * BKV, &v_full[s]);
-          ++jv; progressed = true;
-        }
-      }
-      if (progressed) spins = 0;
-      else if (++spins > (1u << 26)) { printf("lmod attn_fwd_kernel: producer timeout (block %d %d %d)\n", blockIdx.x, blockIdx.y, blockIdx.z); __trap(); }
     }
-  } else if (warp == 1 && lane == 0) {
-    // ===================== MMA issuer =====================
-    const uint32_t idesc_qk = attn_idesc(BKV, false), idesc_pv = attn_idesc(HD, true);
-    const uint32_t aQ = smem_u32(sQ);
-    auto issue_qk = [&](int j) {
-      const int s = j % NST, sb = j & 1;
-      mbar_wait_bounded(&k_full[s], (j / NST) & 1);
-      tc_fence_after();
-      const uint32_t aK = smem_u32(sK0 + s * K_BYTES);
+    float alpha[2], neg_m[2];
 #pragma unroll
-      for (int k = 0; k < HD / 16; ++k) {
-        const uint64_t da = smem_desc(aQ + (k / 4) * (BQ * 128) + (k % 4) * 32, 16, 1024);
-        const uint64_t db = smem_desc(aK + (k / 4) * (BKV * 128) + (k % 4) * 32, 16, 1024);
-        umma_f16(tS0 + sb * BKV, da, db, idesc_qk, k > 0 ? 1u : 0u);
-      }
-      umma_commit(&k_empty[s]);                       // the K slot is reusable as soon as these MMAs have read it
-      umma_commit(&s_full[sb]);
-    };
-    if (nblk > 0) {
-      mbar_wait_bounded(&q_full, 0);
-      issue_qk(0);
-    }
-    for (int j = 0; j < nblk; ++j) {
-      const int s = j % NST, sb = j & 1;
-      ATT_TRACE(7);
-      if (j + 1 < nblk) issue_qk(j + 1);              // tensor core works on S_{j+1} while the softmax warps chew on S_j
-      ATT_TRACE(8);
-      mbar_wait_bounded(&p_full[sb], (j >> 1) & 1);
-      ATT_TRACE(9);
-      mbar_wait_bounded(&v_full[s], (j / NST) & 1);
-      ATT_TRACE(10);
-      tc_fence_after();
-      const uint32_t aV = smem_u32(sV0 + s * V_BYTES);
+    for (int hh = 0; hh < 2; ++hh) {
+      float mx = -INFINITY;
 #pragma unroll
-      for (int k = 0; k < BKV / 16; ++k) {
-        // V_j as B operand, MN-major: 64-wide hd blocks BKV*128 B apart (LBO), 8-key groups 1024 B apart (SBO), 16 keys = 2048 B per MMA
-        const uint64_t db = smem_desc(aV + k * 2048, BKV * 128, 1024);
-        umma_f16_ts(tO, tS0 + sb * BKV + k * 8, db, idesc_pv, (j > 0 || k > 0) ? 1u : 0u);     // P: 16 bf16 = 8 TMEM columns per MMA
-      }
-      umma_commit(&v_empty[s]);
-      umma_commit(&pv_done);
-      ATT_TRACE(11);
-    }
-  } else if (warp >= 2) {
-    // ===================== softmax / correction / epilogue: TWO threads per query row =====================
-    // warps 2..5 (group 0) own key columns [0,32) of every S block and output columns [0,HD/2); warps 6..9 (group 1) the other halves.
-    // The two threads of a row exchange their block maxima through shared memory (one 256-thread named barrier per block); the row sum
-    // stays split until the epilogue.  Half the per-thread work and twice the warps of the one-thread-per-row version.
-    const int q = warp & 3;                           // TMEM lane quarter of this warp
-    const int g = (warp - 2) >> 2;                    // column group
-    const int r = q * 32 + lane;                      // row within the query block == TMEM lane
-    const int qrow = q0 + r;
-    const uint32_t lane_off = (uint32_t)(q * 32) << 16;
-    constexpr int HC = HD / 2;                        // O columns per group
-    // keys this row may see: [klo_r, khi_r)
-    int klo_r = lo, khi_r = p.causal ? min(hi, qrow + 1) : hi;
-    if (all_pad || qrow < lo) { klo_r = 0; khi_r = p.T; }
-    float m = -INFINITY, l0 = 0.f, l1 = 0.f;
-    if (TRACE && threadIdx.x != 64) tr = nullptr;     // stamps of warp 2 lane 0
-    for (int j = 0; j < nblk; ++j) {
-      const int s = j & 1;
-      ATT_TRACE(0);
-      mbar_wait_warp(&s_full[s], (j >> 1) & 1);
-      tc_fence_after();
-      ATT_TRACE(1);
-      uint32_t sv[32];
-      tmem_ld32(tS0 + s * BKV + g * 32 + lane_off, sv);
-      ATT_TRACE(2);
-      const int kv0 = (jb + j) * BKV + g * 32;
-      const bool need_mask = (kv0 < klo_r) || (kv0 + 32 > khi_r);
-      if (need_mask) {
-#pragma unroll
-        for (int c = 0; c < 32; ++c) {
-          const int kv = kv0 + c;
-          if (kv < klo_r || kv >= khi_r) sv[c] = 0xff800000u;      // -inf
-        }
-      }
-      float mx_loc = -INFINITY;
-#pragma unroll
-      for (int c = 0; c < 32; c += 2) mx_loc = fmaxf(mx_loc, fmaxf(__uint_as_float(sv[c]), __uint_as_float(sv[c + 1])));
-      xmax[s][g][r] = mx_loc;
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      ATT_TRACE(3);
-      const float mblk = fmaxf(mx_loc, xmax[s][g ^ 1][r]) * p.scale_log2;     // block max in scaled-log2 units (scale > 0); both threads of a row agree
-      // lazy running max: keep the stale max while the block max stays within 2^TAU of it (P <= 2^TAU, exact in fp32 / fine in bf16); the
-      // O rescale -- a TMEM round trip that also has to wait for the previous P*V -- then happens on a few early blocks only
-      const bool upd = mblk > m + RESCALE_TAU;               // m = -inf on the first block with a visible key
-      const float m_new = upd ? mblk : m;
+      for (int i = 0; i < BKV / 8; ++i) mx = fmaxf(mx, fmaxf(sacc[4 * i + 2 * hh], sacc[4 * i + 2 * hh + 1]));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      const float m_new = fmaxf(m[hh], mx * p.scale_log2);
       const float m_use = (m_new == -INFINITY) ? 0.f : m_new;   // no visible key so far: keep everything finite (P = exp2(-inf) = 0)
-      const float alpha = upd ? ex2f(m - m_new) : 1.f;       // m = -inf -> 0
-      m = m_new;
-      const float neg_m = -m_use;
-      float rs0 = 0.f, rs1 = 0.f;
-      uint32_t pk[16];
-#pragma unroll
-      for (int c = 0; c < 32; c += 2) {
-        float t0, t1;
-        ffma2_bc(t0, t1, __uint_as_float(sv[c]), __uint_as_float(sv[c + 1]), p.scale_log2, neg_m);
-        const float p0 = ex2f(t0), p1 = ex2f(t1);
-        fadd2_acc(rs0, rs1, p0, p1);
-        pk[c >> 1] = pack_bf16x2(p0, p1);
-      }
-      l0 = fmaf(l0, alpha, rs0);
-      l1 = fmaf(l1, alpha, rs1);
-      ATT_TRACE(4);
-      // P_j (bf16x2) over the start of S_j: group g -> columns [16g, 16g+16).  Issued before the (rare) O rescale so that the 16 packed
-      // registers are dead while the rescale holds 32 accumulator columns (the 96-register build of hd 128 spilled across it)
-      tmem_st16(tS0 + s * BKV + g * 16 + lane_off, pk);
-      if (j > 0) {
-        const bool any_upd = __any_sync(0xffffffffu, upd);
-        if (any_upd || j == nblk - 1) {                      // (the last block always waits: it keeps the epilogue's parity wait unambiguous)
-          mbar_wait_warp(&pv_done, (j - 1) & 1);             // O holds blocks 0..j-1
-          tc_fence_after();
-        }
-        if (any_upd) {                                       // rescale this group's half of O
-#pragma unroll
-          for (int c = 0; c < HC / 32; ++c) {
-            uint32_t o[32];
-            tmem_ld32(tO + g * HC + c * 32 + lane_off, o);
-#pragma unroll
-            for (int i = 0; i < 32; i += 2) {
-              float a0 = __uint_as_float(o[i]), a1 = __uint_as_float(o[i + 1]);
-              fmul2_bc(a0, a1, alpha);
-              o[i] = __float_as_uint(a0); o[i + 1] = __float_as_uint(a1);
-            }
-            tmem_st32(tO + g * HC + c * 32 + lane_off, o);
-          }
-        }
-      }
-      ATT_TRACE(5);
-      tmem_st_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&p_full[s]);
-      ATT_TRACE(6);
+      alpha[hh] = ex2f(m[hh] - m_use);                         // m = -inf -> 0
+      m[hh] = m_new;
+      neg_m[hh] = -m_use;
     }
-    // the two partial row sums of a row -> its total; all of this CTA's MMAs done
-    xsum[g][r] = l0 + l1;
-    asm volatile("bar.sync 1, 256;" ::: "memory");
-    lt_fin = ((l0 + l1) + xsum[g ^ 1][r]);
-    m_fin = m;
-    if (nblk > 0) {
-      mbar_wait_warp(&pv_done, (nblk - 1) & 1);
-      tc_fence_after();
+    uint32_t pa[BKV / 16][4];
+    float rs[2] = {0.f, 0.f};
+#pragma unroll
+    for (int i = 0; i < BKV / 8; ++i) {
+      float pv[4];
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        pv[e] = ex2f(fmaf(sacc[4 * i + e], p.scale_log2, neg_m[e >> 1]));
+        rs[e >> 1] += pv[e];
+      }
+      pa[i >> 1][(i & 1) * 2 + 0] = pack_bf16x2(pv[0], pv[1]);
+      pa[i >> 1][(i & 1) * 2 + 1] = pack_bf16x2(pv[2], pv[3]);
     }
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) l[hh] = fmaf(l[hh], alpha[hh], rs[hh]);
+#pragma unroll
+    for (int i = 0; i < HD / 8; ++i) {
+      o[4 * i + 0] *= alpha[0]; o[4 * i + 1] *= alpha[0];
+      o[4 * i + 2] *= alpha[1]; o[4 * i + 3] *= alpha[1];
+    }
+
+    mbar_wait(&v_full[s], ph);
+    const uint32_t aV = smem_u32(sV0 + s * C::KV_BYTES);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < BKV / 16; ++kk)        // V_j as B operand, MN-major: 64-wide hd blocks BKV*128 B apart, 16 keys = 2048 B per k step
+      wgmma_rs_mn<HD>(o, pa[kk], gmma_desc(aV + kk * 2048, BKV * 128, 1024), 1u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence<HD / 2>(o);
+    if (wg_leader) mbar_arrive(&v_empty[s]);
   }
-  __syncwarp();
-  // ---- SPLIT: CTA 1 of the pair hands its partial (m, l, O) to CTA 0 through distributed shared memory (over CTA 0's idle Q/K/V buffers:
-  //      after the first cluster barrier every MMA and TMA load of both CTAs has completed) ----
-  constexpr int HC = HD / 2;
-  float4* xO = reinterpret_cast<float4*>(smem);         // [HD/4][BQ] float4: column quad major, row minor (conflict-free both ways)
-  float* xm = reinterpret_cast<float*>(smem + BQ * HD * 4);
-  float* xl = xm + BQ;
-  if (SPLIT) {
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-    if (warp >= 2 && half == 1) {
-      const int q = warp & 3, g = (warp - 2) >> 2, r = q * 32 + lane;
-      const uint32_t lane_off = (uint32_t)(q * 32) << 16;
-      uint32_t rO, rm, rl;
-      asm volatile("mapa.shared::cluster.u32 %0, %1, 0;" : "=r"(rO) : "r"(smem_u32(xO)));
-      asm volatile("mapa.shared::cluster.u32 %0, %1, 0;" : "=r"(rm) : "r"(smem_u32(xm)));
-      asm volatile("mapa.shared::cluster.u32 %0, %1, 0;" : "=r"(rl) : "r"(smem_u32(xl)));
+
+  // ---- epilogue: normalise, store, LSE ----
 #pragma unroll
-      for (int c = 0; c < HC / 32; ++c) {
-        uint32_t o[32];
-        tmem_ld32(tO + g * HC + c * 32 + lane_off, o);
-#pragma unroll
-        for (int v = 0; v < 8; ++v) {
-          const int c4 = (g * HC + c * 32) / 4 + v;
-          asm volatile("st.shared::cluster.v4.b32 [%0], {%1, %2, %3, %4};" :: "r"(rO + (uint32_t)(c4 * BQ + r) * 16u), "r"(o[v * 4 + 0]),
-                       "r"(o[v * 4 + 1]), "r"(o[v * 4 + 2]), "r"(o[v * 4 + 3]) : "memory");
-        }
-      }
-      if (g == 0) {
-        asm volatile("st.shared::cluster.f32 [%0], %1;" :: "r"(rm + (uint32_t)r * 4u), "f"(m_fin) : "memory");
-        asm volatile("st.shared::cluster.f32 [%0], %1;" :: "r"(rl + (uint32_t)r * 4u), "f"(lt_fin) : "memory");
-      }
-    }
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-  }
-  if (warp >= 2 && half == 0) {
-    // ---- epilogue: normalise, store this group's half of the head dimension (SPLIT: after merging the partner's partial) ----
-    const int q = warp & 3, g = (warp - 2) >> 2, r = q * 32 + lane;
-    const int qrow = q0 + r;
-    const uint32_t lane_off = (uint32_t)(q * 32) << 16;
-    float a0 = 1.f, a1 = 0.f, mm = m_fin, lt = lt_fin;
-    if (SPLIT) {
-      const float m1 = xm[r], l1t = xl[r];
-      mm = fmaxf(m_fin, m1);
-      a0 = (m_fin == -INFINITY) ? 0.f : ex2f(m_fin - mm);
-      a1 = (m1 == -INFINITY) ? 0.f : ex2f(m1 - mm);
-      lt = lt_fin * a0 + l1t * a1;
-    }
+  for (int hh = 0; hh < 2; ++hh) {
+    float lt = l[hh];
+    lt += __shfl_xor_sync(0xffffffffu, lt, 1);
+    lt += __shfl_xor_sync(0xffffffffu, lt, 2);
     const float inv = (lt > 0.f) ? 1.f / lt : 0.f;
-    const bool ok = qrow < p.T;
-    __nv_bfloat16* orow = p.out + (int64_t)(row_base + qrow) * p.ld_o + col_q + g * HC;
+    const int qrow = q0 + r + 8 * hh;
+    if (qrow < p.T) {
+      __nv_bfloat16* orow = p.out + (int64_t)(row_base + qrow) * p.ld_o + col_q + cq;
 #pragma unroll
-    for (int c = 0; c < HC / 32; ++c) {
-      uint32_t o[32];
-      if (!SPLIT || nblk > 0) tmem_ld32(tO + g * HC + c * 32 + lane_off, o);
-      float f[32];
-#pragma unroll
-      for (int i = 0; i < 32; ++i) f[i] = (!SPLIT) ? __uint_as_float(o[i]) : ((a0 > 0.f && nblk > 0) ? __uint_as_float(o[i]) * a0 : 0.f);
-      if (SPLIT) {
-#pragma unroll
-        for (int v = 0; v < 8; ++v) {
-          const float4 x = xO[((g * HC + c * 32) / 4 + v) * BQ + r];
-          f[v * 4 + 0] = fmaf(x.x, a1, f[v * 4 + 0]); f[v * 4 + 1] = fmaf(x.y, a1, f[v * 4 + 1]);
-          f[v * 4 + 2] = fmaf(x.z, a1, f[v * 4 + 2]); f[v * 4 + 3] = fmaf(x.w, a1, f[v * 4 + 3]);
-        }
-      }
-      if (ok) {
-#pragma unroll
-        for (int v = 0; v < 4; ++v) {
-          uint4 w;
-          w.x = pack_bf16x2(f[v * 8 + 0] * inv, f[v * 8 + 1] * inv);
-          w.y = pack_bf16x2(f[v * 8 + 2] * inv, f[v * 8 + 3] * inv);
-          w.z = pack_bf16x2(f[v * 8 + 4] * inv, f[v * 8 + 5] * inv);
-          w.w = pack_bf16x2(f[v * 8 + 6] * inv, f[v * 8 + 7] * inv);
-          *reinterpret_cast<uint4*>(orow + c * 32 + v * 8) = w;
-        }
-      }
+      for (int i = 0; i < HD / 8; ++i)
+        *reinterpret_cast<uint32_t*>(orow + 8 * i) = pack_bf16x2(o[4 * i + 2 * hh] * inv, o[4 * i + 2 * hh + 1] * inv);
+      if (p.lse && (lane & 3) == 0) p.lse[((int64_t)b * p.nh + h) * p.T + qrow] = (m[hh] + lg2f(lt)) * LN2_F;
     }
-    if (g == 0 && ok && p.lse) p.lse[((int64_t)b * p.nh + h) * p.T + qrow] = (mm + lg2f(lt)) * LN2_F;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem, TMEM_COLS);
 }
 
-template <int HD, bool TRACE, bool SPLIT, bool REGCAP>
+template <int HD>
 int launch_attn(const CUtensorMap& tq, const CUtensorMap& tkv, const AttnParams& p, cudaStream_t st) {
-  constexpr int SMEM = BQ * HD * 2 + ((HD == 64) ? 4 : 2) * (2 * BKV * HD * 2) + 1024;
-  static_assert(BQ * HD * 4 + 2 * BQ * 4 + 1024 <= SMEM, "the pair's exchange buffer lives in the Q/K/V area");
+  constexpr int SMEM = AttCfg<HD>::SMEM;
   static bool attr = false;
   if (!attr) {
-    LMOD_CUDA_OK(cudaFuncSetAttribute(attn_fwd_kernel<HD, TRACE, SPLIT, REGCAP>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
+    LMOD_CUDA_OK(cudaFuncSetAttribute(attn_fwd_kernel<HD>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
     attr = true;
   }
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(p.nh * (SPLIT ? 2 : 1), p.B, (p.T + BQ - 1) / BQ);
-  cfg.blockDim = dim3(ATT_THREADS);
-  cfg.dynamicSmemBytes = SMEM;
-  cfg.stream = st;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeClusterDimension;
-  at[0].val.clusterDim.x = SPLIT ? 2 : 1; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-  cfg.attrs = at; cfg.numAttrs = 1;
-  static bool verbose = getenv("LMOD_ATTN_VERBOSE") != nullptr;
-  if (verbose) {
-    int ncl = -1, nb = -1;
-    cudaOccupancyMaxActiveClusters(&ncl, attn_fwd_kernel<HD, TRACE, SPLIT, REGCAP>, &cfg);
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, attn_fwd_kernel<HD, TRACE, SPLIT, REGCAP>, ATT_THREADS, SMEM);
-    cudaFuncAttributes fa = {};
-    cudaFuncGetAttributes(&fa, attn_fwd_kernel<HD, TRACE, SPLIT, REGCAP>);
-    fprintf(stderr, "[lmod] attn_fwd_kernel<%d,%d,%d,%d> grid (%u,%u,%u) cluster %d: %d co-resident clusters, %d CTAs/SM (regs %d, static smem %zu, dynamic %d, local %zu)\n",
-            HD, (int)TRACE, (int)SPLIT, (int)REGCAP, cfg.gridDim.x, cfg.gridDim.y, cfg.gridDim.z, SPLIT ? 2 : 1, ncl, nb, fa.numRegs, fa.sharedSizeBytes, SMEM,
-            fa.localSizeBytes);
-    verbose = false;
-  }
-  LMOD_CUDA_OK(cudaLaunchKernelEx(&cfg, attn_fwd_kernel<HD, TRACE, SPLIT, REGCAP>, tq, tkv, p));
-  lmod_count_launch();
+  const dim3 grid(p.nh, p.B, (p.T + BQ - 1) / BQ);
+  attn_fwd_kernel<HD><<<grid, ATT_THREADS, SMEM, st>>>(tq, tkv, p);
+  LMOD_LAUNCH_OK();
   return LMOD_OK;
-}
-
-// LMOD_ATTN_SPLIT=1: split every query block's keys over a CTA pair (SPLIT above).  Off by default: measured on the shapes it was built for
-// (T 2048 x 16 heads, the CLIP tower) it changes nothing -- cluster launches lose the second co-resident CTA per SM, which costs what the
-// shorter critical path gains (profiles/attn_shapes_r2.txt).  Kept because it is verified (tests/test_attn_gpu.py runs it in a child
-// process) and is the building block for a decode-shaped grid.
-bool attn_split_wanted(const AttnParams&) {
-  static int mode = -1;
-  if (mode < 0) { const char* e = getenv("LMOD_ATTN_SPLIT"); mode = (e && e[0] == '1') ? 1 : 0; }
-  return mode == 1;
 }
 
 }  // namespace
@@ -454,9 +247,9 @@ bool attn_split_wanted(const AttnParams&) {
 // qkv: fused projection output [batch*seq, (nh + 2*nkv)*hd] bf16 (q heads | k heads | v heads), row stride ld_qkv.
 // out: [batch*seq, nh*hd] (row stride ld_o).  lse: [batch, nh, seq] fp32 or NULL.  hd in {64, 128}.
 // kv_lo / kv_hi: int32 [batch] device arrays, the real (un-padded) key range of every batch row, or both NULL for no padding.
-static int attn_fwd_impl(const void* qkv, int64_t ld_qkv, int64_t batch, int64_t seq, int nh, int nkv, int hd, int causal,
-                         float softmax_scale, void* out, int64_t ld_o, float* lse, const int32_t* kv_lo, const int32_t* kv_hi,
-                         long long* trace, void* stream) {
+extern "C" int lmod_attn_fwd(const void* qkv, int64_t ld_qkv, int64_t batch, int64_t seq, int nh, int nkv, int hd, int causal,
+                             float softmax_scale, void* out, int64_t ld_o, float* lse, const int32_t* kv_lo, const int32_t* kv_hi,
+                             void* stream) {
   LMOD_CHECK_ARG((kv_lo == nullptr) == (kv_hi == nullptr), "lmod_attn_fwd: kv_lo and kv_hi come together");
   LMOD_CHECK_ARG(qkv && out && batch > 0 && seq > 0 && nh > 0 && nkv > 0 && nh % nkv == 0, "lmod_attn_fwd: bad arguments");
   LMOD_CHECK_ARG(hd == 64 || hd == 128, "lmod_attn_fwd: head_dim %d not built (64 and 128 are)", hd);
@@ -465,36 +258,11 @@ static int attn_fwd_impl(const void* qkv, int64_t ld_qkv, int64_t batch, int64_t
   const uint64_t cols = (uint64_t)(nh + 2 * nkv) * hd, rows = (uint64_t)(batch * seq);
   int rc = make_map(&tq, qkv, cols, rows, (uint64_t)ld_qkv, 64, BQ);
   if (rc) return rc;
-  rc = make_map(&tkv, qkv, cols, rows, (uint64_t)ld_qkv, 64, BKV);
+  rc = make_map(&tkv, qkv, cols, rows, (uint64_t)ld_qkv, 64, hd == 128 ? AttCfg<128>::BKV : AttCfg<64>::BKV);
   if (rc) return rc;
   AttnParams p;
   p.out = (__nv_bfloat16*)out; p.lse = lse; p.ld_o = ld_o; p.B = (int)batch; p.T = (int)seq; p.nh = nh; p.nkv = nkv; p.causal = causal;
   p.scale_log2 = softmax_scale * LOG2E_F;
-  p.kv_lo = kv_lo; p.kv_hi = kv_hi; p.trace = trace;
-  cudaStream_t st = (cudaStream_t)stream;
-  static int cap = -1;                                  // LMOD_ATTN_REGCAP = 0 | 1 overrides the per-head-dim default (hd 64: capped, hd 128: not)
-  if (cap < 0) { const char* e = getenv("LMOD_ATTN_REGCAP"); cap = (e && (e[0] == '0' || e[0] == '1')) ? e[0] - '0' : 2; }
-  const bool regcap = cap == 2 ? hd == 64 : cap == 1;
-  const bool split = !trace && attn_split_wanted(p);
-#define ATT_GO(H, T, S) (regcap ? launch_attn<H, T, S, true>(tq, tkv, p, st) : launch_attn<H, T, S, false>(tq, tkv, p, st))
-  if (trace) return hd == 128 ? ATT_GO(128, true, false) : ATT_GO(64, true, false);
-  if (split) return hd == 128 ? ATT_GO(128, false, true) : ATT_GO(64, false, true);
-  return hd == 128 ? ATT_GO(128, false, false) : ATT_GO(64, false, false);
-#undef ATT_GO
-}
-
-extern "C" int lmod_attn_fwd(const void* qkv, int64_t ld_qkv, int64_t batch, int64_t seq, int nh, int nkv, int hd, int causal,
-                             float softmax_scale, void* out, int64_t ld_o, float* lse, const int32_t* kv_lo, const int32_t* kv_hi,
-                             void* stream) {
-  return attn_fwd_impl(qkv, ld_qkv, batch, seq, nh, nkv, hd, causal, softmax_scale, out, ld_o, lse, kv_lo, kv_hi, nullptr, stream);
-}
-
-// Diagnostics (profiles/attn_trace.py): the same kernel compiled with clock64 stamps at the pipeline hand-offs of head 0's CTAs.
-// trace: int64 [ceil(seq/128)][64][16] device buffer, zero-filled by the caller (seq <= 4096).  Slots per key block: 0-6 softmax warp
-// (before s_full wait, after it, after tcgen05.ld, after the max exchange, after exp, before the P store, after the p_full arrive),
-// 7-11 MMA thread (top of iteration, after issuing S_{j+1}, after p_full, after v_full, after issuing P*V).
-extern "C" int lmod_attn_fwd_trace(const void* qkv, int64_t ld_qkv, int64_t batch, int64_t seq, int nh, int nkv, int hd, int causal,
-                                   float softmax_scale, void* out, int64_t ld_o, float* lse, long long* trace, void* stream) {
-  LMOD_CHECK_ARG(trace != nullptr && seq <= 4096, "lmod_attn_fwd_trace: trace buffer missing or seq > 4096");
-  return attn_fwd_impl(qkv, ld_qkv, batch, seq, nh, nkv, hd, causal, softmax_scale, out, ld_o, lse, nullptr, nullptr, trace, stream);
+  p.kv_lo = kv_lo; p.kv_hi = kv_hi;
+  return hd == 128 ? launch_attn<128>(tq, tkv, p, (cudaStream_t)stream) : launch_attn<64>(tq, tkv, p, (cudaStream_t)stream);
 }

@@ -1,24 +1,24 @@
-// attn_bwd.cu -- flash-attention BACKWARD on tcgen05 / TMEM / TMA (sm_100a).
+// attn_bwd.cu -- flash-attention BACKWARD on wgmma / TMA (sm_90a).
 //
 // Backward of Qwen2SdpaAttention's scaled_dot_product_attention (modeling_qwen2.py:713-721) for the sparse student: given the fused
 // RoPE'd QKV buffer, the forward output O, dO and the log-sum-exp of the forward kernel, produces dQ|dK|dV in one fused buffer.
 //
 // One CTA owns a block of 128 keys of one (batch, kv-head) and sweeps the 64-query blocks (and the query heads of its GQA group) that can
-// see it.  Five tensor-core products per (key block, query block), all issued by one thread, accumulators in TMEM:
-//     S^T  = K_j Q_i^T            (SS, M=128 N=64)        dP^T = V_j dO_i^T        (SS, M=128 N=64)
-//     dV_j += P^T  dO_i           (TS: A = P^T  bf16 in TMEM, B = dO_i MN-major)   accumulates over the whole sweep
-//     dK_j += dS^T Q_i            (TS: A = dS^T bf16 in TMEM, B = Q_i  MN-major)   accumulates over the whole sweep
-//     dQ_i  = dS K_j              (SS, M=64: A = dS written to 128B-swizzled smem by the softmax threads, MN-major; B = K_j re-read MN-major)
-// 256 softmax threads, two per key row (TMEM lane = key, 32 query columns each): P = exp2(S*c - lse), dS = P (dP - D) * scale with
-// lse / D broadcast per query column.  Four more warps drain dQ_i to an fp32 workspace with red.global.add.v4 (a key block only holds
-// a partial dQ) off the critical path; for head_dim 64 the score accumulators are double-buffered so that the tensor core computes
-// S/dP of the next query block while the softmax threads work on the current one.
-#include "tc05.cuh"
+// see it.  Warpgroup 0 is the TMA producer (K_j, V_j once; Q_i / dO_i through a 2-stage ring); math warpgroups 1 and 2 own 64 keys each
+// and keep their dK_j, dV_j accumulators in registers for the whole sweep.  Per (key block, query block):
+//     S^T  = K_j Q_i^T,  dP^T = V_j dO_i^T      (wgmma, both operands from shared memory, M = 64 keys, N = 64 queries)
+//     P^T  = exp2(S^T c - lse),  dS^T = P^T (dP^T - D) scale      (registers; lse / D per query column)
+//     dV_j += P^T dO_i,  dK_j += dS^T Q_i       (wgmma, A = P^T / dS^T straight from registers, B = dO_i / Q_i MN-major)
+//     dQ_i  = dS K_j                            (wgmma over all 128 keys, A = dS written to 128B-swizzled shared memory by both math
+//                                                warpgroups, MN-major; B = K_j MN-major) -- computed by warpgroup 1 + (i mod 2) and
+//                                                added into an fp32 workspace with red.global.add (a key block only holds a partial dQ)
+#include "sm90.cuh"
 
 namespace {
 
 constexpr int BKVB = 128, BQB = 64;
-constexpr int ATB_THREADS = 448;     // TMA, MMA, 8 softmax warps, 4 dQ-drain warps
+constexpr int ATB_THREADS = 384;     // TMA warpgroup + two math warpgroups
+constexpr int NQ = 2;                // Q_i / dO_i ring
 
 struct AttnBwdParams {
   const float* lse;       // [B, nh, T]
@@ -33,24 +33,13 @@ struct AttnBwdParams {
   const int32_t* kv_hi;
 };
 
-__device__ __forceinline__ uint32_t bwd_idesc(int m, int n, bool a_mn, bool b_mn) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((a_mn ? 1u : 0u) << 15) | ((b_mn ? 1u : 0u) << 16) | ((uint32_t)(n >> 3) << 17) |
-         ((uint32_t)(m >> 4) << 24);
+__device__ __forceinline__ void red_add_v2(float* dst, float a, float b) {
+  asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" :: "l"(dst), "f"(a), "f"(b) : "memory");
 }
-__device__ __forceinline__ void tmem_ld16(uint32_t addr, uint32_t* r) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-                 "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-               : "r"(addr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void red_add_v4(float* dst, const uint32_t* r) {
-  asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" :: "l"(dst), "f"(__uint_as_float(r[0])), "f"(__uint_as_float(r[1])),
-               "f"(__uint_as_float(r[2])), "f"(__uint_as_float(r[3])) : "memory");
-}
-__device__ __forceinline__ void tmem_st8(uint32_t addr, const uint32_t* r) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};"
-               :: "r"(addr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]) : "memory");
+template <int N>
+__device__ __forceinline__ void wgmma_rs_b_mn(float* d, const uint32_t* a, uint64_t db, uint32_t acc) {
+  if constexpr (N == 128) wgmma_rs_n128<1>(d, a, db, acc);
+  else wgmma_rs_n64<1>(d, a, db, acc);
 }
 
 template <int HD>
@@ -58,21 +47,17 @@ __global__ void __launch_bounds__(ATB_THREADS, 1)
 attn_bwd_kernel(const __grid_constant__ CUtensorMap tma_kv, const __grid_constant__ CUtensorMap tma_q, const __grid_constant__ CUtensorMap tma_do,
                 const AttnBwdParams p) {
   constexpr int KSUB = HD / 64;
-  constexpr int NQ = 3;                                // Q_i / dO_i ring
-  constexpr int NBUF = (HD == 64) ? 2 : 1;             // S^T/dP^T (and dS smem) double-buffered when TMEM has room: 2*HD + NBUF*128 + 64 <= 512
   constexpr int KV_BYTES = BKVB * HD * 2;              // one of K_j / V_j
   constexpr int Q_BYTES = BQB * HD * 2;                // one of Q_i / dO_i
   constexpr int DS_BYTES = BKVB * BQB * 2;
   extern __shared__ uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t kv_full, q_full[NQ], q_empty[NQ], s_full[2], ds_ready[2], dq_full, dq_empty, acc_full;
-  __shared__ uint32_t tmem_slot;
-  __shared__ __align__(16) float s_lse2[2][BQB], s_dsum[2][BQB];      // per query block: lse*log2(e) and D, double buffered
+  __shared__ __align__(8) uint64_t kv_full, q_full[NQ], q_empty[NQ];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t* sK = smem;
   uint8_t* sV = sK + KV_BYTES;
   uint8_t* sQ = sV + KV_BYTES;                         // stage s: Q at sQ + s*2*Q_BYTES, dO right after
-  uint8_t* sDS = sQ + NQ * 2 * Q_BYTES;                // NBUF buffers of DS_BYTES
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  uint8_t* sDS = sQ + NQ * 2 * Q_BYTES;                // 2 buffers of DS_BYTES (by iteration parity)
+  const int wg = threadIdx.x >> 7;
 
   // heavy key blocks (small j under the causal mask) are scheduled first: j is the slowest grid index
   const int j = blockIdx.z, hk = blockIdx.x, b = blockIdx.y;
@@ -92,264 +77,165 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tma_kv, const __grid_constan
 
   if (threadIdx.x == 0) {
     mbar_init(&kv_full, 1);
-    for (int s = 0; s < NQ; ++s) { mbar_init(&q_full[s], 1); mbar_init(&q_empty[s], 1); }
-    for (int s = 0; s < 2; ++s) { mbar_init(&s_full[s], 1); mbar_init(&ds_ready[s], 8); }
-    mbar_init(&dq_full, 1); mbar_init(&dq_empty, 4); mbar_init(&acc_full, 1);
+    for (int s = 0; s < NQ; ++s) { mbar_init(&q_full[s], 1); mbar_init(&q_empty[s], 2); }
     mbar_fence_init();
     asm volatile("prefetch.tensormap [%0];" :: "l"(&tma_kv) : "memory");
     asm volatile("prefetch.tensormap [%0];" :: "l"(&tma_q) : "memory");
     asm volatile("prefetch.tensormap [%0];" :: "l"(&tma_do) : "memory");
   }
-  if (warp == 1) tmem_alloc(&tmem_slot, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = tmem_slot;
-  const uint32_t tDK = tmem, tDV = tmem + HD, tS0 = tmem + 2 * HD, tDQ = tS0 + NBUF * 2 * BQB;   // buffer b: S^T at tS0 + b*128, dP^T 64 columns later; dQ: HD columns
 
-  if (warp == 0 && lane == 0) {
+  if (wg == 0) {
     // ===================== TMA producer =====================
-    mbar_expect_tx(&kv_full, 2 * KV_BYTES);
-#pragma unroll
-    for (int i = 0; i < KSUB; ++i) {
-      tma_load_2d(sK + i * (BKVB * 128), &tma_kv, col_k + 64 * i, row_base + kv0, &kv_full);
-      tma_load_2d(sV + i * (BKVB * 128), &tma_kv, col_v + 64 * i, row_base + kv0, &kv_full);
-    }
-    for (int it = 0; it < n_it; ++it) {
-      const int s = it % NQ;
-      const int h = hk * group + it / n_i, qi = i_start + it % n_i;
-      mbar_wait_bounded(&q_empty[s], ((it / NQ) & 1) ^ 1);
-      uint8_t* q = sQ + s * 2 * Q_BYTES;
-      uint8_t* d = q + Q_BYTES;
-      mbar_expect_tx(&q_full[s], 2 * Q_BYTES);
+    regs_dealloc<40>();
+    if (threadIdx.x == 0) {
+      mbar_expect_tx(&kv_full, 2 * KV_BYTES);
 #pragma unroll
       for (int i = 0; i < KSUB; ++i) {
-        tma_load_2d(q + i * (BQB * 128), &tma_q, h * HD + 64 * i, row_base + qi * BQB, &q_full[s]);
-        tma_load_2d(d + i * (BQB * 128), &tma_do, h * HD + 64 * i, row_base + qi * BQB, &q_full[s]);
+        tma_load_2d(sK + i * (BKVB * 128), &tma_kv, col_k + 64 * i, row_base + kv0, &kv_full);
+        tma_load_2d(sV + i * (BKVB * 128), &tma_kv, col_v + 64 * i, row_base + kv0, &kv_full);
       }
-    }
-  } else if (warp == 1 && lane == 0) {
-    // ===================== MMA issuer =====================
-    const uint32_t id_s = bwd_idesc(128, BQB, false, false);       // S^T, dP^T
-    const uint32_t id_acc = bwd_idesc(128, HD, false, true);       // dV, dK   (A from TMEM, B MN-major)
-    const uint32_t id_dq = bwd_idesc(BQB, HD, true, true);         // dQ       (A = dS MN-major: 64 queries contiguous per key row, B = K_j MN-major)
-    const uint32_t aK = smem_u32(sK), aV = smem_u32(sV);
-    // S^T = K Q^T and dP^T = V dO^T of iteration `it` into buffer it % NBUF
-    auto issue_scores = [&](int it) {
-      const int s = it % NQ, buf = it % NBUF;
-      const uint32_t aQ = smem_u32(sQ + s * 2 * Q_BYTES), aDO = aQ + Q_BYTES;
-      const uint32_t tS = tS0 + buf * 2 * BQB, tDP = tS + BQB;
-      mbar_wait_bounded(&q_full[s], (it / NQ) & 1);
-      tc_fence_after();
-#pragma unroll
-      for (int k = 0; k < HD / 16; ++k) {
-        const uint32_t ko = (k / 4), ki = (k % 4) * 32;
-        umma_f16(tS, smem_desc(aK + ko * (BKVB * 128) + ki, 16, 1024), smem_desc(aQ + ko * (BQB * 128) + ki, 16, 1024), id_s, k > 0 ? 1u : 0u);
-      }
-#pragma unroll
-      for (int k = 0; k < HD / 16; ++k) {
-        const uint32_t ko = (k / 4), ki = (k % 4) * 32;
-        umma_f16(tDP, smem_desc(aV + ko * (BKVB * 128) + ki, 16, 1024), smem_desc(aDO + ko * (BQB * 128) + ki, 16, 1024), id_s, k > 0 ? 1u : 0u);
-      }
-      umma_commit(&s_full[buf]);
-    };
-    // dV += P^T dO, dK += dS^T Q, dQ = dS K of iteration `it`
-    auto issue_grads = [&](int it) {
-      const int s = it % NQ, buf = it % NBUF;
-      const uint32_t aQ = smem_u32(sQ + s * 2 * Q_BYTES), aDO = aQ + Q_BYTES, aDS = smem_u32(sDS + buf * DS_BYTES);
-      const uint32_t tS = tS0 + buf * 2 * BQB, tDP = tS + BQB;
-      mbar_wait_bounded(&ds_ready[buf], (it / NBUF) & 1);
-      if (it > 0) mbar_wait_bounded(&dq_empty, (it - 1) & 1);
-      tc_fence_after();
-#pragma unroll
-      for (int k = 0; k < BQB / 16; ++k) {         // reduction over the 64 queries of the block
-        const uint32_t ka = (k >> 1) * 32 + (k & 1) * 8;       // 16 queries = 8 bf16x2 columns; the second 32 queries start at column 32
-        umma_f16_ts(tDV, tS + ka, smem_desc(aDO + k * 2048, BQB * 128, 1024), id_acc, (it > 0 || k > 0) ? 1u : 0u);
-        umma_f16_ts(tDK, tDP + ka, smem_desc(aQ + k * 2048, BQB * 128, 1024), id_acc, (it > 0 || k > 0) ? 1u : 0u);
-      }
-#pragma unroll
-      for (int k = 0; k < BKVB / 16; ++k) {        // reduction over the 128 keys
-        umma_f16(tDQ, smem_desc(aDS + k * 2048, 16, 1024), smem_desc(aK + k * 2048, BKVB * 128, 1024), id_dq, k > 0 ? 1u : 0u);
-      }
-      umma_commit(&q_empty[s]);
-      umma_commit(&dq_full);
-    };
-    mbar_wait_bounded(&kv_full, 0);
-    if (NBUF == 2) {
-      // scores of it+1 are in flight (other S buffer, other Q stage) while the softmax threads work on it
-      issue_scores(0);
       for (int it = 0; it < n_it; ++it) {
-        if (it + 1 < n_it) issue_scores(it + 1);
-        issue_grads(it);
+        const int s = it % NQ;
+        const int h = hk * group + it / n_i, qi = i_start + it % n_i;
+        mbar_wait_bounded(&q_empty[s], ((it / NQ) & 1) ^ 1);
+        uint8_t* q = sQ + s * 2 * Q_BYTES;
+        uint8_t* d = q + Q_BYTES;
+        mbar_expect_tx(&q_full[s], 2 * Q_BYTES);
+#pragma unroll
+        for (int i = 0; i < KSUB; ++i) {
+          tma_load_2d(q + i * (BQB * 128), &tma_q, h * HD + 64 * i, row_base + qi * BQB, &q_full[s]);
+          tma_load_2d(d + i * (BQB * 128), &tma_do, h * HD + 64 * i, row_base + qi * BQB, &q_full[s]);
+        }
       }
-    } else {
-      for (int it = 0; it < n_it; ++it) { issue_scores(it); issue_grads(it); }
     }
-    umma_commit(&acc_full);
-  } else if (warp >= 2 && warp < 10) {
-    // ===================== softmax / dS: two threads per key row (32 of the 64 query columns each) =====================
-    const int q = warp & 3;
-    const int g = (warp - 2) >> 2;
-    const int r = q * 32 + lane;
-    const int kv = kv0 + r;
-    const uint32_t lane_off = (uint32_t)(q * 32) << 16;
-    // lse*log2(e) and D of a query block are staged one iteration ahead: the first 128 threads (g == 0) load them from global memory
-    // before waiting on the scores and publish them after their own math, so the L2 latency is off the critical path
-    auto stage_load = [&](int it) -> float {
-      const int h = hk * group + it / n_i, q0 = (i_start + it % n_i) * BQB;
-      const int qc = min(q0 + (r & 63), p.T - 1);                       // rows >= T are masked below, clamp the address
-      const int64_t base = ((int64_t)b * p.nh + h) * p.T + qc;
-      return (r < 64) ? __ldg(p.lse + base) * LOG2E_F : __ldg(p.dsum + base);
-    };
-    auto stage_store = [&](int it, float v) {
-      if (r < 64) s_lse2[it & 1][r & 63] = v; else s_dsum[it & 1][r & 63] = v;
-    };
-    if (g == 0 && n_it > 0) stage_store(0, stage_load(0));
-    asm volatile("bar.sync 1, 256;" ::: "memory");
-    for (int it = 0; it < n_it; ++it) {
-      const int qi = i_start + it % n_i;
-      const int q0 = qi * BQB;
-      const int buf = it % NBUF;
-      const uint32_t tS = tS0 + buf * 2 * BQB, tDP = tS + BQB;
-      uint8_t* ds_row = sDS + buf * DS_BYTES + r * 128;
-      float staged = 0.f;
-      const bool prefetch = (g == 0) && (it + 1 < n_it);
-      if (prefetch) staged = stage_load(it + 1);
-      const float* lse2 = s_lse2[it & 1] + g * 32;
-      const float* dsm_s = s_dsum[it & 1] + g * 32;
-      // only the blocks on the causal diagonal and the ragged tail need per-element masks
-      const bool masked = padded || (q0 + BQB > p.T) || (kv0 + BKVB > p.T) || (p.causal && q0 < kv0 + BKVB - 1);
-      mbar_wait_warp(&s_full[buf], (it / NBUF) & 1);
-      tc_fence_after();
-      uint32_t sv[32], dv[32];
-      tmem_ld32(tS + g * 32 + lane_off, sv);
-      tmem_ld32(tDP + g * 32 + lane_off, dv);
-      uint32_t pk[16], dk[16];
-      if (masked) {
+    return;
+  }
+
+  // ===================== math warpgroups =====================
+  regs_alloc<232>();
+  const int c = wg - 1;
+  const int w = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+  const bool wg_leader = (threadIdx.x & 127) == 0;
+  const int kr = c * 64 + w * 16 + (lane >> 2);        // key row (within the block) of fragment rows h = 0; h = 1 is kr + 8
+  const int cq = 2 * (lane & 3);
+  const uint32_t aK = smem_u32(sK), aV = smem_u32(sV);
+  float dk[HD / 2], dv[HD / 2];
 #pragma unroll
-        for (int c = 0; c < 32; c += 2) {
-          float pp[2], dd[2];
+  for (int i = 0; i < HD / 2; ++i) { dk[i] = 0.f; dv[i] = 0.f; }
+  mbar_wait(&kv_full, 0);
+  for (int it = 0; it < n_it; ++it) {
+    const int s = it % NQ, buf = it & 1;
+    const int h = hk * group + it / n_i, qi = i_start + it % n_i;
+    const int q0 = qi * BQB;
+    const uint32_t aQ = smem_u32(sQ + s * 2 * Q_BYTES), aDO = aQ + Q_BYTES;
+    const int64_t lbase = ((int64_t)b * p.nh + h) * p.T;
+    // only the blocks on the causal diagonal and the ragged tail need per-element masks
+    const bool masked = padded || (q0 + BQB > p.T) || (kv0 + BKVB > p.T) || (p.causal && q0 < kv0 + BKVB - 1);
+
+    float sacc[32], dpacc[32];
+    mbar_wait(&q_full[s], (it / NQ) & 1);
+    wgmma_fence();
 #pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            const int qidx = q0 + g * 32 + c + e;
-            const bool seen = (all_pad || qidx < lo) ? true : (kv >= lo && kv < hi && (!p.causal || kv <= qidx));
-            const bool ok = (qidx < p.T) && (kv < p.T) && seen;
-            const float pv = ok ? ex2f(fmaf(__uint_as_float(sv[c + e]), p.scale_log2, -lse2[c + e])) : 0.f;
-            pp[e] = pv;
-            dd[e] = pv * (__uint_as_float(dv[c + e]) - dsm_s[c + e]) * p.scale;
-          }
-          pk[c >> 1] = pack_bf16x2(pp[0], pp[1]);
-          dk[c >> 1] = pack_bf16x2(dd[0], dd[1]);
+    for (int k = 0; k < HD / 16; ++k) {
+      const uint32_t ko = (k / 4), ki = (k % 4) * 32;
+      wgmma_ss_n64<0, 0>(sacc, gmma_desc(aK + ko * (BKVB * 128) + c * (64 * 128) + ki, 16, 1024), gmma_desc(aQ + ko * (BQB * 128) + ki, 16, 1024), k > 0 ? 1u : 0u);
+    }
+#pragma unroll
+    for (int k = 0; k < HD / 16; ++k) {
+      const uint32_t ko = (k / 4), ki = (k % 4) * 32;
+      wgmma_ss_n64<0, 0>(dpacc, gmma_desc(aV + ko * (BKVB * 128) + c * (64 * 128) + ki, 16, 1024), gmma_desc(aDO + ko * (BQB * 128) + ki, 16, 1024), k > 0 ? 1u : 0u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence<32>(sacc);
+    reg_fence<32>(dpacc);
+
+    // P^T, dS^T: fragment register 4i + 2hh + e = key kr + 8hh, query q0 + 8i + cq + e
+    uint32_t pa[4][4], da[4][4];
+    uint8_t* dsb = sDS + buf * DS_BYTES;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const int qa = min(q0 + 8 * i + cq, p.T - 1), qb = min(q0 + 8 * i + cq + 1, p.T - 1);   // rows >= T are masked below
+      const float2 l2 = make_float2(__ldg(p.lse + lbase + qa) * LOG2E_F, __ldg(p.lse + lbase + qb) * LOG2E_F);
+      const float2 dd = make_float2(__ldg(p.dsum + lbase + qa), __ldg(p.dsum + lbase + qb));
+      float pv[4], ds[4];
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int kv = kv0 + kr + 8 * (e >> 1), qidx = q0 + 8 * i + cq + (e & 1);
+        bool ok = true;
+        if (masked) {
+          const bool seen = (all_pad || qidx < lo) ? true : (kv >= lo && kv < hi && (!p.causal || kv <= qidx));
+          ok = (qidx < p.T) && (kv < p.T) && seen;
         }
-      } else {
-#pragma unroll
-        for (int c = 0; c < 32; c += 2) {
-          float pp[2], dd[2];
-#pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            const float pv = ex2f(fmaf(__uint_as_float(sv[c + e]), p.scale_log2, -lse2[c + e]));
-            pp[e] = pv;
-            dd[e] = pv * (__uint_as_float(dv[c + e]) - dsm_s[c + e]) * p.scale;
-          }
-          pk[c >> 1] = pack_bf16x2(pp[0], pp[1]);
-          dk[c >> 1] = pack_bf16x2(dd[0], dd[1]);
-        }
+        const float lsev = (e & 1) ? l2.y : l2.x, dsv = (e & 1) ? dd.y : dd.x;
+        pv[e] = ok ? ex2f(fmaf(sacc[4 * i + e], p.scale_log2, -lsev)) : 0.f;
+        ds[e] = pv[e] * (dpacc[4 * i + e] - dsv) * p.scale;
       }
-      // P^T over S^T, dS^T over dP^T (bf16x2: this thread's 32 queries = 16 columns)
-      // each thread overwrites only columns it has read itself (its partner on the same row runs unsynchronised): queries 32g..32g+31
-      // land in columns 32g..32g+15
-      tmem_st8(tS + g * 32 + lane_off, pk);
-      tmem_st8(tS + g * 32 + 8 + lane_off, pk + 8);
-      tmem_st8(tDP + g * 32 + lane_off, dk);
-      tmem_st8(tDP + g * 32 + 8 + lane_off, dk + 8);
+      pa[i >> 1][(i & 1) * 2 + 0] = pack_bf16x2(pv[0], pv[1]);
+      pa[i >> 1][(i & 1) * 2 + 1] = pack_bf16x2(pv[2], pv[3]);
+      da[i >> 1][(i & 1) * 2 + 0] = pack_bf16x2(ds[0], ds[1]);
+      da[i >> 1][(i & 1) * 2 + 1] = pack_bf16x2(ds[2], ds[3]);
       // dS for dQ = dS K: row = key, 64 queries contiguous (MN-major A operand), 128B swizzle (16-byte chunk ^ (row & 7))
 #pragma unroll
-      for (int ch = 0; ch < 4; ++ch) {
-        const int cidx = g * 4 + ch;
-        uint4 w = make_uint4(dk[ch * 4], dk[ch * 4 + 1], dk[ch * 4 + 2], dk[ch * 4 + 3]);
-        *reinterpret_cast<uint4*>(ds_row + ((cidx ^ (r & 7)) << 4)) = w;
-      }
-      tmem_st_wait();
-      fence_proxy_async();                               // generic-proxy smem writes -> visible to the tensor core (async proxy)
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&ds_ready[buf]);
-      if (prefetch) stage_store(it + 1, staged);
-      asm volatile("bar.sync 1, 256;" ::: "memory");     // next block's lse / D visible; this block's are free to be overwritten
-    }
-    // ---- dK_j, dV_j epilogue: the two threads of a row split the 32-column chunks ----
-    mbar_wait_warp(&acc_full, 0);
-    tc_fence_after();
-    {
-      // tcgen05.ld is warp-collective (.sync.aligned): every lane executes the loads, only the stores are predicated on the row
-      const bool row_ok = kv < p.T;
-      __nv_bfloat16* dkrow = p.dqkv + (int64_t)(row_base + kv) * p.ld_dqkv + col_k;
-      __nv_bfloat16* dvrow = p.dqkv + (int64_t)(row_base + kv) * p.ld_dqkv + col_v;
-#pragma unroll
-      for (int cc = 0; cc < HD / 64; ++cc) {
-        const int c = cc * 2 + g;
-        uint32_t o[32];
-        tmem_ld32(tDK + c * 32 + lane_off, o);
-        if (row_ok) {
-#pragma unroll
-          for (int v = 0; v < 4; ++v) {
-            uint4 w;
-            w.x = pack_bf16x2(__uint_as_float(o[v * 8 + 0]), __uint_as_float(o[v * 8 + 1]));
-            w.y = pack_bf16x2(__uint_as_float(o[v * 8 + 2]), __uint_as_float(o[v * 8 + 3]));
-            w.z = pack_bf16x2(__uint_as_float(o[v * 8 + 4]), __uint_as_float(o[v * 8 + 5]));
-            w.w = pack_bf16x2(__uint_as_float(o[v * 8 + 6]), __uint_as_float(o[v * 8 + 7]));
-            *reinterpret_cast<uint4*>(dkrow + c * 32 + v * 8) = w;
-          }
-        }
-        tmem_ld32(tDV + c * 32 + lane_off, o);
-        if (row_ok) {
-#pragma unroll
-          for (int v = 0; v < 4; ++v) {
-            uint4 w;
-            w.x = pack_bf16x2(__uint_as_float(o[v * 8 + 0]), __uint_as_float(o[v * 8 + 1]));
-            w.y = pack_bf16x2(__uint_as_float(o[v * 8 + 2]), __uint_as_float(o[v * 8 + 3]));
-            w.z = pack_bf16x2(__uint_as_float(o[v * 8 + 4]), __uint_as_float(o[v * 8 + 5]));
-            w.w = pack_bf16x2(__uint_as_float(o[v * 8 + 6]), __uint_as_float(o[v * 8 + 7]));
-            *reinterpret_cast<uint4*>(dvrow + c * 32 + v * 8) = w;
-          }
-        }
+      for (int hh = 0; hh < 2; ++hh) {
+        const int row = kr + 8 * hh;
+        *reinterpret_cast<uint32_t*>(dsb + row * 128 + ((i ^ (row & 7)) << 4) + 2 * cq) = da[i >> 1][(i & 1) * 2 + hh];
       }
     }
-  } else if (warp >= 10) {
-    // ===================== dQ_i drain: M = 64 accumulator, query row (16*quarter + lane) in lanes 0..15 of every quarter, columns = head dim;
-    // vector fp32 red.add into the workspace (a key block only holds a partial dQ) =====================
-    const int q = warp & 3;
-    const uint32_t lane_off = (uint32_t)(q * 32) << 16;
-    const int row = q * 16 + lane;
-    for (int it = 0; it < n_it; ++it) {
-      const int h = hk * group + it / n_i, qi = i_start + it % n_i;
-      const int q0 = qi * BQB;
-      const bool row_ok = (lane < 16) && (q0 + row < p.T);
-      float* dst = p.dq32 + (int64_t)(row_base + q0 + row) * p.ld_dq32 + h * HD;
-      mbar_wait_warp(&dq_full, it & 1);
-      tc_fence_after();
+    fence_proxy_async();                               // generic-proxy smem writes -> visible to the tensor core (async proxy)
+    named_bar(1, 256);                                 // both halves of dS are in shared memory
+
+    wgmma_fence();
 #pragma unroll
-      for (int c = 0; c < HD / 64; ++c) {
-        uint32_t o0[32], o1[32];
-        tmem_ld32(tDQ + c * 64 + lane_off, o0);
-        tmem_ld32(tDQ + c * 64 + 32 + lane_off, o1);
-        if (c == HD / 64 - 1) {
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&dq_empty);                        // registers hold the tile: the tensor core may overwrite dQ now
-        }
-        if (row_ok) {
+    for (int kk = 0; kk < 4; ++kk) {                   // reduction over the 64 queries of the block
+      wgmma_rs_b_mn<HD>(dv, pa[kk], gmma_desc(aDO + kk * 2048, BQB * 128, 1024), 1u);
+      wgmma_rs_b_mn<HD>(dk, da[kk], gmma_desc(aQ + kk * 2048, BQB * 128, 1024), 1u);
+    }
+    wgmma_commit();
+    if ((it & 1) == c) {
+      // dQ_i = dS K_j over the 128 keys, 64 head-dim columns per pass
+      const int row = q0 + w * 16 + (lane >> 2);
+      float* dst = p.dq32 + (int64_t)(row_base + row) * p.ld_dq32 + h * HD + cq;
 #pragma unroll
-          for (int v = 0; v < 8; ++v) red_add_v4(dst + c * 64 + v * 4, o0 + v * 4);
+      for (int ps = 0; ps < KSUB; ++ps) {
+        float dq[32];
+        wgmma_fence();
 #pragma unroll
-          for (int v = 0; v < 8; ++v) red_add_v4(dst + c * 64 + 32 + v * 4, o1 + v * 4);
-        }
+        for (int k = 0; k < BKVB / 16; ++k)
+          wgmma_ss_n64<1, 1>(dq, gmma_desc(smem_u32(dsb) + k * 2048, BQB * 128, 1024),
+                             gmma_desc(aK + ps * (BKVB * 128) + k * 2048, BKVB * 128, 1024), k > 0 ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<0>();
+        reg_fence<32>(dq);
+#pragma unroll
+        for (int i = 0; i < 8; ++i)
+#pragma unroll
+          for (int hh = 0; hh < 2; ++hh)
+            if (row + 8 * hh < p.T) red_add_v2(dst + (int64_t)8 * hh * p.ld_dq32 + ps * 64 + 8 * i, dq[4 * i + 2 * hh], dq[4 * i + 2 * hh + 1]);
       }
+    }
+    wgmma_wait<0>();
+    reg_fence<HD / 2>(dv);
+    reg_fence<HD / 2>(dk);
+    reg_fence_u<16>(&pa[0][0]);
+    reg_fence_u<16>(&da[0][0]);
+    if (wg_leader) mbar_arrive(&q_empty[s]);
+  }
+
+  // ---- dK_j, dV_j epilogue ----
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    const int kv = kv0 + kr + 8 * hh;
+    if (kv >= p.T) continue;
+    __nv_bfloat16* dkrow = p.dqkv + (int64_t)(row_base + kv) * p.ld_dqkv + col_k + cq;
+    __nv_bfloat16* dvrow = p.dqkv + (int64_t)(row_base + kv) * p.ld_dqkv + col_v + cq;
+#pragma unroll
+    for (int i = 0; i < HD / 8; ++i) {
+      *reinterpret_cast<uint32_t*>(dkrow + 8 * i) = pack_bf16x2(dk[4 * i + 2 * hh], dk[4 * i + 2 * hh + 1]);
+      *reinterpret_cast<uint32_t*>(dvrow + 8 * i) = pack_bf16x2(dv[4 * i + 2 * hh], dv[4 * i + 2 * hh + 1]);
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem, 512);
 }
 
 // D[b,h,t] = sum_d dO[t,h,d] * O[t,h,d]   (one warp per (t,h))
@@ -389,7 +275,7 @@ __global__ void attn_dq_convert_kernel(const float* __restrict__ dq32, int64_t l
 
 template <int HD>
 int launch_attn_bwd(const CUtensorMap& tkv, const CUtensorMap& tq, const CUtensorMap& tdo, const AttnBwdParams& p, cudaStream_t st) {
-  constexpr int SMEM = 2 * BKVB * HD * 2 + 6 * BQB * HD * 2 + ((HD == 64) ? 2 : 1) * BKVB * BQB * 2 + 1024;
+  constexpr int SMEM = 2 * BKVB * HD * 2 + NQ * 2 * BQB * HD * 2 + 2 * BKVB * BQB * 2 + 1024;
   static bool attr = false;
   if (!attr) {
     LMOD_CUDA_OK(cudaFuncSetAttribute(attn_bwd_kernel<HD>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));

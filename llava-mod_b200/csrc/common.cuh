@@ -1,4 +1,4 @@
-// common.cuh -- shared device helpers for liblmod_b200 (sm_100a only).
+// common.cuh -- shared device helpers for liblmod_b200 (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -7,7 +7,7 @@
 #include "../../include/lmod.h"
 
 #define LMOD_IGNORE_INDEX (-100)
-#define LMOD_NUM_SMS_FALLBACK 148
+#define LMOD_NUM_SMS_FALLBACK 132
 
 // ---- host-side error plumbing -----------------------------------------------------------------
 void lmod_set_error(const char* fmt, ...);

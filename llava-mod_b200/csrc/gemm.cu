@@ -1,20 +1,20 @@
-// gemm.cu -- hand-written tcgen05 + TMA GEMM for sm_100a:  D[M,N] (+)= A[M,K] * B[N,K]^T  (bf16 in, fp32 TMEM accumulate)
+// gemm.cu -- hand-written wgmma + TMA GEMM for sm_90a:  D[M,N] (+)= A[M,K] * B[N,K]^T  (bf16 in, fp32 register accumulate)
 //
 // Replaces the nn.Linear call sites of the path (modeling_qwen2.py:199-200 gate/up/down, :678-680 q/k/v, :726 o_proj, :1176
 // lm_head; CLIP / projector linears) and, in its grouped form, DeepSpeed's per-expert loop (Experts.forward) on COMPACT
 // expert rows -- no capacity padding.
 //
-// Structure (one persistent CTA per SM, 256 threads, warp-specialised):
-//   warp 0 lane 0 : TMA producer  -- cp.async.bulk.tensor.2d into a 4-stage 128B-swizzled shared-memory ring (A 128x64, B 256x64)
-//   warp 1 lane 0 : MMA issuer    -- tcgen05.mma.cta_group::1.kind::f16, M=128 N=256 K=16, accumulators in TMEM (2 x 256 columns,
-//                                    double buffered so the epilogue of tile i overlaps the MMAs of tile i+1)
-//   warp 2        : TMEM allocator
-//   warps 4..7    : epilogue      -- tcgen05.ld 32x32b.x32 -> (+bias) (+D_old) -> bf16 -> 64-byte row segments to global
-//   mbarriers     : full[stage] (TMA complete_tx) / empty[stage] (tcgen05.commit) / tmem_full[2] / tmem_empty[2]
+// Structure (one persistent CTA per SM, 384 threads = three warpgroups, warp-specialised):
+//   warpgroup 0, thread 0 : TMA producer -- cp.async.bulk.tensor.2d into a 128B-swizzled shared-memory ring (A 128x64, B BNx64;
+//                           4 stages for BN = 256, 6 for BN = 128); gives its registers to the math warpgroups (setmaxnreg)
+//   warpgroups 1, 2       : math -- each owns 64 rows of the 128 x BN tile: wgmma.mma_async m64nBNk16 (both operands from shared
+//                           memory), fp32 accumulators in registers; one k-block of MMAs stays in flight while the previous
+//                           stage is handed back; then the epilogue (+bias) (+D_old) ... -> bf16 -> global from the registers
+//   mbarriers             : full[stage] (TMA complete_tx) / empty[stage] (one arrive per math warpgroup)
 // Operand "major-ness" is a template parameter, so dgrad (B = W as stored, MN-major) and wgrad (A = dY^T, B = X^T, both MN-major)
-// run without transposes; the UMMA shared-memory descriptors and the TMA boxes change, the pipeline does not.
+// run without transposes: the wgmma transpose bits and descriptors and the TMA boxes change, the pipeline does not.
 #include <stdlib.h>
-#include "tc05.cuh"
+#include "sm90.cuh"
 
 namespace {
 
@@ -27,7 +27,7 @@ template <int BN> struct Cfg {
   static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
   static constexpr int SMEM = STAGES * STAGE_BYTES + 1024;   // + alignment slack
 };
-constexpr int GEMM_THREADS = 256;
+constexpr int GEMM_THREADS = 384;
 constexpr int MAX_GROUPS = 8;
 
 struct GemmParams {
@@ -63,7 +63,7 @@ struct GemmParams {
   // D = bf16( bf16(acc + bias) + R ) -- the GEMM output is rounded to bf16 first, exactly as the reference materialises it before its add
   const __nv_bfloat16* R;
   int64_t ld_r;
-  int dbg_nostore;                 // timing experiments only (LMOD_GEMM_NOSTORE=1): epilogue drains TMEM but does not write D
+  int dbg_nostore;                 // timing experiments only (LMOD_GEMM_NOSTORE=1): the epilogue does not write D
   // grouped (experts): row ranges from `offsets` (device), B / D32 advance per group
   const int32_t* offsets;          // [groups+1] or null
   int groups;
@@ -83,94 +83,59 @@ __device__ __forceinline__ GemmParams effective_extents(const GemmParams& in) {
   return p;
 }
 
-// K-major 128B-swizzled tile (rows x 64 bf16, 128 B per row, 8-row atoms of 1024 B): LBO unused (=1), SBO = 1024; +32 B per UMMA_K
-// MN-major 128B-swizzled tile (64 k-rows x 64 mn per 8 KB block): LBO = 8192 (next 64-wide mn block), SBO = 1024 (next 8 k-rows);
-//   +2048 B per UMMA_K (16 k-rows)
-template <bool MN>
-__device__ __forceinline__ uint64_t operand_desc(uint32_t tile_saddr, int k16) {
-  if (!MN) return smem_desc(tile_saddr + k16 * 32, 16, 1024);
-  return smem_desc(tile_saddr + k16 * 2048, BK * 128, 1024);
-}
-// cute::UMMA::InstrDescriptor: c_format F32 (1) [4,6) | a_format BF16 (1) [7,10) | b_format BF16 (1) [10,13) | a_major [15] | b_major [16]
-// | N>>3 [17,23) | M>>4 [24,29)
-template <int BN, bool A_MN, bool B_MN>
-__device__ __forceinline__ uint32_t instr_desc() {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((A_MN ? 1u : 0u) << 15) | ((B_MN ? 1u : 0u) << 16) | ((uint32_t)(BN >> 3) << 17) |
-         ((uint32_t)(BM >> 4) << 24);
-}
-
 struct Tile { int m0, n0, kb0, kb1, group, m_end; };
 
+// The epilogue works on what one thread holds of a wgmma accumulator: two adjacent columns (col, col + 1) of one row.
 __device__ __forceinline__ float sigmoid_f(float x) { return 1.f / (1.f + __expf(-x)); }
-// rotate 8 (x1, x2) pairs of one head: x = bf16(acc + bias); o1 = bf16(bf16(x1 c) + bf16(-x2 s)), o2 = bf16(bf16(x2 c) + bf16(x1 s))
+__device__ __forceinline__ void bias2(const __nv_bfloat16* b, float& f0, float& f1) {
+  const uint32_t w = __ldg(reinterpret_cast<const uint32_t*>(b));
+  f0 += bf16lo(w); f1 += bf16hi(w);
+}
+// rotate one (x1, x2) pair of columns of a head: x = bf16(acc + bias); o1 = bf16(bf16(x1 c) + bf16(-x2 s)), o2 = bf16(bf16(x2 c) + bf16(x1 s))
 // (the expression of rope_vec_kernel).  a1 / a2: fp32 accumulators of the first-half / second-half columns, b1 / b2: their bias (or null).
-__device__ __forceinline__ void rope_store8(const uint32_t* a1, const uint32_t* a2, const __nv_bfloat16* b1, const __nv_bfloat16* b2, const __nv_bfloat16* cs,
-                                            const __nv_bfloat16* sn, __nv_bfloat16* d1, __nv_bfloat16* d2) {
-  float x1[8], x2[8], c[8], s[8];
+__device__ __forceinline__ void rope_store2(float a10, float a11, float a20, float a21, const __nv_bfloat16* b1, const __nv_bfloat16* b2,
+                                            const __nv_bfloat16* cs, const __nv_bfloat16* sn, __nv_bfloat16* d1, __nv_bfloat16* d2) {
+  float x1[2] = {a10, a11}, x2[2] = {a20, a21};
+  if (b1) { bias2(b1, x1[0], x1[1]); bias2(b2, x2[0], x2[1]); }
+  const uint32_t cw = __ldg(reinterpret_cast<const uint32_t*>(cs)), sw = __ldg(reinterpret_cast<const uint32_t*>(sn));
+  const float c[2] = {bf16lo(cw), bf16hi(cw)}, s[2] = {bf16lo(sw), bf16hi(sw)};
+  float o1[2], o2[2];
 #pragma unroll
-  for (int j = 0; j < 8; ++j) { x1[j] = __uint_as_float(a1[j]); x2[j] = __uint_as_float(a2[j]); }
-  if (b1) {
-    const uint4 u = __ldg(reinterpret_cast<const uint4*>(b1)), w = __ldg(reinterpret_cast<const uint4*>(b2));
-    x1[0] += bf16lo(u.x); x1[1] += bf16hi(u.x); x1[2] += bf16lo(u.y); x1[3] += bf16hi(u.y);
-    x1[4] += bf16lo(u.z); x1[5] += bf16hi(u.z); x1[6] += bf16lo(u.w); x1[7] += bf16hi(u.w);
-    x2[0] += bf16lo(w.x); x2[1] += bf16hi(w.x); x2[2] += bf16lo(w.y); x2[3] += bf16hi(w.y);
-    x2[4] += bf16lo(w.z); x2[5] += bf16hi(w.z); x2[6] += bf16lo(w.w); x2[7] += bf16hi(w.w);
-  }
-  {
-    const uint4 u = __ldg(reinterpret_cast<const uint4*>(cs)), w = __ldg(reinterpret_cast<const uint4*>(sn));
-    c[0] = bf16lo(u.x); c[1] = bf16hi(u.x); c[2] = bf16lo(u.y); c[3] = bf16hi(u.y); c[4] = bf16lo(u.z); c[5] = bf16hi(u.z); c[6] = bf16lo(u.w); c[7] = bf16hi(u.w);
-    s[0] = bf16lo(w.x); s[1] = bf16hi(w.x); s[2] = bf16lo(w.y); s[3] = bf16hi(w.y); s[4] = bf16lo(w.z); s[5] = bf16hi(w.z); s[6] = bf16lo(w.w); s[7] = bf16hi(w.w);
-  }
-  float o1[8], o2[8];
-#pragma unroll
-  for (int j = 0; j < 8; ++j) {
+  for (int j = 0; j < 2; ++j) {
     const float y1 = bf16_round(x1[j]), y2 = bf16_round(x2[j]);
     o1[j] = bf16_round(y1 * c[j]) + bf16_round(-y2 * s[j]);
     o2[j] = bf16_round(y2 * c[j]) + bf16_round(y1 * s[j]);
   }
-  uint4 w;
-  w.x = pack_bf16x2(o1[0], o1[1]); w.y = pack_bf16x2(o1[2], o1[3]); w.z = pack_bf16x2(o1[4], o1[5]); w.w = pack_bf16x2(o1[6], o1[7]);
-  *reinterpret_cast<uint4*>(d1) = w;
-  w.x = pack_bf16x2(o2[0], o2[1]); w.y = pack_bf16x2(o2[2], o2[3]); w.z = pack_bf16x2(o2[4], o2[5]); w.w = pack_bf16x2(o2[6], o2[7]);
-  *reinterpret_cast<uint4*>(d2) = w;
+  *reinterpret_cast<uint32_t*>(d1) = pack_bf16x2(o1[0], o1[1]);
+  *reinterpret_cast<uint32_t*>(d2) = pack_bf16x2(o2[0], o2[1]);
 }
 // act = bf16(bf16(silu(g)) * u) on bf16-rounded GEMM outputs: the expression of silu_mul_fwd_kernel (bit-identical to GEMM + that kernel)
-__device__ __forceinline__ void swiglu_store8(const uint32_t* g, const uint32_t* u, __nv_bfloat16* act, __nv_bfloat16* h1g, __nv_bfloat16* h1u) {
-  float gb[8], ub[8], f[8];
+__device__ __forceinline__ void swiglu_store2(float g0, float g1, float u0, float u1, __nv_bfloat16* act, __nv_bfloat16* h1g, __nv_bfloat16* h1u) {
+  const float gb[2] = {bf16_round(g0), bf16_round(g1)}, ub[2] = {bf16_round(u0), bf16_round(u1)};
+  float f[2];
 #pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    gb[j] = bf16_round(__uint_as_float(g[j])); ub[j] = bf16_round(__uint_as_float(u[j]));
-    f[j] = bf16_round(gb[j] * sigmoid_f(gb[j])) * ub[j];
-  }
-  uint4 w;
-  w.x = pack_bf16x2(f[0], f[1]); w.y = pack_bf16x2(f[2], f[3]); w.z = pack_bf16x2(f[4], f[5]); w.w = pack_bf16x2(f[6], f[7]);
-  *reinterpret_cast<uint4*>(act) = w;
+  for (int j = 0; j < 2; ++j) f[j] = bf16_round(gb[j] * sigmoid_f(gb[j])) * ub[j];
+  *reinterpret_cast<uint32_t*>(act) = pack_bf16x2(f[0], f[1]);
   if (h1g) {
-    w.x = pack_bf16x2(gb[0], gb[1]); w.y = pack_bf16x2(gb[2], gb[3]); w.z = pack_bf16x2(gb[4], gb[5]); w.w = pack_bf16x2(gb[6], gb[7]);
-    *reinterpret_cast<uint4*>(h1g) = w;
-    w.x = pack_bf16x2(ub[0], ub[1]); w.y = pack_bf16x2(ub[2], ub[3]); w.z = pack_bf16x2(ub[4], ub[5]); w.w = pack_bf16x2(ub[6], ub[7]);
-    *reinterpret_cast<uint4*>(h1u) = w;
+    *reinterpret_cast<uint32_t*>(h1g) = pack_bf16x2(gb[0], gb[1]);
+    *reinterpret_cast<uint32_t*>(h1u) = pack_bf16x2(ub[0], ub[1]);
   }
 }
 // d(gate), d(up) from dact (the fp32 accumulator rounded to bf16, as the unfused path materialises it) and the saved pre-activations:
 // the expression of silu_mul_bwd_kernel
-__device__ __forceinline__ void silu_bwd_store8(const float* dacc, const __nv_bfloat16* gp, const __nv_bfloat16* up, __nv_bfloat16* dgp, __nv_bfloat16* dup) {
-  const uint4 gv = __ldg(reinterpret_cast<const uint4*>(gp)), uv = __ldg(reinterpret_cast<const uint4*>(up));
-  const float g[8] = {bf16lo(gv.x), bf16hi(gv.x), bf16lo(gv.y), bf16hi(gv.y), bf16lo(gv.z), bf16hi(gv.z), bf16lo(gv.w), bf16hi(gv.w)};
-  const float u[8] = {bf16lo(uv.x), bf16hi(uv.x), bf16lo(uv.y), bf16hi(uv.y), bf16lo(uv.z), bf16hi(uv.z), bf16lo(uv.w), bf16hi(uv.w)};
-  float dg[8], du[8];
+__device__ __forceinline__ void silu_bwd_store2(float a0, float a1, const __nv_bfloat16* gp, const __nv_bfloat16* up, __nv_bfloat16* dgp, __nv_bfloat16* dup) {
+  const uint32_t gv = __ldg(reinterpret_cast<const uint32_t*>(gp)), uv = __ldg(reinterpret_cast<const uint32_t*>(up));
+  const float g[2] = {bf16lo(gv), bf16hi(gv)}, u[2] = {bf16lo(uv), bf16hi(uv)}, dacc[2] = {a0, a1};
+  float dg[2], du[2];
 #pragma unroll
-  for (int j = 0; j < 8; ++j) {
+  for (int j = 0; j < 2; ++j) {
     const float d = bf16_round(dacc[j]);
     const float sg = sigmoid_f(g[j]);
     du[j] = d * g[j] * sg;
     dg[j] = d * u[j] * sg * (1.f + g[j] * (1.f - sg));
   }
-  uint4 w;
-  w.x = pack_bf16x2(dg[0], dg[1]); w.y = pack_bf16x2(dg[2], dg[3]); w.z = pack_bf16x2(dg[4], dg[5]); w.w = pack_bf16x2(dg[6], dg[7]);
-  *reinterpret_cast<uint4*>(dgp) = w;
-  w.x = pack_bf16x2(du[0], du[1]); w.y = pack_bf16x2(du[2], du[3]); w.z = pack_bf16x2(du[4], du[5]); w.w = pack_bf16x2(du[6], du[7]);
-  *reinterpret_cast<uint4*>(dup) = w;
+  *reinterpret_cast<uint32_t*>(dgp) = pack_bf16x2(dg[0], dg[1]);
+  *reinterpret_cast<uint32_t*>(dup) = pack_bf16x2(du[0], du[1]);
 }
 
 // tile index -> coordinates.  Dense: M fastest (consecutive CTAs share the B tile in L2).  Grouped forward/dgrad: per-group row
@@ -214,446 +179,172 @@ __device__ __forceinline__ bool get_tile(const GemmParams& p, int t, Tile& o) {
 }
 
 template <int BN, bool A_MN, bool B_MN>
+__device__ __forceinline__ void mma_kblock(float* acc, uint32_t sa, uint32_t sb, uint32_t accumulate) {
+#pragma unroll
+  for (int k = 0; k < BK / 16; ++k) {
+    const uint64_t da = A_MN ? gmma_desc(sa + k * 2048, BK * 128, 1024) : gmma_desc(sa + k * 32, 16, 1024);
+    const uint64_t db = B_MN ? gmma_desc(sb + k * 2048, BK * 128, 1024) : gmma_desc(sb + k * 32, 16, 1024);
+    const uint32_t acc_in = (k > 0) ? 1u : accumulate;
+    if constexpr (BN == 256) wgmma_ss_n256<A_MN, B_MN>(acc, da, db, acc_in);
+    else wgmma_ss_n128<A_MN, B_MN>(acc, da, db, acc_in);
+  }
+}
+
+template <int BN, bool A_MN, bool B_MN>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b, const GemmParams p_in) {
+gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b, const GemmParams p_in) {
   const GemmParams p = effective_extents(p_in);
   constexpr int STAGES = Cfg<BN>::STAGES, STAGE_BYTES = Cfg<BN>::STAGE_BYTES;
   extern __shared__ uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t full_bar[STAGES], empty_bar[STAGES], tmem_full[2], tmem_empty[2];
-  __shared__ uint32_t tmem_base_slot;
+  __shared__ __align__(8) uint64_t full_bar[STAGES], empty_bar[STAGES];
 
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);   // SW128 needs 1024 B
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-    for (int a = 0; a < 2; ++a) { mbar_init(&tmem_full[a], 1); mbar_init(&tmem_empty[a], 4); }
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 2); }
     mbar_fence_init();
     asm volatile("prefetch.tensormap [%0];" :: "l"(&tma_a) : "memory");
     asm volatile("prefetch.tensormap [%0];" :: "l"(&tma_b) : "memory");
   }
-  if (warp == 2) tmem_alloc(&tmem_base_slot, 2 * BN);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_slot;
 
-  if (warp == 0 && lane == 0) {
+  if (wg == 0) {
     // ===================== TMA producer =====================
-    uint32_t stage = 0, phase = 0;
-    Tile t;
-    for (int ti = blockIdx.x; get_tile(p, ti, t); ti += gridDim.x) {
-      const int b_row0 = (int)(t.group * p.b_group_rows);
-      for (int kb = t.kb0; kb < t.kb1; ++kb) {
-        mbar_wait_bounded(&empty_bar[stage], phase ^ 1);
-        uint8_t* sa = smem + stage * STAGE_BYTES;
-        uint8_t* sb = sa + A_STAGE_BYTES;
-        mbar_expect_tx(&full_bar[stage], STAGE_BYTES);
-        if (!A_MN) {
-          tma_load_2d(sa, &tma_a, kb * BK, t.m0, &full_bar[stage]);                      // box (64 k, 128 rows)
-        } else {
+    regs_dealloc<40>();
+    if (threadIdx.x == 0) {
+      uint32_t stage = 0, phase = 0;
+      Tile t;
+      for (int ti = blockIdx.x; get_tile(p, ti, t); ti += gridDim.x) {
+        const int b_row0 = (int)(t.group * p.b_group_rows);
+        for (int kb = t.kb0; kb < t.kb1; ++kb) {
+          mbar_wait_bounded(&empty_bar[stage], phase ^ 1);
+          uint8_t* sa = smem + stage * STAGE_BYTES;
+          uint8_t* sb = sa + A_STAGE_BYTES;
+          mbar_expect_tx(&full_bar[stage], STAGE_BYTES);
+          if (!A_MN) {
+            tma_load_2d(sa, &tma_a, kb * BK, t.m0, &full_bar[stage]);                      // box (64 k, 128 rows)
+          } else {
 #pragma unroll
-          for (int j = 0; j < BM / 64; ++j) tma_load_2d(sa + j * (BK * 128), &tma_a, t.m0 + 64 * j, kb * BK, &full_bar[stage]);   // box (64 mn, 64 k)
-        }
-        if (!B_MN && p.swiglu) {                                                         // box (64 k, 128 rows): gate rows, then the matching up rows
-          tma_load_2d(sb, &tma_b, kb * BK, b_row0 + t.n0, &full_bar[stage]);
-          tma_load_2d(sb + 128 * 128, &tma_b, kb * BK, b_row0 + p.swiglu_I + t.n0, &full_bar[stage]);
-        } else if (!B_MN) {
-          tma_load_2d(sb, &tma_b, kb * BK, b_row0 + t.n0, &full_bar[stage]);             // box (64 k, 256 rows)
-        } else {
+            for (int j = 0; j < BM / 64; ++j) tma_load_2d(sa + j * (BK * 128), &tma_a, t.m0 + 64 * j, kb * BK, &full_bar[stage]);   // box (64 mn, 64 k)
+          }
+          if (!B_MN && p.swiglu) {                                                         // box (64 k, 128 rows): gate rows, then the matching up rows
+            tma_load_2d(sb, &tma_b, kb * BK, b_row0 + t.n0, &full_bar[stage]);
+            tma_load_2d(sb + 128 * 128, &tma_b, kb * BK, b_row0 + p.swiglu_I + t.n0, &full_bar[stage]);
+          } else if (!B_MN) {
+            tma_load_2d(sb, &tma_b, kb * BK, b_row0 + t.n0, &full_bar[stage]);             // box (64 k, BN rows)
+          } else {
 #pragma unroll
-          for (int j = 0; j < BN / 64; ++j) tma_load_2d(sb + j * (BK * 128), &tma_b, t.n0 + 64 * j, b_row0 + kb * BK, &full_bar[stage]);
+            for (int j = 0; j < BN / 64; ++j) tma_load_2d(sb + j * (BK * 128), &tma_b, t.n0 + 64 * j, b_row0 + kb * BK, &full_bar[stage]);
+          }
+          if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp == 1 && lane == 0) {
-    // ===================== MMA issuer =====================
-    const uint32_t idesc = instr_desc<BN, A_MN, B_MN>();
-    uint32_t stage = 0, phase = 0, it = 0;
-    Tile t;
-    for (int ti = blockIdx.x; get_tile(p, ti, t); ti += gridDim.x, ++it) {
-      const uint32_t acc = it & 1u, acc_phase = (it >> 1) & 1u;
-      mbar_wait_bounded(&tmem_empty[acc], acc_phase ^ 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + acc * BN;
-      uint32_t first = 1;
-      for (int kb = t.kb0; kb < t.kb1; ++kb) {
-        mbar_wait_bounded(&full_bar[stage], phase);
-        tc_fence_after();
-        const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES), sb = sa + A_STAGE_BYTES;
-#pragma unroll
-        for (int k = 0; k < BK / 16; ++k) {
-          umma_f16(d_tmem, operand_desc<A_MN>(sa, k), operand_desc<B_MN>(sb, k), idesc, first ? 0u : 1u);
-          first = 0;
-        }
-        umma_commit(&empty_bar[stage]);                    // frees the smem slot once these MMAs have read it
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+    return;
+  }
+  // ===================== math warpgroups: MMA + epilogue =====================
+  regs_alloc<232>();
+  const int c = wg - 1;                                    // rows [64c, 64c + 64) of every tile
+  const int w = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+  const bool wg_leader = (threadIdx.x & 127) == 0;
+  float acc[BN / 2];
+  uint32_t stage = 0, phase = 0;
+  Tile t;
+  for (int ti = blockIdx.x; get_tile(p, ti, t); ti += gridDim.x) {
+    uint32_t prev = 0;
+    for (int kb = t.kb0; kb < t.kb1; ++kb) {
+      mbar_wait(&full_bar[stage], phase);
+      const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES) + c * (64 * 128), sb = smem_u32(smem + stage * STAGE_BYTES + A_STAGE_BYTES);
+      wgmma_fence();
+      mma_kblock<BN, A_MN, B_MN>(acc, sa, sb, kb > t.kb0 ? 1u : 0u);
+      wgmma_commit();
+      if (kb > t.kb0) {                                    // the previous k-block's MMAs are done: hand its stage back
+        wgmma_wait<1>();
+        if (wg_leader) mbar_arrive(&empty_bar[prev]);
       }
-      umma_commit(&tmem_full[acc]);                        // accumulator ready for the epilogue
+      prev = stage;
+      if (++stage == STAGES) { stage = 0; phase ^= 1; }
     }
-  } else if (warp >= 4) {
-    // ===================== epilogue (TMEM -> registers -> global) =====================
-    const int q = warp & 3;                                // TMEM lane quarter this warp may access
-    uint32_t it = 0;
-    Tile t;
-    for (int ti = blockIdx.x; get_tile(p, ti, t); ti += gridDim.x, ++it) {
-      const uint32_t acc = it & 1u, acc_phase = (it >> 1) & 1u;
-      mbar_wait_warp(&tmem_full[acc], acc_phase);
-      tc_fence_after();
-      const int row = t.m0 + q * 32 + lane;
-      const bool row_ok = row < t.m_end;
-      const bool empty_k = t.kb1 <= t.kb0;                 // grouped wgrad of an expert with no rows: contributes zero
-      __nv_bfloat16* drow = p.D ? p.D + (p.wgrad_grouped ? t.group * p.d_group_stride : 0) + (int64_t)row * p.ldd : nullptr;
-      float* d32row = p.D32 ? p.D32 + (p.wgrad_grouped ? t.group * p.d_group_stride : 0) + (int64_t)row * p.ldd : nullptr;
-      if (BN == 256 && p.swiglu) {
-#pragma unroll 1
-        for (int c = 0; c < 4; ++c) {
-          uint32_t g[32], u[32];
-          tmem_ld32(tmem_base + acc * BN + c * 32 + ((uint32_t)(q * 32) << 16), g);
-          tmem_ld32(tmem_base + acc * BN + 128 + c * 32 + ((uint32_t)(q * 32) << 16), u);
-          const int col0 = t.n0 + c * 32;
-          if (!row_ok || col0 >= p.N) continue;
+    const bool empty_k = t.kb1 <= t.kb0;                   // grouped wgrad of an expert with no rows / empty dynamic reduction: zero
+    if (!empty_k) {
+      wgmma_wait<0>();
+      if (wg_leader) mbar_arrive(&empty_bar[prev]);
+    }
+    reg_fence<BN / 2>(acc);
+
+    // accumulator fragment: register 4i + 2h + e holds row 16w + lane/4 + 8h, column 8i + 2(lane%4) + e of this warpgroup's 64 x BN block
+    const int row0 = t.m0 + c * 64 + w * 16 + (lane >> 2);
+    const int cq = 2 * (lane & 3);
+    const int64_t goff = p.wgrad_grouped ? t.group * p.d_group_stride : 0;
+    if (BN == 256 && p.swiglu) {
+      // accumulator columns [0,128) = gate, [128,256) = up of the same 128 act columns
+#pragma unroll
+      for (int i = 0; i < 16; ++i) {
+        const int col = t.n0 + 8 * i + cq;
+        if (col >= p.N) continue;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int row = row0 + 8 * h;
+          if (row >= t.m_end) continue;
+          __nv_bfloat16* drow = p.D + (int64_t)row * p.ldd;
           __nv_bfloat16* h1row = p.H1 ? p.H1 + (int64_t)row * p.ld_h1 : nullptr;
-#pragma unroll
-          for (int v = 0; v < 4; ++v) {
-            const int col = col0 + v * 8;
-            swiglu_store8(g + v * 8, u + v * 8, drow + col, h1row ? h1row + col : nullptr, h1row ? h1row + p.swiglu_I + col : nullptr);
-          }
+          swiglu_store2(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1], acc[4 * (i + 16) + 2 * h], acc[4 * (i + 16) + 2 * h + 1], drow + col,
+                        h1row ? h1row + col : nullptr, h1row ? h1row + p.swiglu_I + col : nullptr);
         }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&tmem_empty[acc]);
+      }
+      continue;
+    }
+#pragma unroll
+    for (int i = 0; i < BN / 8; ++i) {
+      const int col8 = t.n0 + 8 * i, col = col8 + cq;
+      if (p.rope_cos && col8 < p.rope_cols) {
+        // q / k head columns: the first half of a head is processed together with its partner half a head further on (same thread)
+        const int hoff = col8 % p.rope_hd, half = p.rope_hd >> 1;
+        if (hoff >= half) continue;                                     // done with its partner
+        const int ip = (half == 32) ? i + 4 : i + 8;
+        if (ip >= BN / 8) continue;                                     // (a head never straddles a tile: tiles start at multiples of 128)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int row = row0 + 8 * h;
+          if (row >= t.m_end) continue;
+          float x20, x21;
+          if (half == 32) { x20 = acc[4 * ((i + 4) % (BN / 8)) + 2 * h]; x21 = acc[4 * ((i + 4) % (BN / 8)) + 2 * h + 1]; }
+          else { x20 = acc[4 * ((i + 8) % (BN / 8)) + 2 * h]; x21 = acc[4 * ((i + 8) % (BN / 8)) + 2 * h + 1]; }
+          const int64_t pp = __ldg(p.rope_pos + row);
+          __nv_bfloat16* drow = p.D + (int64_t)row * p.ldd;
+          rope_store2(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1], x20, x21, p.bias ? p.bias + col : nullptr, p.bias ? p.bias + col + half : nullptr,
+                      p.rope_cos + pp * p.rope_hd + hoff + cq, p.rope_sin + pp * p.rope_hd + hoff + cq, drow + col, drow + col + half);
+        }
         continue;
       }
-#pragma unroll 1
-      for (int c = 0; c < BN / 32; ++c) {
-        uint32_t r[32];
-        const int col0 = t.n0 + c * 32;
-        if (p.rope_cos && col0 < p.rope_cols) {
-          // q / k head columns: the chunk of the first half of a head is processed together with its partner half a head further on
-          const int hoff = col0 % p.rope_hd, half = p.rope_hd >> 1;
-          if (hoff >= half) continue;                                   // done with its partner
-          uint32_t r2[32];
-          tmem_ld32(tmem_base + acc * BN + c * 32 + ((uint32_t)(q * 32) << 16), r);
-          tmem_ld32(tmem_base + acc * BN + c * 32 + half + ((uint32_t)(q * 32) << 16), r2);
-          if (!row_ok) continue;
-          const int64_t pp = __ldg(p.rope_pos + row);
+      if (col >= p.N || p.dbg_nostore) continue;
 #pragma unroll
-          for (int v = 0; v < 4; ++v) {
-            const int col = col0 + v * 8, d = hoff + v * 8;
-            rope_store8(r + v * 8, r2 + v * 8, p.bias ? p.bias + col : nullptr, p.bias ? p.bias + col + half : nullptr,
-                        p.rope_cos + pp * p.rope_hd + d, p.rope_sin + pp * p.rope_hd + d, drow + col, drow + col + half);
-          }
-          continue;
-        }
-        tmem_ld32(tmem_base + acc * BN + c * 32 + ((uint32_t)(q * 32) << 16), r);
-        if (!row_ok || col0 >= p.N || p.dbg_nostore) continue;
-#pragma unroll
-        for (int v = 0; v < 4; ++v) {
-          const int col = col0 + v * 8;
-          if (col >= p.N) break;
-          float f[8];
-#pragma unroll
-          for (int j = 0; j < 8; ++j) f[j] = empty_k ? 0.f : __uint_as_float(r[v * 8 + j]);
-          if (p.bias) {
-            const uint4 b = __ldg(reinterpret_cast<const uint4*>(p.bias + col));
-            f[0] += bf16lo(b.x); f[1] += bf16hi(b.x); f[2] += bf16lo(b.y); f[3] += bf16hi(b.y);
-            f[4] += bf16lo(b.z); f[5] += bf16hi(b.z); f[6] += bf16lo(b.w); f[7] += bf16hi(b.w);
-          }
-          if (p.silu_bwd) {
-            const __nv_bfloat16* gurow = p.GU + (int64_t)row * p.ld_gu;
-            silu_bwd_store8(f, gurow + col, gurow + p.N + col, drow + col, drow + p.N + col);
-          } else if (d32row && p.splits > 1) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) atomicAdd(d32row + col + j, f[j]);
-          } else if (d32row) {
-            float4* o = reinterpret_cast<float4*>(d32row + col);
-            float4 a = o[0], b2 = o[1];
-            a.x += f[0]; a.y += f[1]; a.z += f[2]; a.w += f[3]; b2.x += f[4]; b2.y += f[5]; b2.z += f[6]; b2.w += f[7];
-            o[0] = a; o[1] = b2;
-          } else {
-            uint4* o = reinterpret_cast<uint4*>(drow + col);
-            if (p.beta) {
-              const uint4 old = *o;
-              f[0] += bf16lo(old.x); f[1] += bf16hi(old.x); f[2] += bf16lo(old.y); f[3] += bf16hi(old.y);
-              f[4] += bf16lo(old.z); f[5] += bf16hi(old.z); f[6] += bf16lo(old.w); f[7] += bf16hi(old.w);
-            }
-            if (p.R) {
-              const uint4 rr = __ldg(reinterpret_cast<const uint4*>(p.R + (int64_t)row * p.ld_r + col));
-              f[0] = bf16_round(f[0]) + bf16lo(rr.x); f[1] = bf16_round(f[1]) + bf16hi(rr.x);
-              f[2] = bf16_round(f[2]) + bf16lo(rr.y); f[3] = bf16_round(f[3]) + bf16hi(rr.y);
-              f[4] = bf16_round(f[4]) + bf16lo(rr.z); f[5] = bf16_round(f[5]) + bf16hi(rr.z);
-              f[6] = bf16_round(f[6]) + bf16lo(rr.w); f[7] = bf16_round(f[7]) + bf16hi(rr.w);
-            }
-            uint4 w;
-            w.x = pack_bf16x2(f[0], f[1]); w.y = pack_bf16x2(f[2], f[3]); w.z = pack_bf16x2(f[4], f[5]); w.w = pack_bf16x2(f[6], f[7]);
-            *o = w;
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty[acc]);
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) tmem_dealloc(tmem_base, 2 * BN);
-}
-
-// =================================================================================================================================
-// 2-CTA variant (cta_group::2): a CTA PAIR (cluster of 2, same TPC) owns a 256 x 256 output tile.  Each CTA stages its own 128 rows
-// of A and only HALF of B (128 of the 256 columns) -- the UMMA reads B from both CTAs' shared memory -- so shared-memory and L2
-// traffic per FLOP halve.  The leader CTA (rank 0) issues tcgen05.mma.cta_group::2 (M = 256); both CTAs run a TMA producer (their
-// loads complete_tx on the LEADER's full barrier) and an epilogue over their own 128 TMEM lanes.  tcgen05.commit multicasts the
-// "stage free" / "accumulator ready" arrivals to both CTAs; the peer's epilogue warps arrive remotely on the leader's tmem_empty.
-// Two tile widths: 256 x 256 (each CTA stages 16 KB of A + 16 KB of B per k-block: 64 B/clk of shared-memory fill at full tensor rate) for
-// the big GEMMs, and 256 x 128 (16 + 8 KB: 96 B/clk, against 128 B/clk of the 1-CTA 128 x 128 tile) for the N ~ 1024 problems of the
-// 0.5B student, whose 256 x 256 tiling would leave most CTA pairs idle.
-template <int BN2> struct Cfg2 {
-  static constexpr int STAGES = (BN2 == 256) ? 6 : 8;
-  static constexpr int B_STAGE_BYTES = (BN2 / 2) * BK * 2;       // half of the B tile per CTA
-  static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
-  static constexpr int SMEM = STAGES * STAGE_BYTES + 1024;
-};
-constexpr uint32_t PEER_MASK = 0xFEFFFFFFu;                     // clears the CTA-pair rank bit of a shared::cluster address -> leader CTA
-
-__device__ __forceinline__ void tma_load_2d_2sm(void* smem_dst, const CUtensorMap* map, int c0, int c1, uint64_t* leader_bar) {
-  asm volatile("cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
-               :: "r"(smem_u32(smem_dst)), "l"(map), "r"(c0), "r"(c1), "r"(smem_u32(leader_bar) & PEER_MASK) : "memory");
-}
-__device__ __forceinline__ void umma2_f16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      :: "r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void umma2_commit_mc(uint64_t* bar) {       // arrive on the same-offset barrier of BOTH CTAs of the pair
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               :: "r"(smem_u32(bar)), "h"((uint16_t)3) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_leader(uint64_t* bar) {     // arrive on the leader CTA's copy of `bar`
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" :: "r"(smem_u32(bar) & PEER_MASK) : "memory");
-}
-
-template <int BN2, bool A_MN, bool B_MN>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GEMM_THREADS, 1)
-gemm2_tcgen05_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b, const GemmParams p_in) {
-  const GemmParams p = effective_extents(p_in);
-  constexpr int STAGES2 = Cfg2<BN2>::STAGES, STAGE2_BYTES = Cfg2<BN2>::STAGE_BYTES;
-  extern __shared__ uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t full_bar[STAGES2], empty_bar[STAGES2], tmem_full[2], tmem_empty[2];
-  __shared__ uint32_t tmem_base_slot;
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-  const int cluster = blockIdx.x >> 1, nclusters = gridDim.x >> 1;
-  // SwiGLU forward: N = I and a pair's tile is 256 rows x 128 act columns (accumulator: 128 gate | 128 up columns, one half per CTA's B)
-  const int num_m = (p.M + 255) / 256, num_n = p.swiglu ? (p.N + 127) / 128 : (p.N + BN2 - 1) / BN2, num_k = (p.K + BK - 1) / BK;
-  const int ntiles = num_m * num_n;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES2; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-    for (int a = 0; a < 2; ++a) { mbar_init(&tmem_full[a], 1); mbar_init(&tmem_empty[a], 8); }     // 4 epilogue warps x 2 CTAs (leader's copy)
-    mbar_fence_init();
-    asm volatile("prefetch.tensormap [%0];" :: "l"(&tma_a) : "memory");
-    asm volatile("prefetch.tensormap [%0];" :: "l"(&tma_b) : "memory");
-  }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" :: "r"(smem_u32(&tmem_base_slot)), "r"(2 * BN2) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();                                   // both CTAs' barriers initialised before any remote arrive / multicast commit
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_slot;
-
-  if (warp == 0 && lane == 0) {
-    // ===================== TMA producer (both CTAs: own half of A rows and of B rows) =====================
-    uint32_t stage = 0, phase = 0;
-    for (int t = cluster; t < ntiles; t += nclusters) {
-      const int m0 = (t % num_m) * 256 + 128 * (int)rank;
-      const int n0 = p.swiglu ? (t / num_m) * 128 + (int)rank * p.swiglu_I           // rank 0 stages the gate rows, rank 1 the matching up rows
-                              : (t / num_m) * BN2 + (BN2 / 2) * (int)rank;
-      for (int kb = 0; kb < num_k; ++kb) {
-        mbar_wait_bounded(&empty_bar[stage], phase ^ 1);
-        uint8_t* sa = smem + stage * STAGE2_BYTES;
-        uint8_t* sb = sa + A_STAGE_BYTES;
-        if (leader) mbar_expect_tx(&full_bar[stage], 2 * STAGE2_BYTES);          // bytes of BOTH CTAs land on the leader's barrier
-        if (!A_MN) {
-          tma_load_2d_2sm(sa, &tma_a, kb * BK, m0, &full_bar[stage]);
+      for (int h = 0; h < 2; ++h) {
+        const int row = row0 + 8 * h;
+        if (row >= t.m_end) continue;
+        float f0 = empty_k ? 0.f : acc[4 * i + 2 * h], f1 = empty_k ? 0.f : acc[4 * i + 2 * h + 1];
+        if (p.bias) bias2(p.bias + col, f0, f1);
+        if (p.silu_bwd) {
+          const __nv_bfloat16* gurow = p.GU + (int64_t)row * p.ld_gu;
+          __nv_bfloat16* drow = p.D + (int64_t)row * p.ldd;
+          silu_bwd_store2(f0, f1, gurow + col, gurow + p.N + col, drow + col, drow + p.N + col);
+        } else if (p.D32) {
+          float* d32 = p.D32 + goff + (int64_t)row * p.ldd + col;
+          if (p.splits > 1) { atomicAdd(d32, f0); atomicAdd(d32 + 1, f1); }
+          else { float2 o = *reinterpret_cast<float2*>(d32); o.x += f0; o.y += f1; *reinterpret_cast<float2*>(d32) = o; }
         } else {
-#pragma unroll
-          for (int j = 0; j < 2; ++j) tma_load_2d_2sm(sa + j * (BK * 128), &tma_a, m0 + 64 * j, kb * BK, &full_bar[stage]);
-        }
-        if (!B_MN) {
-          tma_load_2d_2sm(sb, &tma_b, kb * BK, n0, &full_bar[stage]);
-        } else {
-#pragma unroll
-          for (int j = 0; j < BN2 / 128; ++j) tma_load_2d_2sm(sb + j * (BK * 128), &tma_b, n0 + 64 * j, kb * BK, &full_bar[stage]);
-        }
-        if (++stage == STAGES2) { stage = 0; phase ^= 1; }
-      }
-    }
-  } else if (warp == 1 && lane == 0 && leader) {
-    // ===================== MMA issuer (leader CTA only) =====================
-    const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((A_MN ? 1u : 0u) << 15) | ((B_MN ? 1u : 0u) << 16) | ((uint32_t)(BN2 >> 3) << 17) |
-                           ((uint32_t)(256 >> 4) << 24);
-    uint32_t stage = 0, phase = 0, it = 0;
-    for (int t = cluster; t < ntiles; t += nclusters, ++it) {
-      const uint32_t acc = it & 1u, acc_phase = (it >> 1) & 1u;
-      mbar_wait_bounded(&tmem_empty[acc], acc_phase ^ 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + acc * BN2;
-      uint32_t first = 1;
-      for (int kb = 0; kb < num_k; ++kb) {
-        mbar_wait_bounded(&full_bar[stage], phase);
-        tc_fence_after();
-        const uint32_t sa = smem_u32(smem + stage * STAGE2_BYTES), sb = sa + A_STAGE_BYTES;
-#pragma unroll
-        for (int k = 0; k < BK / 16; ++k) {
-          umma2_f16(d_tmem, operand_desc<A_MN>(sa, k), operand_desc<B_MN>(sb, k), idesc, first ? 0u : 1u);
-          first = 0;
-        }
-        umma2_commit_mc(&empty_bar[stage]);
-        if (++stage == STAGES2) { stage = 0; phase ^= 1; }
-      }
-      umma2_commit_mc(&tmem_full[acc]);
-    }
-  } else if (warp >= 4) {
-    // ===================== epilogue (both CTAs: own 128 rows x 256 columns) =====================
-    const int q = warp & 3;
-    uint32_t it = 0;
-    for (int t = cluster; t < ntiles; t += nclusters, ++it) {
-      const uint32_t acc = it & 1u, acc_phase = (it >> 1) & 1u;
-      mbar_wait_warp(&tmem_full[acc], acc_phase);
-      tc_fence_after();
-      const int row = (t % num_m) * 256 + 128 * (int)rank + q * 32 + lane;
-      const int n00 = (t / num_m) * BN2;
-      const bool row_ok = row < p.M;
-      __nv_bfloat16* drow = p.D ? p.D + (int64_t)row * p.ldd : nullptr;
-      float* d32row = p.D32 ? p.D32 + (int64_t)row * p.ldd : nullptr;
-      if (BN2 == 256 && p.swiglu) {
-        // fused SwiGLU epilogue: accumulator columns [0,128) = gate, [128,256) = up of the same 128 act columns
-        const int c00 = (t / num_m) * 128;
-        __nv_bfloat16* h1row = p.H1 ? p.H1 + (int64_t)row * p.ld_h1 : nullptr;
-#pragma unroll 1
-        for (int c = 0; c < 4; ++c) {
-          uint32_t g[32], u[32];
-          tmem_ld32(tmem_base + acc * BN2 + c * 32 + ((uint32_t)(q * 32) << 16), g);
-          tmem_ld32(tmem_base + acc * BN2 + 128 + c * 32 + ((uint32_t)(q * 32) << 16), u);
-          const int col0 = c00 + c * 32;
-          if (!row_ok || col0 >= p.N) continue;
-#pragma unroll
-          for (int v = 0; v < 4; ++v) {
-            const int col = col0 + v * 8;
-            swiglu_store8(g + v * 8, u + v * 8, drow + col, h1row ? h1row + col : nullptr, h1row ? h1row + p.swiglu_I + col : nullptr);
+          uint32_t* o = reinterpret_cast<uint32_t*>(p.D + goff + (int64_t)row * p.ldd + col);
+          if (p.beta) { const uint32_t old = *o; f0 += bf16lo(old); f1 += bf16hi(old); }
+          if (p.R) {
+            const uint32_t rr = __ldg(reinterpret_cast<const uint32_t*>(p.R + (int64_t)row * p.ld_r + col));
+            f0 = bf16_round(f0) + bf16lo(rr); f1 = bf16_round(f1) + bf16hi(rr);
           }
-        }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive_leader(&tmem_empty[acc]);
-        continue;
-      }
-#pragma unroll 1
-      for (int c = 0; c < BN2 / 32; ++c) {
-        uint32_t r[32];
-        const int col0 = n00 + c * 32;
-        if (p.rope_cos && col0 < p.rope_cols) {
-          const int hoff = col0 % p.rope_hd, half = p.rope_hd >> 1;
-          if (hoff >= half) continue;
-          uint32_t r2[32];
-          tmem_ld32(tmem_base + acc * BN2 + c * 32 + ((uint32_t)(q * 32) << 16), r);
-          tmem_ld32(tmem_base + acc * BN2 + c * 32 + half + ((uint32_t)(q * 32) << 16), r2);
-          if (!row_ok) continue;
-          const int64_t pp = __ldg(p.rope_pos + row);
-#pragma unroll
-          for (int v = 0; v < 4; ++v) {
-            const int col = col0 + v * 8, d = hoff + v * 8;
-            rope_store8(r + v * 8, r2 + v * 8, p.bias ? p.bias + col : nullptr, p.bias ? p.bias + col + half : nullptr,
-                        p.rope_cos + pp * p.rope_hd + d, p.rope_sin + pp * p.rope_hd + d, drow + col, drow + col + half);
-          }
-          continue;
-        }
-        tmem_ld32(tmem_base + acc * BN2 + c * 32 + ((uint32_t)(q * 32) << 16), r);
-        if (!row_ok || col0 >= p.N || p.dbg_nostore) continue;
-#pragma unroll
-        for (int v = 0; v < 4; ++v) {
-          const int col = col0 + v * 8;
-          if (col >= p.N) break;
-          float f[8];
-#pragma unroll
-          for (int j = 0; j < 8; ++j) f[j] = (num_k == 0) ? 0.f : __uint_as_float(r[v * 8 + j]);   // empty (dynamic) reduction: nothing was accumulated
-          if (p.bias) {
-            const uint4 b = __ldg(reinterpret_cast<const uint4*>(p.bias + col));
-            f[0] += bf16lo(b.x); f[1] += bf16hi(b.x); f[2] += bf16lo(b.y); f[3] += bf16hi(b.y);
-            f[4] += bf16lo(b.z); f[5] += bf16hi(b.z); f[6] += bf16lo(b.w); f[7] += bf16hi(b.w);
-          }
-          if (p.silu_bwd) {
-            const __nv_bfloat16* gurow = p.GU + (int64_t)row * p.ld_gu;
-            silu_bwd_store8(f, gurow + col, gurow + p.N + col, drow + col, drow + p.N + col);
-          } else if (d32row) {
-            float4* o = reinterpret_cast<float4*>(d32row + col);
-            float4 a = o[0], b2 = o[1];
-            a.x += f[0]; a.y += f[1]; a.z += f[2]; a.w += f[3]; b2.x += f[4]; b2.y += f[5]; b2.z += f[6]; b2.w += f[7];
-            o[0] = a; o[1] = b2;
-          } else {
-            uint4* o = reinterpret_cast<uint4*>(drow + col);
-            if (p.beta) {
-              const uint4 old = *o;
-              f[0] += bf16lo(old.x); f[1] += bf16hi(old.x); f[2] += bf16lo(old.y); f[3] += bf16hi(old.y);
-              f[4] += bf16lo(old.z); f[5] += bf16hi(old.z); f[6] += bf16lo(old.w); f[7] += bf16hi(old.w);
-            }
-            if (p.R) {
-              const uint4 rr = __ldg(reinterpret_cast<const uint4*>(p.R + (int64_t)row * p.ld_r + col));
-              f[0] = bf16_round(f[0]) + bf16lo(rr.x); f[1] = bf16_round(f[1]) + bf16hi(rr.x);
-              f[2] = bf16_round(f[2]) + bf16lo(rr.y); f[3] = bf16_round(f[3]) + bf16hi(rr.y);
-              f[4] = bf16_round(f[4]) + bf16lo(rr.z); f[5] = bf16_round(f[5]) + bf16hi(rr.z);
-              f[6] = bf16_round(f[6]) + bf16lo(rr.w); f[7] = bf16_round(f[7]) + bf16hi(rr.w);
-            }
-            uint4 w;
-            w.x = pack_bf16x2(f[0], f[1]); w.y = pack_bf16x2(f[2], f[3]); w.z = pack_bf16x2(f[4], f[5]); w.w = pack_bf16x2(f[6], f[7]);
-            *o = w;
-          }
+          *o = pack_bf16x2(f0, f1);
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_leader(&tmem_empty[acc]);
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();                                   // the pair frees its tensor memory together
-  if (warp == 2) asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" :: "r"(tmem_base), "r"(2 * BN2) : "memory");
-}
-
-template <int BN2, bool A_MN, bool B_MN>
-int launch2(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, cudaStream_t st) {
-  static bool attr = false;
-  if (!attr) {
-    LMOD_CUDA_OK(cudaFuncSetAttribute(gemm2_tcgen05_kernel<BN2, A_MN, B_MN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg2<BN2>::SMEM));
-    attr = true;
-  }
-  const int tiles = ((p.M + 255) / 256) * (p.swiglu ? (p.N + 127) / 128 : (p.N + BN2 - 1) / BN2);
-  int clusters = lmod_num_sms() / 2;
-  if (tiles < clusters) clusters = tiles;
-  gemm2_tcgen05_kernel<BN2, A_MN, B_MN><<<2 * clusters, GEMM_THREADS, Cfg2<BN2>::SMEM, st>>>(ta, tb, p);
-  LMOD_LAUNCH_OK();
-  return LMOD_OK;
-}
-template <int BN2>
-int dispatch2_bn(bool a_mn, bool b_mn, const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, cudaStream_t st) {
-  if (!a_mn && !b_mn) return launch2<BN2, false, false>(ta, tb, p, st);
-  if (!a_mn && b_mn) return launch2<BN2, false, true>(ta, tb, p, st);
-  if (a_mn && b_mn) return launch2<BN2, true, true>(ta, tb, p, st);
-  return launch2<BN2, true, false>(ta, tb, p, st);
-}
-int dispatch2(bool a_mn, bool b_mn, const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, cudaStream_t st) {
-  return p.bn == 128 ? dispatch2_bn<128>(a_mn, b_mn, ta, tb, p, st) : dispatch2_bn<256>(a_mn, b_mn, ta, tb, p, st);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------------------
@@ -661,13 +352,13 @@ template <int BN, bool A_MN, bool B_MN>
 int launch(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, int tiles_upper, cudaStream_t st) {
   static bool attr = false;
   if (!attr) {
-    LMOD_CUDA_OK(cudaFuncSetAttribute(gemm_tcgen05_kernel<BN, A_MN, B_MN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<BN>::SMEM));
+    LMOD_CUDA_OK(cudaFuncSetAttribute(gemm_wgmma_kernel<BN, A_MN, B_MN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<BN>::SMEM));
     attr = true;
   }
   int grid = lmod_num_sms();
   if (tiles_upper < grid) grid = tiles_upper;
   if (grid < 1) grid = 1;
-  gemm_tcgen05_kernel<BN, A_MN, B_MN><<<grid, GEMM_THREADS, Cfg<BN>::SMEM, st>>>(ta, tb, p);
+  gemm_wgmma_kernel<BN, A_MN, B_MN><<<grid, GEMM_THREADS, Cfg<BN>::SMEM, st>>>(ta, tb, p);
   LMOD_LAUNCH_OK();
   return LMOD_OK;
 }
@@ -692,7 +383,7 @@ int pick_bn(int64_t m_tiles, int64_t N) {
 
 // D[M,N] = A * B^T.  a_mn_major = 0: A stored [M,K] (row stride lda) ; 1: A stored [K,M].  b_mn_major = 0: B stored [N,K] ; 1: B stored [K,N].
 // epilogue bit 0: D = bf16(D + acc) ;  d_f32_accum != null: fp32 D32 += acc (ldd applies to it) instead of the bf16 output;
-// epilogue bit 1: fused SwiGLU (B rows tile-interleaved [128 gate | 128 up] per 256; D has N/2 columns; CTA-pair kernel only);
+// epilogue bit 1: retired (the fused SwiGLU forward is lmod_gemm_swiglu);
 // epilogue bits 8..: split-K factor (fp32 atomic accumulation into D32, which the caller zero-initialises).
 struct RopeArgs { const void* cos; const void* sin; const int64_t* pos; int hd; int cols; };
 struct ResidArgs { const void* R; int64_t ld_r; };
@@ -706,36 +397,7 @@ static int gemm_dense(const void* A, int64_t lda, int a_mn_major, const void* B,
   CUtensorMap ta, tb;
   int rc;
   const int splits_req = (epilogue >> 8) > 1 ? (epilogue >> 8) : 1;
-  static const int two_cta_env = getenv("LMOD_GEMM_2CTA") ? atoi(getenv("LMOD_GEMM_2CTA")) : 1;
-  // measured (round 2, profiles/README.md): student dgrad 2048x1024x5632 619 vs 642 TFLOP/s, wgrad 561 vs 580, step 25.69 vs 25.92 samples/s
-  // with / without the 256 x 128 pair tiles -- the 1-CTA 128 x 128 tiles stay the default, the variant is kept behind LMOD_GEMM_PAIR128=1
-  static const int pair128_env = getenv("LMOD_GEMM_PAIR128") ? atoi(getenv("LMOD_GEMM_PAIR128")) : 0;
-  const int64_t tiles256 = ((M + 255) / 256) * ((N + 255) / 256);
-  const int64_t tiles128 = ((M + 255) / 256) * ((N + 127) / 128);
-  const int npairs = lmod_num_sms() / 2;
-  const bool pair256 = two_cta_env && splits_req == 1 && tiles256 >= (int64_t)npairs * 3 / 2;
-  // 256 x 128 pair tiles: the N ~ 1024..3072 problems (0.5B student, CLIP) whose 256 x 256 tiling cannot fill the pairs; needs most pairs busy
-  const bool pair128 = two_cta_env && pair128_env && splits_req == 1 && !pair256 && tiles128 >= (int64_t)npairs * 6 / 7;
-  const bool pair = pair256 || pair128;
   LMOD_CHECK_ARG(!(epilogue & 2), "lmod_gemm_bf16: epilogue bit 1 is retired -- the fused SwiGLU forward is lmod_gemm_swiglu");
-  if (pair) {
-    // CTA-pair kernel: 256 x 256 (or 256 x 128) tiles, each CTA stages 128 rows of A and half of the B tile
-    const int bn2 = pair256 ? 256 : 128;
-    if (!a_mn_major) rc = make_map(&ta, A, (uint64_t)K, (uint64_t)M, (uint64_t)lda, BK, 128);
-    else rc = make_map(&ta, A, (uint64_t)M, (uint64_t)K, (uint64_t)lda, 64, BK);
-    if (rc) return rc;
-    if (!b_mn_major) rc = make_map(&tb, B, (uint64_t)K, (uint64_t)N, (uint64_t)ldb, BK, bn2 / 2);
-    else rc = make_map(&tb, B, (uint64_t)N, (uint64_t)K, (uint64_t)ldb, 64, BK);
-    if (rc) return rc;
-    GemmParams p2 = {};
-    p2.D = (__nv_bfloat16*)D; p2.bias = (const __nv_bfloat16*)bias; p2.D32 = d_f32_accum; p2.ldd = ldd;
-    p2.M = (int)M; p2.N = (int)N; p2.K = (int)K; p2.beta = epilogue & 1; p2.splits = 1; p2.groups = 1; p2.bn = bn2;
-    p2.dbg_nostore = getenv("LMOD_GEMM_NOSTORE") ? 1 : 0;
-    p2.m_dev = m_rows_dev; p2.k_dev = k_rows_dev;
-    if (resid) { p2.R = (const __nv_bfloat16*)resid->R; p2.ld_r = resid->ld_r; }
-    if (rope) { p2.rope_cos = (const __nv_bfloat16*)rope->cos; p2.rope_sin = (const __nv_bfloat16*)rope->sin; p2.rope_pos = rope->pos; p2.rope_hd = rope->hd; p2.rope_cols = rope->cols; }
-    return dispatch2(a_mn_major != 0, b_mn_major != 0, ta, tb, p2, (cudaStream_t)stream);
-  }
   const int BN = pick_bn(((M + BM - 1) / BM) * splits_req, N);
   if (!a_mn_major) rc = make_map(&ta, A, (uint64_t)K, (uint64_t)M, (uint64_t)lda, BK, BM);
   else rc = make_map(&ta, A, (uint64_t)M, (uint64_t)K, (uint64_t)lda, 64, BK);
@@ -803,15 +465,6 @@ static int swiglu_common(const void* A, int64_t lda, const void* W, int64_t ldb,
   GemmParams p = {};
   p.D = (__nv_bfloat16*)act; p.ldd = ld_act; p.M = (int)M; p.N = (int)I; p.K = (int)K; p.splits = 1; p.groups = G > 0 ? G : 1;
   p.swiglu = 1; p.swiglu_I = (int)I; p.H1 = (__nv_bfloat16*)h1; p.ld_h1 = ld_h1; p.bn = 128;     // tile enumeration: 128 act columns per tile
-  static const int two_cta_env = getenv("LMOD_GEMM_2CTA") ? atoi(getenv("LMOD_GEMM_2CTA")) : 1;
-  const int64_t pair_tiles = ((M + 255) / 256) * (I / 128);
-  if (!offsets && two_cta_env && pair_tiles >= (int64_t)(lmod_num_sms() / 2) * 3 / 2) {
-    rc = make_map(&ta, A, (uint64_t)K, (uint64_t)M, (uint64_t)lda, BK, 128);
-    if (rc) return rc;
-    rc = make_map(&tb, W, (uint64_t)K, (uint64_t)(2 * I), (uint64_t)ldb, BK, 128);
-    if (rc) return rc;
-    return dispatch2_bn<256>(false, false, ta, tb, p, st);       // (p.bn = 128 only enumerates the 128 act columns of a tile)
-  }
   rc = make_map(&ta, A, (uint64_t)K, (uint64_t)M, (uint64_t)lda, BK, BM);
   if (rc) return rc;
   rc = make_map(&tb, W, (uint64_t)K, (uint64_t)((offsets ? G : 1) * 2 * I), (uint64_t)ldb, BK, 128);
@@ -850,16 +503,6 @@ static int silu_bwd_common(const void* dY, int64_t lda, const void* W, int64_t l
   GemmParams p = {};
   p.D = (__nv_bfloat16*)dh1; p.ldd = ld_dh1; p.M = (int)M; p.N = (int)I; p.K = (int)K; p.splits = 1; p.groups = G > 0 ? G : 1;
   p.silu_bwd = 1; p.GU = (const __nv_bfloat16*)h1; p.ld_gu = ld_h1;
-  static const int two_cta_env = getenv("LMOD_GEMM_2CTA") ? atoi(getenv("LMOD_GEMM_2CTA")) : 1;
-  const int64_t tiles256 = ((M + 255) / 256) * ((I + 255) / 256);
-  if (!offsets && two_cta_env && tiles256 >= (int64_t)(lmod_num_sms() / 2) * 3 / 2) {
-    rc = make_map(&ta, dY, (uint64_t)K, (uint64_t)M, (uint64_t)lda, BK, 128);
-    if (rc) return rc;
-    rc = make_map(&tb, W, (uint64_t)I, (uint64_t)K, (uint64_t)ldb, 64, BK);
-    if (rc) return rc;
-    p.bn = 256;
-    return dispatch2(false, true, ta, tb, p, st);
-  }
   const int BN = pick_bn((M + BM - 1) / BM, I);
   p.bn = BN;
   rc = make_map(&ta, dY, (uint64_t)K, (uint64_t)M, (uint64_t)lda, BK, BM);

@@ -24,7 +24,7 @@ namespace {
 constexpr int KL_CHUNKS = 4;       // mbarrier-tracked load chunks per slice
 constexpr int KL_MAX_CS = 8;
 constexpr int KL_MIN_CTAS = 2;       // two CTAs per SM (2 x 76 KB of shared memory)
-constexpr int KL_DEFAULT_MODE = 5;      // sb128.  measured (profiles/kl_modes_r1.txt, all rows active): sb128 0.60 ms, sb256 0.64, sb384 0.72, sb512 0.90, db256 1.10, db512 1.24
+constexpr int KL_DEFAULT_MODE = 5;      // sb128: the fastest of the shared-memory-resident modes
 
 struct KlParams {
   const __nv_bfloat16* s;
@@ -75,7 +75,7 @@ __device__ __forceinline__ void accum_pair(uint32_t sw, uint32_t tw, float nms, 
   a = fmaf(et1, s1, a);
 }
 
-// NBUF = 1 (default): one slice buffer, two CTAs per SM hide each other's loads AND each other's barrier waits (33 co-resident clusters).
+// NBUF = 1 (default): one slice buffer, two CTAs per SM hide each other's loads AND each other's barrier waits.
 // NBUF = 2 (LMOD_KL_MODE=db256/db512, experiment kept for the record): one CTA per SM with two slice buffers, the loads of the cluster's
 // NEXT active row issued before the math of the current one.  Measured 1.6-1.8x SLOWER: with one CTA per SM nothing fills the SM while
 // the CTA sits in __syncthreads / barrier.cluster (22 % of warp samples), and only 15 clusters of 8 single-CTA SMs fit the GPCs.
@@ -328,14 +328,17 @@ __global__ void __launch_bounds__(KL_THREADS, NBUF == 2 ? 1 : KL_MIN_CTAS) kl_fu
 // it through a shared-memory ring fed by a dedicated TMA-producer warp, twice:
 //   pass 1  online max / sum-exp / sum p_T*s over the half row (no per-row shared-memory residency, so no 76 KB-per-row limit and no
 //           load latency in front of the math: the ring always holds the next chunks);
-//   pass 2  the same chunks again -- issued by the producer right behind pass 1, so they come out of the 126 MB L2 (74 rows x 0.6 MB
-//           in flight) -- turned into the gradient and written back in place.
+//   pass 2  the same chunks again -- issued by the producer right behind pass 1, so they come out of L2 as long as the rows in flight
+//           fit in it -- turned into the gradient and written back in place.
+// On H100 (50 MB L2, 132 SMs) one CTA per row keeps 132 rows x 0.6 MB = 79 MB in flight and pass 2 partly misses; two CTAs per row
+// (a cluster of 2 sharing the row through DSMEM) keep 66 rows = 40 MB in flight.  Timed on one H100 (400 W limit), 885 rows x 151936:
+// 0.338 ms with two CTAs per row against 0.415 ms with one -> two is the default.
 // The per-row fixed cost (block reduction + exchange between the CTAs of a row) is paid once per HALF row of 76 K logit pairs instead
 // of once per 19 K-pair slice, and the exchange is a DSMEM store + remote mbarrier arrive instead of a barrier.cluster, so the producer
 // warp never stops prefetching.  HBM traffic stays the algorithmic 4V read + 2V written per token as long as pass 2 hits L2
-// (ncu dram__bytes is the check; profiles/).
+// (DRAM bytes read per launch is the check).
 // =====================================================================================================================
-constexpr int KS_CS = 1;                 // CTAs per row (LMOD_KL_MODE=stream2 / stream4: a cluster shares a row through DSMEM)
+constexpr int KS_CS = 2;                 // CTAs per row (a cluster shares a row through DSMEM; LMOD_KL_MODE=stream1 / stream4 override)
 constexpr int KS_CH = 8192;              // logit pairs per ring stage (16 KB student + 16 KB teacher)
 constexpr int KS_STAGES = 6;             // 192 KB ring
 
@@ -393,50 +396,38 @@ __device__ __forceinline__ void bulk_g2s_hint(void* smem_dst, const void* gsrc, 
 }
 
 
-// ---- packed fp32x2 arithmetic + exp2 on the FMA / ALU pipes --------------------------------------------------------------------
+// ---- two-lane arithmetic + exp2 on the FMA / ALU pipes ----------------------------------------------------------------------------
 // The kernel needs 4 exponentials per (student, teacher) logit pair and the MUFU pipe retires 16 per clock per SM: at V = 151936 that
-// is exactly the HBM time of the row.  A share of the exponentials is therefore evaluated WITHOUT the MUFU: Cody-Waite split
-// x = n + f, f in [-0.5, 0.5], 2^f by a degree-4 minimax polynomial (max relative error 3.7e-6), 2^n by an integer add into the exponent,
-// two values per instruction (FFMA2 / FADD2).  Inputs are <= 0 here (logit - running max), clamped at -126.
+// is about the HBM time of the row.  A share of the exponentials is therefore evaluated WITHOUT the MUFU: Cody-Waite split
+// x = n + f, f in [-0.5, 0.5], 2^f by a degree-4 minimax polynomial (max relative error 3.7e-6), 2^n by an integer add into the exponent.
+// Inputs are <= 0 here (logit - running max), clamped at -126.  Every operation is rounded to nearest (no contraction into other FMAs).
+__device__ __forceinline__ float exp2_poly1(float x, uint32_t& t) {
+  const float tf = __fadd_rn(x, 12582912.f);          // t = x + 1.5*2^23: the integer part sits in the low mantissa bits
+  const float n = __fadd_rn(tf, -12582912.f);         // n = round(x)
+  const float f = __fmaf_rn(n, -1.f, x);              // f = x - n
+  float p = 9.676037098e-03f;
+  p = __fmaf_rn(p, f, 5.592203565e-02f);
+  p = __fmaf_rn(p, f, 2.402210736e-01f);
+  p = __fmaf_rn(p, f, 6.931210340e-01f);
+  p = __fmaf_rn(p, f, 1.000000075f);
+  t = __float_as_uint(tf);
+  return p;
+}
 __device__ __forceinline__ void exp2_poly2(float x0, float x1, float& y0, float& y1) {
   x0 = fmaxf(x0, -126.f); x1 = fmaxf(x1, -126.f);
-  uint32_t t0, t1, p0, p1;
-  asm("{\n\t.reg .b64 x, t, n, f, p, k;\n\t"
-      "mov.b64 x, {%4, %5};\n\t"
-      "mov.b64 k, {%6, %6};\n\t"
-      "add.rn.f32x2 t, x, k;\n\t"                 // t = x + 1.5*2^23: the integer part sits in the low mantissa bits
-      "mov.b64 k, {%7, %7};\n\t"
-      "add.rn.f32x2 n, t, k;\n\t"                 // n = round(x)
-      "mov.b64 k, {%8, %8};\n\t"
-      "fma.rn.f32x2 f, n, k, x;\n\t"              // f = x - n
-      "mov.b64 p, {%9, %9};\n\t"
-      "mov.b64 k, {%10, %10};\n\t"
-      "fma.rn.f32x2 p, p, f, k;\n\t"
-      "mov.b64 k, {%11, %11};\n\t"
-      "fma.rn.f32x2 p, p, f, k;\n\t"
-      "mov.b64 k, {%12, %12};\n\t"
-      "fma.rn.f32x2 p, p, f, k;\n\t"
-      "mov.b64 k, {%13, %13};\n\t"
-      "fma.rn.f32x2 p, p, f, k;\n\t"
-      "mov.b64 {%0, %1}, t;\n\t"
-      "mov.b64 {%2, %3}, p;\n\t}"
-      : "=r"(t0), "=r"(t1), "=r"(p0), "=r"(p1)
-      : "f"(x0), "f"(x1), "f"(12582912.f), "f"(-12582912.f), "f"(-1.f), "f"(9.676037098e-03f), "f"(5.592203565e-02f), "f"(2.402210736e-01f),
-        "f"(6.931210340e-01f), "f"(1.000000075f));
-  y0 = __uint_as_float(p0 + (t0 << 23));
-  y1 = __uint_as_float(p1 + (t1 << 23));
+  uint32_t t0, t1;
+  const float p0 = exp2_poly1(x0, t0), p1 = exp2_poly1(x1, t1);
+  y0 = __uint_as_float(__float_as_uint(p0) + (t0 << 23));
+  y1 = __uint_as_float(__float_as_uint(p1) + (t1 << 23));
 }
 __device__ __forceinline__ void ffma2_bcast(float& d0, float& d1, float a0, float a1, float b, float c) {      // d = a * b + c
-  asm("{ .reg .b64 ra, rb, rc, rd; mov.b64 ra, {%2,%3}; mov.b64 rb, {%4,%4}; mov.b64 rc, {%5,%5}; fma.rn.f32x2 rd, ra, rb, rc; mov.b64 {%0,%1}, rd; }"
-      : "=f"(d0), "=f"(d1) : "f"(a0), "f"(a1), "f"(b), "f"(c));
+  d0 = __fmaf_rn(a0, b, c); d1 = __fmaf_rn(a1, b, c);
 }
 __device__ __forceinline__ void fadd2_into(float& d0, float& d1, float a0, float a1) {                         // d += a
-  asm("{ .reg .b64 ra, rd; mov.b64 ra, {%2,%3}; mov.b64 rd, {%0,%1}; add.rn.f32x2 rd, rd, ra; mov.b64 {%0,%1}, rd; }"
-      : "+f"(d0), "+f"(d1) : "f"(a0), "f"(a1));
+  d0 = __fadd_rn(d0, a0); d1 = __fadd_rn(d1, a1);
 }
 __device__ __forceinline__ void ffma2_into(float& d0, float& d1, float a0, float a1, float b0, float b1) {     // d += a * b
-  asm("{ .reg .b64 ra, rb, rd; mov.b64 ra, {%2,%3}; mov.b64 rb, {%4,%5}; mov.b64 rd, {%0,%1}; fma.rn.f32x2 rd, ra, rb, rd; mov.b64 {%0,%1}, rd; }"
-      : "+f"(d0), "+f"(d1) : "f"(a0), "f"(a1), "f"(b0), "f"(b1));
+  d0 = __fmaf_rn(a0, b0, d0); d1 = __fmaf_rn(a1, b1, d1);
 }
 // two-lane accumulators of the online pass
 struct Acc2 { float zs0, zs1, zt0, zt1, a0, a1; };
@@ -463,8 +454,7 @@ __device__ __forceinline__ uint32_t grad_word(uint32_t sw, uint32_t tw, float es
   if (T_POLY) exp2_poly2(xt0, xt1, p0, p1); else { p0 = ex2f(xt0); p1 = ex2f(xt1); }
   float c0, c1;
   ffma2_bcast(c0, c1, p0, p1, ncb, 0.f);                  // -cb * p
-  asm("{ .reg .b64 ra, rb, rc, rd; mov.b64 ra, {%2,%3}; mov.b64 rb, {%4,%4}; mov.b64 rc, {%5,%6}; fma.rn.f32x2 rd, ra, rb, rc; mov.b64 {%0,%1}, rd; }"
-      : "=f"(g0), "=f"(g1) : "f"(q0), "f"(q1), "f"(ca), "f"(c0), "f"(c1));
+  g0 = __fmaf_rn(q0, ca, c0); g1 = __fmaf_rn(q1, ca, c1);
   return 0u;
 }
 
@@ -571,7 +561,7 @@ __global__ void __launch_bounds__(KS_THREADS + 32, 1) kl_stream_kernel(const KlP
         const int e0 = c * KS_CH, nv = min(KS_CH, len - e0) >> 3;
         const uint4* s_buf = reinterpret_cast<const uint4*>(smem_raw + (size_t)st * (KS_CH * 4));
         const uint4* t_buf = reinterpret_cast<const uint4*>(smem_raw + (size_t)st * (KS_CH * 4) + KS_CH * 2);
-        ks_wait(&full[st], (n / KS_STAGES) & 1);      // every thread polls: one-lane polling + __syncwarp measured 25 % slower here
+        ks_wait(&full[st], (n / KS_STAGES) & 1);      // every thread polls
         for (int i = tid; i < nv; i += KS_THREADS) {
           const uint4 sv = s_buf[i], tv = t_buf[i];
           const uint32_t pmx_s = hmax2_u32(hmax2_u32(sv.x, sv.y), hmax2_u32(sv.z, sv.w));
@@ -826,8 +816,8 @@ static int kl_stream_launch_t(KlParams p, int cs, int64_t n_rows, cudaStream_t s
   lmod_count_launch();
   return LMOD_OK;
 }
-// measured (profiles/kl_modes_r2.txt, bench-like rows): polynomial shares 0/8 0.214 ms, 2/8 0.218, 3/8 0.230, 4/8 0.244 -- the kernel is
-// not MUFU-bound, the extra FMA-pipe instructions only cost issue slots; the MUFU-only form is the default and <3,3> stays as the A/B arm
+// the kernel is not MUFU-bound, so the extra FMA-pipe instructions of the polynomial exponentials only cost issue slots; the MUFU-only
+// form is the default and <3,3> stays as the A/B arm
 static int kl_stream_launch(KlParams p, int cs, int64_t n_rows, cudaStream_t stream) {
   static const char* e = getenv("LMOD_KL_POLY");       // "33": polynomial share 3/8 in both passes
   static const char* th = getenv("LMOD_KL_THREADS");   // "256" / "768": consumer threads (default 512)
@@ -849,7 +839,7 @@ extern "C" int lmod_kl_fwd_bwd_rows(const void* s_logits, int64_t ld_s, const vo
   LMOD_CHECK_ARG(((uintptr_t)s_logits % 16 == 0) && ((uintptr_t)t_logits % 16 == 0), "lmod_kl_fwd_bwd: pointers must be 16B aligned");
   if (dlogits) LMOD_CHECK_ARG(ld_d % 8 == 0 && ld_d >= vocab && ((uintptr_t)dlogits % 16 == 0), "lmod_kl_fwd_bwd: bad dlogits stride");
 
-  int cs = (vocab >= 512) ? KL_MAX_CS : 1;      // (a 16-CTA cluster with 38 KB slices, 4 CTAs/SM, measured 2.1x slower)
+  int cs = (vocab >= 512) ? KL_MAX_CS : 1;
   int64_t per = (vocab + cs - 1) / cs;
   int slice = (int)((per + 7) / 8 * 8);
   size_t smem = (size_t)slice * 2 * 2;
@@ -865,12 +855,12 @@ extern "C" int lmod_kl_fwd_bwd_rows(const void* s_logits, int64_t ld_s, const vo
   LMOD_CHECK_ARG((perm == nullptr) == (count == nullptr), "lmod_kl_fwd_bwd_rows: perm and count go together");
   p.perm = perm; p.count = count;
 
-  // LMOD_KL_MODE: unset / "stream" = the streaming kernel (1 CTA per row, ring + L2 re-read); "stream2" / "stream4" = 2 / 4 CTAs per row;
-  // "sb128" the round-1 shared-memory-resident 8-CTA kernel (kept as the A/B arm of profiles/kl_bench.py), "sb256"/"sb384"/"sb512" its
+  // LMOD_KL_MODE: unset / "stream" = the streaming kernel (KS_CS CTAs per row, ring + L2 re-read); "stream1" / "stream2" / "stream4" = 1 / 2 / 4 CTAs per row;
+  // "sb128" the shared-memory-resident 8-CTA kernel (kept as an A/B arm), "sb256"/"sb384"/"sb512" its
   // thread-count variants, "db256"/"db512" its double-buffered experiments
   static const char* mode_env = getenv("LMOD_KL_MODE");
   if (!mode_env || !strncmp(mode_env, "stream", 6)) {
-    int scs = 1;                                     // one CTA per row measured fastest (profiles/kl_modes_r2.txt): 148 rows x 0.6 MB in flight stay in L2
+    int scs = KS_CS;
     if (mode_env && mode_env[6] >= '1' && mode_env[6] <= '8') scs = mode_env[6] - '0';
     int64_t sper = (vocab + scs - 1) / scs;
     p.slice = (int)((sper + 7) / 8 * 8);

@@ -1,4 +1,4 @@
-// moe.cu -- DeepSpeed-0.9.5 top-2 MoE routing on B200: gate (GEMV + softmax + top-2) and seat+scatter (stable capacity positions by
+// moe.cu -- DeepSpeed-0.9.5 top-2 MoE routing on H100: gate (GEMV + softmax + top-2) and seat+scatter (stable capacity positions by
 // warp ballots, token copy) as two ordinary launches of small CTAs; weighted gather/combine; and their backward kernels.
 //
 // Replaces (third-party, call site llavamod/model/language_model/llava_qwen1_5_moe.py:536-546)

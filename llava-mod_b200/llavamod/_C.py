@@ -63,7 +63,6 @@ SIGNATURES = {
     "lmod_grouped_gemm_bf16": [_P, _L, _P, _L, _P, _L, _P, _I, _L, _L, _L, _L, _I, _I, _P],
     "lmod_gemm_residual": [_P, _L, _P, _L, _P, _P, _L, _P, _L, _L, _L, _L, _P],
     "lmod_attn_fwd": [_P, _L, _L, _L, _I, _I, _I, _I, _F, _P, _L, _P, _P, _P, _P],
-    "lmod_attn_fwd_trace": [_P, _L, _L, _L, _I, _I, _I, _I, _F, _P, _L, _P, _P, _P],
     "lmod_attn_bwd": [_P, _L, _P, _L, _P, _L, _P, _L, _L, _I, _I, _I, _I, _F, _P, _L, _P, _P, _P, _P, _P],
     "lmod_version": [],
     "lmod_launch_count_reset": [],

@@ -2,7 +2,7 @@
 shells/train/qwen/dense2sparse_distillation.sh:48-88 and preference_distillation.sh:48-88).
 
 ``TrainingArguments`` restates the subset of ``transformers.TrainingArguments`` the shells set (HF Trainer / accelerate /
-DeepSpeed are not on the B200 path); unknown HF flags are accepted and ignored with a warning so the reference's shell
+DeepSpeed are not on this path); unknown HF flags are accepted and ignored with a warning so the reference's shell
 command lines keep working (``--deepspeed <json>`` is accepted and ignored: plain data parallelism replaces ZeRO-2)."""
 import argparse
 import dataclasses

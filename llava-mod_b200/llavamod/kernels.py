@@ -42,7 +42,7 @@ def _need_cuda(*ts):
 
 
 # ---------------------------------------------------------------------------------------------------
-# GEMM plumbing.  Every dense contraction of the path (forward, dgrad, wgrad, grouped expert forms) runs on the hand-written tcgen05 /
+# GEMM plumbing.  Every dense contraction of the path (forward, dgrad, wgrad, grouped expert forms) runs on the hand-written wgmma /
 # TMA GEMM of csrc/gemm.cu through lmod_gemm_bf16 / lmod_grouped_gemm_bf16; no library GEMM is called.
 # ---------------------------------------------------------------------------------------------------
 def _rows(t):
@@ -51,7 +51,7 @@ def _rows(t):
 
 
 def mm_nt(x, w, bias=None):
-    """y[..,N] = x[..,K] @ w[N,K]^T (+bias) -- nn.Linear forward on the tcgen05 GEMM."""
+    """y[..,N] = x[..,K] @ w[N,K]^T (+bias) -- nn.Linear forward on the wgmma GEMM."""
     y = gemm(_rows(x), w, bias=bias)
     return y if x.dim() == 2 else y.view(*x.shape[:-1], w.shape[0])     # no view object for the 2-D case (RoPE writes in place)
 
@@ -64,7 +64,7 @@ def mm_nn(dy, w, m_dev=None):
     Kout = w.shape[1]
     tiles = ((M + 127) // 128) * ((Kout + 255) // 256)
     if tiles < 100 and N >= 16384:
-        split = max(2, min(16, 148 // max(1, tiles)))
+        split = max(2, min(16, torch.cuda.get_device_properties(dy.device).multi_processor_count // max(1, tiles)))
         acc = torch.zeros(M, Kout, dtype=torch.float32, device=dy.device)
         gemm(dy2, w, b_mn=True, out_f32=acc, split_k=split, m_dev=m_dev)
         return acc.to(dy.dtype)
@@ -114,7 +114,7 @@ def scatter_rows(xc, perm, count, n):
 
 
 def gemm(a, b, a_mn=False, b_mn=False, bias=None, out=None, accumulate=False, out_f32=None, split_k=1, m_dev=None, k_dev=None):
-    """Hand-written tcgen05/TMA GEMM (lmod_gemm_bf16).  D[M,N] (+)= A * B^T with
+    """Hand-written wgmma/TMA GEMM (lmod_gemm_bf16).  D[M,N] (+)= A * B^T with
        a_mn=False: a is [M,K] ; True: a is [K,M]     b_mn=False: b is [N,K] ; True: b is [K,N].
        m_dev / k_dev: int32 device scalars bounding the rows of D / the reduction (lmod_gemm_bf16_dyn; active-row loss head)."""
     _need_cuda(a, b)
@@ -132,16 +132,14 @@ def gemm(a, b, a_mn=False, b_mn=False, bias=None, out=None, accumulate=False, ou
     return out
 
 
-# Epilogue fusions run on the GEMM's 4 epilogue warps, so they pay off only when the main loop is long enough to hide them
-# (profiles/microbench_r2.txt): at the teacher's K = 4096 the fused SwiGLU forward is 8 % faster than GEMM + silu_mul (0.275 vs 0.299 ms),
-# at the student's K = 1024 it is 30 % SLOWER (49 vs 37 us; the silu-backward epilogue 58 vs 34 us) -- there the element-wise kernels,
-# which use every warp of the SM, win.  The (lighter) RoPE epilogue of the q|k|v projection wins at both.  LLAVAMOD_FUSE_SWIGLU: "auto" (by
+# Epilogue fusions pay off only when the GEMM's main loop is long enough to hide them: the fused SwiGLU forward is used from a reduction
+# length of FUSE_MIN_K on (the teacher's K = 4096); at the student's K = 1024 the element-wise kernels, which use every warp of the SM,
+# are preferred.  The (lighter) RoPE epilogue of the q|k|v projection is always fused.  LLAVAMOD_FUSE_SWIGLU: "auto" (by
 # reduction length), "1" always, "0" never; LLAVAMOD_FUSE_ROPE: "0" = GEMM + lmod_rope.
 FUSE_SWIGLU = _os.environ.get("LLAVAMOD_FUSE_SWIGLU", "auto")
 FUSE_ROPE = _os.environ.get("LLAVAMOD_FUSE_ROPE", "auto")
 # residual add in the o_proj / down_proj (CLIP: out_proj / fc2) epilogue of no-grad forwards.  Bit-identical to the add inside the next norm's
-# kernel; measured (profiles/microbench_r2.txt, profiles/ab_bench_r2.txt): the teacher GEMMs run at 0.96 of the tensor peak and have no epilogue
-# slack, so projection + norm is 0.071 vs 0.067 ms with the add in the epilogue and the step does not move (25.0 vs 25.0 samples/s) -> opt-in
+# kernel; opt-in (the add is cheap inside the norm kernel, and the epilogue of a long GEMM has little slack)
 FUSE_RESIDUAL = _os.environ.get("LLAVAMOD_FUSE_RESIDUAL", "0")
 FUSE_MIN_K = 2048
 
@@ -328,7 +326,7 @@ ATTN_HEAD_DIMS = (64, 128)
 
 
 def attention_fwd(qkv, B, T, nh, nkv, hd, causal, scale=None, need_lse=False, pad=None):
-    """Hand-written tcgen05 flash-attention forward on the fused QKV buffer [B*T, (nh+2nkv)*hd] -> [B*T, nh*hd] (+ lse [B,nh,T]).
+    """Hand-written wgmma flash-attention forward on the fused QKV buffer [B*T, (nh+2nkv)*hd] -> [B*T, nh*hd] (+ lse [B,nh,T]).
     pad = (kv_lo, kv_hi): int32 [B] device tensors, the real key range of every batch row (padded batches), or None."""
     _need_cuda(qkv)
     out = torch.empty(B * T, nh * hd, dtype=qkv.dtype, device=qkv.device)
@@ -340,7 +338,7 @@ def attention_fwd(qkv, B, T, nh, nkv, hd, causal, scale=None, need_lse=False, pa
 
 
 class AttnFn(Function):
-    """Qwen2SdpaAttention core (modeling_qwen2.py:713-721, 4-D mask :1035-1040): our tcgen05 forward (lmod_attn_fwd) and backward
+    """Qwen2SdpaAttention core (modeling_qwen2.py:713-721, 4-D mask :1035-1040): our wgmma forward (lmod_attn_fwd) and backward
     (lmod_attn_bwd); dq|dk|dv come back as one fused buffer."""
 
     @staticmethod
@@ -361,7 +359,7 @@ class AttnFn(Function):
 
 
 def attention_bwd(qkv, out, dout, lse, B, T, nh, nkv, hd, causal, scale, pad=None):
-    """Hand-written tcgen05 flash-attention backward -> fused dqkv (same layout as qkv)."""
+    """Hand-written wgmma flash-attention backward -> fused dqkv (same layout as qkv)."""
     dqkv = torch.empty_like(qkv)
     dq32 = torch.empty(B * T, nh * hd, dtype=torch.float32, device=qkv.device)
     dsum = torch.empty(B, nh, T, dtype=torch.float32, device=qkv.device)
@@ -372,7 +370,7 @@ def attention_bwd(qkv, out, dout, lse, B, T, nh, nkv, hd, causal, scale, pad=Non
 
 
 def attention(qkv, B, T, nh, nkv, hd, causal=True, scale=None, pad=None):
-    """Self-attention on the fused, RoPE'd QKV buffer [B*T, (nh+2nkv)*hd] -> [B*T, nh*hd], always on the tcgen05 kernels.
+    """Self-attention on the fused, RoPE'd QKV buffer [B*T, (nh+2nkv)*hd] -> [B*T, nh*hd], always on the wgmma kernels.
     Head dims other than 64 / 128 (the reference's tiny test shapes) are zero-padded per head to the next built width: the extra
     q/k columns add 0 to every score and the extra v columns produce output columns that are sliced away (softmax scale = hd^-0.5 of
     the TRUE head dim); the pad / slice are plain tensor ops, so autograd carries the gradient back to the unpadded buffer."""
@@ -543,7 +541,7 @@ class QKVRopeFn(Function):
 
 def qkv_rope(x, w, bias, cos, sin, pos, nh, nkv, hd, wgrad=None, bgrad=None):
     """Fused q|k|v projection + RoPE for the head dims the epilogue is built for; other head dims (tiny test shapes) take GEMM + lmod_rope."""
-    if hd not in ATTN_HEAD_DIMS or FUSE_ROPE == "0":       # the RoPE epilogue wins at every reduction length measured (K 1024: 29 vs 33 us, K 4096: 167 vs 178 us)
+    if hd not in ATTN_HEAD_DIMS or FUSE_ROPE == "0":
         return rope_(linear(x, w, bias, wgrad, bgrad), cos, sin, pos, nh, nkv, hd)
     if torch.is_grad_enabled() and (x.requires_grad or wgrad is not None):
         return QKVRopeFn.apply(x, w, bias, cos, sin, pos, nh, nkv, hd, wgrad, bgrad)
@@ -724,7 +722,7 @@ def moe_gather_combine(y, row, w, residual=None):
 
 class MoEFn(Function):
     """x: post-attention-layernorm hidden [S,H]; res: residual stream [S,H].  Experts are SwiGLU MLPs with fused gate|up weights
-    w_gu [E,2I,H] and w_dn [E,H,I].  Expert GEMMs run as ONE grouped tcgen05 GEMM each over COMPACT expert rows (no capacity
+    w_gu [E,2I,H] and w_dn [E,H,I].  Expert GEMMs run as ONE grouped wgmma GEMM each over COMPACT expert rows (no capacity
     padding; the reference computes E*C = 1.5x the routed rows).  Returns (res + moe_out, l_aux)."""
 
     @staticmethod

@@ -3,7 +3,7 @@
 The reference's evaluation scripts call HF `generate` with `use_cache=False` (llavamod/eval/model_vqa_loader.py:119-130; the
 DeepSpeed-MoE eval classes do not carry a KV cache through `MoEQwen1_5Model_forward`), i.e. every new token re-runs the multimodal
 splice and the whole decoder on the sequence so far.  This module does the same thing on the CUDA path -- the prefill kernels
-(tcgen05 GEMMs, flash attention, fused router) are the hot path here -- with two savings that do not change the result: the CLIP tower
+(wgmma GEMMs, flash attention, fused router) are the hot path here -- with two savings that do not change the result: the CLIP tower
 + projector run once per call instead of once per token, and lm_head is applied to the last position only.  Routing uses
 `eval_capacity_factor` (model.eval()), and, as in the reference, fresh Gumbel noise for the second expert at every step
 (DeepSpeed top2gating adds it regardless of train / eval).

@@ -1,11 +1,11 @@
-"""Qwen2 decoder engine for the B200 build (dense and DeepSpeed-style sparse-MoE layers).
+"""Qwen2 decoder engine for the H100 build (dense and DeepSpeed-style sparse-MoE layers).
 
 Stands in for the reference's vendored ``qwen1_5/modeling_qwen2.py`` (RMSNorm :96-110, RoPE :114-184, MLP :188-200,
 SDPA attention :644-728, decoder layer :738-812, model :932-1107) and the patched MoE forwards of
 ``llava_qwen1_5_moe.py:112-339``.  Parameter modules keep the reference's attribute / checkpoint key names;
 the arithmetic is issued through ``llavamod.kernels`` (our CUDA: GEMM, attention, norms, RoPE, MoE, loss heads).
 
-Layout decisions (B200-first):
+Layout decisions (GPU-first):
   * q|k|v and gate|up weights live in ONE fused buffer each (one GEMM instead of three / two); the per-projection
     ``nn.Parameter``s the reference exposes are views into it, so ``state_dict()`` keeps the reference layout;
   * the E experts of an MoE layer are one [E,2I,H] + one [E,H,I] buffer (batched / grouped GEMM operands);

@@ -3,7 +3,7 @@
 Stands in for ``llavamod/model/llava_arch.py`` (LlavaMetaModel :27-128, encode_images :143-148,
 prepare_inputs_labels_for_multimodal :155-334; image branch only -- 4-D video entries are out of scope).
 
-The splice is split the B200 way: the INTEGER plan (which embedding row / image-feature row feeds every output
+The splice is split in two: the INTEGER plan (which embedding row / image-feature row feeds every output
 position, the new labels, mask and position ids) is computed on the host from the host copy of ``input_ids`` --
 the reference does the same work on the device with two host syncs (llava_arch.py:237,247) -- and the float part
 is one gather kernel (``lmod_splice_embed``) whose backward scatters into the projector output.

@@ -16,7 +16,7 @@ ARCH = {
                          num_key_value_heads=16, vocab_size=151936, rope_theta=1e6, tie_word_embeddings=False),
     "qwen1.5-7b": dict(hidden_size=4096, intermediate_size=11008, num_hidden_layers=32, num_attention_heads=32,
                        num_key_value_heads=32, vocab_size=151936, rope_theta=1e6, tie_word_embeddings=False),
-    # config 1 of BASELINE.json (2-layer / 128-d); 2 heads -> head_dim 64, so the tcgen05 attention kernel is the one that runs
+    # config 1 of BASELINE.json (2-layer / 128-d); 2 heads -> head_dim 64, so the wgmma attention kernel is the one that runs
     "tiny": dict(hidden_size=128, intermediate_size=256, num_hidden_layers=2, num_attention_heads=2,
                  num_key_value_heads=2, vocab_size=512, rope_theta=1e6, tie_word_embeddings=False),
 }

@@ -5,7 +5,7 @@ Reference: llavamod/train/align_trainer.py (AlignTrainer :180; get_p :455-477; g
 slice 151936, ``moe_loss`` counted inside the model loss AND again by the trainer under ``kd_lm``, ``-1.0`` sentinel metric,
 0/0 -> NaN for a fully masked batch.
 
-B200 hot loop (``compute_loss``): frozen teacher forward (no grad) -> bf16 teacher logits; student forward; the student's
+Hot loop (``compute_loss``): frozen teacher forward (no grad) -> bf16 teacher logits; student forward; the student's
 lm_head GEMM output goes straight into ONE fused kernel that produces the mimic loss, the LM loss and d(logits) in a single
 sweep (no fp32 [N,V] probability tensors -- the reference materialises five of them); when teacher and student hold the
 same frozen CLIP tower it runs once per micro-batch instead of twice.

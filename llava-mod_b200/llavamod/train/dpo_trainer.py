@@ -4,7 +4,7 @@ Reference: llavamod/train/dpo_trainer.py (DPOTrainer :180; get_logp :462-495; dp
 Kept: shift by one, NO vocabulary slice, masked sequence SUM of gathered log-probs, the four loss types with beta=0.1,
 ``chosen_moe + rejected_moe`` added when enabled, the ten logged metrics.
 
-B200 hot loop: two frozen-teacher forwards (no grad) and two student forwards; each lm_head GEMM feeds the fused
+Hot loop: two frozen-teacher forwards (no grad) and two student forwards; each lm_head GEMM feeds the fused
 log-softmax+gather kernel (online LSE + pick, 2*V bytes/token) instead of materialising log_softmax over [B,T,V]; the DPO
 scalar math runs on [B] device tensors; backward re-reads the bf16 logits once and writes d(logits) in place.
 """

@@ -2,7 +2,7 @@
 fused AdamW, gradient all-reduce over NCCL.
 
 Replaces what the reference gets from HF Trainer + accelerate + DeepSpeed ZeRO-2 with CPU-offloaded Adam
-(llavamod/train/align_trainer.py:326-453, llavamod/config/dpconfig/zero2_offload.json): on a 180 GB B200 nothing is
+(llavamod/train/align_trainer.py:326-453, llavamod/config/dpconfig/zero2_offload.json): on an 80 GB H100 nothing is
 sharded or offloaded -- the trainable student parameters (0.5B-4E: 521 M) keep bf16 model copy + fp32 master + two fp32
 moments + a bf16 gradient buffer resident (16 B/param = 8.3 GB), the frozen teacher is replicated, and the only
 collective of a step is ONE all-reduce over the flat gradient buffer (student grads only; SURVEY.md section 8e).

@@ -65,9 +65,8 @@ class BaseTrainer:
         self._graph_pool = None
         self._statics = {}                   # base signature -> static input buffers shared by the graphs of that signature
         # data parallel experiment (LLAVAMOD_GRAPH_ALLREDUCE=1, OFF by default): capture the gradient all-reduce INSIDE the graph of the step's
-        # last micro-batch, behind the student's backward and ahead of the join with the teacher stream.  Measured on 2 GPUs (round 2,
-        # profiles/README.md): 320.0 ms/step against 316.6 ms with the plain blocking all-reduce after the replay -- NCCL's CTAs compete with
-        # the teacher's persistent GEMMs instead of hiding behind them -- and c10d aborts at shutdown with captured NCCL work outstanding.
+        # last micro-batch, behind the student's backward and ahead of the join with the teacher stream.  NCCL's CTAs then compete with the
+        # teacher's persistent GEMMs instead of hiding behind them, and c10d aborts at shutdown with captured NCCL work outstanding.
         self.graph_allreduce = bool(int(os.environ.get("LLAVAMOD_GRAPH_ALLREDUCE", "0")))
         self._suppress_store = False
         self.graph_replayed_launches = 0     # liblmod kernels executed through graph replays (not seen by the host-side counter)

@@ -47,11 +47,11 @@ def load():
     """Returns a namespace with the reference classes of the dense path.
 
     The reference uses absolute ``llavamod.*`` imports, so it has to live under that name in ``sys.modules`` -- the same
-    name as the B200 package.  The two therefore never share a process: tests reach the reference through
+    name as this project's package.  The two therefore never share a process: tests reach the reference through
     ``run_child`` (a subprocess running ``oracle/ref_child.py``); only ``tests/golden/make_golden.py`` and that child
     call ``load()`` directly."""
     if "llavamod" in sys.modules and not getattr(sys.modules["llavamod"], "__path__", [""])[0].startswith(REF_ROOT):
-        raise RuntimeError("the B200 llavamod package is already imported in this process; use ref_shim.run_child()")
+        raise RuntimeError("this project's llavamod package is already imported in this process; use ref_shim.run_child()")
     if _loaded:
         return types.SimpleNamespace(**_loaded)
     if not available():
@@ -153,7 +153,7 @@ def build_tiny_dense(tmpdir, hidden=128, inter=256, layers=2, heads=4, kv_heads=
 
 
 def run_child(request: dict, timeout=600):
-    """Runs oracle/ref_child.py in a clean subprocess (reference namespace isolated from the B200 package).
+    """Runs oracle/ref_child.py in a clean subprocess (reference namespace isolated from this project's package).
     ``request`` = dict(kw=<build_tiny_dense kwargs>, input_ids, labels, attention_mask, images, padding_side).
     Returns dict(state_dict, logits, labels, loss)."""
     import subprocess

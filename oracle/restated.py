@@ -1,6 +1,6 @@
 """TEST INFRASTRUCTURE ONLY -- CPU restatement (plain PyTorch) of the LLaVA-MoD distillation step.
 
-This is the parity oracle for the B200 build.  Only ``tests/``, ``__graft_entry__.smoke()`` and
+This is the parity oracle for the H100 build.  Only ``tests/``, ``__graft_entry__.smoke()`` and
 ``bench.py``'s ``cpu_baseline`` / ``--impl reference`` legs may import it; the product package
 (``llava-mod_b200/llavamod``) must never do so.
 

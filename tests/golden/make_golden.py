@@ -1,10 +1,11 @@
-"""Generates tests/golden/dense_*.pt by running the REFERENCE's own dense path
+"""Generates tests/golden/dense_*.<i>.pt (shards, see shards.py) by running the REFERENCE's own dense path
 (LlavaQwen1_5ForCausalLM, imported in place through oracle/ref_shim.py) on seeded tiny inputs.
 Run in the build container only (needs /root/reference):  python tests/golden/make_golden.py
 
 Each fixture holds: the reference model's state_dict (reference key names), config numbers, the
 inputs, and the reference outputs (logits fp32, post-splice labels, loss, a few parameter grads).
 """
+import glob
 import os
 import sys
 import tempfile
@@ -14,6 +15,7 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, ROOT)
 from oracle import ref_shim  # noqa: E402
+from tests.golden import shards  # noqa: E402
 
 OUT = os.path.dirname(os.path.abspath(__file__))
 
@@ -23,7 +25,7 @@ CASES = {
                       B=2, T=20, img_pos=[[3], [7]], pad=[0, 3]),
     "dense_gqa": dict(kw=dict(hidden=128, inter=192, layers=2, heads=4, kv_heads=2, vocab=384, seed=1),
                       B=3, T=24, img_pos=[[2, 11], [], [0]], pad=[0, 5, 9]),
-    # head_dim 64 (2 heads x 64, CLIP 1 head x 64): the shapes our tcgen05 attention kernel is built for
+    # head_dim 64 (2 heads x 64, CLIP 1 head x 64): the shapes our wgmma attention kernel is built for
     "dense_hd64": dict(kw=dict(hidden=128, inter=256, layers=2, heads=2, kv_heads=1, vocab=512, seed=3, clip_heads=1),
                        B=2, T=30, img_pos=[[4], [9]], pad=[0, 0]),
     "dense_nopad": dict(kw=dict(hidden=128, inter=256, layers=2, heads=4, kv_heads=4, vocab=512, seed=2),
@@ -69,9 +71,9 @@ def main():
         fx = dict(kw=case["kw"], input_ids=ids, labels=labels, attention_mask=mask, images=images,
                   state_dict=sd, logits=out.logits.detach(), out_labels=out.labels, loss=out.loss.detach(),
                   grads=grads)
-        torch.save(fx, os.path.join(OUT, name + ".pt"))
-        print(name, "logits", tuple(out.logits.shape), "loss", float(out.loss),
-              "size", os.path.getsize(os.path.join(OUT, name + ".pt")) // 1024, "KiB")
+        shards.save(fx, OUT, name)
+        size = sum(os.path.getsize(p) for p in glob.glob(os.path.join(OUT, name + ".*.pt")))
+        print(name, "logits", tuple(out.logits.shape), "loss", float(out.loss), "size", size // 1024, "KiB")
 
 
 if __name__ == "__main__":

@@ -1,4 +1,4 @@
-"""Generates tests/golden/trainer_losses.pt by running the REFERENCE's own trainer methods on seeded fake model outputs:
+"""Generates tests/golden/trainer_losses.<i>.pt (shards, see shards.py) by running the REFERENCE's own trainer methods on seeded fake model outputs:
     python tests/golden/make_loss_golden.py
 
 llavamod/train/align_trainer.py and dpo_trainer.py cannot be imported here (accelerate, transformers 4.37 internals), but the loss code in
@@ -12,6 +12,7 @@ The vocabulary is 256 (so the hard-coded [:151936] slice is a no-op here, as in 
 logits, all-masked labels (0/0 -> NaN), distill_all_tokens, every DPO loss type and both moe-loss branches (incl. the -1.0 sentinel)."""
 import ast
 import os
+import sys
 import types
 
 import torch
@@ -20,6 +21,8 @@ import torch.nn.functional as F
 from typing import Any, Dict, List, Literal, Optional, Tuple, Union
 
 HERE = os.path.dirname(os.path.abspath(__file__))
+sys.path.insert(0, os.path.dirname(os.path.dirname(HERE)))
+from tests.golden import shards  # noqa: E402
 REF = os.environ.get("LLAVAMOD_REFERENCE", "/root/reference")
 
 
@@ -110,8 +113,8 @@ def main():
     me = make_self(D, loss_type="sigmoid", label_smoothing=0.1)
     lp = [torch.randn(5, generator=g) for _ in range(4)]
     cases["dpo_smoothed"] = dict(logps=lp, out=D.dpo_loss(me, *lp))
-    torch.save(cases, os.path.join(HERE, "trainer_losses.pt"))
-    print("wrote trainer_losses.pt:", {k: (len(v) if isinstance(v, list) else 1) for k, v in cases.items()})
+    shards.save(cases, HERE, "trainer_losses")
+    print("wrote trainer_losses.<i>.pt:", {k: (len(v) if isinstance(v, list) else 1) for k, v in cases.items()})
 
 
 if __name__ == "__main__":

@@ -1,5 +1,5 @@
-"""tcgen05/TMA GEMM (lmod_gemm_bf16 / lmod_grouped_gemm_bf16) vs an fp32 reference of the same bf16 inputs.
-Tolerance: the reference accumulates in fp32 as the kernel does (TMEM), so the only difference is the summation order and the
+"""wgmma/TMA GEMM (lmod_gemm_bf16 / lmod_grouped_gemm_bf16) vs an fp32 reference of the same bf16 inputs.
+Tolerance: the reference accumulates in fp32 as the kernel does (registers), so the only difference is the summation order and the
 final bf16 rounding: |err| <= 2^-8 * |ref| + 2^-8 * sqrt(K) * 2e-2."""
 import pytest
 import torch
@@ -37,8 +37,8 @@ def test_gemm_all_layouts(M, N, K, a_mn, b_mn):
 @pytest.mark.parametrize("a_mn,b_mn", [(False, False), (False, True), (True, True), (True, False)])
 @pytest.mark.parametrize("M,N,K", [(2048, 4096, 512), (1900, 3904, 520), (2048, 1024, 2816), (5632, 1024, 2048), (2048, 3072, 1024), (1990, 1000, 520)])
 def test_gemm_two_cta_path(M, N, K, a_mn, b_mn):
-    """Problems with >= 111 256x256 tiles run on the CTA-pair (cta_group::2) kernel with 256x256 tiles (the 256x128 variant for the
-    N ~ 1024..3072 problems is opt-in, LMOD_GEMM_PAIR128=1, and covered when the suite runs with that switch)."""
+    """Large problems (what used to run on a two-CTA kernel): 128x256 or 128x128 tiles depending on how well they fill the SMs, with a
+    bias epilogue and the fp32-accumulate output."""
     from llavamod import kernels as Kk
     g = torch.Generator(device="cuda").manual_seed(M + N + K + 1)
     pad = lambda n: (n + 7) // 8 * 8          # noqa: E731
@@ -249,4 +249,4 @@ def test_gemm_throughput_report():
             e1.record()
             torch.cuda.synchronize()
             res.append(2.0 * M * N * K * 10 / (e0.elapsed_time(e1) * 1e-3) / 1e12)
-        print(f"GEMM {M}x{N}x{K}: lmod tcgen05 {res[0]:.0f} TFLOP/s, cuBLAS {res[1]:.0f} TFLOP/s")
+        print(f"GEMM {M}x{N}x{K}: lmod wgmma {res[0]:.0f} TFLOP/s, cuBLAS {res[1]:.0f} TFLOP/s")

@@ -7,6 +7,7 @@ import pytest
 import torch
 
 from oracle import restated as R
+from tests.golden import shards
 
 
 def test_splice_plan_bit_exact_vs_oracle():
@@ -65,7 +66,7 @@ def test_cosine_schedule_matches_oracle():
 def test_checkpoint_key_layout_equals_reference(name, golden_dir):
     """The reference's own state_dict (golden fixture) must load into our dense class key-for-key, shape-for-shape."""
     from llavamod.model import LlavaQwen1_5Config, LlavaQwen1_5ForCausalLM
-    fx = torch.load(os.path.join(golden_dir, name + ".pt"), weights_only=False)
+    fx = shards.load(golden_dir, name)
     kw = fx["kw"]
     clip = dict(hidden_size=64, intermediate_size=128, num_hidden_layers=3, num_attention_heads=kw.get("clip_heads", 4), image_size=32, patch_size=8)
     cfg = LlavaQwen1_5Config(vocab_size=kw["vocab"], hidden_size=kw["hidden"], intermediate_size=kw["inter"],

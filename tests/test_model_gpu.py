@@ -9,6 +9,7 @@ pytestmark = pytest.mark.gpu
 
 from oracle import restated as R  # noqa: E402
 from tests import helpers as Hh  # noqa: E402
+from tests.golden import shards  # noqa: E402
 
 
 def _rel(a, b):
@@ -20,7 +21,7 @@ def test_dense_model_matches_reference_golden(name, golden_dir):
     """Reference outputs (fp32, from the reference's own code) vs our bf16 CUDA model loaded with the same weights."""
     from llavamod.model import LlavaQwen1_5Config, LlavaQwen1_5ForCausalLM
     from llavamod.model.builder_io import load_into
-    fx = torch.load(os.path.join(golden_dir, name + ".pt"), weights_only=False)
+    fx = shards.load(golden_dir, name)
     kw = fx["kw"]
     clip = dict(hidden_size=64, intermediate_size=128, num_hidden_layers=3, num_attention_heads=kw.get("clip_heads", 4), image_size=32, patch_size=8)
     cfg = LlavaQwen1_5Config(vocab_size=kw["vocab"], hidden_size=kw["hidden"], intermediate_size=kw["inter"], num_hidden_layers=kw["layers"],
@@ -233,7 +234,7 @@ def test_loss_curve_tracks_oracle_20_steps():
 def test_loss_curve_100_steps_config1():
     """BASELINE.json config 1, 100 optimizer steps (AdamW + cosine schedule + clipping): bf16 CUDA path vs the fp32 CPU oracle started
     from the same weights and fed the same batches / router noise.  Stated tolerance (BASELINE.json north star): |loss - oracle| <= 1e-3
-    at every step; measured on B200: max 6.4e-4 absolute = 5e-5 relative."""
+    at every step."""
     student, teacher = Hh.tiny_pair()
     sd_s, sd_t = Hh.oracle_state(student), Hh.oracle_state(teacher)
     keys = [n for n, p in student.named_parameters() if p.requires_grad]
@@ -373,7 +374,7 @@ def test_dpo_gradients_match_oracle_autograd(loss_type):
     """Backward of the preference step through the fused log-prob head (lmod_logp_gather_bwd), two student forwards sharing one set of
     weights: every trainable gradient against fp32 autograd of the oracle, same bar as the mimic step (8 % of the tensor norm)."""
     student, teacher = Hh.tiny_pair()
-    # seeds whose top-2 gate logits are never closer than the bf16-vs-fp32 activation noise (profiles/route_diag.py): one token routed to a
+    # seeds whose top-2 gate logits are never closer than the bf16-vs-fp32 activation noise: one token routed to a
     # different expert on the two sides moves ~2 % of an expert's rows and would drown the arithmetic being compared -- the test first
     # proves that both sides route identically, then compares gradients
     bc, nc, br, nr, inputs = _dpo_inputs(student, seeds=(24, 26))

@@ -1,9 +1,10 @@
 """Pins oracle/restated.py against the reference's own dense path.
 
-* golden leg (runs everywhere): tests/golden/dense_*.pt were produced by the reference's
+* golden leg (runs everywhere): tests/golden/dense_*.<i>.pt (shards, tests/golden/shards.py) were produced by the reference's
   LlavaQwen1_5ForCausalLM (tests/golden/make_golden.py); the restatement must reproduce logits,
   post-splice labels, loss and parameter gradients.
-* live leg (only where /root/reference exists): fresh seeds / shapes through oracle/ref_shim.py.
+* live leg: fresh seeds / GQA / left padding, against the reference's answers stored by tests/golden/make_ref_golden.py
+  (tests/golden/ref_live_*.pt).
 """
 import os
 
@@ -11,7 +12,8 @@ import pytest
 import torch
 
 from oracle import restated as R
-from oracle import ref_shim
+from tests.golden.make_ref_golden import LIVE_CASES, live_key, live_request
+from tests.golden import shards
 
 CASES = ["dense_mha", "dense_gqa", "dense_nopad", "dense_hd64"]
 
@@ -34,7 +36,7 @@ def run_restated(fx, with_grad=True):
 
 @pytest.mark.parametrize("name", CASES)
 def test_restated_matches_reference_golden(name, golden_dir):
-    fx = torch.load(os.path.join(golden_dir, name + ".pt"), weights_only=False)
+    fx = shards.load(golden_dir, name)
     sd, out = run_restated(fx)
     assert torch.equal(out["labels"], fx["out_labels"])           # integer splice logic: bit exact
     valid = out["attention_mask"]
@@ -45,20 +47,12 @@ def test_restated_matches_reference_golden(name, golden_dir):
         torch.testing.assert_close(sd[k].grad, g, rtol=2e-3, atol=2e-6, msg=lambda m: f"{k}: {m}")
 
 
-@pytest.mark.skipif(not ref_shim.available(), reason="reference tree not on this box")
-@pytest.mark.parametrize("seed,heads,kv,side", [(11, 4, 4, "right"), (12, 4, 1, "right"), (13, 2, 2, "left")])
-def test_restated_matches_reference_live(seed, heads, kv, side):
-    """Fresh seeds / GQA / left padding through the reference itself (run in a child process, see ref_shim.load)."""
-    g = torch.Generator().manual_seed(seed)
-    B, T = 3, 12
-    ids = torch.randint(0, 97, (B, T), generator=g)
-    ids[0, 1] = -200; ids[2, 4] = -200; ids[2, 9] = -200
-    mask = torch.ones(B, T, dtype=torch.bool); mask[1, 8:] = False
-    labels = ids.clone(); labels[:, :3] = -100
-    images = [torch.randn(3, 32, 32, generator=g) for _ in range(4)]
-    kw = dict(hidden=64, inter=96, layers=1, heads=heads, kv_heads=kv, vocab=97, seed=seed)
-    ref = ref_shim.run_child(dict(kw=kw, input_ids=ids, labels=labels, attention_mask=mask, images=images, padding_side=side,
-                                  clip_images=torch.stack(images[:2])))
+@pytest.mark.parametrize("seed,heads,kv,side", LIVE_CASES)
+def test_restated_matches_reference_live(seed, heads, kv, side, golden_dir):
+    """Fresh seeds / GQA / left padding: the reference's own outputs on these inputs (stored; see tests/golden/make_ref_golden.py)."""
+    req = live_request(seed, heads, kv, side)
+    ids, labels, mask, images = req["input_ids"], req["labels"], req["attention_mask"], req["images"]
+    ref = torch.load(os.path.join(golden_dir, "ref_live_%s.pt" % live_key(seed, heads, kv, side)), weights_only=False)
     cc = R.ClipCfg(hidden=64, inter=128, layers=3, heads=4, image=32, patch=8)
     lc = R.LMCfg(hidden=64, inter=96, layers=1, heads=heads, kv_heads=kv, vocab=97, kd_vocab=97)
     sd = ref["state_dict"]

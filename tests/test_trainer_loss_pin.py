@@ -1,6 +1,6 @@
 """Pins the oracle's loss code (oracle/restated.py: get_p / get_logp / compute_align_loss / mimic_compute_loss, dpo_get_logp / dpo_loss /
 dpo_compute_loss) against outputs of the REFERENCE's own AlignTrainer / DPOTrainer method bodies, executed at golden-generation time on
-fake model outputs (tests/golden/make_loss_golden.py -> trainer_losses.pt).  fp32 CPU on both sides: exact up to summation order."""
+fake model outputs (tests/golden/make_loss_golden.py -> trainer_losses.<i>.pt).  fp32 CPU on both sides: exact up to summation order."""
 import math
 import os
 
@@ -8,11 +8,12 @@ import pytest
 import torch
 
 from oracle import restated as R
+from tests.golden import shards
 
 
 @pytest.fixture(scope="module")
 def gold(golden_dir):
-    return torch.load(os.path.join(golden_dir, "trainer_losses.pt"), weights_only=False)
+    return shards.load(golden_dir, "trainer_losses")
 
 
 def _close(a, b, what):
