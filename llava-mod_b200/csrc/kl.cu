@@ -808,7 +808,9 @@ static int kl_stream_launch_t(KlParams p, int cs, int64_t n_rows, cudaStream_t s
   if (max_clusters <= 0) {
     cudaError_t e = cudaOccupancyMaxActiveClusters(&max_clusters, kl_stream_kernel<P1, P2, KS_THREADS>, &cfg);
     if (e != cudaSuccess || max_clusters <= 0) { (void)cudaGetLastError(); max_clusters = lmod_num_sms() / cs; }
-    if (getenv("LMOD_KL_VERBOSE")) fprintf(stderr, "[lmod] kl_stream_kernel<%d,%d,%d>: cluster %d, %zu B smem, %d co-resident clusters\n", P1, P2, KS_THREADS, cs, smem, max_clusters);
+    if (getenv("LMOD_KL_VERBOSE"))
+      fprintf(stderr, "[lmod] kl_stream_kernel<%d,%d,%d>: cluster %d, %zu B smem, %d co-resident clusters, keep_tail %d\n", P1, P2, KS_THREADS, cs,
+              smem, max_clusters, p.keep_tail);
   }
   int64_t ncl = n_rows < max_clusters ? n_rows : max_clusters;
   cfg.gridDim = dim3((unsigned)(ncl * cs));
