@@ -244,7 +244,8 @@ int lmod_grouped_gemm_bf16(const void* A, int64_t lda, const void* B, int64_t ld
  * lse [batch, nh, seq] fp32 (natural-log LSE of the scaled scores, consumed by lmod_attn_bwd) or NULL.
  * Padded batches (the additive 4-D mask of modeling_qwen2.py:1035-1040; the varlen un-pad of :600-641): kv_lo / kv_hi are int32
  * [batch] device arrays giving the real key range [kv_lo[b], kv_hi[b]) of every batch row (right or left padding); a query row with
- * no visible key attends to all keys (HF _unmask_unattended).  Both NULL = no padding. */
+ * no visible key attends to all keys (HF _unmask_unattended).  Both NULL = no padding.  Padding needs causal = 1: a non-causal
+ * call with kv_lo / kv_hi is rejected (LMOD_ERR_ARG), since those un-masked rows are not what a key-padding mask would give. */
 int lmod_attn_fwd(const void* qkv, int64_t ld_qkv, int64_t batch, int64_t seq, int nh, int nkv, int hd, int causal,
                   float softmax_scale, void* out, int64_t ld_o, float* lse, const int32_t* kv_lo, const int32_t* kv_hi,
                   void* stream);

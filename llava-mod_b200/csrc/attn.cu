@@ -251,6 +251,9 @@ extern "C" int lmod_attn_fwd(const void* qkv, int64_t ld_qkv, int64_t batch, int
                              float softmax_scale, void* out, int64_t ld_o, float* lse, const int32_t* kv_lo, const int32_t* kv_hi,
                              void* stream) {
   LMOD_CHECK_ARG((kv_lo == nullptr) == (kv_hi == nullptr), "lmod_attn_fwd: kv_lo and kv_hi come together");
+  // The kernel un-masks every query row in front of kv_lo (no visible key under the causal mask).  Without the causal mask those rows
+  // would see [kv_lo, kv_hi) under a key-padding mask, so the combination would silently give a different answer: refuse it.
+  LMOD_CHECK_ARG(causal || kv_lo == nullptr, "lmod_attn_fwd: key padding (kv_lo / kv_hi) is only supported with causal = 1");
   LMOD_CHECK_ARG(qkv && out && batch > 0 && seq > 0 && nh > 0 && nkv > 0 && nh % nkv == 0, "lmod_attn_fwd: bad arguments");
   LMOD_CHECK_ARG(hd == 64 || hd == 128, "lmod_attn_fwd: head_dim %d not built (64 and 128 are)", hd);
   LMOD_CHECK_ARG(ld_qkv % 8 == 0 && ld_o % 8 == 0 && ((uintptr_t)qkv % 16 == 0) && ((uintptr_t)out % 16 == 0), "lmod_attn_fwd: alignment");

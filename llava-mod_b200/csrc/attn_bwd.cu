@@ -296,6 +296,7 @@ extern "C" int lmod_attn_bwd(const void* qkv, int64_t ld_qkv, const void* out, i
                              int64_t batch, int64_t seq, int nh, int nkv, int hd, int causal, float softmax_scale, void* dqkv, int64_t ld_dqkv,
                              float* dq32_ws, float* dsum_ws, const int32_t* kv_lo, const int32_t* kv_hi, void* stream) {
   LMOD_CHECK_ARG((kv_lo == nullptr) == (kv_hi == nullptr), "lmod_attn_bwd: kv_lo and kv_hi come together");
+  LMOD_CHECK_ARG(causal || kv_lo == nullptr, "lmod_attn_bwd: key padding (kv_lo / kv_hi) is only supported with causal = 1 (see lmod_attn_fwd)");
   LMOD_CHECK_ARG(qkv && out && dout && lse && dqkv && dq32_ws && dsum_ws && batch > 0 && seq > 0 && nh % nkv == 0, "lmod_attn_bwd: bad arguments");
   LMOD_CHECK_ARG(hd == 64 || hd == 128, "lmod_attn_bwd: head_dim %d not built (64 and 128 are)", hd);
   LMOD_CHECK_ARG(ld_qkv % 8 == 0 && ld_o % 8 == 0 && ld_do % 8 == 0 && ld_dqkv % 8 == 0, "lmod_attn_bwd: strides must be multiples of 8");

@@ -325,9 +325,18 @@ def gemm_residual(x, w, bias, res, inplace=False):
 ATTN_HEAD_DIMS = (64, 128)
 
 
+def _check_pad(causal, pad):
+    """The kernels un-mask the query rows in front of a left-padded sequence (they see no key under the causal mask) and give them
+    every key.  Without the causal mask a key-padding mask would restrict those rows to [kv_lo, kv_hi) instead, so padding is only
+    accepted together with causal=True (what the decoder passes); CLIP attends without padding."""
+    if pad is not None and pad[0] is not None and not causal:
+        raise _C.LmodError("attention: key padding (pad / kv_lo, kv_hi) is only supported with causal=True")
+
+
 def attention_fwd(qkv, B, T, nh, nkv, hd, causal, scale=None, need_lse=False, pad=None):
     """Hand-written wgmma flash-attention forward on the fused QKV buffer [B*T, (nh+2nkv)*hd] -> [B*T, nh*hd] (+ lse [B,nh,T]).
-    pad = (kv_lo, kv_hi): int32 [B] device tensors, the real key range of every batch row (padded batches), or None."""
+    pad = (kv_lo, kv_hi): int32 [B] device tensors, the real key range of every batch row (padded batches), or None; needs causal."""
+    _check_pad(causal, pad)
     _need_cuda(qkv)
     out = torch.empty(B * T, nh * hd, dtype=qkv.dtype, device=qkv.device)
     lse = torch.empty(B, nh, T, dtype=torch.float32, device=qkv.device) if need_lse else None
@@ -360,6 +369,7 @@ class AttnFn(Function):
 
 def attention_bwd(qkv, out, dout, lse, B, T, nh, nkv, hd, causal, scale, pad=None):
     """Hand-written wgmma flash-attention backward -> fused dqkv (same layout as qkv)."""
+    _check_pad(causal, pad)
     dqkv = torch.empty_like(qkv)
     dq32 = torch.empty(B * T, nh * hd, dtype=torch.float32, device=qkv.device)
     dsum = torch.empty(B, nh, T, dtype=torch.float32, device=qkv.device)
@@ -375,6 +385,7 @@ def attention(qkv, B, T, nh, nkv, hd, causal=True, scale=None, pad=None):
     q/k columns add 0 to every score and the extra v columns produce output columns that are sliced away (softmax scale = hd^-0.5 of
     the TRUE head dim); the pad / slice are plain tensor ops, so autograd carries the gradient back to the unpadded buffer."""
     scale = float(scale if scale is not None else hd ** -0.5)
+    _check_pad(causal, pad)
     if hd not in ATTN_HEAD_DIMS:
         hp = 64 if hd < 64 else 128
         if hd > 128:

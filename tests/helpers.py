@@ -197,6 +197,184 @@ def check_out4(out4, ref, msg="out4"):
         assert abs(o[j].item() - ref[key]) <= 2e-5 * abs(ref[key]) + 1e-6, (msg, key, o[j].item(), ref[key])
 
 
+# ---------------------------------------------------------------------------------------------------
+# flash attention (csrc/attn.cu, csrc/attn_bwd.cu): float64 reference and element-wise bounds
+# ---------------------------------------------------------------------------------------------------
+def attn_visible(B, T, causal, keep=None, device="cpu"):
+    """[B, T, T] bool: may query row i see key j.  The semantics of R.sdpa_mask: the causal mask plus key padding (keep [B, T] bool,
+    contiguous real tokens), and a row with no visible key (in front of a left-padded sequence, or a sample that is all padding) sees every
+    key.  Key padding goes with causal=True only, as in the kernels."""
+    assert causal or keep is None, "key padding is only defined together with the causal mask"
+    vis = torch.ones(T, T, dtype=torch.bool, device=device)
+    if causal:
+        vis = vis.tril()
+    vis = vis[None].expand(B, T, T)
+    if keep is not None:
+        vis = vis & keep.to(device=device, dtype=torch.bool)[:, None, :]
+    return vis | ~vis.any(-1, keepdim=True)
+
+
+# Element-wise bounds of the kernels against attn_reference_fp64, from the kernels' own arithmetic.  u = 2^-8 is the unit roundoff of bf16,
+# 2^-24 that of fp32.  Per query row i (natural-log units, s_ij = q_i.k_j the raw dot product, c = scale):
+#   A_i     = max_j sum_d |q_id k_jd| over the visible keys, Smax_i = max_j |s_ij|.
+#   delta_i bounds the relative error of every fp32 P_ij = ex2(fma(s_ij, c log2e, -m)) the kernels form:
+#             c (hd/16 + 1) 2^-23 A_i   the fp32 score from wgmma, which truncates its accumulator at each k = 16 step (hd/16 steps, +1 for
+#                                       the alignment inside a step);
+#             2^-22 c Smax_i            the fp32 constant c log2e (2^-23 relative) and the rounding of the fma residual (|.| <= 2 c Smax log2e);
+#             2^-22                     ex2.approx.
+#   gamma_i = (n_i/4 + 2 nblk_i + 4) 2^-24, the fp32 sum l (each of the 4 threads of a row adds n/4 terms in order, one fma per key block,
+#             then two shuffles) and the rescales of o and l by alpha once per key block; n_i visible keys, nblk_i <= n_i/BKV + 2 blocks.
+#   o:   |o_k - o| <= 2^-8 |o| + (2^-8 + (n_i/16 + 2) 2^-23 + 2 delta_i + gamma_i) (P|V|)_i
+#             2^-8 |o| is the bf16 store.  P is rounded to bf16 before P V (2^-8) while l sums the unrounded P; the fp32 accumulator of P V
+#             truncates at each of the (n_i/16 + 2) k = 16 steps that hold a visible key; o/l carries delta_i from the numerator and from the
+#             denominator, and gamma_i from l.  P|V| = sum_j p_ij |v_j| majorises every one of these sums.
+#   lse: |lse_k - lse| <= delta_i + gamma_i + 2^-22 (2 + log2 n_i + |lse_i|)
+#             the shift m cancels between m and the P it scales; lg2.approx (2^-22 absolute per unit of log2 l) and the fp32 roundings of
+#             m + lg2(l) and of the product by ln2.
+# Backward (P recomputed as ex2(fma(s, c log2e, -lse_k log2e)) from the forward's fp32 lse_k):
+#   deltab_i = the score and ex2 terms of delta_i + 2^-22 |lse_i| (lse_k log2e rounded, the fma residual) + |lse_k,i - lse_i|.
+#   dP_ij = dO_i.V_j in fp32 wgmma: error (hd/16 + 1) 2^-23 (|dO_i|.|V_j|).  D_i from attn_dsum_kernel is rowsum(dO_i o_k,i) of the
+#   forward's bf16 output: its difference from the exact rowsum(dO_i O_i) is dD_i = rowsum(dO_i (o_k,i - O_i)), computed exactly here, plus
+#   the fp32 sum (hd/32 fmas per lane, then five shuffles): (hd/32 + 6) 2^-24 sum |dO_i o_k,i|.
+#   dS = P (dP - D) c goes to bf16 before both of its products, so every dS_ij is off by at most c E_ij with
+#     E_ij = P_ij ((2^-8 + deltab_i + 2^-22) |dP_ij - D_i| + (1 + 2^-7) (err(dP_ij) + |dD_i| + err(D_i))),   F_ij = P_ij |dP_ij - D_i|.
+#   The bf16 rounding of dS acts on the kernel's dS, which already carries the dP and D errors: in a peaked row dP - D nearly cancels
+#   and those errors can be most of dS, so they are counted (1 + 2^-8)(1 + deltab) <= 1 + 2^-7 times.
+#   dV: |dV_k - dV| <= 2^-8 |dV| + (2^-8 + (n_kv + 1) 2^-23) (P^T |dO|) + (P^T (deltab |dO|))
+#   dK: |dK_k - dK| <= 2^-8 |dK| + c (E^T |Q|) + c (n_kv + 1) 2^-23 (F^T |Q|)
+#             n_kv = group (T/16 + 1) bounds the k = 16 steps of the register accumulators of dK and dV over every query of every head of the
+#             GQA group (the heads' terms are summed here in float64 too).
+#   dQ: |dQ_k - dQ| <= 2^-8 |dQ| + c (E |K|) + c (9 2^-23 + n_kb 2^-24) (F |K|)
+#             each 128-key block adds its partial dS K (8 wgmma k-steps) with an fp32 red.add; n_kb = T/128 + 1 adds in any order.
+#   Every bound also gets ATTN_ABS_FLOOR: ex2.approx.ftz flushes P below 2^-126 to zero, which moves no sum by more than T 2^-126 max|v|.
+ATTN_ABS_FLOOR = 2.0 ** -100
+
+
+def attn_reference_fp64(qkv, B, T, nh, nkv, hd, causal, scale, keep=None, dout=None, out_kernel=None, lse_kernel=None,
+                        block_bytes=3 << 29):
+    """Plain float64 attention on the fused bf16 QKV buffer [B*T, (nh + 2 nkv) hd] (q heads | k heads | v heads, GQA by index: query head h
+    reads kv head h // (nh / nkv)), under the mask of attn_visible.  Runs on qkv's device in blocks of heads, so that the float64 [T, T]
+    temporaries of one block stay near `block_bytes`.
+
+    Returns a dict: o [B*T, nh*hd] and lse [B, nh, T] (float64, the kernel's layouts) with their bounds o_tol and lse_tol, and the majorants
+    behind them (PV = P|V|, delta, nvis per row).  With dout [B*T, nh*hd], also dqkv [B*T, (nh + 2 nkv) hd] from the analytic gradients
+    (P, dP = dO V^T, D = rowsum(dO O), dS = P (dP - D)) and its bound dqkv_tol.  out_kernel / lse_kernel, the forward kernel's outputs that
+    the backward kernel consumes, make the dD and lse terms of the gradient bounds exact; without them the forward bounds stand in."""
+    dev = qkv.device
+    f64 = torch.float64
+    x = qkv.detach().to(f64).view(B, T, nh + 2 * nkv, hd)
+    q, k, v = (x[:, :, a:b].permute(0, 2, 1, 3) for a, b in ((0, nh), (nh, nh + nkv), (nh + nkv, nh + 2 * nkv)))
+    vis = attn_visible(B, T, causal, keep, dev)
+    nvis = vis.sum(-1).to(f64)                                       # [B, T]
+    group = nh // nkv
+    bkv = 128 if hd <= 64 else 64
+    u, e23, e22, e24 = 2.0 ** -8, 2.0 ** -23, 2.0 ** -22, 2.0 ** -24
+    o = torch.zeros(B, nh, T, hd, dtype=f64, device=dev)
+    o_tol, PVall = torch.zeros_like(o), torch.zeros_like(o)
+    lse = torch.zeros(B, nh, T, dtype=f64, device=dev)
+    lse_tol, delta_all = torch.zeros_like(lse), torch.zeros_like(lse)
+    grads = dout is not None
+    if grads:
+        do = dout.detach().to(dev, f64).view(B, T, nh, hd).permute(0, 2, 1, 3)
+        ok = None if out_kernel is None else out_kernel.detach().to(dev, f64).view(B, T, nh, hd).permute(0, 2, 1, 3)
+        lk = None if lse_kernel is None else lse_kernel.detach().to(dev, f64)
+        dq, dq_tol = torch.zeros_like(o), torch.zeros_like(o)
+        dk = torch.zeros(B, nkv, T, hd, dtype=f64, device=dev)
+        dv, dk_tol, dv_tol = torch.zeros_like(dk), torch.zeros_like(dk), torch.zeros_like(dk)
+        n_kv = group * (T / 16 + 1)
+        n_kb = T / 128 + 1
+    hb = max(1, min(nh, block_bytes // (12 * 8 * T * T)))
+    ninf = float("-inf")
+    for b in range(B):
+        visb, nv = vis[b], nvis[b][:, None]                          # [T, T], [T, 1]
+        for h0 in range(0, nh, hb):
+            h1 = min(nh, h0 + hb)
+            kvi = torch.arange(h0, h1, device=dev) // group
+            qb, kb, vb = q[b, h0:h1], k[b][kvi], v[b][kvi]           # [h, T, hd]
+            s = (qb @ kb.transpose(-1, -2)).masked_fill(~visb, ninf)
+            lse_b = torch.logsumexp(s * scale, -1)                   # [h, T]
+            P = torch.exp(s * scale - lse_b[..., None])
+            ob = P @ vb
+            A = (qb.abs() @ kb.abs().transpose(-1, -2)).masked_fill(~visb, 0).amax(-1)
+            Smax = s.abs().masked_fill(~visb, 0).amax(-1)
+            d_score = scale * ((hd / 16 + 1) * e23 * A + e22 * Smax)
+            delta = d_score + e22
+            gamma = (nv[:, 0] / 4 + 2 * (nv[:, 0] / bkv + 2) + 4) * e24
+            PV = P @ vb.abs()
+            o[b, h0:h1], lse[b, h0:h1], PVall[b, h0:h1], delta_all[b, h0:h1] = ob, lse_b, PV, delta
+            o_tol[b, h0:h1] = u * ob.abs() + (u + (nv / 16 + 2) * e23 + 2 * delta[..., None] + gamma[..., None]) * PV + ATTN_ABS_FLOOR
+            lse_t = delta + gamma + e22 * (2 + torch.log2(nv[:, 0]) + lse_b.abs()) + ATTN_ABS_FLOOR
+            lse_tol[b, h0:h1] = lse_t
+            if not grads:
+                continue
+            dob = do[b, h0:h1]
+            okb = ob if ok is None else ok[b, h0:h1]
+            lerr = lse_t if lk is None else (lk[b, h0:h1] - lse_b).abs()
+            deltab = d_score + e22 * (1 + lse_b.abs()) + lerr        # [h, T]
+            dP = dob @ vb.transpose(-1, -2)
+            D = (dob * ob).sum(-1)
+            if ok is None:
+                dD = (dob.abs() * o_tol[b, h0:h1]).sum(-1)
+            else:
+                dD = (dob * (okb - ob)).sum(-1).abs()
+            eD = (hd / 32 + 6) * e24 * (dob.abs() * okb.abs()).sum(-1)
+            edP = (hd / 16 + 1) * e23 * (dob.abs() @ vb.abs().transpose(-1, -2))
+            R = dP - D[..., None]
+            dS = P * R
+            F = P * R.abs()
+            E = (u + deltab[..., None] + e22) * F + (1 + 2.0 ** -7) * P * (edP + (dD + eD)[..., None])
+            del s, dP, R, edP
+            qa, ka = qb.abs(), kb.abs()
+            dq[b, h0:h1] = scale * (dS @ kb)
+            dq_tol[b, h0:h1] = scale * (E @ ka + (9 * e23 + n_kb * e24) * (F @ ka))
+            Pt = P.transpose(-1, -2)
+            dk[b].index_add_(0, kvi, scale * (dS.transpose(-1, -2) @ qb))
+            dv[b].index_add_(0, kvi, Pt @ dob)
+            dk_tol[b].index_add_(0, kvi, scale * (E.transpose(-1, -2) @ qa + (n_kv + 1) * e23 * (F.transpose(-1, -2) @ qa)))
+            dv_tol[b].index_add_(0, kvi, (u + (n_kv + 1) * e23) * (Pt @ dob.abs()) + Pt @ (deltab[..., None] * dob.abs()))
+            del P, Pt, dS, F, E
+    rows = lambda t: t.permute(0, 2, 1, 3).reshape(B * T, -1)       # noqa: E731  [B, H, T, hd] -> [B*T, H*hd]
+    res = dict(o=rows(o), lse=lse, o_tol=rows(o_tol), lse_tol=lse_tol, PV=rows(PVall), delta=delta_all, nvis=nvis)
+    if grads:
+        res["dqkv"] = torch.cat([rows(dq), rows(dk), rows(dv)], 1)
+        res["dqkv_tol"] = torch.cat([rows(dq_tol + u * dq.abs()), rows(dk_tol + u * dk.abs()), rows(dv_tol + u * dv.abs())], 1) + ATTN_ABS_FLOOR
+    return res
+
+
+def check_attn(name, got, want, tol, T, hd=None, report=None):
+    """Element-wise |got - want| <= tol.  got / want / tol in the kernel's layouts: [B*T, H*hd] (row b*T + t, column h*hd + d; pass hd) or
+    lse [B, H, T].  On failure names the worst element by (sample, head, row, column), the count out of bound and max(err / bound).
+    Returns max(err / bound); `report`, a dict, collects it under `name`."""
+    got = got.detach().to(want.device, torch.float64)
+    err = (got - want).abs()
+    ratio = (err / tol).nan_to_num(float("inf"))                    # a NaN in got counts as out of bound
+    bad = ~(err <= tol)
+    worst = float(ratio.max()) if ratio.numel() else 0.0
+    if report is not None:
+        report[name] = max(worst, report.get(name, 0.0))
+    nbad = int(bad.sum())
+    if nbad:
+        i = int(ratio.reshape(-1).argmax())
+        if got.dim() == 3:
+            H = got.shape[1]
+            where = dict(sample=i // (H * T), head=(i // T) % H, row=i % T, column=None)
+        else:
+            r, c = divmod(i, got.shape[1])
+            where = dict(sample=r // T, head=c // hd, row=r % T, column=c % hd)
+        g, w, t = got.reshape(-1)[i].item(), want.reshape(-1)[i].item(), tol.reshape(-1)[i].item()
+        raise AssertionError(f"{name}: {nbad} / {got.numel()} elements out of bound, max err/bound {worst:.3g}; worst at {where}: "
+                             f"got {g!r} want {w!r} bound {t:.3g}")
+    return worst
+
+
+def check_attn_grads(name, dqkv, ref, T, nh, nkv, hd, report=None):
+    """dq, dk and dv of a fused gradient buffer against attn_reference_fp64(..., dout=...)."""
+    out = {}
+    for part, sl in (("dq", slice(0, nh * hd)), ("dk", slice(nh * hd, (nh + nkv) * hd)), ("dv", slice((nh + nkv) * hd, None))):
+        out[part] = check_attn(f"{name} {part}", dqkv[:, sl], ref["dqkv"][:, sl], ref["dqkv_tol"][:, sl], T, hd, report)
+    return out
+
+
 def make_trainer(student, teacher, loss_type="kd_lm", accum=1, lr=2e-5, max_steps=100, kind="align", moe_loss_enable=True):
     from llavamod.config.args import TrainingArguments
     from llavamod.train.align_trainer import AlignTrainer
