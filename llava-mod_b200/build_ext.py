@@ -16,7 +16,14 @@ OUT = os.path.join(HERE, "llavamod", "liblmod_b200.so")
 OBJ = os.path.join(HERE, "build")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
-         "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-diag-suppress", "177"]
+         "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-diag-suppress", "177", "-Xptxas", "-v"]
+# ptxas messages that mean it serialized the wgmma pipeline of a kernel (every MMA waited on before the next issues): a function call
+# in the kernel (C7510) or accumulator registers read on a path without a wgmma.wait_group (C7517).  A build that has one fails.
+WGMMA_SERIALIZED = ("C7510", "C7517", "wgmma.mma_async instructions are serialized", "warpgroup.wait is injected")
+
+
+def wgmma_serialization_messages(ptxas_output):
+    return [ln for ln in ptxas_output.splitlines() if any(m in ln for m in WGMMA_SERIALIZED)]
 
 
 def sources():
@@ -42,10 +49,15 @@ def build(force=False, verbose=False):
 
     def cc(f):
         o = os.path.join(OBJ, f[:-3] + ".o")
-        cmd = [NVCC] + FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-c", os.path.join(CSRC, f), "-o", o]
+        cmd = [NVCC] + FLAGS + ["-c", os.path.join(CSRC, f), "-o", o]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError("nvcc failed for %s:\n%s\n%s" % (f, r.stdout, r.stderr))
+        bad = wgmma_serialization_messages(r.stdout + r.stderr)
+        if bad:
+            os.remove(o)
+            raise RuntimeError("ptxas serialized the wgmma pipeline in %s (keep calls such as printf out of wgmma kernels, and wait on "
+                               "every path before reading an accumulator):\n%s" % (f, "\n".join(bad)))
         if verbose:
             sys.stderr.write(r.stderr)
         return o

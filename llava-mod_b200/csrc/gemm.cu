@@ -267,10 +267,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_consta
       if (++stage == STAGES) { stage = 0; phase ^= 1; }
     }
     const bool empty_k = t.kb1 <= t.kb0;                   // grouped wgrad of an expert with no rows / empty dynamic reduction: zero
-    if (!empty_k) {
-      wgmma_wait<0>();
-      if (wg_leader) mbar_arrive(&empty_bar[prev]);
-    }
+    wgmma_wait<0>();                                       // on every path: a conditional wait makes ptxas drain after each MMA (C7517)
+    if (!empty_k && wg_leader) mbar_arrive(&empty_bar[prev]);
     reg_fence<BN / 2>(acc);
 
     // accumulator fragment: register 4i + 2h + e holds row 16w + lane/4 + 8h, column 8i + 2(lane%4) + e of this warpgroup's 64 x BN block

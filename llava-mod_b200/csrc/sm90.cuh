@@ -8,7 +8,8 @@ namespace {
 
 // ---------------------------------------------------------------------------------------------------------------------------------
 // try_wait with a suspend-time hint: the thread sleeps in hardware until the phase completes (or ~20 us pass) instead of spinning through
-// issue slots the math warps need; the spin bound (~2.6 s) turns a protocol bug into a trap instead of a hung GPU
+// issue slots the math warps need; the spin bound (~2.6 s) turns a protocol bug into a trap instead of a hung GPU.
+// No printf (or any other call) here: a call anywhere in a wgmma kernel makes ptxas serialize every MMA in it (C7510).
 __device__ __forceinline__ bool mbar_try_wait_hint(uint64_t* bar, uint32_t phase) {
   uint32_t ok;
   asm volatile(
@@ -22,7 +23,7 @@ __device__ __forceinline__ void mbar_wait_bounded(uint64_t* bar, uint32_t phase)
   if (mbar_try_wait(bar, phase)) return;
   uint32_t spins = 0;
   while (!mbar_try_wait_hint(bar, phase)) {
-    if (++spins > (1u << 17)) { printf("lmod wgmma kernel: mbarrier timeout (block %d thread %d)\n", blockIdx.x, threadIdx.x); __trap(); }
+    if (++spins > (1u << 17)) __trap();
   }
 }
 __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {

@@ -135,11 +135,12 @@ def gemm(a, b, a_mn=False, b_mn=False, bias=None, out=None, accumulate=False, ou
 # Epilogue fusions pay off only when the GEMM's main loop is long enough to hide them: the fused SwiGLU forward is used from a reduction
 # length of FUSE_MIN_K on (the teacher's K = 4096); at the student's K = 1024 the element-wise kernels, which use every warp of the SM,
 # are preferred.  The (lighter) RoPE epilogue of the q|k|v projection is always fused.  LLAVAMOD_FUSE_SWIGLU: "auto" (by
-# reduction length), "1" always, "0" never; LLAVAMOD_FUSE_ROPE: "0" = GEMM + lmod_rope.
+# reduction length), "1" always, "0" never; LLAVAMOD_FUSE_ROPE: "0" = GEMM + lmod_rope.  Measured again with asynchronous MMAs
+# (DESIGN.md section 4): "1" is within the step's run-to-run spread of "auto".
 FUSE_SWIGLU = _os.environ.get("LLAVAMOD_FUSE_SWIGLU", "auto")
 FUSE_ROPE = _os.environ.get("LLAVAMOD_FUSE_ROPE", "auto")
 # residual add in the o_proj / down_proj (CLIP: out_proj / fc2) epilogue of no-grad forwards.  Bit-identical to the add inside the next norm's
-# kernel; opt-in (the add is cheap inside the norm kernel, and the epilogue of a long GEMM has little slack)
+# kernel; opt-in: the add is cheap inside the norm kernel, and the fused form measures within the step's spread (DESIGN.md section 4)
 FUSE_RESIDUAL = _os.environ.get("LLAVAMOD_FUSE_RESIDUAL", "0")
 FUSE_MIN_K = 2048
 
