@@ -112,9 +112,9 @@ int lmod_align_loss_dense(const float* logp, const float* probs, int64_t ld, con
  * multiple of 128 rows (what lmod_grouped_gemm_bf16 wants).  The padding rows of xp (alignment / unused capacity) are zeroed by the
  * op itself, so xp needs no initialisation; rows past offsets[E] are not touched.
  * meta = {l_aux, capacity, rows_used, rows_end(=offsets[E]), exp_counts[E]}. */
-int lmod_moe_capacity(int64_t S, int E, float capacity_factor, int64_t min_capacity);
+int lmod_moe_capacity(int64_t S, int E, double capacity_factor, int64_t min_capacity);
 int lmod_moe_route_scatter(const void* x, const float* wg, const float* noise, int64_t S, int64_t H,
-                           int E, float capacity_factor, int64_t min_capacity, int layout,
+                           int E, double capacity_factor, int64_t min_capacity, int layout,
                            float* logits, float* gates, int32_t* idx, int32_t* row, float* w,
                            int32_t* offsets, float* meta, void* xp, int32_t* ws, void* stream);
 int64_t lmod_moe_route_ws_elems(int64_t S, int E);

@@ -89,12 +89,20 @@ __global__ void __launch_bounds__(RT_THREADS) moe_gate_kernel(const RouteParams 
     if (lane == 0 || (lane == 1 && has1)) {          // lane 0 finishes token t0, lane 1 token t0+1
       const int tok = t0 + lane;
       float mx = -INFINITY;
-      int i1 = 0;
 #pragma unroll
-      for (int e = 0; e < MAXE; ++e) if (e < E && acc0[e] > mx) { mx = acc0[e]; i1 = e; }   // first max wins ties
-      float ex[MAXE], den = 0.f;
+      for (int e = 0; e < MAXE; ++e) if (e < E) mx = fmaxf(mx, acc0[e]);
+      float ex[MAXE], g[MAXE], den = 0.f;
 #pragma unroll
       for (int e = 0; e < MAXE; ++e) { ex[e] = (e < E) ? expf(acc0[e] - mx) : 0.f; den += ex[e]; }
+      // top2gating takes argmax(softmax(logits)): the first choice is the first maximal GATE.  Logits closer than exp can resolve
+      // (about 2^-25 apart) give equal gates, and then the lower expert wins even if its logit is the smaller one.
+      int i1 = 0;
+      float gmx = -1.f;
+#pragma unroll
+      for (int e = 0; e < MAXE; ++e) {
+        g[e] = ex[e] / den;
+        if (e < E && g[e] > gmx) { gmx = g[e]; i1 = e; }
+      }
       float best = -INFINITY;
       int i2 = (i1 == 0) ? 1 : 0;
 #pragma unroll
@@ -106,9 +114,8 @@ __global__ void __launch_bounds__(RT_THREADS) moe_gate_kernel(const RouteParams 
       }
 #pragma unroll
       for (int e = 0; e < MAXE; ++e) {
-        const float g = ex[e] / den;
-        if (e < E) { p.logits[(size_t)tok * E + e] = acc0[e]; p.gates[(size_t)tok * E + e] = g; }
-        s_gates[(tok - b0) * MAXE + e] = (e < E) ? g : 0.f;
+        if (e < E) { p.logits[(size_t)tok * E + e] = acc0[e]; p.gates[(size_t)tok * E + e] = g[e]; }
+        s_gates[(tok - b0) * MAXE + e] = (e < E) ? g[e] : 0.f;
       }
       p.idx[2 * tok] = i1; p.idx[2 * tok + 1] = i2;
       atomicAdd(&s_cnt[i1], 1);
@@ -439,9 +446,10 @@ __global__ void moe_wg_grad_reduce_kernel(const float* __restrict__ ws, int H, i
 
 }  // namespace
 
-extern "C" int lmod_moe_capacity(int64_t S, int E, float capacity_factor, int64_t min_capacity) {
-  // deepspeed _capacity: ceil(S/E * (cf*2)) ; computed in double like Python, raised to min_capacity
-  double c = ceil(((double)S / (double)E) * ((double)capacity_factor * 2.0));
+extern "C" int lmod_moe_capacity(int64_t S, int E, double capacity_factor, int64_t min_capacity) {
+  // deepspeed _capacity: ceil(S/E * (cf*2)) ; computed in double like Python, raised to min_capacity.  The factor is taken as a double:
+  // a user-set factor such as 0.3 rounded to float first moves the product across an integer (S=320, E=4: C=49 instead of 48).
+  double c = ceil(((double)S / (double)E) * (capacity_factor * 2.0));
   int64_t ci = (int64_t)c;
   if (ci < min_capacity) ci = min_capacity;
   return (int)ci;
@@ -462,7 +470,7 @@ extern "C" int64_t lmod_moe_route_ws_elems(int64_t S, int E) {
 }
 
 extern "C" int lmod_moe_route_scatter(const void* x, const float* wg, const float* noise, int64_t S, int64_t H, int E,
-                                      float capacity_factor, int64_t min_capacity, int layout, float* logits, float* gates,
+                                      double capacity_factor, int64_t min_capacity, int layout, float* logits, float* gates,
                                       int32_t* idx, int32_t* row, float* w, int32_t* offsets, float* meta, void* xp,
                                       int32_t* ws, void* stream) {
   LMOD_CHECK_ARG(x && wg && noise && logits && gates && idx && row && w && offsets && meta && xp && ws,

@@ -14,10 +14,10 @@ LIB_PATH = os.path.join(_HERE, "liblmod_b200.so")
 
 _lib = None
 
-c_void_p, c_int, c_int64, c_float = ctypes.c_void_p, ctypes.c_int, ctypes.c_int64, ctypes.c_float
+c_void_p, c_int, c_int64, c_float, c_double = ctypes.c_void_p, ctypes.c_int, ctypes.c_int64, ctypes.c_float, ctypes.c_double
 
 # name -> argtypes (all return int unless listed in _RESTYPES)
-_P, _I, _L, _F = c_void_p, c_int, c_int64, c_float
+_P, _I, _L, _F, _D = c_void_p, c_int, c_int64, c_float, c_double
 SIGNATURES = {
     "lmod_kl_counts": [_P, _L, _L, _I, _P, _P],
     "lmod_kl_fwd_bwd": [_P, _L, _P, _L, _P, _L, _L, _L, _I, _F, _F, _P, _P, _P, _L, _P],
@@ -30,9 +30,9 @@ SIGNATURES = {
     "lmod_logp_gather_bwd": [_P, _L, _P, _L, _L, _L, _P, _P, _I, _P, _L, _P],
     "lmod_softmax_rows": [_P, _L, _L, _L, _I, _P, _L, _P],
     "lmod_align_loss_dense": [_P, _P, _L, _P, _L, _L, _I, _P, _P, _P],
-    "lmod_moe_capacity": [_L, _I, _F, _L],
+    "lmod_moe_capacity": [_L, _I, _D, _L],
     "lmod_moe_route_ws_elems": [_L, _I],
-    "lmod_moe_route_scatter": [_P, _P, _P, _L, _L, _I, _F, _L, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P],
+    "lmod_moe_route_scatter": [_P, _P, _P, _L, _L, _I, _D, _L, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P],
     "lmod_moe_gather_combine": [_P, _P, _P, _P, _L, _L, _P, _P],
     "lmod_moe_combine_bwd": [_P, _P, _P, _P, _L, _L, _P, _P, _P],
     "lmod_moe_gate_bwd": [_P, _P, _P, _P, _P, _P, _L, _I, _P, _P],

@@ -692,6 +692,7 @@ def splice_embed(feats, embed_w, src, img_index, n_patches, embed_grad=None):
 # MoE layer (DeepSpeed 0.9.5 MoE; call site llava_qwen1_5_moe.py:536-546, SURVEY.md Appendix A)
 # ---------------------------------------------------------------------------------------------------
 def moe_capacity(S, E, capacity_factor, min_capacity):
+    """DeepSpeed's _capacity, ceil(S/E * cf * 2) raised to min_capacity, with cf as the Python double the user set."""
     return int(_C.lib().lmod_moe_capacity(S, E, float(capacity_factor), int(min_capacity)))
 
 
@@ -732,6 +733,66 @@ def moe_gather_combine(y, row, w, residual=None):
     return out
 
 
+def moe_forward_stages(x, res, wg, w_gu, w_dn, noise, cf, min_cap, fused):
+    """The MoE forward as MoEFn runs it, returning every intermediate (the router's record, xp, h1, act, y, out).  fused: SwiGLU in the
+    grouped GEMM's epilogue instead of GEMM + silu_mul (bit-identical)."""
+    E, I2, H = w_gu.shape
+    r = moe_route_scatter(x, wg, noise, cf, min_cap, LAYOUT_ALIGNED)
+    R = r["max_rows"]
+    xp, offs = r["xp"], r["offsets"]
+    # only xp (and dy in the backward) are zero-filled: in the 128-aligned layout the grouped GEMM writes EVERY row below offsets[E],
+    # so the padding rows of h1 / act / y come out as exact zeros (0 @ W); rows past offsets[E] are never read by a GEMM
+    if fused:
+        act, h1 = grouped_gemm_swiglu(xp, w_gu, offs, R, True)         # act [R,I], pre-activations [R,2I]: SwiGLU in the GEMM epilogue
+    else:
+        h1 = torch.empty(R, I2, dtype=x.dtype, device=x.device)
+        grouped_gemm(xp, w_gu, h1, offs, 0)                            # [R,2I] = xp @ w_gu[e]^T
+        act = silu_mul(h1)                                             # [R,I]
+    y = torch.empty(R, H, dtype=x.dtype, device=x.device)
+    grouped_gemm(act, w_dn, y, offs, 0)                                # [R,H] = act @ w_dn[e]^T
+    r.update(h1=h1, act=act, y=y, out=moe_gather_combine(y, r["row"], r["w"], res), fused=fused)
+    return r
+
+
+def moe_backward_stages(st, x, wg, w_gu, w_dn, dout, dlaux, grads):
+    """The MoE backward as MoEFn runs it, from moe_forward_stages' record; returns every intermediate (dy, dw, dact on the unfused
+    path, dh1, dxp, dlogits, dx).  Weight gradients accumulate in place into grads['wg'|'w_gu'|'w_dn'] (None or a missing key = frozen)."""
+    E, I2, H = w_gu.shape
+    xp, h1, act, y, row, w, gates, idx, meta, offs = (st[k] for k in ("xp", "h1", "act", "y", "row", "w", "gates", "idx", "meta", "offsets"))
+    R = xp.shape[0]
+    S = x.shape[0]
+    dy = torch.zeros(R, H, dtype=dout.dtype, device=dout.device)
+    dw = torch.empty(S, 2, dtype=torch.float32, device=dout.device)
+    call("lmod_moe_combine_bwd", ptr(dout), ptr(y), ptr(row), ptr(w), S, H, ptr(dy), ptr(dw))
+    g = grads
+    out = dict(dy=dy, dw=dw, dact=None)
+    if st["fused"]:
+        dh1 = grouped_gemm_silu_bwd(dy, w_dn, h1, offs, R)             # d(gate)|d(up) straight from the dgrad GEMM's epilogue
+    else:
+        dact = torch.empty(R, I2 // 2, dtype=dout.dtype, device=dout.device)
+        grouped_gemm(dy, w_dn, dact, offs, 1)                          # dact = dy @ w_dn[e]
+        dh1 = silu_mul_bwd(dact, h1)
+        out["dact"] = dact
+    if g is not None and g.get("w_dn") is not None:
+        grouped_gemm(dy, act, g["w_dn"], offs, 2, accumulate=True)      # dW_dn[e] += dy_e^T @ act_e
+    dxp = torch.empty(R, H, dtype=dout.dtype, device=dout.device)
+    grouped_gemm(dh1, w_gu, dxp, offs, 1)                              # dxp = dh1 @ w_gu[e]
+    if g is not None and g.get("w_gu") is not None:
+        grouped_gemm(dh1, xp, g["w_gu"], offs, 2, accumulate=True)      # dW_gu[e] += dh1_e^T @ xp_e
+    dlogits = torch.empty(S, E, dtype=torch.float32, device=dout.device)
+    gl = None
+    if dlaux is not None:
+        gl = dlaux.to(torch.float32).reshape(1).contiguous()
+    call("lmod_moe_gate_bwd", ptr(gates), ptr(idx), ptr(row), ptr(dw), ptr(meta), ptr(gl) if gl is not None else None, S, E, ptr(dlogits))
+    dx = torch.empty_like(x)
+    call("lmod_moe_scatter_bwd", ptr(dxp), ptr(row), ptr(dlogits), ptr(wg), None, S, H, E, ptr(dx))
+    if g is not None and g.get("wg") is not None:
+        ws = torch.empty(32, E, H, dtype=torch.float32, device=dout.device)
+        call("lmod_moe_wg_grad", ptr(x), ptr(dlogits), S, H, E, ptr(ws), ptr(g["wg"]))
+    out.update(dh1=dh1, dxp=dxp, dlogits=dlogits, dx=dx)
+    return out
+
+
 class MoEFn(Function):
     """x: post-attention-layernorm hidden [S,H]; res: residual stream [S,H].  Experts are SwiGLU MLPs with fused gate|up weights
     w_gu [E,2I,H] and w_dn [E,H,I].  Expert GEMMs run as ONE grouped wgmma GEMM each over COMPACT expert rows (no capacity
@@ -742,59 +803,21 @@ class MoEFn(Function):
         x = _c(x)
         res = _c(res)
         E, I2, H = w_gu.shape
-        r = moe_route_scatter(x, wg, noise, cf, min_cap, LAYOUT_ALIGNED)
-        R = r["max_rows"]
-        xp, offs = r["xp"], r["offsets"]
-        # only xp (and dy in the backward) are zero-filled: in the 128-aligned layout the grouped GEMM writes EVERY row below offsets[E],
-        # so the padding rows of h1 / act / y come out as exact zeros (0 @ W); rows past offsets[E] are never read by a GEMM
-        ctx.fused = swiglu_fusable(I2 // 2, H, training=True)
-        if ctx.fused:
-            act, h1 = grouped_gemm_swiglu(xp, w_gu, offs, R, True)     # act [R,I], pre-activations [R,2I]: SwiGLU in the GEMM epilogue
-        else:
-            h1 = torch.empty(R, I2, dtype=x.dtype, device=x.device)
-            grouped_gemm(xp, w_gu, h1, offs, 0)                        # [R,2I] = xp @ w_gu[e]^T
-            act = silu_mul(h1)                                         # [R,I]
-        y = torch.empty(R, H, dtype=x.dtype, device=x.device)
-        grouped_gemm(act, w_dn, y, offs, 0)                            # [R,H] = act @ w_dn[e]^T
-        out = moe_gather_combine(y, r["row"], r["w"], res)
-        ctx.save_for_backward(x, wg, w_gu, w_dn, xp, h1, act, y, r["row"], r["w"], r["gates"], r["idx"], r["meta"], offs)
+        st = moe_forward_stages(x, res, wg, w_gu, w_dn, noise, cf, min_cap, swiglu_fusable(I2 // 2, H, training=True))
+        ctx.save_for_backward(x, wg, w_gu, w_dn, *(st[k] for k in _MOE_SAVED))
+        ctx.fused = st["fused"]
         ctx.grads = grads
-        return out, r["meta"][0].clone()
+        return st["out"], st["meta"][0].clone()
 
     @staticmethod
     def backward(ctx, dout, dlaux):
-        x, wg, w_gu, w_dn, xp, h1, act, y, row, w, gates, idx, meta, offs = ctx.saved_tensors
-        E, I2, H = w_gu.shape
-        R = xp.shape[0]
-        S = x.shape[0]
-        dout = _c(dout)
-        dy = torch.zeros(R, H, dtype=dout.dtype, device=dout.device)
-        dw = torch.empty(S, 2, dtype=torch.float32, device=dout.device)
-        call("lmod_moe_combine_bwd", ptr(dout), ptr(y), ptr(row), ptr(w), S, H, ptr(dy), ptr(dw))
-        g = ctx.grads
-        if ctx.fused:
-            dh1 = grouped_gemm_silu_bwd(dy, w_dn, h1, offs, R)         # d(gate)|d(up) straight from the dgrad GEMM's epilogue
-        else:
-            dact = torch.empty(R, I2 // 2, dtype=dout.dtype, device=dout.device)
-            grouped_gemm(dy, w_dn, dact, offs, 1)                      # dact = dy @ w_dn[e]
-            dh1 = silu_mul_bwd(dact, h1)
-        if g is not None and g.get("w_dn") is not None:
-            grouped_gemm(dy, act, g["w_dn"], offs, 2, accumulate=True)  # dW_dn[e] += dy_e^T @ act_e
-        dxp = torch.empty(R, H, dtype=dout.dtype, device=dout.device)
-        grouped_gemm(dh1, w_gu, dxp, offs, 1)                          # dxp = dh1 @ w_gu[e]
-        if g is not None and g.get("w_gu") is not None:
-            grouped_gemm(dh1, xp, g["w_gu"], offs, 2, accumulate=True)  # dW_gu[e] += dh1_e^T @ xp_e
-        dlogits = torch.empty(S, E, dtype=torch.float32, device=dout.device)
-        gl = None
-        if dlaux is not None:
-            gl = dlaux.to(torch.float32).reshape(1).contiguous()
-        call("lmod_moe_gate_bwd", ptr(gates), ptr(idx), ptr(row), ptr(dw), ptr(meta), ptr(gl) if gl is not None else None, S, E, ptr(dlogits))
-        dx = torch.empty_like(x)
-        call("lmod_moe_scatter_bwd", ptr(dxp), ptr(row), ptr(dlogits), ptr(wg), None, S, H, E, ptr(dx))
-        if g is not None and g.get("wg") is not None:
-            ws = torch.empty(32, E, H, dtype=torch.float32, device=dout.device)
-            call("lmod_moe_wg_grad", ptr(x), ptr(dlogits), S, H, E, ptr(ws), ptr(g["wg"]))
+        x, wg, w_gu, w_dn, *saved = ctx.saved_tensors
+        st = dict(zip(_MOE_SAVED, saved), fused=ctx.fused)
+        dx = moe_backward_stages(st, x, wg, w_gu, w_dn, _c(dout), dlaux, ctx.grads)["dx"]
         return dx, dout, None, None, None, None, None, None, None
+
+
+_MOE_SAVED = ("xp", "h1", "act", "y", "row", "w", "gates", "idx", "meta", "offsets")
 
 
 def moe_forward_nograd(x, res, wg, w_gu, w_dn, noise, cf, min_cap):

@@ -1,5 +1,6 @@
 """Shared fixtures for the GPU parity tests, smoke() and bench.py: tiny config-1 models, seeded batches, and the
 oracle-side evaluation of the same step."""
+import math
 import types
 
 import torch
@@ -387,3 +388,415 @@ def make_trainer(student, teacher, loss_type="kd_lm", accum=1, lr=2e-5, max_step
     tr = cls(model=student, ref_model=teacher, args=args, loss_type=loss_type, moe_loss_enable=moe_loss_enable)
     tr._total_steps = max_steps
     return tr
+
+
+# ---------------------------------------------------------------------------------------------------
+# sparse MoE block (csrc/moe.cu, grouped modes of csrc/gemm.cu, kernels.MoEFn): float64 reference and element-wise bounds
+# ---------------------------------------------------------------------------------------------------
+# Every stage is recomputed in float64 from the tensors the kernels produced at the stage before it, so each bound covers the arithmetic
+# of one stage and errors do not compound.  u = 2^-8 is the unit roundoff of bf16, 2^-24 that of fp32.
+#   GEMM stages (h1, y, dact, dxp; the wgrads dW_gu, dW_dn with the old buffer value in ref):
+#       |got - ref| <= 2^-8 |ref| + (1 + 2^-8) (ceil(K/16) + 1) 2^-23 (|A| |B|)  [+ 2^-23 |ref| for the fp32 add of the old value]
+#     the wgmma fp32 accumulator truncates toward zero at each k = 16 step (relative 2^-23 per step, +1 for the alignment inside a step),
+#     so (|A||B|) majorises the error element by element; the bf16 store adds half an ulp (2^-8 relative) of the rounded value.  K is the
+#     reduction length: H or I (or 2I) for the row GEMMs, the group's 128-aligned row count for the wgrads.
+#   fp32 FMA chains: n 2^-24 sum|a||b|, n the chain the kernel runs:
+#     logits   H/32 FMAs per lane + 5 butterfly adds             dw      (combine_bwd) the same over dout . y
+#     dwg      ceil(S/32) FMAs per split + 32 split sums + the add to the old value
+#     dx       dxp[r1] + dxp[r2] + E FMAs of dlogits . wg (E + 2 roundings), then the bf16 store (2^-8 |ref|)
+#   gates: softmax of the kernel's fp32 logits with expf (<= 2 ulp), the rounded shift l - max, an E-term sum and a division:
+#       |got - ref| <= 2^-22 (E + 4 + max_e |l - max|) g
+#   act / dh1: SwiGLU of the kernel's bf16 h1.  bf16(silu(g)) and the bf16 store are 2^-8 each; the sigmoid (__expf: relative error
+#     about 2^-22 (2 + |g|)) and the fp32 products are covered by 2^-16.  dh1 also carries the error of dact (bf16 of a GEMM accumulator,
+#     never materialised on the fused path): 2^-8 |dact| + the GEMM term above, times |d dh1 / d dact|.
+#   dlogits: gate_bwd's fp32 arithmetic.  dg_e (l_aux term + renormalisation term) is off by at most 16 2^-24 D_e (D_e the sum of the
+#     terms' magnitudes), the dot sum_j g_j dg_j by sum_j g_j (16 2^-24 D_j + E 2^-24 |dg_j|), the final g (dg - dot) by 2 2^-24 of itself.
+#   l_aux: E sum_e mean(g_e) count_e / S over the tiles' fp32 sums (tpb + ntiles + E + 8 roundings of positive terms).
+# Bit-exact stages (compared by bits against a torch fp32 emulation): the scatter copy (xp rows = x rows); w = g / max(g1 + g2, eps) of
+# the kernel's gates; dy = bf16(bf16(w) dout); out = bf16(res + bf16(fp32(bf16(w1) y1 + bf16(w2) y2))) (both products are exact in fp32,
+# so the sum is one rounding, as the kernel's fma); zero padding rows of xp, h1, act and y below offsets[E].
+FLT_EPS = 2.0 ** -23
+
+
+def moe_route_tpb(S):
+    """Tokens per CTA of the router (route_tpb in csrc/moe.cu): a multiple of 16 that keeps the grid at <= 1024 CTAs."""
+    tpb = 16
+    while -(-S // tpb) > 1024:
+        tpb += 16
+    return tpb
+
+
+def _gemm_tol(ref, maj, K):
+    return 2.0 ** -8 * ref.abs() + (1 + 2.0 ** -8) * (math.ceil(K / 16) + 1) * 2.0 ** -23 * maj
+
+
+def moe_reference_fp64(x, res, wg, w_gu, w_dn, noise, cf, min_cap, dout=None, g_laux=0.0, old=None, k=None, eps=FLT_EPS, w_bf16=True,
+                       store=torch.float64):
+    """Float64 restatement of the sparse-MoE block (DeepSpeed top-2 gating, SwiGLU experts, combine) stage by stage.
+
+    x, res [S, H] bf16; wg [E, H] fp32; w_gu [E, 2I, H], w_dn [E, H, I] bf16; noise [S, E] fp32.  With dout [S, H] (and g_laux, the
+    upstream gradient of l_aux) the backward stages too; old: the gradient buffers' values before the call ({'wg', 'w_gu', 'w_dn'}).
+    k: the kernels' tensors per stage (kernels.moe_forward_stages / moe_backward_stages, plus the grads under 'g_wg', 'g_w_gu', 'g_w_dn');
+    every stage takes its inputs from k.  Without k the reference chains its own float64 stages.  eps is the clamp of the renormalisation
+    (fp32's in the kernels), w_bf16 rounds the combine weights to bf16 (the einsum's type_as in the model).  Works on x's device.
+
+    Returns {stage: (want, tol)} -- tol None for bit-exact stages -- plus the routing record under 'rec' (top2gating of the fp32 logits:
+    idx [S, 2], row [S, 2] in the 128-aligned compact layout, offsets [E+1], used [E], counts [E], capacity) and, for each GEMM stage, its
+    rows (the routed rows below offsets[E]); want/tol of the large stages are kept as `store`."""
+    dev = x.device
+    f64 = torch.float64
+    S, H = x.shape
+    E, I2, _ = w_gu.shape
+    I = I2 // 2
+    kk = k if k is not None else {}
+    out = {}
+    own = {}
+
+    def src(name):
+        return (kk[name] if name in kk and kk[name] is not None else own[name])
+
+    x64, wg64 = x.to(f64), wg.to(dev, f64)
+    # ---- gate: logits (fp32 GEMV), softmax, routing record
+    logits = x64 @ wg64.t()
+    own["logits"] = logits
+    lane_fmas = 8 * -(-H // 256)                                 # per lane: ceil(H / 8 / 32) vectors of 8 (gate GEMV, combine_bwd)
+    out["logits"] = (logits, (lane_fmas + 6) * 2.0 ** -24 * (x64.abs() @ wg64.abs().t()))
+    lk = src("logits").to(f64)
+    gates = torch.softmax(lk, 1)
+    own["gates"] = gates
+    out["gates"] = (gates, 2.0 ** -22 * (E + 4 + (lk - lk.amax(1, keepdim=True)).abs().amax(1, keepdim=True)) * gates)
+    o = R.top2gating(lk.float().cpu(), noise.float().cpu(), cf, min_cap)
+    C = o["capacity"]
+    idx = torch.stack([o["idx1"], o["idx2"]], 1).to(dev)
+    keep = torch.stack([o["keep1"], o["keep2"]], 1).to(dev)
+    counts = o["exp_counts"].to(dev)
+    cnt = torch.minimum(torch.bincount(idx[:, 0], minlength=E) + torch.bincount(idx[:, 1], minlength=E), torch.tensor(C, device=dev))
+    offsets = torch.zeros(E + 1, dtype=torch.long, device=dev)
+    offsets[1:] = ((cnt + 127) // 128 * 128).cumsum(0)
+    slot = torch.stack([o["slot1"], o["slot2"]], 1).to(dev)
+    row = torch.where(keep, offsets[idx] + slot, torch.full_like(slot, -1))
+    rec = dict(idx=idx, row=row, keep=keep, offsets=offsets, used=cnt, counts=counts, capacity=C)
+    out["rec"] = rec
+    gk = src("gates")
+    # ---- renormalised weights (bit exact in fp32 from the kernel's gates) and l_aux
+    g32 = gk.float() if "gates" in kk else gk
+    gsel = torch.where(keep, g32.gather(1, idx), torch.zeros_like(g32[:, :2]))
+    den = (gsel[:, 0] + gsel[:, 1]).clamp(min=eps)
+    w = gsel / den[:, None]
+    own["w"] = w
+    out["w"] = (w, None)
+    ce = counts.to(f64) / S
+    laux = E * (gk.to(f64).mean(0) * ce).sum()
+    tpb = moe_route_tpb(S)
+    out["l_aux"] = (laux, (tpb + -(-S // tpb) + E + 8) * 2.0 ** -24 * laux.abs())
+    wk = src("w")
+    wr = wk.to(torch.bfloat16).to(f64) if w_bf16 else wk.to(f64)
+    # ---- scatter: xp rows are the token rows; padding rows are zero
+    n_rows = int(offsets[-1])
+    tok = torch.full((n_rows,), -1, dtype=torch.long, device=dev)
+    for c in range(2):
+        tok[row[:, c][keep[:, c]]] = torch.arange(S, device=dev)[keep[:, c]]
+    rec["tok"] = tok
+    xp = torch.zeros(n_rows, H, dtype=x.dtype, device=dev)
+    xp[tok >= 0] = x[tok[tok >= 0]]
+    own["xp"] = xp
+    out["xp"] = (xp, None)
+    groups = [(int(offsets[e]), int(offsets[e]) + int(cnt[e]), int(offsets[e + 1])) for e in range(E)]   # (first, end of routed, end)
+    rec["groups"] = groups
+
+    def per_expert(name, a_name, wfun, K, n_out):
+        want = torch.zeros(n_rows, n_out, dtype=store, device=dev)
+        tol = torch.zeros_like(want)
+        a = src(a_name)
+        for e, (r0, r1, _) in enumerate(groups):
+            if r1 > r0:
+                A = a[r0:r1].to(f64)
+                B = wfun(e)
+                want[r0:r1] = (A @ B).to(store)
+                tol[r0:r1] = _gemm_tol(want[r0:r1].to(f64), A.abs() @ B.abs(), K).to(store)
+        own[name] = want
+        out[name] = (want, tol)
+        return want
+
+    # ---- expert forward
+    per_expert("h1", "xp", lambda e: w_gu[e].to(dev, f64).t(), H, I2)
+    h1k = src("h1")[:n_rows].to(f64)
+    gg, uu = h1k[:, :I], h1k[:, I:]
+    sg = torch.sigmoid(gg)
+    act = gg * sg * uu
+    own["act"] = act.to(store)
+    out["act"] = (own["act"], ((2.0 ** -7 + 2.0 ** -16) * act.abs()).to(store))
+    del h1k, gg, uu, sg
+    per_expert("y", "act", lambda e: w_dn[e].to(dev, f64).t(), I, H)
+    # ---- combine (bit exact in fp32 from the kernel's y and w)
+    yk = src("y")
+    yt = torch.float32 if "y" in kk else f64
+    ysel = [torch.where(keep[:, c:c + 1], yk[row[:, c].clamp(min=0)].to(yt), torch.zeros(S, H, dtype=yt, device=dev)) for c in range(2)]
+    if "y" in kk:
+        wb = wk.to(torch.bfloat16).float()
+        comb = (wb[:, :1] * ysel[0] + wb[:, 1:] * ysel[1]).to(torch.bfloat16)
+        outv = (res.float() + comb.float()).to(torch.bfloat16)
+    else:
+        outv = res.to(f64) + wr[:, :1] * ysel[0].to(f64) + wr[:, 1:] * ysel[1].to(f64)
+    own["out"] = outv
+    out["out"] = (outv, None)
+    del ysel
+    if dout is None:
+        return out
+    # ---- backward: combine -> dy (bit exact), dw (fp32 chains)
+    d64 = dout.to(f64)
+    dy = torch.zeros(n_rows, H, dtype=torch.bfloat16 if "w" in kk else f64, device=dev)
+    for c in range(2):
+        m = keep[:, c]
+        if "w" in kk:
+            dy[row[m, c]] = (wk[m, c:c + 1].to(torch.bfloat16).float() * dout[m].float()).to(torch.bfloat16)
+        else:
+            dy[row[m, c]] = wr[m, c:c + 1] * d64[m]
+    own["dy"] = dy
+    out["dy"] = (dy, None)
+    dw = torch.zeros(S, 2, dtype=f64, device=dev)
+    dwt = torch.zeros_like(dw)
+    for c in range(2):
+        m = keep[:, c]
+        yr = yk[row[m, c]].to(f64)
+        dw[m, c] = (d64[m] * yr).sum(1)
+        dwt[m, c] = (lane_fmas + 6) * 2.0 ** -24 * (d64[m].abs() * yr.abs()).sum(1)
+    own["dw"] = dw
+    out["dw"] = (dw, dwt)
+    # ---- expert backward: dact = dy W_dn, dh1 = SwiGLU backward (from the kernel's h1), wgrads, dxp
+    per_expert("dact", "dy", lambda e: w_dn[e].to(dev, f64), H, I)
+    dact, dact_tol = own["dact"].to(f64), out["dact"][1].to(f64)
+    h1k = src("h1")[:n_rows].to(f64)
+    gg, uu = h1k[:, :I], h1k[:, I:]
+    sg = torch.sigmoid(gg)
+    cg, cu = uu * sg * (1 + gg * (1 - sg)), gg * sg
+    dh1 = torch.cat([dact * cg, dact * cu], 1)
+    derr = dact_tol + 2.0 ** -16 * dact.abs()
+    dh1_tol = 2.0 ** -8 * dh1.abs() + (1 + 2.0 ** -8) * torch.cat([derr * cg.abs(), derr * cu.abs()], 1)
+    own["dh1"] = dh1.to(store)
+    out["dh1"] = (own["dh1"], dh1_tol.to(store))
+    del h1k, gg, uu, sg, cg, cu, dact, dact_tol, derr, dh1, dh1_tol
+    per_expert("dxp", "dh1", lambda e: w_gu[e].to(dev, f64), I2, H)
+    olds = old or {}
+    for gname, a_name, b_name, M, N in (("w_dn", "dy", "act", H, I), ("w_gu", "dh1", "xp", I2, H)):
+        want = torch.zeros(E, M, N, dtype=store, device=dev)
+        tol = torch.zeros_like(want)
+        A, B = src(a_name), src(b_name)
+        for e, (r0, r1, r2) in enumerate(groups):
+            o_e = olds[gname][e].to(dev, f64) if gname in olds else torch.zeros(M, N, dtype=f64, device=dev)
+            if r1 > r0:
+                a, b = A[r0:r1].to(f64), B[r0:r1].to(f64)
+                ref = a.t() @ b + o_e
+                tol[e] = (_gemm_tol(ref, a.abs().t() @ b.abs(), r2 - r0) + 2.0 ** -23 * ref.abs()).to(store)
+                want[e] = ref.to(store)
+            else:
+                want[e] = o_e.to(store)                      # an expert without rows leaves its gradient untouched, bit for bit
+        out["g_" + gname] = (want, tol)
+    # ---- gate backward: dlogits through the renormalisation (clamped or not) and the softmax, plus the l_aux term
+    gk64 = gk.to(f64)
+    dwk = src("dw").to(f64)
+    a = torch.where(keep[:, 0], gk64.gather(1, idx[:, :1])[:, 0], torch.zeros(S, dtype=f64, device=dev))
+    b = torch.where(keep[:, 1], gk64.gather(1, idx[:, 1:])[:, 0], torch.zeros(S, dtype=f64, device=dev))
+    ssum = a + b
+    lterm = (g_laux * E * counts.to(f64) / S / S)[None].expand(S, E)
+    clamp = ssum <= eps                                          # torch.clamp(min=eps): zero derivative of the sum below eps
+    inv2 = 1.0 / (ssum * ssum).clamp(min=1e-300)
+    da = torch.where(clamp, dwk[:, 0] / eps, (dwk[:, 0] - dwk[:, 1]) * b * inv2)
+    db = torch.where(clamp, dwk[:, 1] / eps, (dwk[:, 1] - dwk[:, 0]) * a * inv2)
+    da, db = da * keep[:, 0], db * keep[:, 1]
+    rterm = torch.zeros(S, E, dtype=f64, device=dev)
+    rterm.scatter_add_(1, idx[:, :1], da[:, None])
+    rterm.scatter_add_(1, idx[:, 1:], db[:, None])
+    dg = lterm + rterm
+    D = lterm.abs() + rterm.abs()
+    dot = (gk64 * dg).sum(1, keepdim=True)
+    dl = gk64 * (dg - dot)
+    u = 2.0 ** -24
+    dl_tol = gk64 * (16 * u * D + (gk64 * (16 * u * D + E * u * dg.abs())).sum(1, keepdim=True)) + 2 * u * dl.abs() + 2.0 ** -140
+    own["dlogits"] = dl
+    out["dlogits"] = (dl, dl_tol)
+    # ---- dx = dxp[r1] + dxp[r2] + dlogits wg ;  dwg += dlogits^T x
+    dxpk, dlk = src("dxp"), src("dlogits").to(f64)
+    gate_term = dlk @ wg64
+    maj = dlk.abs() @ wg64.abs()
+    dx = gate_term.clone()
+    for c in range(2):
+        m = keep[:, c]
+        v = dxpk[row[m, c]].to(f64)
+        dx[m] += v
+        maj[m] += v.abs()
+    own["dx"] = dx
+    out["dx"] = (dx, 2.0 ** -8 * dx.abs() + (1 + 2.0 ** -8) * (E + 2) * u * maj)
+    out["dx_gate"] = gate_term
+    o_wg = olds["wg"].to(dev, f64) if "wg" in olds else torch.zeros(E, H, dtype=f64, device=dev)
+    dwg = o_wg + dlk.t() @ x64
+    out["g_wg"] = (dwg, (-(-S // 32) + 34) * u * (dlk.abs().t() @ x64.abs() + o_wg.abs()))
+    return out
+
+
+def check_moe(name, got, want, tol=None, report=None, rows=None):
+    """One stage of moe_reference_fp64: bit for bit when tol is None, else element-wise |got - want| <= tol.  rows (optional) restricts the
+    comparison to a bool mask or index of the first dimension (the routed rows of an expert-row tensor).  On failure names the worst
+    element by (token or expert row, column), the count out of bound and max(err / bound).  Returns max(err / bound) (0 for exact stages);
+    `report`, a dict, collects it under `name`."""
+    if rows is not None:
+        got, want = got[rows], want[rows]
+        tol = None if tol is None else tol[rows]
+    if tol is None:
+        g, w = got.detach().to(want.device), want
+        assert g.dtype == w.dtype and g.shape == w.shape, (name, g.dtype, w.dtype, g.shape, w.shape)
+        bad = g.view(torch.int16 if g.element_size() == 2 else torch.int32) != w.view(torch.int16 if w.element_size() == 2 else torch.int32) \
+            if g.is_floating_point() else g != w
+        nbad = int(bad.sum())
+        if nbad:
+            i = tuple(int(t) for t in torch.nonzero(bad)[0])
+            raise AssertionError(f"{name}: {nbad} / {g.numel()} elements differ in bits; first at {i}: got {g[i].item()!r} want {w[i].item()!r}")
+        if report is not None:
+            report.setdefault(name, 0.0)
+        return 0.0
+    got = got.detach().to(want.device, torch.float64)
+    want, tol = want.to(torch.float64), tol.to(torch.float64)
+    err = (got - want).abs()
+    ratio = (err / tol).nan_to_num(float("inf"), float("inf"), 0.0)   # a NaN in got counts as out of bound; 0/0 is in bound
+    ratio = torch.where(err == 0, torch.zeros_like(ratio), ratio)
+    worst = float(ratio.max()) if ratio.numel() else 0.0
+    if report is not None:
+        report[name] = max(worst, report.get(name, 0.0))
+    nbad = int((~(err <= tol)).sum())
+    if nbad:
+        i = int(ratio.reshape(-1).argmax())
+        where = tuple(int(t) for t in torch.unravel_index(torch.tensor(i), ratio.shape))
+        g, w, t = got.reshape(-1)[i].item(), want.reshape(-1)[i].item(), tol.reshape(-1)[i].item()
+        raise AssertionError(f"{name}: {nbad} / {got.numel()} elements out of bound, max err/bound {worst:.3g}; worst at (row, col) {where}: "
+                             f"got {g!r} want {w!r} bound {t:.3g}")
+    return worst
+
+
+def moe_plan_pairs(S, E, n1, n2, seed=0):
+    """[S, 2] (first, second) expert of every token with n1[e] first and n2[e] second choices, first != second, in a seeded order."""
+    g = torch.Generator().manual_seed(seed)
+    assert sum(n1) == S and sum(n2) == S
+    e1 = torch.cat([torch.full((n,), e, dtype=torch.long) for e, n in enumerate(n1)])[torch.randperm(S, generator=g)]
+    left = list(n2)
+    e2 = torch.empty(S, dtype=torch.long)
+    done = []
+    for s in torch.randperm(S, generator=g).tolist():          # the expert with the most second choices left, other than the first
+        c = max((e for e in range(E) if e != int(e1[s]) and left[e] > 0), key=lambda e: left[e], default=None)
+        if c is None:                                          # only the token's own first choice is left: trade with a placed token
+            c = int(e1[s])
+            t = next((t for t in done if int(e2[t]) != c and int(e1[t]) != c), None)
+            assert t is not None, "moe_plan_pairs: counts cannot be met with first != second"
+            e2[s], e2[t] = e2[t].clone(), c
+        else:
+            e2[s] = c
+        left[c] -= 1
+        done.append(s)
+    return torch.stack([e1, e2], 1)
+
+
+def moe_planted_inputs(pairs, E, H, specials=(), seed=0, x_scale=1.0):
+    """Inputs whose routing is exactly `pairs` [S, 2] (first, second expert per token).  Column e < E of x carries the token's first
+    choice: x[s, e1] in [0.75, 1.25], wg[e, e] = 4, so logit e1 leads the random part (x[:, 16:] . wg[:, 16:], std about 0.3) by a clear
+    margin; the noise adds 10 to the second choice.  specials: (token, logits, noise) rows planted exactly: x[s] is one-hot in a column
+    of its own (16 - E > index), wg's column holds the logits (fp32, so the kernel's GEMV gives them bit for bit), noise[s] = noise.
+    Returns x [S, H] bf16, wg [E, H] fp32, noise [S, E] fp32 (CPU)."""
+    S = pairs.shape[0]
+    g = torch.Generator().manual_seed(seed)
+    x = torch.randn(S, H, generator=g) * x_scale
+    x[:, :16] = 0
+    x[torch.arange(S), pairs[:, 0]] = 0.75 + 0.5 * torch.rand(S, generator=g)
+    wg = torch.randn(E, H, generator=g) * (0.3 / math.sqrt(H - 16) / x_scale)
+    wg[:, :16] = 0
+    wg[torch.arange(E), torch.arange(E)] = 4.0
+    noise = torch.zeros(S, E)
+    noise[torch.arange(S), pairs[:, 1]] = 10.0
+    for i, (s, logits, nz) in enumerate(specials):
+        col = E + i
+        assert col < 16
+        x[s] = 0
+        x[s, col] = 1
+        wg[:, col] = torch.as_tensor(logits, dtype=torch.float32)
+        noise[s] = torch.as_tensor(nz, dtype=torch.float32)
+    return x.to(torch.bfloat16), wg.contiguous(), noise
+
+
+def moe_special_rows(E, S, clamp_to=None):
+    """The planted routing edges (token, logits, noise, expected (first, second), what) on tokens S-1, S-2 (late: their first choice,
+    expert 0, has overflowed; pairs must give them first choice 0) and tokens 0, 1, 2 (early):
+      equal logits -> first choice 0, second choice a tie of logits + noise between experts 1 and 2 -> 1;
+      1-ulp near tie at |logit| ~ 0.1 (gates tie, logits do not) -> first choice 0;
+      a tie in logits + noise for the second choice with distinct logits;
+      late: first choice dropped, second (clamp_to, default E-1) kept with a gate below FLT_EPSILON (clamped renormalisation);
+      late: both choices dropped (second choice 1, which must be full by then)."""
+    ct = E - 1 if clamp_to is None else clamp_to
+    f = torch.tensor
+    nt = float(torch.nextafter(f(0.1, dtype=torch.float32), f(1.0, dtype=torch.float32)))
+    pad = lambda v, fill: (list(v) + [fill] * E)[:E]             # noqa: E731
+    rows = [
+        (0, [0.5] * E, pad([0.0, 3.0, 3.0], 0.0), (0, 1), "equal logits"),
+        (1, pad([0.1, nt], -1.0) if E == 2 else pad([0.1, nt, -1.0, -2.0], -2.5), pad([0.0, 0.0, 10.0], 0.0) if E > 2 else [0.0, 0.0],
+         (0, 2) if E > 2 else (0, 1), "1-ulp near tie"),
+        (2, pad([1.0, 0.5, 0.25], -1.0), pad([0.0, 1.0, 1.25], 0.0) if E > 2 else [0.0, 1.0], (0, 1), "tie in logits + noise"),
+        (S - 2, [8.0] + [-8.2 if e == ct else -9.0 for e in range(1, E)], [10.0 if e == ct else 0.0 for e in range(E)], (0, ct),
+         "dropped first, clamped second"),
+        (S - 1, pad([3.0, 1.0], -1.0), pad([0.0, 10.0], 0.0), (0, 1), "both dropped"),
+    ]
+    return rows
+
+
+def moe_force_pairs(pairs, rows):
+    """Give the special tokens their (first, second) pair by swapping with a token that has it (the counts stay as planned)."""
+    pairs = pairs.clone()
+    fixed = set()
+    for s, _, _, want, _ in rows:
+        want = torch.tensor(want)
+        if not torch.equal(pairs[s], want):
+            cand = [t for t in torch.nonzero((pairs == want).all(1))[:, 0].tolist() if t not in fixed and t != s]
+            assert cand, ("moe_force_pairs: no token has the pair", tuple(want.tolist()))
+            t = cand[0]
+            pairs[[s, t]] = pairs[[t, s]]
+        fixed.add(s)
+    return pairs
+
+
+def moe_run_stages(x, res, wg, w_gu, w_dn, noise, cf, mc, dout, g_laux, old, fused):
+    """kernels.moe_forward_stages + moe_backward_stages with weight gradients accumulated into copies of `old`; one dict of every
+    intermediate, the gradients under 'g_wg', 'g_w_gu', 'g_w_dn'."""
+    from llavamod import kernels as K
+    grads = {k: v.clone() for k, v in old.items()}
+    st = K.moe_forward_stages(x, res, wg, w_gu, w_dn, noise, cf, mc, fused)
+    bw = K.moe_backward_stages(st, x, wg, w_gu, w_dn, dout, torch.tensor(g_laux, device="cuda"), grads)
+    k = {**st, **bw, **{"g_" + n: v for n, v in grads.items()}}
+    return k
+
+
+def check_moe_stages(k, ref, E, old, report=None):
+    """Every stage of moe_run_stages against moe_reference_fp64(..., k=k): the routing record bit for bit, then each stage's bound."""
+    rec = ref["rec"]
+    n_rows = int(rec["offsets"][-1])
+    assert torch.equal(k["idx"].long(), rec["idx"]), "routing record (first / second expert)"
+    assert torch.equal(k["row"].long(), rec["row"]), "routing record (rows: slots and drops)"
+    assert torch.equal(k["offsets"].long(), rec["offsets"])
+    assert k["capacity"] == rec["capacity"] and int(k["meta"][1]) == rec["capacity"]
+    assert torch.equal(k["meta"][4:4 + E].long(), rec["counts"])
+    routed = rec["tok"] >= 0
+    pad = ~routed
+    for name in ("logits", "gates", "dw", "dlogits", "dx"):
+        check_moe(name, k[name], *ref[name], report=report)
+    check_moe("w", k["w"], ref["w"][0], None, report)
+    la_want, la_tol = ref["l_aux"]
+    assert abs(float(k["meta"][0]) - float(la_want)) <= float(la_tol), ("l_aux", float(k["meta"][0]), float(la_want))
+    check_moe("xp", k["xp"][:n_rows], ref["xp"][0], None, report)
+    for name in ("h1", "act", "y", "dh1", "dxp") + (("dact",) if k["dact"] is not None else ()):
+        check_moe(name, k[name][:n_rows], *ref[name], report=report, rows=routed)
+        if name in ("h1", "act", "y"):                           # padding rows below offsets[E] are exact zeros
+            assert int(k[name][:n_rows][pad].ne(0).sum()) == 0, f"{name}: non-zero padding row"
+    check_moe("out", k["out"], ref["out"][0], None, report)
+    check_moe("dy", k["dy"][:n_rows], ref["dy"][0], None, report)
+    assert int(k["dy"][n_rows:].ne(0).sum()) == 0
+    check_moe("g_wg", k["g_wg"], *ref["g_wg"], report=report)
+    for gname in ("w_gu", "w_dn"):
+        check_moe("g_" + gname, k["g_" + gname], *ref["g_" + gname], report=report)
+        for e in range(E):
+            if int(rec["used"][e]) == 0:                       # an expert without rows leaves its pre-filled gradient untouched
+                check_moe(f"g_{gname}[{e}] (empty expert)", k["g_" + gname][e], old[gname][e], None)

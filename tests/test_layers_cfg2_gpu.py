@@ -145,15 +145,19 @@ def test_moe_block_forward_backward_at_config2_shape():
     assert torch.equal(r["idx"].cpu().long()[:, 0], o["idx1"]) and torch.equal(r["idx"].cpu().long()[:, 1], o["idx2"])
     assert torch.equal(r["row"].cpu()[:, 0] >= 0, o["keep1"]) and torch.equal(r["row"].cpu()[:, 1] >= 0, o["keep2"])
     assert int((~o["keep1"]).sum() + (~o["keep2"]).sum()) > 0
-    assert rel(out, (ro + y)) < 8e-3
     assert abs(l_aux.item() - la.item()) < 1e-4 * abs(la.item())
-    assert rel(xd.grad, xo.grad) < 2e-2
     assert rel(rd.grad, ro.grad) < 1e-6 + 2.0 ** -8
-    assert rel(grads["wg"], sdo[pre + "gate.wg.weight"].grad) < 2e-2
-    for e in range(E):
-        gg = torch.cat([sdo[pre + f"experts.deepspeed_experts.{e}.gate_proj.weight"].grad, sdo[pre + f"experts.deepspeed_experts.{e}.up_proj.weight"].grad])
-        assert rel(grads["w_gu"][e], gg) < 1.5e-2, e
-        assert rel(grads["w_dn"][e], sdo[pre + f"experts.deepspeed_experts.{e}.down_proj.weight"].grad) < 1.5e-2, e
+    # element by element: every stage against the float64 reference from the kernels' previous stage (a missing or misrouted token row,
+    # about 2 % of the Frobenius norm here, fails), and MoEFn gives the stage functions' bytes
+    from tests.helpers import check_moe_stages, moe_reference_fp64, moe_run_stages
+    zeros = {k: torch.zeros_like(v) for k, v in grads.items()}
+    k = moe_run_stages(xd.detach(), rd.detach(), wg, w_gu, w_dn, noise.cuda(), cf, 0, go.cuda(), 0.37, zeros, False)
+    assert torch.equal(out, k["out"]) and torch.equal(xd.grad, k["dx"])
+    for name in ("wg", "w_gu", "w_dn"):
+        assert torch.equal(grads[name], k["g_" + name]), name
+    ref = moe_reference_fp64(xd.detach(), rd.detach(), wg, w_gu, w_dn, noise, cf, 0, dout=go.cuda(), g_laux=0.37, old=zeros, k=k,
+                             store=torch.float32)
+    check_moe_stages(k, ref, E, zeros)
 
 
 def test_loss_head_full_vocab_on_supervised_rows():
