@@ -256,6 +256,24 @@ int lmod_attn_bwd(const void* qkv, int64_t ld_qkv, const void* out, int64_t ld_o
                   void* dqkv, int64_t ld_dqkv, float* dq32_ws, float* dsum_ws, const int32_t* kv_lo, const int32_t* kv_hi,
                   void* stream);
 
+/* ------------------------------------------------------------------------------------------
+ * KV-cache decoding (csrc/decode.cu).  The cache of a layer is one K and one V buffer [batch, nkv, max_len, hd] bf16 (HF's legacy layout);
+ * sequence b holds rows [0, len[b]).
+ * lmod_kv_append: DynamicCache.update (the reference's cache_utils.py) -- copies the k and v heads of n_new rows per sequence of the fused,
+ *   RoPE'd QKV buffer [batch*n_new, (nh+2*nkv)*hd] (row stride ld_qkv) to cache rows offsets[b] + [0, n_new), offsets int32 [batch] on the
+ *   device.  Bit-exact; no other row is written (rows that would land at or past max_len are skipped; callers bounds-check).  hd %% 8 == 0.
+ * lmod_attn_decode: the past_key_value path of Qwen2SdpaAttention.forward (modeling_qwen2.py:652-728) for one new query per sequence:
+ *   q [batch, ld_q] (query heads at columns [h*hd, (h+1)*hd), e.g. the fused QKV rows) against cache rows [0, len[b]), len int32 [batch] on
+ *   the device; GQA by index (query head h reads KV head h / (nh/nkv), nh/nkv <= 8).  out [batch, nh*hd] bf16 (row stride ld_o); lse
+ *   [batch, nh] fp32 (natural-log LSE of the scaled scores) or NULL.  hd in {64,128}.  Split-KV: the launch grid depends on max_len, not
+ *   on len, so a captured graph serves every step.  ws: fp32 workspace of at least lmod_attn_decode_ws_elems(...) elements. */
+int lmod_kv_append(const void* qkv, int64_t ld_qkv, int64_t batch, int64_t n_new, int nh, int nkv, int hd, const int32_t* offsets,
+                   void* k_cache, void* v_cache, int64_t max_len, void* stream);
+int64_t lmod_attn_decode_ws_elems(int64_t batch, int nh, int nkv, int hd, int64_t max_len);
+int lmod_attn_decode(const void* q, int64_t ld_q, const void* k_cache, const void* v_cache, const int32_t* len, int64_t batch, int nh,
+                     int nkv, int hd, int64_t max_len, float softmax_scale, void* out, int64_t ld_o, float* lse, float* ws,
+                     int64_t ws_elems, void* stream);
+
 
 #ifdef __cplusplus
 }

@@ -64,11 +64,14 @@ SIGNATURES = {
     "lmod_gemm_residual": [_P, _L, _P, _L, _P, _P, _L, _P, _L, _L, _L, _L, _P],
     "lmod_attn_fwd": [_P, _L, _L, _L, _I, _I, _I, _I, _F, _P, _L, _P, _P, _P, _P],
     "lmod_attn_bwd": [_P, _L, _P, _L, _P, _L, _P, _L, _L, _I, _I, _I, _I, _F, _P, _L, _P, _P, _P, _P, _P],
+    "lmod_kv_append": [_P, _L, _L, _L, _I, _I, _I, _P, _P, _P, _L, _P],
+    "lmod_attn_decode_ws_elems": [_L, _I, _I, _I, _L],
+    "lmod_attn_decode": [_P, _L, _P, _P, _P, _L, _I, _I, _I, _L, _F, _P, _L, _P, _P, _L, _P],
     "lmod_version": [],
     "lmod_launch_count_reset": [],
 }
 _RESTYPES = {"lmod_last_error": ctypes.c_char_p, "lmod_launch_count": c_int64, "lmod_launch_count_reset": None,
-             "lmod_moe_route_ws_elems": c_int64}
+             "lmod_moe_route_ws_elems": c_int64, "lmod_attn_decode_ws_elems": c_int64}
 
 
 class LmodError(RuntimeError):

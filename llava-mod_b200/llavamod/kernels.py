@@ -400,6 +400,75 @@ def attention(qkv, B, T, nh, nkv, hd, causal=True, scale=None, pad=None):
     return attention_fwd(qkv, B, T, nh, nkv, hd, causal, scale, pad=pad)[0]
 
 
+def attn_head_dim(hd):
+    """Head width the attention kernels run for a model head dim: 64 / 128 as they are, smaller ones zero-padded (see attention)."""
+    if hd > 128:
+        raise _C.LmodError("head_dim %d > 128 is not built" % hd)
+    return hd if hd in ATTN_HEAD_DIMS else (64 if hd < 64 else 128)
+
+
+def _pad_heads(x, heads, hd, hp):
+    """[rows, heads*hd] (row stride free) -> contiguous [rows, heads*hp], every head zero-padded to hp columns."""
+    return torch.nn.functional.pad(x.view(x.shape[0], heads, hd), (0, hp - hd)).view(x.shape[0], heads * hp)
+
+
+def _check_cache(k_cache, v_cache, B, nkv, hd):
+    """The kernels index the cache as dense bf16 [B, nkv, max_len, attn_head_dim(hd)]."""
+    want = (B, nkv, k_cache.shape[2] if k_cache.dim() == 4 else -1, attn_head_dim(hd))
+    for t in (k_cache, v_cache):
+        if t.dtype != BF16 or tuple(t.shape) != want or not t.is_contiguous():
+            raise _C.LmodError("KV cache must be contiguous bf16 %s, got %s %s%s" % (want, t.dtype, tuple(t.shape),
+                                                                                    "" if t.is_contiguous() else " (strided)"))
+
+
+def _check_i32(t, B, name):
+    if t.dtype != torch.int32 or t.numel() != B or not t.is_contiguous():
+        raise _C.LmodError("%s must be a contiguous int32 tensor of %d elements, got %s %s" % (name, B, t.dtype, tuple(t.shape)))
+
+
+def kv_append(qkv, B, n_new, nh, nkv, hd, k_cache, v_cache, offsets):
+    """DynamicCache.update: the k / v heads of the fused, RoPE'd QKV rows [B*n_new, (nh+2nkv)*hd] -> cache rows offsets[b] + [0, n_new)
+    of k_cache / v_cache [B, nkv, max_len, hp] (hp = attn_head_dim(hd); padded heads get zero columns).  offsets: int32 [B] on the device."""
+    _need_cuda(qkv, k_cache, v_cache, offsets)
+    _check_cache(k_cache, v_cache, B, nkv, hd)
+    _check_i32(offsets, B, "offsets")
+    if qkv.dim() != 2 or qkv.shape[0] != B * n_new or qkv.shape[1] != (nh + 2 * nkv) * hd or qkv.stride(1) != 1:
+        raise _C.LmodError("kv_append: qkv must be [B*n_new, (nh+2nkv)*hd] with unit column stride, got %s" % (tuple(qkv.shape),))
+    hp = k_cache.shape[-1]
+    if hp != hd:
+        qkv = _pad_heads(qkv, nh + 2 * nkv, hd, hp)
+    call("lmod_kv_append", ptr(qkv), qkv.stride(0), B, n_new, nh, nkv, hp, ptr(offsets), ptr(k_cache), ptr(v_cache), k_cache.shape[2])
+
+
+def attn_decode_ws_elems(B, nh, nkv, hd, max_len):
+    return int(_C.lib().lmod_attn_decode_ws_elems(B, nh, nkv, attn_head_dim(hd), max_len))
+
+
+def attn_decode(q, nh, nkv, hd, k_cache, v_cache, lens, ws, scale=None, need_lse=False):
+    """Single-query attention of every sequence over its cached keys [0, lens[b]) (split-KV, lmod_attn_decode).  q: [B, >= nh*hd] rows
+    whose first nh*hd columns are the query heads (the fused QKV rows of a decode step); k_cache / v_cache [B, nkv, max_len, hp];
+    lens int32 [B] on the device; ws fp32 of at least attn_decode_ws_elems(...).  -> (out [B, nh*hd] bf16, lse [B, nh] fp32 or None)."""
+    _need_cuda(q, k_cache, v_cache, lens, ws)
+    B = q.shape[0]
+    _check_cache(k_cache, v_cache, B, nkv, hd)
+    _check_i32(lens, B, "lens")
+    if q.dim() != 2 or q.shape[1] < nh * hd or q.stride(1) != 1 or q.dtype != BF16:
+        raise _C.LmodError("attn_decode: q must be bf16 [B, >= nh*hd] with unit column stride, got %s %s" % (q.dtype, tuple(q.shape)))
+    if ws.dtype != torch.float32 or not ws.is_contiguous():
+        raise _C.LmodError("attn_decode: ws must be a contiguous fp32 tensor")
+    hp, max_len = k_cache.shape[-1], k_cache.shape[2]
+    scale = float(scale if scale is not None else hd ** -0.5)
+    if hp != hd:
+        q = _pad_heads(q[:, :nh * hd], nh, hd, hp)
+    out = torch.empty(B, nh * hp, dtype=q.dtype, device=q.device)
+    lse = torch.empty(B, nh, dtype=torch.float32, device=q.device) if need_lse else None
+    call("lmod_attn_decode", ptr(q), q.stride(0), ptr(k_cache), ptr(v_cache), ptr(lens), B, nh, nkv, hp, max_len, scale, ptr(out), out.stride(0),
+         ptr(lse), ptr(ws), ws.numel())
+    if hp != hd:
+        out = out.view(B, nh, hp)[:, :, :hd].reshape(B, nh * hd)
+    return out, lse
+
+
 def pad_ranges(attention_mask):
     """[B,T] bool mask (contiguous real tokens, right or left padded -- what the collators and the multimodal splice produce) ->
     (kv_lo, kv_hi) int32 [B] on the device, no host sync."""

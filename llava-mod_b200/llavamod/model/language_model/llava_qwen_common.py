@@ -14,11 +14,13 @@ import torch.nn as nn
 from torch.autograd import Function
 
 from ... import kernels as K
-from ...constants import IGNORE_INDEX
+from ...constants import IGNORE_INDEX, IMAGE_TOKEN_INDEX
 from ..builder_io import load_into, load_state_dict_files
 from ..llava_arch import LlavaMetaForCausalLM, LlavaMetaModel
 from ..utils import CausalLMOutputWithPast, MoECausalLMOutputWithPast
-from .qwen2_core import MoE, ParamLinear, Qwen2Config, Qwen2Model
+from .qwen2_core import KVCache, MoE, ParamLinear, Qwen2Config, Qwen2Model
+
+CACHE_ROOM = 512          # positions a cache allocated by forward(use_cache=True) keeps free after the prompt
 
 
 class LlavaQwenModelBase(LlavaMetaModel, Qwen2Model):
@@ -128,9 +130,20 @@ class LlavaQwenForCausalLMBase(nn.Module, LlavaMetaForCausalLM):
         return self.model.embed_tokens
 
     # ---- forward -------------------------------------------------------------------------------------
+    def new_kv_cache(self, batch, max_len):
+        """A KVCache for `batch` equal-length sequences of up to max_len spliced positions (prompt incl. image patches + new tokens)."""
+        return KVCache(self.model, batch, max_len)
+
     def forward_hidden(self, input_ids=None, attention_mask=None, position_ids=None, inputs_embeds=None, labels=None,
-                       images=None, moe_noise=None, tower_features=None, plan=None):
-        """Splice + decoder.  Returns dict(hidden [B,T',H], labels [B,T'], attention_mask, l_aux list)."""
+                       images=None, moe_noise=None, tower_features=None, plan=None, cache=None):
+        """Splice + decoder.  Returns dict(hidden [B,T',H], labels [B,T'], attention_mask, l_aux list).
+        cache: a KVCache -- empty: prefill into it; holding a prefix: input_ids [B,1] is one decode step (no splice, as llava_arch.py:162)."""
+        if cache is not None and cache.length > 0 and inputs_embeds is None:
+            ids = input_ids.to(self.device)
+            if ids.shape[1] != 1:
+                raise NotImplementedError("a cached step decodes one token per sequence (got %d)" % ids.shape[1])
+            inputs_embeds = torch.nn.functional.embedding(ids, self.model.embed_tokens.weight)
+            attention_mask = None
         if inputs_embeds is None:
             (_, position_ids, attention_mask, _, inputs_embeds, labels) = self.prepare_inputs_labels_for_multimodal(
                 input_ids, position_ids, attention_mask, None, labels, images, tower_features=tower_features, plan=plan)
@@ -142,7 +155,7 @@ class LlavaQwenForCausalLMBase(nn.Module, LlavaMetaForCausalLM):
                 if labels is not None:
                     labels = labels.to(self.device)
         hidden, l_auxes, records = self.model(inputs_embeds, attention_mask, position_ids, moe_noise=moe_noise,
-                                              training_moe=self.training)
+                                              training_moe=self.training, cache=cache)
         if hasattr(attention_mask, "mask"):
             attention_mask = attention_mask.mask
         return dict(hidden=hidden, labels=labels, attention_mask=attention_mask, l_aux=l_auxes, records=records)
@@ -166,9 +179,19 @@ class LlavaQwenForCausalLMBase(nn.Module, LlavaMetaForCausalLM):
     def forward(self, input_ids=None, attention_mask=None, position_ids=None, past_key_values=None, inputs_embeds=None,
                 labels=None, use_cache=None, output_attentions=None, output_hidden_states=None, images=None,
                 return_dict=None, moe_noise=None):
+        cache = None
         if past_key_values is not None or use_cache:
-            raise NotImplementedError("KV-cache generation is outside the distillation hot path (SURVEY.md N4)")
-        r = self.forward_hidden(input_ids, attention_mask, position_ids, inputs_embeds, labels, images, moe_noise)
+            # KV-cache path (modeling_qwen2.py:1110-1217 with past_key_values; llava_arch.py:162-172 for the cached multimodal step).
+            # Without a cache one is allocated for the prompt plus CACHE_ROOM positions; pass new_kv_cache(B, max_len) for longer runs.
+            if past_key_values is not None and not isinstance(past_key_values, KVCache):
+                raise NotImplementedError("past_key_values must be the KVCache this model returned (or new_kv_cache made)")
+            if labels is not None:
+                raise NotImplementedError("labels with a KV cache: the cached path is for decoding")
+            cache = past_key_values
+            if cache is None:
+                n = inputs_embeds.shape[1] if inputs_embeds is not None else self.spliced_length(input_ids, images)
+                cache = self.new_kv_cache(input_ids.shape[0] if input_ids is not None else inputs_embeds.shape[0], n + CACHE_ROOM)
+        r = self.forward_hidden(input_ids, attention_mask, position_ids, inputs_embeds, labels, images, moe_noise, cache=cache)
         hidden, labels = r["hidden"], r["labels"]
         B, T, H = hidden.shape
         logits_lp = K.linear(hidden.reshape(B * T, H), self.lm_head.weight, None, self.lm_head_grad, None).view(B, T, -1)
@@ -181,8 +204,14 @@ class LlavaQwenForCausalLMBase(nn.Module, LlavaMetaForCausalLM):
         logits = logits_lp.float()                                            # reference returns fp32 logits (:408)
         if self.is_moe:
             return MoECausalLMOutputWithPast(loss=loss, moe_loss=moe_loss, logits=logits, labels=labels,
-                                             moe_loss_list=tuple(r["l_aux"]))
-        return CausalLMOutputWithPast(loss=loss, logits=logits, labels=labels)
+                                             moe_loss_list=tuple(r["l_aux"]), past_key_values=cache)
+        return CausalLMOutputWithPast(loss=loss, logits=logits, labels=labels, past_key_values=cache)
+
+    def spliced_length(self, input_ids, images=None):
+        """Length of the decoder input of unpadded prompts: every image placeholder becomes the tower's patch count."""
+        tower = self.get_image_tower()
+        n_img = int((input_ids[0] == IMAGE_TOKEN_INDEX).sum()) if images is not None and tower is not None else 0
+        return input_ids.shape[1] + n_img * (tower.num_patches - 1)
 
 
 

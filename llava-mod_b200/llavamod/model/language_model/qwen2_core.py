@@ -256,12 +256,20 @@ class Qwen2Model(nn.Module):
         return self.grad_views.get(id(t))
 
     # -- forward -------------------------------------------------------------------------------------
-    def forward(self, inputs_embeds, attention_mask=None, position_ids=None, moe_noise=None, training_moe=True):
+    def forward(self, inputs_embeds, attention_mask=None, position_ids=None, moe_noise=None, training_moe=True, cache=None):
         """inputs_embeds [B,T,H] bf16; attention_mask [B,T] bool or None; position_ids [B,T] int64 or None.
+        cache: a KVCache.  Empty: the prefill -- this forward, plus the K / V of every layer appended to the cache.  Holding a prefix and
+        T == 1: one decode step at position len (modeling_qwen2.py:652-728 with past_key_value), attention over the cached keys.
         Returns (final-normed hidden [B,T,H], [l_aux per MoE layer], routing records)."""
+        if cache is not None and cache.length > 0:
+            return self._decode_step(inputs_embeds, moe_noise, training_moe, cache)
         cfg = self.config
         B, T, H = inputs_embeds.shape
         dev = inputs_embeds.device
+        if cache is not None:
+            if attention_mask is not None and not bool(attention_mask.all()):
+                raise NotImplementedError("KV-cache prefill of padded prompts: decode equal-length, unpadded prompts")
+            cache.check(B, T)
         if position_ids is None:
             position_ids = torch.arange(T, device=dev, dtype=torch.int64).unsqueeze(0).expand(B, T)
         pos = position_ids.reshape(-1).to(torch.int64).contiguous()
@@ -281,7 +289,7 @@ class Qwen2Model(nn.Module):
             moes = [l.mlp for l in self.layers if isinstance(l.mlp, MoE)]
             if moes and len({m.num_experts for m in moes}) == 1:
                 moe_noise = gumbel_noise((len(moes), B * T, moes[0].num_experts), dev).unbind(0)
-        for layer in self.layers:
+        for li, layer in enumerate(self.layers):
             at = layer.self_attn
             nh, nkv, hd = at.num_heads, at.num_key_value_heads, at.head_dim
             if branch is None:
@@ -289,6 +297,8 @@ class Qwen2Model(nn.Module):
             else:
                 x, stream = K.rmsnorm(branch, layer.input_layernorm.weight, cfg.rms_norm_eps, res=stream, wgrad=self.gview(layer.input_layernorm.weight))
             qkv = K.qkv_rope(x, at.qkv_weight, at.qkv_bias, cos, sin, pos, nh, nkv, hd, self.gview(at.qkv_weight), self.gview(at.qkv_bias))
+            if cache is not None:
+                K.kv_append(qkv, B, T, nh, nkv, hd, cache.k[li], cache.v[li], cache.len)
             attn = K.attention(qkv, B, T, nh, nkv, hd, True, None, pad)
             if K.residual_fusable(attn, stream, self.gview(at.o_proj.weight), self.gview(layer.post_attention_layernorm.weight)):
                 # frozen / no-grad forward: o_proj's epilogue writes residual + branch (modeling_qwen2.py:796), the norm reads one tensor
@@ -325,7 +335,114 @@ class Qwen2Model(nn.Module):
             out, _ = K.rmsnorm(stream, self.norm.weight, cfg.rms_norm_eps, wgrad=self.gview(self.norm.weight))
         else:
             out, _ = K.rmsnorm(branch, self.norm.weight, cfg.rms_norm_eps, res=stream, wgrad=self.gview(self.norm.weight))
+        if cache is not None:
+            cache.len.add_(T)
+            cache.length += T
         return out.view(B, T, H), l_auxes, records
+
+    def _decode_step(self, inputs_embeds, moe_noise, training_moe, cache):
+        """One cached step: each sequence's new token sits at position len[b] (the reference's rule for a cached step,
+        llava_arch.py:162-172, on unpadded prompts), its k / v are appended at row len[b], and its query attends to rows [0, len[b] + 1).
+        Everything the step reads about the position is on the device, so the step can be captured once and replayed.  MoE layers route
+        the B new tokens alone (top2gating with S = B, as MoEQwen1_5Model_forward does with a cache, llava_qwen1_5_moe.py:223-236).
+        The layer body is forward's no-grad layer body with the attention swapped for append + decode attention: the same norm and
+        residual-fusion choices, the same MoE call and final norm.  A change to one loop must be made to the other;
+        tests/test_decode_gpu.py checks that the two give the same K / V, bit for bit."""
+        cfg = self.config
+        B, T, H = inputs_embeds.shape
+        if T != 1:
+            raise NotImplementedError("a cached step decodes one token per sequence (got %d)" % T)
+        cache.check(B, 1)
+        dev = inputs_embeds.device
+        cos, sin = cache.rope
+        torch.add(cache.len, 1, out=cache.end)
+        cache.pos.copy_(cache.len)
+        stream = inputs_embeds.reshape(B, H)
+        branch = None
+        l_auxes, records = [], []
+        moe_i = 0
+        for li, layer in enumerate(self.layers):
+            at = layer.self_attn
+            nh, nkv, hd = at.num_heads, at.num_key_value_heads, at.head_dim
+            if branch is None:
+                x, stream = K.rmsnorm(stream, layer.input_layernorm.weight, cfg.rms_norm_eps)
+            else:
+                x, stream = K.rmsnorm(branch, layer.input_layernorm.weight, cfg.rms_norm_eps, res=stream)
+            qkv = K.qkv_rope(x, at.qkv_weight, at.qkv_bias, cos, sin, cache.pos, nh, nkv, hd)
+            K.kv_append(qkv, B, 1, nh, nkv, hd, cache.k[li], cache.v[li], cache.len)
+            attn, _ = K.attn_decode(qkv, nh, nkv, hd, cache.k[li], cache.v[li], cache.end, cache.ws)
+            if K.residual_fusable(attn, stream):
+                stream = K.gemm_residual(attn, at.o_proj.weight, None, stream)
+                x, stream = K.rmsnorm(stream, layer.post_attention_layernorm.weight, cfg.rms_norm_eps)
+            else:
+                branch = K.linear(attn, at.o_proj.weight)
+                x, stream = K.rmsnorm(branch, layer.post_attention_layernorm.weight, cfg.rms_norm_eps, res=stream)
+            mlp = layer.mlp
+            if isinstance(mlp, MoE):
+                ds = mlp.deepspeed_moe
+                noise = moe_noise[moe_i] if moe_noise is not None else gumbel_noise((B, mlp.num_experts), dev)
+                moe_i += 1
+                cf = mlp.capacity_factor if training_moe else mlp.eval_capacity_factor
+                stream, l_aux, rec = K.moe_forward_nograd(x, stream, ds.gate.wg.weight, ds.experts.gu_weight, ds.experts.dn_weight, noise,
+                                                          cf, mlp.min_capacity)
+                records.append(rec)
+                l_auxes.append(l_aux)
+                branch = None
+            elif K.residual_fusable(x, stream):
+                stream = K.mlp(x, mlp.gu_weight, mlp.down_proj.weight, res=stream)
+                branch = None
+            else:
+                branch = K.mlp(x, mlp.gu_weight, mlp.down_proj.weight)
+        if branch is None:
+            out, _ = K.rmsnorm(stream, self.norm.weight, cfg.rms_norm_eps)
+        else:
+            out, _ = K.rmsnorm(branch, self.norm.weight, cfg.rms_norm_eps, res=stream)
+        cache.len.copy_(cache.end)
+        cache.length += 1
+        return out.view(B, 1, H), l_auxes, records
+
+
+class KVCache:
+    """Decoding cache of a Qwen2Model for B equal-length sequences of up to max_len positions.
+
+    Per layer one K and one V buffer [B, nkv, max_len, hp] bf16 (HF's legacy layout; hp = the head width the attention kernels run,
+    head dims below 64 zero-padded), the valid length of every sequence on the device (``len`` int32 [B], which the kernels read, so a
+    captured decode step serves every position) and its host mirror ``length``: the host always knows how many rows a forward adds, so
+    every append is bounds-checked without a sync.  ``cache[i]`` gives layer i's (k, v) views [B, nkv, length, hd], the legacy tuple layout
+    llava_arch.py:165 indexes.  The RoPE tables cover max_len at allocation, so nothing is rebuilt inside a captured step."""
+
+    def __init__(self, model, batch, max_len):
+        cfg = model.config
+        w = model.embed_tokens.weight
+        dev, dt = w.device, w.dtype
+        nh, nkv = cfg.num_attention_heads, cfg.num_key_value_heads
+        self.head_dim = cfg.hidden_size // nh
+        hp = K.attn_head_dim(self.head_dim)
+        self.batch, self.max_len = int(batch), int(max_len)
+        self.k = [torch.empty(batch, nkv, max_len, hp, device=dev, dtype=dt) for _ in model.layers]
+        self.v = [torch.empty(batch, nkv, max_len, hp, device=dev, dtype=dt) for _ in model.layers]
+        self.len = torch.zeros(batch, dtype=torch.int32, device=dev)
+        self.end = torch.zeros(batch, dtype=torch.int32, device=dev)          # len + 1 during a decode step
+        self.pos = torch.zeros(batch, dtype=torch.int64, device=dev)          # RoPE positions of a decode step
+        self.ws = torch.empty(max(1, K.attn_decode_ws_elems(batch, nh, nkv, self.head_dim, max_len)), dtype=torch.float32, device=dev)
+        self.rope = model.rope(max_len, dev, dt)
+        self.length = 0
+
+    def check(self, batch, n_new):
+        if batch != self.batch:
+            raise ValueError("KVCache holds %d sequences, got a batch of %d" % (self.batch, batch))
+        if self.length + n_new > self.max_len:
+            raise ValueError("KVCache is full: %d cached + %d new positions > max_len %d" % (self.length, n_new, self.max_len))
+
+    def get_seq_length(self, layer_idx=0):
+        return self.length
+
+    def __len__(self):
+        return len(self.k)
+
+    def __getitem__(self, i):
+        n, hd = self.length, self.head_dim
+        return self.k[i][:, :, :n, :hd], self.v[i][:, :, :n, :hd]
 
 
 def gumbel_noise(shape, device):
