@@ -138,6 +138,22 @@ __device__ __forceinline__ void silu_bwd_store2(float a0, float a1, const __nv_b
   *reinterpret_cast<uint32_t*>(dup) = pack_bf16x2(du[0], du[1]);
 }
 
+// 4 x 4 transpose within each quad of lanes: lane q holds w[j] = word j of its own; afterwards w[j] = word q of lane j (the lane index
+// within the quad is q).  The sender picks the word its receiver needs, so no register is indexed dynamically.
+__device__ __forceinline__ uint32_t pick4(const uint32_t (&w)[4], int i) { return i == 0 ? w[0] : i == 1 ? w[1] : i == 2 ? w[2] : w[3]; }
+__device__ __forceinline__ void quad_transpose(uint32_t (&w)[4], int q) {
+  uint32_t o[4];
+#pragma unroll
+  for (int r = 0; r < 4; ++r) {
+    const int s = (q + r) & 3;                               // lane s sends its word q, chosen there as word (s - r) & 3
+    const uint32_t v = r == 0 ? pick4(w, q) : __shfl_sync(0xffffffffu, pick4(w, (q - r) & 3), s, 4);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) o[j] = (j == s) ? v : (r == 0 ? 0u : o[j]);
+  }
+#pragma unroll
+  for (int j = 0; j < 4; ++j) w[j] = o[j];
+}
+
 // tile index -> coordinates.  Dense: M fastest (consecutive CTAs share the B tile in L2).  Grouped forward/dgrad: per-group row
 // ranges [offsets[g], offsets[g+1]) (128-row aligned by the router), B rows offset by g*b_group_rows.  Grouped wgrad: each group owns
 // the reduction range [offsets[g], offsets[g+1]) and its own D.
@@ -289,6 +305,30 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_consta
           __nv_bfloat16* h1row = p.H1 ? p.H1 + (int64_t)row * p.ld_h1 : nullptr;
           swiglu_store2(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1], acc[4 * (i + 16) + 2 * h], acc[4 * (i + 16) + 2 * h + 1], drow + col,
                         h1row ? h1row + col : nullptr, h1row ? h1row + p.swiglu_I + col : nullptr);
+        }
+      }
+      continue;
+    }
+    if (!p.rope_cos && !p.silu_bwd && !p.D32 && !p.beta && !p.R && !p.dbg_nostore && (reinterpret_cast<uintptr_t>(p.D) & 15) == 0) {
+      // plain bf16 output (+bias): the four lanes of a quad trade their packed column pairs so that each stores one 16-byte block of
+      // 8 columns -- a quad writes 64 contiguous bytes of a row per instruction instead of 16, with a quarter of the store instructions
+      const int q = lane & 3;
+#pragma unroll
+      for (int k = 0; k < BN / 32; ++k) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          uint32_t wd[4];
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+            const int col = t.n0 + 8 * (4 * k + j) + cq;
+            float f0 = empty_k ? 0.f : acc[4 * (4 * k + j) + 2 * h], f1 = empty_k ? 0.f : acc[4 * (4 * k + j) + 2 * h + 1];
+            if (p.bias && col < p.N) bias2(p.bias + col, f0, f1);
+            wd[j] = pack_bf16x2(f0, f1);
+          }
+          quad_transpose(wd, q);
+          const int row = row0 + 8 * h, col8 = t.n0 + 8 * (4 * k + q);
+          if (row < t.m_end && col8 < p.N)                 // N % 8 == 0: a block of 8 columns is in or out as a whole
+            *reinterpret_cast<uint4*>(p.D + goff + (int64_t)row * p.ldd + col8) = make_uint4(wd[0], wd[1], wd[2], wd[3]);
         }
       }
       continue;

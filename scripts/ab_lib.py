@@ -8,8 +8,9 @@ An arm is NAME=LIB[,VAR=VALUE...]: the library is copied over llavamod/liblmod_b
 the end), and the variables are set in the arm's child processes.  Build each library beforehand with llava-mod_b200/build_ext.py from
 the sources it stands for, and keep it in an ignored directory (ab_libs/).  For every arm the script
 
-  * runs the GEMM in every epilogue form at the teacher's shapes, the grouped expert GEMM and the attention forward (hd 64 / 128,
-    causal and padded) on seeded inputs, writes the outputs as .npy and times each call with CUDA events;
+  * runs the GEMM in every epilogue form at the teacher's shapes (and the teacher lm_head on 1229 compact rows), the grouped expert
+    GEMM and the attention forward (hd 64 / 128, causal and padded) on seeded inputs, writes the outputs as .npy and times each call
+    with CUDA events, next to the same dense product through torch.mm (`<case>_torch_mm`);
   * runs `bench.py --no-secondary --no-cpu-baseline` --runs times, the arms alternating, the first run also with --dump-outputs;
   * for the arms named in --detail: with --reports the GEMM and attention throughput reports of the test suite and one
     `bench.py --torch-profile` run, with --full one `bench.py --no-cpu-baseline` run (the headline and configs 3, 4 and 5).
@@ -49,14 +50,7 @@ def dump_kernels(out_dir):
     def rnd(*shape, scale=1.0):
         return (torch.randn(*shape, device=dev, generator=g) * scale).to(torch.bfloat16)
 
-    def case(name, fn, dump=True):
-        out = fn()
-        torch.cuda.synchronize()
-        outs = out if isinstance(out, tuple) else (out,)
-        for i, o in enumerate(x for x in outs if x is not None and dump):
-            a = o.detach().contiguous().cpu()
-            a = a.view(torch.int16).numpy() if a.dtype == torch.bfloat16 else a.numpy()
-            np.save(os.path.join(out_dir, "%s%s.npy" % (name, "" if i == 0 else "_%d" % i)), a)
+    def timed(fn):
         for _ in range(2):
             fn()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -65,7 +59,20 @@ def dump_kernels(out_dir):
             fn()
         e1.record()
         torch.cuda.synchronize()
-        times[name] = e0.elapsed_time(e1) / 10
+        return e0.elapsed_time(e1) / 10
+
+    def case(name, fn, dump=True, mm=None):
+        """mm: the same product through torch.mm (cuBLAS), timed as name + "_torch_mm" for the fraction of cuBLAS"""
+        out = fn()
+        torch.cuda.synchronize()
+        outs = out if isinstance(out, tuple) else (out,)
+        for i, o in enumerate(x for x in outs if x is not None and dump):
+            a = o.detach().contiguous().cpu()
+            a = a.view(torch.int16).numpy() if a.dtype == torch.bfloat16 else a.numpy()
+            np.save(os.path.join(out_dir, "%s%s.npy" % (name, "" if i == 0 else "_%d" % i)), a)
+        times[name] = timed(fn)
+        if mm is not None:
+            times[name + "_torch_mm"] = timed(mm)
 
     M = 2048
     # teacher (qwen1.5-7b): H 4096, I 11008, 32 heads of 128
@@ -79,25 +86,38 @@ def dump_kernels(out_dir):
     res, act = rnd(M, H), rnd(M, I)
     dy, h1 = rnd(M, H), rnd(M, 2 * I)
     with torch.no_grad():
-        case("teacher_plain_MxNxK_2048x4096x4096", lambda: K.gemm(x, w_o))
-        case("teacher_bias_2048x12288x4096", lambda: K.gemm(x, w_qkv, bias=b_qkv))
+        case("teacher_plain_MxNxK_2048x4096x4096", lambda: K.gemm(x, w_o), mm=lambda: torch.mm(x, w_o.t()))
+        case("teacher_bias_2048x12288x4096", lambda: K.gemm(x, w_qkv, bias=b_qkv), mm=lambda: torch.mm(x, w_qkv.t()))
         case("teacher_qkv_rope_2048x12288x4096", lambda: K.qkv_rope(x, w_qkv, b_qkv, cos, sin, pos, nh, nh, hd))
-        case("teacher_swiglu_2048x22016x4096", lambda: K.gemm_swiglu(x, w_gu, True))
+        case("teacher_swiglu_2048x22016x4096", lambda: K.gemm_swiglu(x, w_gu, True), mm=lambda: torch.mm(x, w_gu.t()))
         case("teacher_residual_2048x4096x11008", lambda: K.gemm_residual(act, w_dn, None, res))
-        case("teacher_down_2048x4096x11008", lambda: K.gemm(act, w_dn))
-        case("teacher_silu_bwd_2048x11008x4096", lambda: K.gemm_silu_bwd(dy, w_dn, h1))
-        case("teacher_dgrad_2048x4096x4096", lambda: K.mm_nn(dy, w_o))
-        case("teacher_wgrad_4096x4096x2048", lambda: K.gemm(dy, x, a_mn=True, b_mn=True))
+        case("teacher_down_2048x4096x11008", lambda: K.gemm(act, w_dn), mm=lambda: torch.mm(act, w_dn.t()))
+        case("teacher_silu_bwd_2048x11008x4096", lambda: K.gemm_silu_bwd(dy, w_dn, h1), mm=lambda: torch.mm(dy, w_dn))
+        case("teacher_dgrad_2048x4096x4096", lambda: K.mm_nn(dy, w_o), mm=lambda: torch.mm(dy, w_o))
+        case("teacher_wgrad_4096x4096x2048", lambda: K.gemm(dy, x, a_mn=True, b_mn=True), mm=lambda: torch.mm(dy.t(), x))
+        # a ragged M: an odd number of 128-row tiles, the last one partial
+        case("odd_m_tiles_1282x4096x4096", lambda: K.gemm(x[:1282], w_o), mm=lambda: torch.mm(x[:1282], w_o.t()))
+        # teacher lm_head on the supervised rows of a compact batch: 1229 of 2048 rows, row count read from device memory
+        w_lmt = rnd(151936, H, scale=0.02)
+        cnt = torch.tensor([1229], device=dev, dtype=torch.int32)
+        lm_out = torch.zeros(M, 151936, device=dev, dtype=torch.bfloat16)
+        case("teacher_lm_head_1229x151936x4096", lambda: K.gemm(x, w_lmt, out=lm_out, m_dev=cnt), dump=False,
+             mm=lambda: torch.mm(x[:1229], w_lmt.t()))
+        # the full output is 622 MB: the first rows and the last supervised ones are compared
+        np.save(os.path.join(out_dir, "teacher_lm_head_rows_0_64.npy"), lm_out[:64].cpu().view(torch.int16).numpy())
+        np.save(os.path.join(out_dir, "teacher_lm_head_rows_1165_1229.npy"), lm_out[1165:1229].cpu().view(torch.int16).numpy())
+        del w_lmt, lm_out
         # student (qwen1.5-0.5b): H 1024, I 2816, 16 heads of 64; the experts' grouped GEMM on 4 groups of compact rows
         Hs, Is = 1024, 2816
         xs, w_s, w_gus = rnd(M, Hs), rnd(3 * Hs, Hs, scale=Hs ** -0.5), rnd(2 * Is, Hs, scale=Hs ** -0.5)
         dys = rnd(M, 3 * Hs)
-        case("student_plain_2048x3072x1024", lambda: K.gemm(xs, w_s))
-        case("student_plain_2048x1024x1024", lambda: K.gemm(xs, w_s[:Hs]))
-        case("student_swiglu_2048x5632x1024", lambda: K.gemm_swiglu(xs, w_gus, True))
-        case("student_wgrad_3072x1024x2048", lambda: K.gemm(dys, xs, a_mn=True, b_mn=True))
+        case("student_plain_2048x3072x1024", lambda: K.gemm(xs, w_s), mm=lambda: torch.mm(xs, w_s.t()))
+        case("student_plain_2048x1024x1024", lambda: K.gemm(xs, w_s[:Hs]), mm=lambda: torch.mm(xs, w_s[:Hs].t()))
+        case("student_swiglu_2048x5632x1024", lambda: K.gemm_swiglu(xs, w_gus, True), mm=lambda: torch.mm(xs, w_gus.t()))
+        case("student_wgrad_3072x1024x2048", lambda: K.gemm(dys, xs, a_mn=True, b_mn=True), mm=lambda: torch.mm(dys.t(), xs))
         w_lm = rnd(151936, Hs, scale=0.02)
-        case("student_lm_head_2048x151936x1024", lambda: K.gemm(xs, w_lm), dump=False)    # timed only: a 622 MB output
+        case("student_lm_head_2048x151936x1024", lambda: K.gemm(xs, w_lm), dump=False,    # timed only: a 622 MB output
+             mm=lambda: torch.mm(xs, w_lm.t()))
         del w_lm
         E, R = 4, 4096
         offsets = torch.tensor([0, 1152, 2048, 3200, 4096], device=dev, dtype=torch.int32)
