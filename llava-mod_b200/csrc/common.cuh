@@ -160,11 +160,6 @@ __device__ __forceinline__ uint32_t cluster_ctarank() {
   asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
   return r;
 }
-__device__ __forceinline__ uint32_t cluster_nctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_nctarank;" : "=r"(r));
-  return r;
-}
 __device__ __forceinline__ uint32_t cluster_id_x() {
   uint32_t r;
   asm volatile("mov.u32 %0, %%clusterid.x;" : "=r"(r));
@@ -182,11 +177,3 @@ __device__ __forceinline__ void cluster_wait() {
   asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
 __device__ __forceinline__ void cluster_sync_all() { cluster_arrive(); cluster_wait(); }
-// read a float from the same shared-memory offset in CTA `rank` of this cluster (DSMEM)
-__device__ __forceinline__ float dsmem_ld_f32(const float* local_ptr, uint32_t rank) {
-  uint32_t a = smem_u32(local_ptr), ra;
-  float v;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra) : "r"(a), "r"(rank));
-  asm volatile("ld.shared::cluster.f32 %0, [%1];" : "=f"(v) : "r"(ra) : "memory");
-  return v;
-}

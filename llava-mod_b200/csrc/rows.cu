@@ -14,7 +14,7 @@
 
 namespace {
 
-// active(row) = KD mask || CE mask, the same predicate kl_fused_kernel evaluates: labels[row] != -100 (or distill_all) ||
+// active(row) = KD mask || CE mask, the same predicate kl_stream_kernel evaluates: labels[row] != -100 (or distill_all) ||
 // (row is not the last of its sequence && labels[row+1] != -100)
 __global__ void __launch_bounds__(1024) active_rows_kernel(const int64_t* __restrict__ labels, int64_t n, int64_t T, int distill_all,
                                                           int32_t* __restrict__ perm, int32_t* __restrict__ count) {

@@ -9,8 +9,8 @@ the end), and the variables are set in the arm's child processes.  Build each li
 the sources it stands for, and keep it in an ignored directory (ab_libs/).  For every arm the script
 
   * runs the GEMM in every epilogue form at the teacher's shapes (and the teacher lm_head on 1229 compact rows), the grouped expert
-    GEMM and the attention forward (hd 64 / 128, causal and padded) on seeded inputs, writes the outputs as .npy and times each call
-    with CUDA events, next to the same dense product through torch.mm (`<case>_torch_mm`);
+    GEMM, the attention forward (hd 64 / 128, causal and padded) and the KL + CE loss head (dense and compact rows) on seeded inputs,
+    writes the outputs as .npy and times each call with CUDA events, next to the same dense product through torch.mm (`<case>_torch_mm`);
   * runs `bench.py --no-secondary --no-cpu-baseline` --runs times, the arms alternating, the first run also with --dump-outputs;
   * for the arms named in --detail: with --reports the GEMM and attention throughput reports of the test suite and one
     `bench.py --torch-profile` run, with --full one `bench.py --no-cpu-baseline` run (the headline and configs 3, 4 and 5).
@@ -37,6 +37,23 @@ LIB = os.path.join(PKG, "llavamod", "liblmod_b200.so")
 # ---------------------------------------------------------------------------------------------------------------------------------
 # child: seeded kernel outputs of one library
 # ---------------------------------------------------------------------------------------------------------------------------------
+def kl_labels(n, T, V, prompt, seed=0):
+    """Labels of n rows in sequences of T: an ignored prompt, then labelled and ignored runs of mixed lengths, so that the loss head
+    meets KD-only rows (next label ignored or sequence end), CE-only rows (own label ignored, next one set) and inactive rows."""
+    import torch
+    g = torch.Generator().manual_seed(seed)
+    lab = torch.randint(0, V, (n,), generator=g)
+    for b in range(0, n, T):
+        lab[b:b + prompt] = -100
+        i, on = b + prompt, True
+        while i < b + T:
+            k = int(torch.randint(1, 9 if on else 5, (1,), generator=g))
+            if not on:
+                lab[i:i + k] = -100
+            i, on = i + k, not on
+    return lab
+
+
 def dump_kernels(out_dir):
     import numpy as np
     import torch
@@ -138,6 +155,27 @@ def dump_kernels(out_dir):
             lo = torch.tensor([0, 300], device=dev, dtype=torch.int32)
             hi = torch.tensor([M, M], device=dev, dtype=torch.int32)
             case("attn_fwd_hd%d_padded" % hdx, lambda: K.attention_fwd(qkv2, 2, M, nhx, nhx, hdx, True, need_lse=True, pad=(lo, hi)))
+        # loss head (KL + CE) over the full vocabulary, dense on all 2048 rows and compact on the 1229 active ones (active_rows +
+        # gather_rows).  out4 and row_out are dumped (the compact call leaves row_out of inactive rows unwritten: active rows only), the
+        # 622 MB dlogits by its SHA-256
+        V, T = 151936, 512
+        lab = kl_labels(M, T, V, prompt=114).to(dev)
+        s_l, t_l = rnd(M, V, scale=3.0), rnd(M, V, scale=3.0)
+        perm, cnt = K.active_rows(lab, T)
+        assert int(cnt) == 1229, int(cnt)
+        active = perm[:1229].long()
+        s_c, t_c = K.gather_rows(s_l, perm, cnt), K.gather_rows(t_l, perm, cnt)
+        for form, s_x, t_x, rows in (("dense_2048", s_l, t_l, None), ("compact_1229", s_c, t_c, (perm, cnt))):
+            d_x = torch.zeros_like(s_x)
+            for w_ce in (1.0, 0.0):
+                name = "kl_%s_x151936_wce%d" % (form, w_ce)
+                fn = lambda: K.kl_fused(s_x, t_x, lab, T, V, 1.0, w_ce, False, dlogits=d_x, rows=rows)   # noqa: E731
+                out4, row_out = fn()
+                np.save(os.path.join(out_dir, name + "_out4.npy"), out4.cpu().numpy())
+                np.save(os.path.join(out_dir, name + "_row_out.npy"), (row_out if rows is None else row_out[active]).cpu().numpy())
+                digest = hashlib.sha256(d_x.cpu().view(torch.int16).numpy().tobytes()).digest()
+                np.save(os.path.join(out_dir, name + "_dlogits_sha256.npy"), np.frombuffer(digest, dtype=np.uint8))
+                case(name, fn, dump=False)
     with open(os.path.join(out_dir, "times_ms.json"), "w") as f:
         json.dump(times, f, indent=1)
 

@@ -148,8 +148,8 @@ def kl_reference_fp64(s, t, labels, T, V, w_kd, w_ce, distill_all=False, g_dtype
 #                lse_S itself: max + lg2(Z)*ln2 rounded to fp32 (half ulp at 64..128 = 3.8e-6) + the fp32 sum Z (~1e-6)   ~4.8e-6
 #                -lse_S*log2e rounded (|.| < 256: half ulp 7.6e-6 in log2 units, x ln2)                                         5.3e-6
 #                the fma s*log2e + (-lse_S*log2e) rounded (|.| < 128: 3.8e-6 x ln2)                                             2.6e-6
-#                ex2.approx (2^-22.5) / the degree-4 polynomial of the LMOD_KL_POLY arm (3.7e-6)                                <= 3.7e-6
-#              sum 1.6e-5.  The fp32 roundings of -cb*p and of the fma ca*q + (-cb*p) add at most 2^-23 (ca q + cb p), i.e. 1.2e-7 to eps;
+#                ex2.approx (2^-22.5)                                                                                           1.7e-7
+#              sum 1.3e-5.  The fp32 roundings of -cb*p and of the fma ca*q + (-cb*p) add at most 2^-23 (ca q + cb p), i.e. 1.2e-7 to eps;
 #              all of it rounded up to 2e-5.
 #   2^-126     ex2.approx.ftz flushes results below the smallest normal fp32 to zero.
 KL_GRAD_EPS = 2e-5

@@ -1,6 +1,6 @@
 """The loss head at full vocabulary, element by element: the streaming KL+CE kernel (csrc/kl.cu kl_stream_kernel) with many rows per
-cluster, its numeric edges and its documented variants against the float64 reference of tests/helpers.py, and the split-K lm_head dgrad
-(kernels.mm_nn) against a float64 GEMM.
+cluster and its numeric edges against the float64 reference of tests/helpers.py, the kernel as the only one kl.cu builds, and the split-K
+lm_head dgrad (kernels.mm_nn) against a float64 GEMM.
 
 The stream kernel gives each cluster of two CTAs the rows cid, cid + ncl, ... (ncl = co-resident clusters, ~66 on an H100), and carries
 its ring stage / phase counters, the held pass-1 chunks and the alternating exchange slot from one active row to the next; a test with
@@ -8,8 +8,10 @@ fewer rows than clusters sees one row per cluster and none of that state.  Every
 
 Bounds (derived in tests/helpers.py): dlogits |g_k - g| <= 2^-8 |g| + 2e-5 (ca q + cb p); row_out lse / nll within 1e-5 + 2e-6 |lse|,
 x within 2e-5 |x| + 1e-5; the loss scalars within 2e-5 relative."""
+import importlib.util
 import os
 import re
+import shutil
 import subprocess
 import sys
 
@@ -165,12 +167,12 @@ def test_many_row_tests_give_every_cluster_several_rows():
               "s = torch.zeros(4, 1024, dtype=torch.bfloat16, device='cuda')\n"
               "K.kl_fused(s, s, torch.arange(4, device='cuda'), 4, 1024, 1.0, 1.0, dlogits=torch.empty_like(s))\n"
               "torch.cuda.synchronize()\n", {"LMOD_KL_VERBOSE": "1"})
-    m = re.search(r"kl_stream_kernel<[^>]*>: cluster (\d+), \d+ B smem, (\d+) co-resident clusters", r.stderr)
+    m = re.search(r"kl_stream_kernel: cluster (\d+), \d+ B smem, (\d+) co-resident clusters", r.stderr)
     assert m, r.stderr
     cs, ncl = int(m.group(1)), int(m.group(2))
     assert cs == 2 and ncl > 0
     assert N_MANY >= 3 * ncl, (N_MANY, ncl)
-    assert VARIANT_N >= 3 * ncl                                # the variant tests and the 600-row compact case of test_rows_gpu
+    assert SWITCH_N >= 3 * ncl                                 # the removed-switch test and the 600-row compact case of test_rows_gpu
 
 
 # V and the chunking case it forces: per half of the row (length, chunks, chunks held in the ring into pass 2, chunks re-fetched from L2)
@@ -196,6 +198,20 @@ def test_stream_kernel_many_rows_per_cluster(V, w_ce, distill_all):
     run_and_check(s, t, lab, T_MANY, V, w_ce, distill_all, msg=f"V={V} w_ce={w_ce} distill_all={distill_all}")
 
 
+@pytest.mark.gpu
+def test_largest_accepted_vocab_and_one_vector_more():
+    """KL_MAX_VOCAB (csrc/kl.cu) = 450560 is accepted and computed right (28 chunks per half, 22 of them re-fetched for pass 2); eight
+    logits more are rejected before anything is launched."""
+    from llavamod import _C, kernels as K
+    N, T, V = 300, 100, 450560
+    s, t = make_logits(N, V, seed=V)
+    lab = run_labels(N, T, V, seed=V + 1)
+    run_and_check(s, t, lab, T, V, 1.0, False, msg=f"V={V}")
+    pad = torch.zeros(N, 8, dtype=torch.bfloat16, device="cuda")
+    with pytest.raises(_C.LmodError, match="vocab 450568"):
+        K.kl_fused(torch.cat([s, pad], 1), torch.cat([t, pad], 1), lab.to(dev()), T, V + 8, 1.0, 1.0)
+
+
 def kernel_constant(name):
     src = open(os.path.join(PKG, "csrc", "kl.cu")).read()
     m = re.search(r"constexpr int %s = (\d+);" % name, src)
@@ -218,6 +234,31 @@ def test_vocab_cases_force_their_chunking():
             held = min(stages, nchunks)
             got.append((n, nchunks, held, nchunks - held))
         assert got == halves, (V, got)
+
+
+def test_kl_cu_builds_only_the_stream_kernel(tmp_path):
+    """kl.cu compiled for sm_90a with the build's flags (no GPU needed) holds the loss head's three kernels and no other, and ptxas reports
+    no spills for the stream kernel."""
+    spec = importlib.util.spec_from_file_location("lmod_build_ext", os.path.join(PKG, "build_ext.py"))
+    be = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(be)
+    if not (os.path.isfile(be.NVCC) or shutil.which(be.NVCC)):
+        pytest.skip("nvcc not found at %s (set NVCC): the check compiles kl.cu for sm_90a" % be.NVCC)
+    r = subprocess.run([be.NVCC] + be.FLAGS + ["-c", os.path.join(be.CSRC, "kl.cu"), "-o", str(tmp_path / "kl.o")], capture_output=True,
+                       text=True)
+    assert r.returncode == 0, r.stderr
+    spills, name = {}, None                                    # ptxas -v: per entry function, then its stack frame and spill bytes
+    for ln in (r.stdout + r.stderr).splitlines():
+        m = re.search(r"Compiling entry function '(\S+)'", ln)
+        if m:
+            name = m.group(1)
+            spills[name] = None
+        m = re.search(r"(\d+) bytes spill stores, (\d+) bytes spill loads", ln)
+        if m and name:
+            spills[name] = (int(m.group(1)), int(m.group(2)))
+    kernels = {re.search(r"(kl_[a-z]+_kernel)", k).group(1): v for k, v in spills.items()}
+    assert len(spills) == 3 and sorted(kernels) == ["kl_counts_kernel", "kl_finalize_kernel", "kl_stream_kernel"], sorted(spills)
+    assert kernels["kl_stream_kernel"] == (0, 0), kernels
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -274,23 +315,10 @@ def test_stream_kernel_numeric_edges(target, c):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# the documented A/B variants (README), each in its own process: the kernel reads these variables once into statics
+# one configuration: the environment variables that used to select other loss-head kernels select nothing
 # ---------------------------------------------------------------------------------------------------------------------
-# name: (environment, the launch line the kernel prints under LMOD_KL_VERBOSE=1 for it -- proof that the variant, not the default, ran)
-VARIANTS = {
-    "stream1": ({"LMOD_KL_MODE": "stream1"},         # one CTA per row: the single-CTA exchange (named barrier)
-                r"kl_stream_kernel<0,0,512>: cluster 1, .* keep_tail 1"),
-    "stream4": ({"LMOD_KL_MODE": "stream4"}, r"kl_stream_kernel<0,0,512>: cluster 4, .* keep_tail 1"),
-    "sb128": ({"LMOD_KL_MODE": "sb128"},             # the shared-memory-resident 8-CTA kernel
-              r"kl_fused_kernel<128,1>: cluster 8,"),
-    "keep0": ({"LMOD_KL_KEEP": "0"},                 # nothing held over: pass 2 re-fetches every chunk
-              r"kl_stream_kernel<0,0,512>: cluster 2, .* keep_tail 0"),
-    "poly33": ({"LMOD_KL_POLY": "33"},               # 3/8 of the exponentials by polynomial
-               r"kl_stream_kernel<3,3,512>: cluster 2, .* keep_tail 1"),
-    "threads256": ({"LMOD_KL_THREADS": "256"}, r"kl_stream_kernel<0,0,256>: cluster 2, .* keep_tail 1"),
-    "threads768": ({"LMOD_KL_THREADS": "768"}, r"kl_stream_kernel<0,0,768>: cluster 2, .* keep_tail 1"),
-}
-VARIANT_N, VARIANT_T = 600, 200
+REMOVED_SWITCHES = {"LMOD_KL_MODE": "sb128", "LMOD_KL_POLY": "33", "LMOD_KL_THREADS": "256", "LMOD_KL_KEEP": "0"}
+SWITCH_N, SWITCH_T = 600, 200
 
 CHILD_RUN = """import torch
 from llavamod import kernels as K
@@ -299,37 +327,27 @@ s, t, lab = x["s"].cuda(), x["t"].cuda(), x["lab"].cuda()
 d = torch.empty_like(s)
 out4, row_out = K.kl_fused(s, t, lab, x["T"], x["V"], 1.0, 1.0, False, dlogits=d)
 torch.cuda.synchronize()
-torch.save({"out4": out4.cpu(), "row_out": row_out.cpu(), "d": d.cpu(), "peak": torch.cuda.max_memory_allocated()}, sys.argv[2])
+torch.save({"out4": out4.cpu(), "row_out": row_out.cpu(), "d": d.cpu()}, sys.argv[2])
 """
 
 
-@pytest.fixture(scope="module")
-def variant_inputs(tmp_path_factory):
-    V = V_FULL
-    s, t = make_logits(VARIANT_N, V, seed=23)
-    lab = run_labels(VARIANT_N, VARIANT_T, V, seed=24)
-    path = tmp_path_factory.mktemp("kl_variants") / "inputs.pt"
-    torch.save({"s": s.cpu(), "t": t.cpu(), "lab": lab, "T": VARIANT_T, "V": V}, path)
-    ref = kl_reference_fp64(s, t, lab.to(dev()), VARIANT_T, V, 1.0, 1.0, False, g_dtype=torch.float32)
-    return path, ref, lab
-
-
 @pytest.mark.gpu
-@pytest.mark.parametrize("name", list(VARIANTS))
-def test_stream_kernel_variants(name, variant_inputs, tmp_path):
-    inputs, ref, lab = variant_inputs
-    out = tmp_path / f"{name}.pt"
-    env, launch = VARIANTS[name]
-    r = child(CHILD_RUN, dict(env, LMOD_KL_VERBOSE="1"), inputs, out)
-    assert re.search(launch, r.stderr), (name, r.stderr)
-    got = torch.load(out)
-    print(f"{name}: child peak GPU memory {got['peak'] / 2**30:.2f} GiB")
-    check_out4(got["out4"], ref, name)
-    check_row_out(got["row_out"], ref, name)
-    d = got["d"].to(dev())
-    check_dlogits(d, ref, name)
-    m_kd, m_ce, _ = kl_row_masks(lab, VARIANT_T)
-    assert bool((d[~(m_kd | m_ce).to(dev())] == 0).all()), name
+def test_removed_kl_switches_select_nothing(tmp_path):
+    """With the removed A/B switches set, the same stream kernel runs (its launch line under LMOD_KL_VERBOSE=1) and writes the same bytes
+    as without them.  Each setting runs in a process of its own: a switch read once into a static would not see a change within one."""
+    s, t = make_logits(SWITCH_N, V_FULL, seed=23)
+    lab = run_labels(SWITCH_N, SWITCH_T, V_FULL, seed=24)
+    inputs = tmp_path / "inputs.pt"
+    torch.save({"s": s.cpu(), "t": t.cpu(), "lab": lab, "T": SWITCH_T, "V": V_FULL}, inputs)
+    got = {}
+    for name, env in (("default", {}), ("removed_switches", REMOVED_SWITCHES)):
+        r = child(CHILD_RUN, dict(env, LMOD_KL_VERBOSE="1"), inputs, tmp_path / f"{name}.pt")
+        assert re.search(r"kl_stream_kernel: cluster 2, ", r.stderr), (name, r.stderr)
+        got[name] = torch.load(tmp_path / f"{name}.pt")
+    a, b = got["default"], got["removed_switches"]
+    assert torch.equal(a["out4"].view(torch.int32), b["out4"].view(torch.int32))
+    assert torch.equal(a["row_out"].view(torch.int32), b["row_out"].view(torch.int32))
+    assert torch.equal(a["d"].view(torch.int16), b["d"].view(torch.int16))
 
 
 # ---------------------------------------------------------------------------------------------------------------------
