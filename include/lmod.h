@@ -150,9 +150,12 @@ int lmod_rmsnorm_bwd(const void* dy, const void* x, const void* w, const float* 
  * Only needed when the norm weights train (dense-student distillation, full SFT); the sparse recipes freeze them. */
 int lmod_rmsnorm_wgrad(const void* dy, const void* x, const float* rstd, int64_t rows, int64_t H, float* ws_zeroed, void* wgrad, void* stream);
 
-/* Token-embedding gradient behind the multimodal splice (nn.Embedding backward; llava_arch.py:262-274): for every row with src[row] >= 0,
- * grad[src[row], :] += dout[row, :] (bf16 atomics; rows that hold image patches or padding carry src < 0, as in lmod_splice_embed). */
-int lmod_embed_grad(const void* dout, const int64_t* src, int64_t n_rows, int64_t H, void* grad, void* stream);
+/* Token-embedding gradient behind the multimodal splice (nn.Embedding backward; llava_arch.py:262-274): for every token t,
+ * grad[t, :] = bf16(grad[t, :] + bf16(sum over the rows r with src[r] == t of dout[r, :])), the sum in fp32 in row order, so the result
+ * is deterministic.  Rows that hold image patches or padding carry src < 0, as in lmod_splice_embed, and add nothing.
+ * order [n_rows] int64: the row indices grouped by token, a stable sort of src with the rows src < 0 last (llava_arch.embed_grad_order).
+ * H % 8 == 0; dout and grad 16-byte aligned. */
+int lmod_embed_grad(const void* dout, const int64_t* src, const int64_t* order, int64_t n_rows, int64_t H, void* grad, void* stream);
 int lmod_layernorm_fwd(const void* x, const void* w, const void* b, int64_t rows, int64_t H, float eps,
                        void* y, void* stream);
 /* rotate-half RoPE applied in place to q [rows, nh*hd] and k [rows, nkv*hd] (rows of a fused QKV buffer via ld).

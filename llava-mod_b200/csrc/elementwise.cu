@@ -302,18 +302,35 @@ __global__ void rmsnorm_wgrad_finish_kernel(float* __restrict__ ws, int H, __nv_
   ws[i] = 0.f;                                                   // the workspace is handed back zeroed
 }
 
-// dW of the token embedding (nn.Embedding backward behind the multimodal splice, llava_arch.py:262-274): every text row adds its
-// upstream gradient to the row of its token id; duplicates collide, hence bf16x2 atomics straight into the gradient buffer.
-__global__ void __launch_bounds__(256) embed_grad_kernel(const __nv_bfloat16* __restrict__ dout, const int64_t* __restrict__ src, int64_t n_rows,
-                                                        int H, __nv_bfloat16* __restrict__ grad) {
-  const int64_t row = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int lane = threadIdx.x & 31;
-  if (row >= n_rows) return;
-  const int64_t tok = src[row];
-  if (tok < 0) return;                                           // image-patch row or padding
-  const __nv_bfloat162* from = reinterpret_cast<const __nv_bfloat162*>(dout + row * H);
-  __nv_bfloat162* to = reinterpret_cast<__nv_bfloat162*>(grad + tok * H);
-  for (int i = lane; i < (H >> 1); i += 32) atomicAdd(to + i, from[i]);
+// dW of the token embedding (nn.Embedding backward behind the multimodal splice, llava_arch.py:262-274, then the bf16 accumulation
+// into .grad): grad[t] = bf16(grad[t] + bf16(sum of the rows of token t)).  `order` lists the rows grouped by token id (a stable sort of
+// src with the rows src < 0 last, built on the host with the splice plan).  The CTA at the first row of a token's run sums the run in
+// fp32 in row order and rounds once, like the reference's fp32 backward; each token has one owner, so no atomics and the same bytes
+// on every run.  Rows of image patches and padding (src < 0) add nothing.
+constexpr int EMB_THREADS = 128;
+__global__ void __launch_bounds__(EMB_THREADS) embed_grad_kernel(const __nv_bfloat16* __restrict__ dout, const int64_t* __restrict__ src,
+                                                                const int64_t* __restrict__ order, int64_t n_rows, int H,
+                                                                __nv_bfloat16* __restrict__ grad) {
+  const int64_t i = blockIdx.x;
+  const int64_t tok = src[order[i]];
+  if (tok < 0 || (i > 0 && src[order[i - 1]] == tok)) return;   // padding / image row, or not the first row of its token's run
+  int64_t end = i + 1;
+  while (end < n_rows && src[order[end]] == tok) ++end;
+  uint4* to = reinterpret_cast<uint4*>(grad + tok * H);
+  for (int v = threadIdx.x; v < (H >> 3); v += EMB_THREADS) {
+    float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    for (int64_t j = i; j < end; ++j) {
+      float f[8];
+      unpack8(ldg_nc_v4(reinterpret_cast<const uint4*>(dout + order[j] * H) + v), f);
+#pragma unroll
+      for (int k = 0; k < 8; ++k) acc[k] += f[k];
+    }
+    float g[8];
+    unpack8(to[v], g);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) g[k] += bf16_round(acc[k]);
+    to[v] = pack8(g);
+  }
 }
 
 __device__ __forceinline__ float sigmoidf_(float x) { return 1.f / (1.f + __expf(-x)); }
@@ -473,9 +490,12 @@ extern "C" int lmod_rmsnorm_wgrad(const void* dy, const void* x, const float* rs
   LMOD_LAUNCH_OK();
   return LMOD_OK;
 }
-extern "C" int lmod_embed_grad(const void* dout, const int64_t* src, int64_t n_rows, int64_t H, void* grad, void* stream) {
-  LMOD_CHECK_ARG(dout && src && grad && n_rows > 0 && H > 0 && H % 2 == 0, "lmod_embed_grad: bad arguments");
-  embed_grad_kernel<<<GRID1D(n_rows * 32, 256), 256, 0, (cudaStream_t)stream>>>((const __nv_bfloat16*)dout, src, n_rows, (int)H, (__nv_bfloat16*)grad);
+extern "C" int lmod_embed_grad(const void* dout, const int64_t* src, const int64_t* order, int64_t n_rows, int64_t H, void* grad,
+                               void* stream) {
+  LMOD_CHECK_ARG(dout && src && order && grad && n_rows > 0 && H > 0 && H % 8 == 0 && (uintptr_t)dout % 16 == 0 && (uintptr_t)grad % 16 == 0,
+                 "lmod_embed_grad: bad arguments (H %% 8 == 0, 16-byte aligned buffers required)");
+  embed_grad_kernel<<<(unsigned)n_rows, EMB_THREADS, 0, (cudaStream_t)stream>>>((const __nv_bfloat16*)dout, src, order, n_rows, (int)H,
+                                                                               (__nv_bfloat16*)grad);
   LMOD_LAUNCH_OK();
   return LMOD_OK;
 }

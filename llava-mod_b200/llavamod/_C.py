@@ -41,7 +41,7 @@ SIGNATURES = {
     "lmod_rmsnorm_fwd": [_P, _P, _P, _L, _L, _F, _P, _P, _P, _P],
     "lmod_rmsnorm_bwd": [_P, _P, _P, _P, _P, _L, _L, _P, _P],
     "lmod_rmsnorm_wgrad": [_P, _P, _P, _L, _L, _P, _P, _P],
-    "lmod_embed_grad": [_P, _P, _L, _L, _P, _P],
+    "lmod_embed_grad": [_P, _P, _P, _L, _L, _P, _P],
     "lmod_layernorm_fwd": [_P, _P, _P, _L, _L, _F, _P, _P],
     "lmod_rope": [_P, _L, _I, _P, _L, _I, _I, _P, _P, _P, _L, _I, _P],
     "lmod_silu_mul_fwd": [_P, _L, _L, _L, _P, _P],

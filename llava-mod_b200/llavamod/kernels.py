@@ -722,13 +722,13 @@ def gelu(x):
 # ---------------------------------------------------------------------------------------------------
 class SpliceFn(Function):
     @staticmethod
-    def forward(ctx, feats, embed_w, src, img_index, n_patches, embed_grad=None):
+    def forward(ctx, feats, embed_w, src, img_index, n_patches, embed_grad=None, order=None):
         B, T = src.shape
         H = embed_w.shape[1]
         out = torch.empty(B, T, H, dtype=embed_w.dtype, device=embed_w.device)
         call("lmod_splice_embed", ptr(embed_w), ptr(feats) if feats is not None else None, ptr(src), ptr(img_index),
              B * T, H, n_patches, ptr(out))
-        ctx.save_for_backward(src, img_index)
+        ctx.save_for_backward(src, img_index, order)
         ctx.fshape = feats.shape
         ctx.n_patches = n_patches
         ctx.embed_grad = embed_grad                         # view of the flat gradient buffer when embed_tokens trains
@@ -736,20 +736,30 @@ class SpliceFn(Function):
 
     @staticmethod
     def backward(ctx, d):
-        src, img_index = ctx.saved_tensors
+        src, img_index, order = ctx.saved_tensors
         dfeats = torch.zeros(ctx.fshape, dtype=d.dtype, device=d.device)
         B, T = src.shape
         d = _c(d)
         call("lmod_splice_embed_bwd", ptr(d), ptr(src), ptr(img_index), B * T, d.shape[-1], ctx.n_patches, ptr(dfeats))
         if ctx.embed_grad is not None:
-            call("lmod_embed_grad", ptr(d), ptr(src), B * T, d.shape[-1], ptr(ctx.embed_grad))
-        return dfeats, None, None, None, None, None
+            call("lmod_embed_grad", ptr(d), ptr(src), ptr(order), B * T, d.shape[-1], ptr(ctx.embed_grad))
+        return dfeats, None, None, None, None, None, None
 
 
-def splice_embed(feats, embed_w, src, img_index, n_patches, embed_grad=None):
+def embed_grad_(dout, src, order, grad):
+    """grad[t] = bf16(grad[t] + bf16(sum of the rows of dout whose src is t)) (lmod_embed_grad); order from llava_arch.embed_grad_order."""
+    H = grad.shape[-1]
+    call("lmod_embed_grad", ptr(_c(dout)), ptr(_c(src)), ptr(_c(order)), src.numel(), H, ptr(grad))
+    return grad
+
+
+def splice_embed(feats, embed_w, src, img_index, n_patches, embed_grad=None, order=None):
+    """order (the rows grouped by token, llava_arch.embed_grad_order) is required with embed_grad."""
     feats = _c(feats)
+    if embed_grad is not None and order is None:
+        raise ValueError("splice_embed: the embedding gradient needs the plan's row order (llava_arch.embed_grad_order)")
     if torch.is_grad_enabled() and (feats.requires_grad or embed_grad is not None):
-        return SpliceFn.apply(feats, embed_w, src, img_index, n_patches, embed_grad)
+        return SpliceFn.apply(feats, embed_w, src, img_index, n_patches, embed_grad, order)
     B, T = src.shape
     H = embed_w.shape[1]
     out = torch.empty(B, T, H, dtype=embed_w.dtype, device=embed_w.device)

@@ -65,6 +65,14 @@ def splice_plan(input_ids, attention_mask, labels, n_patches, padding_side="righ
     return src, nl, nm, pos, img
 
 
+def embed_grad_order(src):
+    """Row order of the token-embedding gradient (lmod_embed_grad): the flat indices of ``src`` grouped by token id, in row order within a
+    token (a stable sort), with the image and padding rows (src < 0) last.  Same shape as ``src``."""
+    s = np.asarray(src)
+    key = np.where(s >= 0, s, np.iinfo(np.int64).max).reshape(-1)
+    return np.argsort(key, kind="stable").astype(np.int64).reshape(s.shape)
+
+
 class MaskInfo:
     """Attention mask + the host-side knowledge whether it contains padding, so the decoder never has to ask the device
     (``bool(mask.all())`` would be a host sync and would break CUDA-graph capture)."""
@@ -156,11 +164,15 @@ class LlavaMetaForCausalLM(ABC):
         lb_h = None if labels is None else (labels.cpu().numpy() if torch.is_tensor(labels) else labels)
         side = getattr(self.config, "tokenizer_padding_side", "right")
         src, nl, nm, pos, img = splice_plan(ids_h, am_h, lb_h, n_patches, side, getattr(self.config, "tokenizer_model_max_length", None))
-        host = torch.from_numpy(np.stack([src, nl, pos, img, nm.astype(np.int64)]))
+        core = self.get_model()
+        embed_trains = core.gview(core.embed_tokens.weight) is not None       # the row order is only needed by the embedding gradient
+        parts = [src, nl, pos, img, nm.astype(np.int64)] + ([embed_grad_order(src)] if embed_trains else [])
+        host = torch.from_numpy(np.stack(parts))
         if dev.type == "cuda":
             host = host.pin_memory()
         plan = host.to(dev, non_blocking=True)
         return dict(src=plan[0].contiguous(), labels=plan[1], pos=plan[2], img=plan[3].contiguous(), mask=plan[4].bool(),
+                    order=plan[5] if embed_trains else None,
                     all_true=bool(nm.all()), has_labels=labels is not None, has_mask=attention_mask is not None, n_patches=n_patches)
 
     def prepare_inputs_labels_for_multimodal(self, input_ids, position_ids, attention_mask, past_key_values, labels, images,
@@ -178,7 +190,7 @@ class LlavaMetaForCausalLM(ABC):
             plan = self.make_splice_plan(input_ids, attention_mask, labels, n_patches, dev)
         core = self.get_model()
         embeds = K.splice_embed(feats, core.embed_tokens.weight, plan["src"], plan["img"], n_patches,
-                                embed_grad=core.gview(core.embed_tokens.weight) if torch.is_grad_enabled() else None)
+                                embed_grad=core.gview(core.embed_tokens.weight) if torch.is_grad_enabled() else None, order=plan["order"])
         if not plan["has_mask"]:
             new_mask = None
         else:       # "no padding" is known on the host, the decoder must not sync to find out

@@ -672,6 +672,298 @@ def check_moe(name, got, want, tol=None, report=None, rows=None):
     return worst
 
 
+# ---------------------------------------------------------------------------------------------------
+# norm / rotary / activation / splice / embedding-gradient / optimizer kernels (csrc/elementwise.cu, csrc/optim.cu): float64 references
+# ---------------------------------------------------------------------------------------------------
+# Each reference states the formula of the kernel (include/lmod.h), keeps the bf16 roundings the reference model materialises and computes
+# the rest in float64.  Stages are checked from the kernel's own previous stage (y from the kernel's rstd), so a rounding that flips because
+# of an fp32 input does not need a loose bound.  u = 2^-8 is the unit roundoff of bf16, 2^-24 that of fp32; a bound "u |ref| + (1 + u) E"
+# is the bf16 store of a value the kernel computed in fp32 with error at most E.  A chain of n fp32 additions of terms t (in any order)
+# is off by at most n 2^-24 sum|t|.  Every kernel of these files reduces a row with one CTA of 128 threads: H / 128 terms per thread, then
+# block_sum (5 shuffle levels, a shared-memory hop, 5 more levels), so a row reduction is a chain of at most H / 128 + 11 additions.
+BF16_U = 2.0 ** -8
+FP32_U = 2.0 ** -24
+ELEM_ABS_FLOOR = 2.0 ** -100          # fp32 flushes / __expf overflow (silu(g) = -0 below g = -88.7) move nothing by more than ~2^-120
+
+
+def bf16_of(t):
+    """Round to bf16 the way the kernels do (fp32 value, round to nearest even) and return float64."""
+    return t.float().to(torch.bfloat16).to(torch.float64)
+
+
+def _row_chain(H):
+    return H / 128 + 11
+
+
+def rmsnorm_reference_fp64(x, w, eps, res=None, rstd_k=None):
+    """lmod_rmsnorm_fwd:  s = bf16(x + res) (or x),  rstd = 1 / sqrt(mean(s^2) + eps),  y = bf16(w * bf16(s * rstd)).
+    Returns s (bf16, bit exact), rstd (float64) with rstd_tol, and y (bf16) computed from rstd_k, the kernel's fp32 rstd (the fp32
+    product s * rstd_k rounded to bf16, times w -- exact in fp32 -- rounded again: bit exact), or from float32(rstd) without it.
+      rstd_tol: the sum of squares is a chain of H / 128 + 11 fmas (relative (H/128 + 11) 2^-24, all terms positive), the division by H and
+      the + eps one rounding each, rsqrtf at most 2 ulp (2^-22): relative 0.5 (H/128 + 13) 2^-24 + 2^-22."""
+    s = x if res is None else (x.float() + res.float()).to(torch.bfloat16)
+    H = s.shape[-1]
+    s64 = s.double()
+    rstd = torch.rsqrt((s64 * s64).mean(-1) + eps)
+    rstd_tol = (0.5 * (_row_chain(H) + 2) * FP32_U + 2.0 ** -22) * rstd
+    r32 = (rstd_k if rstd_k is not None else rstd).float()
+    y = (w.float() * (s.float() * r32[..., None]).to(torch.bfloat16).float()).to(torch.bfloat16)
+    return dict(s=s, rstd=rstd, rstd_tol=rstd_tol, y=y)
+
+
+def rmsnorm_bwd_reference_fp64(dy, s, w, rstd_k, dres=None):
+    """lmod_rmsnorm_bwd from the kernel's rstd:  g = dy w,  xhat = s rstd,  dx = rstd (g - xhat mean(g xhat)) (+ dres).
+    The kernel keeps g in fp32; the reference model's autograd rounds it to bf16 first (the weight multiply is a bf16 op).
+      tol:     the fp32 arithmetic.  g and xhat are one product each (2^-24 relative); dot = sum(g xhat) / H is a chain of H/128 + 11 fmas over
+               terms |g xhat| plus the division; xhat dot and the difference, the product by rstd and the + dres are 4 more roundings:
+                 E = 2^-24 (4 rstd |g| + rstd^2 |s| (6 |dot| + (H/128 + 13) sum|g xhat| / H) + |ref|)
+      tol_g:   what the reference model's bf16(dy w) adds on top: |delta g| <= u |g| moves dx by rstd (u |g| + |xhat| mean(u |g xhat|))."""
+    H = s.shape[-1]
+    r = rstd_k.double()[..., None]
+    g = dy.double() * w.double()
+    xh = s.double() * r
+    dot = (g * xh).mean(-1, keepdim=True)
+    adot = (g * xh).abs().mean(-1, keepdim=True)
+    dx = r * (g - xh * dot)
+    if dres is not None:
+        dx = dx + dres.double()
+    E = FP32_U * (4 * r * g.abs() + r * r * s.double().abs() * (6 * dot.abs() + (_row_chain(H) + 2) * adot) + dx.abs())
+    tol = BF16_U * dx.abs() + (1 + BF16_U) * E + ELEM_ABS_FLOOR
+    tol_g = r * BF16_U * (g.abs() + xh.abs() * adot)
+    return dict(dx=dx, tol=tol, tol_g=tol_g)
+
+
+def accumulate_tol(old, S, e):
+    """Bound of grad = bf16(fp32(old + bf16(S'))) against the exact old + S, where the kernel's fp32 sum S' is within e of S:
+    |bf16(S') - S| <= u |S| + (1 + u) e;  the fp32 add and the bf16 rounding of old + bf16(S') add (u + 2^-24) |old + bf16(S')|."""
+    return (BF16_U + FP32_U) * (old + S).abs() + (1 + 2 * BF16_U) * (BF16_U * S.abs() + (1 + BF16_U) * e) + ELEM_ABS_FLOOR
+
+
+def rmsnorm_wgrad_reference_fp64(dy, s, rstd_k, old):
+    """lmod_rmsnorm_wgrad:  wgrad = bf16(old + bf16(sum_r t_r)),  t_r = bf16(dy_r * bf16(s_r * rstd_r)) (autograd of `w * h.to(bf16)`).
+    The terms are bit exact in fp32 from the kernel's rstd; the kernel sums them in fp32: a warp walks 32 of a 256-row chunk, 8 warps are
+    folded, and the chunks meet in red.add in any order -- a chain of at most min(rows, 32) + 8 + ceil(rows / 256) additions."""
+    rows = s.shape[0]
+    xh = (s.float() * rstd_k.float()[:, None]).to(torch.bfloat16).float()
+    t = (dy.float() * xh).to(torch.bfloat16).double()
+    S = t.sum(0)
+    n = min(rows, 32) + 8 + -(-rows // 256)
+    e = n * FP32_U * t.abs().sum(0)
+    o = old.double()
+    return dict(want=o + S, tol=accumulate_tol(o, S, e))
+
+
+def layernorm_reference_fp64(x, w, b, eps):
+    """lmod_layernorm_fwd:  y = bf16((x - mean) rstd w + b),  rstd = 1 / sqrt(mean((x - mean)^2) + eps)  (CLIP LayerNorm).
+      The fp32 mean is off by e_mu <= (H/128 + 12) 2^-24 mean|x| (the chain and the division); that shifts every x - mean by e_mu and the
+      variance by e_mu^2 (sum(x - mean) = 0), the variance chain is relative (H/128 + 12) 2^-24, rsqrtf 2^-22, + eps one rounding:
+        rho_r = 0.5 ((H/128 + 12) 2^-24 + e_mu^2 / var) + 2^-22 + 2^-24
+      y = fma((x - mean) rstd, w, b) rounds x - mean, its product by rstd and the fma:  E = rstd |w| (|x - mean| (rho_r + 3 2^-24) + e_mu)
+      + 2^-24 |y|."""
+    H = x.shape[-1]
+    x64 = x.double()
+    mu = x64.mean(-1, keepdim=True)
+    d = x64 - mu
+    var = (d * d).mean(-1, keepdim=True)
+    r = torch.rsqrt(var + eps)
+    y = d * r * w.double() + b.double()
+    e_mu = (_row_chain(H) + 1) * FP32_U * x64.abs().mean(-1, keepdim=True)
+    rho = 0.5 * ((_row_chain(H) + 1) * FP32_U + e_mu * e_mu / (var + eps)) + 2.0 ** -22 + FP32_U
+    E = r * w.double().abs() * (d.abs() * (rho + 3 * FP32_U) + e_mu) + FP32_U * y.abs()
+    return dict(y=y, tol=BF16_U * y.abs() + (1 + BF16_U) * E + ELEM_ABS_FLOOR)
+
+
+def rope_bwd_reference_fp64(dq, cos, sin, pos, hd):
+    """Backward of lmod_rope (the transpose rotation) on a [rows, n_heads * hd] block of heads:  d1' = d1 c + d2 s,  d2' = d2 c - d1 s
+    with c, s the bf16 table rows of pos.  The kernel computes each in fp32 (two products and an add, or an fma) and stores bf16 once:
+      tol = u |ref| + (1 + u) 2 2^-24 (|d1 c| + |d2 s|).
+    tol_ag bounds the distance to autograd of R.apply_rope in bf16, which rounds d c, d s and their sum to bf16: one ulp (2^-7 relative)
+    of |d1 c| + |d2 s|."""
+    rows = dq.shape[0]
+    x = dq.double().view(rows, -1, hd)
+    c = cos[pos].double()[:, None, : hd // 2]
+    s_ = sin[pos].double()[:, None, : hd // 2]
+    d1, d2 = x[..., : hd // 2], x[..., hd // 2:]
+    o = torch.cat([d1 * c + d2 * s_, d2 * c - d1 * s_], -1)
+    mag = (d1 * c).abs() + (d2 * s_).abs()
+    mag = torch.cat([mag, (d2 * c).abs() + (d1 * s_).abs()], -1)
+    tol = BF16_U * o.abs() + (1 + BF16_U) * 2 * FP32_U * mag + ELEM_ABS_FLOOR
+    return dict(d=o.reshape(rows, -1), tol=tol.reshape(rows, -1), tol_ag=(2.0 ** -7 * mag + ELEM_ABS_FLOOR).reshape(rows, -1))
+
+
+def _sig_rel(z):
+    """Relative error bound of the kernels' fp32 sigmoid 1 / (1 + __expf(-z)): __expf is ex2.approx of the fp32 product z log2e (2 ulp +
+    |z| 2^-24 in the exponent), then an add and an IEEE division:  (|z| + 8) 2^-22."""
+    return (z.abs() + 8) * 2.0 ** -22
+
+
+def silu_mul_reference_fp64(gu, I):
+    """lmod_silu_mul_fwd / _bwd on [rows, >= 2I] gate | up (row stride = gu's):  out = bf16(bf16(silu(g)) u);
+    dg = d u sg (1 + g (1 - sg)),  du = d g sg,  sg = sigmoid(g).
+      fwd tol: |u| (u |silu| + (1 + u) |silu| rho),  rho = _sig_rel(g) (silu = g sg, one more product)
+      bwd tol: the fp32 sg carries sg rho; 1 - sg, g (1 - sg) and the products add 2^-24 terms:  E = |d u| sg (1 + |g|) (|g| + 8) 2^-21,
+               E = |d g| sg (|g| + 8) 2^-21 for du."""
+    g, u = gu[:, :I].double(), gu[:, I:2 * I].double()
+    sg = torch.sigmoid(g)
+    si = g * sg
+    rho = _sig_rel(g) + FP32_U
+    out = si * u
+    out_tol = BF16_U * out.abs() + (1 + BF16_U) * u.abs() * si.abs() * (BF16_U + (1 + BF16_U) * rho) + ELEM_ABS_FLOOR
+
+    def bwd(d):
+        d = d.double()
+        dg = d * u * sg * (1 + g * (1 - sg))
+        du = d * g * sg
+        Eg = (d * u).abs() * sg * (1 + g.abs()) * (g.abs() + 8) * 2.0 ** -21
+        Eu = (d * g).abs() * sg * (g.abs() + 8) * 2.0 ** -21
+        return dict(dg=dg, du=du, dg_tol=BF16_U * dg.abs() + (1 + BF16_U) * Eg + ELEM_ABS_FLOOR,
+                    du_tol=BF16_U * du.abs() + (1 + BF16_U) * Eu + ELEM_ABS_FLOOR)
+    return dict(out=out, out_tol=out_tol, bwd=bwd)
+
+
+ACT_GELU_REF, ACT_QUICK_GELU_REF, ACT_NONE_REF = 0, 1, 2
+
+
+def bias_act_reference_fp64(x, bias, act):
+    """lmod_bias_act_fwd:  y = bf16(act(bf16(x + bias))) (the bias add is one bf16 op, bit exact in fp32; the CLIP fc1 bias path).
+      GELU (erf):    0.5 z (1 + erf(z / sqrt2)); erff is within 2 ulp (2^-23 absolute near |erf| = 1, where 1 + erf cancels), the argument
+                     product shifts erf by at most 2^-24: E = 0.5 |z| 2^-22 + 2^-23 |y|
+      quick-GELU:    z sigmoid(1.702 z):  E = |y| (_sig_rel(1.702 z) + 2^-23)
+      identity:      exact."""
+    z = x.float()
+    if bias is not None:
+        z = (z + bias.float()).to(torch.bfloat16).float()
+    z = z.double()
+    if act == ACT_GELU_REF:
+        y = 0.5 * z * (1 + torch.erf(z / math.sqrt(2)))
+        E = 0.5 * z.abs() * 2.0 ** -22 + 2.0 ** -23 * y.abs()
+    elif act == ACT_QUICK_GELU_REF:
+        y = z * torch.sigmoid(1.702 * z)
+        E = y.abs() * (_sig_rel(1.702 * z) + 2.0 ** -23)
+    else:
+        y, E = z, torch.zeros_like(z)
+    return dict(y=y, tol=BF16_U * y.abs() + (1 + BF16_U) * E + ELEM_ABS_FLOOR)
+
+
+def gelu_bwd_reference_fp64(dy, x):
+    """lmod_gelu_bwd:  dx = dy (cdf(x) + x pdf(x)).  cdf via erff (2^-22 absolute with the argument product), pdf via __expf(-x^2 / 2)
+    (relative _sig_rel(x^2 / 2)), three more roundings:  E = |dy| (2^-22 + |x| pdf (_sig_rel(x^2/2) + 2^-24) + 3 2^-24 (cdf + |x| pdf))."""
+    x64, d = x.double(), dy.double()
+    cdf = 0.5 * (1 + torch.erf(x64 / math.sqrt(2)))
+    pdf = torch.exp(-0.5 * x64 * x64) / math.sqrt(2 * math.pi)
+    ref = d * (cdf + x64 * pdf)
+    xp = x64.abs() * pdf
+    E = d.abs() * (2.0 ** -22 + xp * (_sig_rel(0.5 * x64 * x64) + FP32_U) + 3 * FP32_U * (cdf + xp))
+    return dict(dx=ref, tol=BF16_U * ref.abs() + (1 + BF16_U) * E + ELEM_ABS_FLOOR)
+
+
+def embed_grad_reference_fp64(dout, src, old):
+    """lmod_embed_grad (nn.Embedding backward behind the splice, then the bf16 accumulation into .grad):  for every token t with rows
+    R_t = {r : src[r] = t},  grad[t] = bf16(old[t] + bf16(sum_{r in R_t} dout[r]));  rows with src < 0 (image patches, padding) add nothing.
+    The kernel sums a token's n_t rows in one fp32 chain: e = n_t 2^-24 sum|dout| (accumulate_tol).
+    Returns the touched token ids (sorted), want = old + S and tol for their rows [U, H], and the counts n_t."""
+    flat = src.reshape(-1)
+    keep = flat >= 0
+    rows = torch.nonzero(keep)[:, 0]
+    toks, inv, cnt = torch.unique(flat[keep], return_inverse=True, return_counts=True)
+    H = dout.shape[-1]
+    d = dout.reshape(-1, H)[rows].double()
+    S = torch.zeros(toks.numel(), H, dtype=torch.float64, device=dout.device).index_add_(0, inv, d)
+    A = torch.zeros_like(S).index_add_(0, inv, d.abs())
+    o = old[toks].double()
+    return dict(toks=toks, counts=cnt, want=o + S, tol=accumulate_tol(o, S, cnt.double()[:, None] * FP32_U * A))
+
+
+def splice_reference(embed_w, feats, src, img, n_patches):
+    """lmod_splice_embed: row r is embed_w[src] (src >= 0), feats[img, -1 - src] (src < 0, img >= 0) or zero -- a copy, bit exact."""
+    flat, im = src.reshape(-1), img.reshape(-1)
+    H = embed_w.shape[1]
+    out = torch.zeros(flat.numel(), H, dtype=embed_w.dtype, device=embed_w.device)
+    t = flat >= 0
+    out[t] = embed_w[flat[t]]
+    f = (flat < 0) & (im >= 0)
+    out[f] = feats.reshape(-1, H)[im[f] * n_patches + (-1 - flat[f])]
+    return out
+
+
+def splice_bwd_reference(dout, src, img, n_img, n_patches):
+    """lmod_splice_embed_bwd: dfeats[img, -1 - src] = dout[r] for the image rows (each feature row is spliced once), zero elsewhere."""
+    flat, im = src.reshape(-1), img.reshape(-1)
+    H = dout.shape[-1]
+    d = torch.zeros(n_img * n_patches, H, dtype=dout.dtype, device=dout.device)
+    f = (flat < 0) & (im >= 0)
+    d[im[f] * n_patches + (-1 - flat[f])] = dout.reshape(-1, H)[f]
+    return d.view(n_img, n_patches, H)
+
+
+def sumsq_reference_fp64(g, chunk=1 << 27):
+    """sum(g^2) in float64, in chunks (a 10^9-element buffer)."""
+    flat = g.reshape(-1)
+    tot = 0.0
+    for i in range(0, flat.numel(), chunk):
+        c = flat[i:i + chunk].double()
+        tot += float((c * c).sum())
+    return tot
+
+
+def sumsq_chain(n, blocks):
+    """Length of lmod_sumsq's fp32 chain: each of the 256 threads of `blocks` CTAs adds ceil(n / (blocks 256)) squares (one fma each; the
+    bf16 path rounds up to whole vectors of 8 and a tail), block_sum (11), the last CTA adds ceil(blocks / 256) partials per thread,
+    block_sum again (11) and the add into out."""
+    return -(-n // (blocks * 256)) + 8 + -(-blocks // 256) + 23
+
+
+def sumsq_blocks(n, n_sms):
+    """The grid of lmod_sumsq: one CTA per 2048 elements, capped at 8 CTAs per SM (and at 4096)."""
+    return max(1, min((n // 8 + 255) // 256, n_sms * 8, 4096))
+
+
+def adamw_reference_fp64(master, m, v, grad, step, lr, beta1, beta2, eps, wd, gnorm_sq=None, max_norm=0.0, grad_scale=1.0,
+                         bias_correction=True, fp32_hyper=True):
+    """lmod_adamw (torch.optim.AdamW with clip_grad_norm_ folded into a scalar) in float64 on the fp32 inputs, with the hyperparameters as
+    the fp32 values the kernel receives:
+      coef = grad_scale min(1, max_norm / (sqrt(gnorm_sq) grad_scale + 1e-6))  (no clipping when gnorm_sq is None or max_norm = 0)
+      g = grad coef;  p' = p (1 - lr wd);  m' = b1 m + (1 - b1) g;  v' = b2 v + (1 - b2) g^2
+      p'' = p' - (lr / bc1) m' / (sqrt(v') / sqrt(bc2) + eps),  bc_i = 1 - b_i^step.
+    Bounds (the kernel's fp32 arithmetic; IEEE sqrtf and division):
+      coef: sqrtf, two products, an add, a division, fminf: relative rho_c = 6 2^-24;  g = grad coef: rho_g = rho_c + 2^-24
+      m: E_m = 3 2^-24 (|b1 m| + |(1 - b1) g|) + (1 - b1) |g| rho_g
+      v: E_v = 4 2^-24 (b2 v + (1 - b2) g^2) + 2 rho_g (1 - b2) g^2
+      denom: relative rho_d = E_v / (2 v') + 5 2^-24 (sqrtf, bc2_sqrt rounded to fp32, the division, the + eps)
+      p: E_p = 3 2^-24 |p'| + (lr / bc1) / denom (E_m + |m'| (rho_d + 4 2^-24)) + 2^-24 |p''|   (1 - lr wd, lr / bc1 with bc1 in fp32,
+         m / denom, the product, the difference).
+    bias_correction=False drops bc1 and bc2 (a planted defect for the tests of the bound).  fp32_hyper=False takes the hyperparameters as
+    the Python floats torch.optim.AdamW uses (1 - beta2 formed in double): the kernel's 1 - fp32(0.999) differs from fp32(0.001) by
+    1.3e-5 relative, a deviation of the second-moment increment that the oracle pin must not mistake for arithmetic error."""
+    f = (lambda a: float(torch.tensor(a, dtype=torch.float32))) if fp32_hyper else float    # noqa: E731  the value the kernel receives
+    lr, b1, b2, eps, wd, mn, gs = f(lr), f(beta1), f(beta2), f(eps), f(wd), f(max_norm), f(grad_scale)
+    coef = gs
+    if gnorm_sq is not None and mn > 0:
+        total = math.sqrt(float(gnorm_sq)) * gs
+        coef = gs * min(1.0, mn / (total + f(1e-6)))
+    u = FP32_U
+    rho_g = 7 * u
+    g = grad.double() * coef
+    p0, m0, v0 = master.double(), m.double(), v.double()
+    bc1 = 1 - b1 ** step if bias_correction else 1.0
+    bc2 = 1 - b2 ** step if bias_correction else 1.0
+    p1 = p0 * (1 - lr * wd)
+    m1 = b1 * m0 + (1 - b1) * g
+    v1 = b2 * v0 + (1 - b2) * g * g
+    den = torch.sqrt(v1) / math.sqrt(bc2) + eps
+    p2 = p1 - (lr / bc1) * m1 / den
+    E_m = 3 * u * ((b1 * m0).abs() + ((1 - b1) * g).abs()) + (1 - b1) * g.abs() * rho_g
+    E_v = 4 * u * (b2 * v0 + (1 - b2) * g * g) + 2 * rho_g * (1 - b2) * g * g
+    rho_d = torch.where(v1 > 0, E_v / (2 * v1), torch.zeros_like(v1)) + 5 * u
+    E_p = 3 * u * p1.abs() + (lr / bc1) / den * (E_m + m1.abs() * (rho_d + 4 * u)) + u * p2.abs()
+    return dict(master=p2, m=m1, v=v1, master_tol=E_p + ELEM_ABS_FLOOR, m_tol=E_m + ELEM_ABS_FLOOR, v_tol=E_v + ELEM_ABS_FLOOR, coef=coef)
+
+
+def check_bound(name, got, want, tol=None, report=None):
+    """Element-wise |got - want| <= tol (bit for bit when tol is None) with a message naming the worst element; see check_moe."""
+    return check_moe(name, got, want, tol, report)
+
+
 def moe_plan_pairs(S, E, n1, n2, seed=0):
     """[S, 2] (first, second) expert of every token with n1[e] first and n2[e] second choices, first != second, in a seeded order."""
     g = torch.Generator().manual_seed(seed)

@@ -9,8 +9,8 @@ import torch
 pytestmark = pytest.mark.gpu
 
 from oracle import restated as R  # noqa: E402
-from tests.helpers import (check_dlogits, check_moe_stages, check_row_out, kl_reference_fp64, moe_reference_fp64,  # noqa: E402
-                           moe_run_stages)
+from tests.helpers import (check_bound, check_dlogits, check_moe_stages, check_row_out, kl_reference_fp64, moe_reference_fp64,  # noqa: E402
+                           moe_run_stages, rope_bwd_reference_fp64)
 
 BF16_EPS = 2.0 ** -8
 
@@ -324,14 +324,14 @@ def test_rope_matches_reference_rounding():
     assert torch.equal(out[:, : nh * hd].view(B, T, nh, hd).transpose(1, 2), qr)                 # bit exact (same bf16 roundings)
     assert torch.equal(out[:, nh * hd:(nh + nkv) * hd].view(B, T, nkv, hd).transpose(1, 2), kr)
     assert torch.equal(out[:, (nh + nkv) * hd:], qkv[:, (nh + nkv) * hd:])                       # v untouched
-    # backward = transpose rotation: <rope(x), y> == <x, rope_bwd(y)>
-    y = torch.randn_like(qkv.float()).to(torch.bfloat16)
+    # backward = transpose rotation, element by element against float64 (tests/helpers.py); v untouched
+    y = torch.randn(qkv.shape, generator=g).to(torch.bfloat16)
     yb = y.to(dev()).clone()
     pos_d = pos.to(dev())
     K.call("lmod_rope", K.ptr(yb), yb.shape[1], nh, yb.data_ptr() + nh * hd * 2, yb.shape[1], nkv, hd, K.ptr(cd), K.ptr(sn), K.ptr(pos_d), B * T, 1)
-    lhs = (out[:, :(nh + nkv) * hd].float() * y[:, :(nh + nkv) * hd].float()).sum()
-    rhs = (qkv[:, :(nh + nkv) * hd].float() * yb.cpu()[:, :(nh + nkv) * hd].float()).sum()
-    assert abs(lhs - rhs) < 2e-2 * abs(lhs) + 0.5
+    ref = rope_bwd_reference_fp64(y[:, :(nh + nkv) * hd], cos, sin, pos, hd)
+    check_bound("rope bwd", yb.cpu()[:, :(nh + nkv) * hd], ref["d"], ref["tol"])
+    assert torch.equal(yb.cpu()[:, (nh + nkv) * hd:], y[:, (nh + nkv) * hd:])
 
 
 def test_silu_mul_gelu_layernorm():
