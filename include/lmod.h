@@ -272,6 +272,12 @@ int lmod_attn_bwd(const void* qkv, int64_t ld_qkv, const void* out, int64_t ld_o
  *   on len, so a captured graph serves every step.  ws: fp32 workspace of at least lmod_attn_decode_ws_elems(...) elements. */
 int lmod_kv_append(const void* qkv, int64_t ld_qkv, int64_t batch, int64_t n_new, int nh, int nkv, int hd, const int32_t* offsets,
                    void* k_cache, void* v_cache, int64_t max_len, void* stream);
+/* lmod_kv_append_rows: the prefill of a padded batch -- of the n_rows rows per sequence of the fused QKV buffer [batch*n_rows, ...], copies
+ *   rows [src_lo[b], src_hi[b]) of sequence b to cache rows offsets[b] + (r - src_lo[b]), so each sequence's real rows land packed from
+ *   offsets[b].  src_lo / src_hi / offsets int32 [batch] on the device (the ranges the attention kernels mask with).  Bit-exact, no host
+ *   sync; no other row is written (rows at or past max_len are skipped; callers bounds-check).  hd %% 8 == 0. */
+int lmod_kv_append_rows(const void* qkv, int64_t ld_qkv, int64_t batch, int64_t n_rows, int nh, int nkv, int hd, const int32_t* src_lo,
+                        const int32_t* src_hi, const int32_t* offsets, void* k_cache, void* v_cache, int64_t max_len, void* stream);
 int64_t lmod_attn_decode_ws_elems(int64_t batch, int nh, int nkv, int hd, int64_t max_len);
 int lmod_attn_decode(const void* q, int64_t ld_q, const void* k_cache, const void* v_cache, const int32_t* len, int64_t batch, int nh,
                      int nkv, int hd, int64_t max_len, float softmax_scale, void* out, int64_t ld_o, float* lse, float* ws,

@@ -228,6 +228,29 @@ __global__ void kv_append_kernel(const __nv_bfloat16* qkv, int64_t ld, int n_new
   *reinterpret_cast<uint4*>(dst) = *reinterpret_cast<const uint4*>(src);
 }
 
+// rows [lo[b], hi[b]) of sequence b's n_rows rows of the fused qkv buffer -> cache rows off[b] + (r - lo[b]): the padded prefill's real
+// rows, packed at the front of each sequence's cache.  One thread per 16 B of a k or v head row; rows outside the range return at once.
+__global__ void kv_append_rows_kernel(const __nv_bfloat16* qkv, int64_t ld, int n_rows, int nh, int nkv, int hd, const int32_t* lo,
+                                      const int32_t* hi, const int32_t* off, __nv_bfloat16* kc, __nv_bfloat16* vc, int max_len,
+                                      int64_t chunks) {
+  const int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= chunks) return;
+  const int per = hd / 8;
+  int64_t i = c;
+  const int d8 = (int)(i % per); i /= per;
+  const int j = (int)(i % nkv); i /= nkv;
+  const int isv = (int)(i % 2); i /= 2;
+  const int64_t row = i;
+  const int b = (int)(row / n_rows), r = (int)(row % n_rows);
+  const int r0 = lo[b];
+  if (r < r0 || r >= hi[b]) return;
+  const int pos = off[b] + (r - r0);
+  if (pos < 0 || pos >= max_len) return;                // the host bounds-checks every append; never write outside the cache
+  const __nv_bfloat16* src = qkv + row * ld + (int64_t)(nh + isv * nkv + j) * hd + d8 * 8;
+  __nv_bfloat16* dst = (isv ? vc : kc) + (((int64_t)b * nkv + j) * max_len + pos) * hd + d8 * 8;
+  *reinterpret_cast<uint4*>(dst) = *reinterpret_cast<const uint4*>(src);
+}
+
 // split count and length (in key blocks) from max_len, nkv and the SM count: about two waves of CTAs at B = 1, at least
 // DEC_MIN_BLOCKS blocks per split
 int decode_splits(int64_t max_len, int nkv, int* split_blocks) {
@@ -278,6 +301,22 @@ extern "C" int lmod_kv_append(const void* qkv, int64_t ld_qkv, int64_t batch, in
   kv_append_kernel<<<(unsigned)((chunks + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
       (const __nv_bfloat16*)qkv, ld_qkv, (int)n_new, nh, nkv, hd, offsets, (__nv_bfloat16*)k_cache, (__nv_bfloat16*)v_cache, (int)max_len,
       chunks);
+  LMOD_LAUNCH_OK();
+  return LMOD_OK;
+}
+
+extern "C" int lmod_kv_append_rows(const void* qkv, int64_t ld_qkv, int64_t batch, int64_t n_rows, int nh, int nkv, int hd,
+                                   const int32_t* src_lo, const int32_t* src_hi, const int32_t* offsets, void* k_cache, void* v_cache,
+                                   int64_t max_len, void* stream) {
+  LMOD_CHECK_ARG(qkv && src_lo && src_hi && offsets && k_cache && v_cache && batch > 0 && n_rows > 0 && nh > 0 && nkv > 0 && max_len > 0,
+                 "lmod_kv_append_rows: bad arguments");
+  LMOD_CHECK_ARG(hd % 8 == 0 && ld_qkv % 8 == 0 && ld_qkv >= (int64_t)(nh + 2 * nkv) * hd, "lmod_kv_append_rows: hd / ld_qkv");
+  LMOD_CHECK_ARG((uintptr_t)qkv % 16 == 0 && (uintptr_t)k_cache % 16 == 0 && (uintptr_t)v_cache % 16 == 0,
+                 "lmod_kv_append_rows: alignment");
+  const int64_t chunks = batch * n_rows * 2 * nkv * (hd / 8);
+  kv_append_rows_kernel<<<(unsigned)((chunks + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
+      (const __nv_bfloat16*)qkv, ld_qkv, (int)n_rows, nh, nkv, hd, src_lo, src_hi, offsets, (__nv_bfloat16*)k_cache,
+      (__nv_bfloat16*)v_cache, (int)max_len, chunks);
   LMOD_LAUNCH_OK();
   return LMOD_OK;
 }

@@ -65,6 +65,7 @@ SIGNATURES = {
     "lmod_attn_fwd": [_P, _L, _L, _L, _I, _I, _I, _I, _F, _P, _L, _P, _P, _P, _P],
     "lmod_attn_bwd": [_P, _L, _P, _L, _P, _L, _P, _L, _L, _I, _I, _I, _I, _F, _P, _L, _P, _P, _P, _P, _P],
     "lmod_kv_append": [_P, _L, _L, _L, _I, _I, _I, _P, _P, _P, _L, _P],
+    "lmod_kv_append_rows": [_P, _L, _L, _L, _I, _I, _I, _P, _P, _P, _P, _P, _L, _P],
     "lmod_attn_decode_ws_elems": [_L, _I, _I, _I, _L],
     "lmod_attn_decode": [_P, _L, _P, _P, _P, _L, _I, _I, _I, _L, _F, _P, _L, _P, _P, _L, _P],
     "lmod_version": [],

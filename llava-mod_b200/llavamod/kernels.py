@@ -440,6 +440,23 @@ def kv_append(qkv, B, n_new, nh, nkv, hd, k_cache, v_cache, offsets):
     call("lmod_kv_append", ptr(qkv), qkv.stride(0), B, n_new, nh, nkv, hp, ptr(offsets), ptr(k_cache), ptr(v_cache), k_cache.shape[2])
 
 
+def kv_append_rows(qkv, B, T, nh, nkv, hd, k_cache, v_cache, src_lo, src_hi, offsets):
+    """The prefill of a padded batch into the cache: rows [src_lo[b], src_hi[b]) of sequence b's T rows of the fused, RoPE'd QKV buffer
+    [B*T, (nh+2nkv)*hd] -> cache rows offsets[b] + (r - src_lo[b]), so every sequence's real rows are packed from offsets[b].  src_lo /
+    src_hi / offsets: int32 [B] on the device (pad_ranges gives the ranges); no other cache row is written."""
+    _need_cuda(qkv, k_cache, v_cache, src_lo, src_hi, offsets)
+    _check_cache(k_cache, v_cache, B, nkv, hd)
+    for t, name in ((src_lo, "src_lo"), (src_hi, "src_hi"), (offsets, "offsets")):
+        _check_i32(t, B, name)
+    if qkv.dim() != 2 or qkv.shape[0] != B * T or qkv.shape[1] != (nh + 2 * nkv) * hd or qkv.stride(1) != 1:
+        raise _C.LmodError("kv_append_rows: qkv must be [B*T, (nh+2nkv)*hd] with unit column stride, got %s" % (tuple(qkv.shape),))
+    hp = k_cache.shape[-1]
+    if hp != hd:
+        qkv = _pad_heads(qkv, nh + 2 * nkv, hd, hp)
+    call("lmod_kv_append_rows", ptr(qkv), qkv.stride(0), B, T, nh, nkv, hp, ptr(src_lo), ptr(src_hi), ptr(offsets), ptr(k_cache),
+         ptr(v_cache), k_cache.shape[2])
+
+
 def attn_decode_ws_elems(B, nh, nkv, hd, max_len):
     return int(_C.lib().lmod_attn_decode_ws_elems(B, nh, nkv, attn_head_dim(hd), max_len))
 

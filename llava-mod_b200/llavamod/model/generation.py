@@ -15,7 +15,17 @@ The decode step (embedding, layers, final norm, lm_head over B rows) is captured
 (LLAVAMOD_CUDA_GRAPHS=0: eager).  Caches are sized to a multiple of CACHE_BUCKET positions, so an eval loop over prompts of different
 lengths reuses a few graphs; at most LLAVAMOD_MAX_GRAPHS (cache, graph) pairs are kept, least recently used dropped first.
 
-Supported: greedy, temperature / top-p sampling, num_beams == 1, EOS and `stopping_criteria` callables, batch of equal-length prompts."""
+Padded prompt batches (attention_mask with zeros; each row's real tokens contiguous, on either side): every sequence is decoded as if
+it were alone.  Any input padding side and any config.tokenizer_padding_side give the same tokens.  Positions run 0 .. n_b - 1 over
+sequence b's n_b real spliced rows and cached steps continue at n_b + s; every step reads the next-token logits from each sequence's last
+real row; a sequence attends to its own real keys only.  So for the dense models a sequence's result does not depend on the other
+prompts.  The sparse student's prefill is the padded forward: pad rows are routed and count toward S and the capacity, as DeepSpeed
+routes every row of a batch, and each cached step routes its B tokens; prompts are coupled only through routing, as in any batch.
+The result is HF's layout: the input ids as given, pads included, followed by the new tokens.  Prompts without padding take the
+unpadded path unchanged.  (The reference's own batched decoding differs from this for padded image batches and right-padded batches,
+DESIGN section 8.)
+
+Supported: greedy, temperature / top-p sampling, num_beams == 1, EOS and `stopping_criteria` callables, padded or unpadded batches."""
 import collections
 import os
 import weakref
@@ -30,11 +40,19 @@ _GRAPH_POOL = None
 
 
 @torch.no_grad()
-def next_token_logits(model, input_ids, images=None, tower_features=None, attention_mask=None, cache=None):
-    """fp32 logits of the position after the last one: [B, V].  cache: prefill into it (empty) or decode one step (input_ids [B,1])."""
+def next_token_logits(model, input_ids, images=None, tower_features=None, attention_mask=None, cache=None, ragged=False):
+    """fp32 logits of the position after the last one: [B, V].  cache: prefill into it (empty) or decode one step (input_ids [B,1]).
+    ragged: attention_mask has padding -- the logits of each sequence's last real row (of the spliced mask), gathered on the device."""
     r = model.forward_hidden(input_ids=input_ids, attention_mask=attention_mask, labels=None, images=images, tower_features=tower_features,
                              cache=cache)
-    last = r["hidden"][:, -1, :].contiguous()
+    h = r["hidden"]
+    if ragged:
+        B, T, H = h.shape
+        rows = ((K.pad_ranges(r["attention_mask"])[1] - 1) + torch.arange(B, device=h.device, dtype=torch.int32) * T).to(torch.int32)
+        last = K.gather_rows(h.reshape(B * T, H), rows, torch.full((1,), B, dtype=torch.int32, device=h.device),
+                             out=torch.empty(B, H, dtype=h.dtype, device=h.device))
+    else:
+        last = h[:, -1, :].contiguous()
     return K.mm_nt(last, model.lm_head.weight).float()
 
 
@@ -69,8 +87,7 @@ def _decoder_entry(model, B, max_len):
     _STEP_GRAPHS[key] = ent
     while len(_STEP_GRAPHS) > max(1, int(os.environ.get("LLAVAMOD_MAX_GRAPHS", "6"))):
         _STEP_GRAPHS.popitem(last=False)
-    ent["cache"].len.zero_()
-    ent["cache"].length = 0
+    ent["cache"].reset()
     return ent
 
 
@@ -82,33 +99,43 @@ def _decode_step(model, ent, tok, eager):
         return next_token_logits(model, tok[:, None], cache=cache)
     if ent["graph"] is None:
         ent["ids"] = tok.clone()
-        n0 = cache.length
+        n0 = list(cache.lengths)
         g = torch.cuda.CUDAGraph()
         if _GRAPH_POOL is None:
             _GRAPH_POOL = torch.cuda.graph_pool_handle()
         with torch.cuda.graph(g, pool=_GRAPH_POOL):
             ent["logits"] = next_token_logits(model, ent["ids"][:, None], cache=cache)
-        cache.length = n0                       # the capture ran the host code of a step; nothing ran on the device
+        cache.lengths = n0                      # the capture ran the host code of a step; nothing ran on the device
         ent["graph"] = g
     cache.check(tok.shape[0], 1)
     ent["ids"].copy_(tok)
     ent["graph"].replay()
-    cache.length += 1
+    cache.advance(1)
     return ent["logits"].clone()
 
 
 @torch.no_grad()
 def generate(model, inputs=None, images=None, attention_mask=None, max_new_tokens=20, do_sample=False, temperature=1.0, top_p=None,
              num_beams=1, use_cache=False, stopping_criteria=None, eos_token_id=None, pad_token_id=None, generator=None, **unused):
-    """-> [B, T_in + n_new] int64: the prompt ids (image placeholders -200 included, as HF returns them) followed by the new tokens."""
+    """-> [B, T_in + n_new] int64: the prompt ids (image placeholders -200 included, pads included, as HF returns them) followed by the
+    new tokens."""
     if num_beams != 1:
         raise NotImplementedError("beam search is not built (the reference's eval shells run num_beams=1)")
-    if attention_mask is not None and not bool(attention_mask.all()):
-        raise NotImplementedError("padded prompt batches: decode one prompt (or equal-length prompts) per call, as the reference's eval loaders do")
-    was_training = model.training
-    model.eval()
     dev = model.device
     ids = inputs.to(dev)
+    mask = None
+    if attention_mask is not None:
+        m = attention_mask.cpu().bool()
+        if not bool(m.all()):
+            n_real = m.sum(1)
+            if bool((n_real == 0).any()):
+                raise ValueError("generate: prompt %d has no real token" % int((n_real == 0).nonzero()[0]))
+            first = m.int().argmax(1)
+            if not bool((m.int().cumsum(1).gather(1, (first + n_real - 1)[:, None]).squeeze(1) == n_real).all()):
+                raise ValueError("generate: every prompt's real tokens must be contiguous (left or right padding)")
+            mask = m
+    was_training = model.training
+    model.eval()
     eos = eos_token_id if eos_token_id is not None else getattr(model.config, "eos_token_id", None)
     eos = [eos] if isinstance(eos, int) else (list(eos) if eos is not None else [])
     pad = pad_token_id if pad_token_id is not None else (eos[0] if eos else 0)
@@ -121,12 +148,22 @@ def generate(model, inputs=None, images=None, attention_mask=None, max_new_token
     B = ids.shape[0]
     done = torch.zeros(B, dtype=torch.bool, device=dev)
     ent = None
+    ragged = mask is not None
     if use_cache and int(max_new_tokens) > 0:
-        need = model.spliced_length(ids, images) + int(max_new_tokens)
+        need = max(model.spliced_length(ids, images, mask)) + int(max_new_tokens)
         ent = _decoder_entry(model, B, (need + CACHE_BUCKET - 1) // CACHE_BUCKET * CACHE_BUCKET)
-        logits = next_token_logits(model, ids, images=images, tower_features=feats, cache=ent["cache"])
+        logits = next_token_logits(model, ids, images=images, tower_features=feats, attention_mask=mask.to(dev) if ragged else None,
+                                   cache=ent["cache"], ragged=ragged)
+    elif ragged:
+        # the no-cache loop re-reads every prompt with its new tokens appended: each row holds its real tokens first, then the new ones,
+        # then padding, so a row stays one run of real tokens and the unspliced text rows sit at positions 0 .. n_b - 1
+        work = ids.gather(1, torch.argsort((~mask).to(torch.int8), dim=1, stable=True).to(dev))
+        wlen = mask.sum(1).to(dev)
     for step in range(int(max_new_tokens)):
-        if ent is None:
+        if ent is None and ragged:
+            wmask = torch.arange(work.shape[1], device=dev)[None, :] < wlen[:, None]
+            logits = next_token_logits(model, work, images=images, tower_features=feats, attention_mask=wmask, ragged=True)
+        elif ent is None:
             logits = next_token_logits(model, ids, images=images, tower_features=feats)
         elif step > 0:
             eager = not _graphs_enabled() or (step == 1 and ent["graph"] is None)      # one eager step before the capture
@@ -143,6 +180,9 @@ def generate(model, inputs=None, images=None, attention_mask=None, max_new_token
             nxt = logits.argmax(dim=-1)
         nxt = torch.where(done, torch.full_like(nxt, pad), nxt)
         ids = torch.cat([ids, nxt[:, None]], dim=1)
+        if ent is None and ragged:
+            work = torch.cat([work, torch.full_like(nxt[:, None], pad)], dim=1).scatter_(1, wlen[:, None], nxt[:, None])
+            wlen = wlen + 1
         for e in eos:
             done |= nxt == e
         stop = bool(done.all())

@@ -131,7 +131,7 @@ class LlavaQwenForCausalLMBase(nn.Module, LlavaMetaForCausalLM):
 
     # ---- forward -------------------------------------------------------------------------------------
     def new_kv_cache(self, batch, max_len):
-        """A KVCache for `batch` equal-length sequences of up to max_len spliced positions (prompt incl. image patches + new tokens)."""
+        """A KVCache for `batch` sequences of up to max_len spliced positions each (prompt incl. image patches + new tokens)."""
         return KVCache(self.model, batch, max_len)
 
     def forward_hidden(self, input_ids=None, attention_mask=None, position_ids=None, inputs_embeds=None, labels=None,
@@ -183,13 +183,14 @@ class LlavaQwenForCausalLMBase(nn.Module, LlavaMetaForCausalLM):
         if past_key_values is not None or use_cache:
             # KV-cache path (modeling_qwen2.py:1110-1217 with past_key_values; llava_arch.py:162-172 for the cached multimodal step).
             # Without a cache one is allocated for the prompt plus CACHE_ROOM positions; pass new_kv_cache(B, max_len) for longer runs.
+            # A padded prompt batch prefills each sequence's real rows; the step's attention_mask is not read (the cache's lengths decide).
             if past_key_values is not None and not isinstance(past_key_values, KVCache):
                 raise NotImplementedError("past_key_values must be the KVCache this model returned (or new_kv_cache made)")
             if labels is not None:
                 raise NotImplementedError("labels with a KV cache: the cached path is for decoding")
             cache = past_key_values
             if cache is None:
-                n = inputs_embeds.shape[1] if inputs_embeds is not None else self.spliced_length(input_ids, images)
+                n = inputs_embeds.shape[1] if inputs_embeds is not None else max(self.spliced_length(input_ids, images, attention_mask))
                 cache = self.new_kv_cache(input_ids.shape[0] if input_ids is not None else inputs_embeds.shape[0], n + CACHE_ROOM)
         r = self.forward_hidden(input_ids, attention_mask, position_ids, inputs_embeds, labels, images, moe_noise, cache=cache)
         hidden, labels = r["hidden"], r["labels"]
@@ -207,11 +208,17 @@ class LlavaQwenForCausalLMBase(nn.Module, LlavaMetaForCausalLM):
                                              moe_loss_list=tuple(r["l_aux"]), past_key_values=cache)
         return CausalLMOutputWithPast(loss=loss, logits=logits, labels=labels, past_key_values=cache)
 
-    def spliced_length(self, input_ids, images=None):
-        """Length of the decoder input of unpadded prompts: every image placeholder becomes the tower's patch count."""
+    def spliced_length(self, input_ids, images=None, attention_mask=None):
+        """Per sequence, the number of real decoder positions of its prompt: its real tokens (attention_mask, or all of them), every image
+        placeholder among them counting as the tower's patch count, cut at tokenizer_model_max_length as the splice cuts.  -> [B] ints."""
+        ids = input_ids.cpu()
+        real = torch.ones_like(ids, dtype=torch.bool) if attention_mask is None else attention_mask.cpu().bool()
+        n = real.sum(1)
         tower = self.get_image_tower()
-        n_img = int((input_ids[0] == IMAGE_TOKEN_INDEX).sum()) if images is not None and tower is not None else 0
-        return input_ids.shape[1] + n_img * (tower.num_patches - 1)
+        if images is not None and tower is not None:
+            n = n + ((ids == IMAGE_TOKEN_INDEX) & real).sum(1) * (tower.num_patches - 1)
+        cap = getattr(self.config, "tokenizer_model_max_length", None)
+        return [min(int(x), cap) if cap is not None else int(x) for x in n]
 
 
 

@@ -260,24 +260,40 @@ class Qwen2Model(nn.Module):
         """inputs_embeds [B,T,H] bf16; attention_mask [B,T] bool or None; position_ids [B,T] int64 or None.
         cache: a KVCache.  Empty: the prefill -- this forward, plus the K / V of every layer appended to the cache.  Holding a prefix and
         T == 1: one decode step at position len (modeling_qwen2.py:652-728 with past_key_value), attention over the cached keys.
+        A padded prefill (attention_mask with zeros; real tokens contiguous, either side) is this same padded forward, with positions
+        0 .. n_b - 1 over sequence b's real rows when position_ids is None; only the real rows go to the cache, packed at [0, n_b).
         Returns (final-normed hidden [B,T,H], [l_aux per MoE layer], routing records)."""
         if cache is not None and cache.length > 0:
             return self._decode_step(inputs_embeds, moe_noise, training_moe, cache)
         cfg = self.config
         B, T, H = inputs_embeds.shape
         dev = inputs_embeds.device
-        if cache is not None:
-            if attention_mask is not None and not bool(attention_mask.all()):
-                raise NotImplementedError("KV-cache prefill of padded prompts: decode equal-length, unpadded prompts")
+        padded = attention_mask is not None and not bool(attention_mask.all())      # MaskInfo answers on the host (no sync)
+        host_lengths = getattr(attention_mask, "lengths", None)
+        if hasattr(attention_mask, "mask"):
+            attention_mask = attention_mask.mask
+        pad = K.pad_ranges(attention_mask) if padded else None       # per-row real key range; the attention kernels mask from it
+        ragged = cache is not None and padded
+        if ragged:
+            lengths = host_lengths
+            if lengths is None:          # a raw mask: its real tokens must be one run per row, which is what pad_ranges assumes
+                span, real = torch.stack([pad[1] - pad[0], attention_mask.to(torch.int32).sum(1, dtype=torch.int32)]).tolist()
+                if span != real:
+                    raise ValueError("KV-cache prefill: every row's real tokens must be contiguous (left or right padding)")
+                lengths = span
+            lengths = [int(n) for n in lengths]
+            if min(lengths) <= 0:
+                raise ValueError("KV-cache prefill: sequence %d has no real token" % lengths.index(min(lengths)))
+            cache.check(B, lengths)
+            if position_ids is None:                        # compact positions (the splice plan gives them for spliced prompts)
+                m = attention_mask.to(torch.int64)
+                position_ids = (m.cumsum(1) - 1) * m
+        elif cache is not None:
             cache.check(B, T)
         if position_ids is None:
             position_ids = torch.arange(T, device=dev, dtype=torch.int64).unsqueeze(0).expand(B, T)
         pos = position_ids.reshape(-1).to(torch.int64).contiguous()
         cos, sin = self.rope(T, dev, inputs_embeds.dtype)
-        padded = attention_mask is not None and not bool(attention_mask.all())      # MaskInfo answers on the host (no sync)
-        if hasattr(attention_mask, "mask"):
-            attention_mask = attention_mask.mask
-        pad = K.pad_ranges(attention_mask) if padded else None       # per-row real key range; the attention kernels mask from it
 
         stream = inputs_embeds.reshape(B * T, H)
         branch = None                                   # pending residual-branch output (added inside the next norm)
@@ -297,7 +313,9 @@ class Qwen2Model(nn.Module):
             else:
                 x, stream = K.rmsnorm(branch, layer.input_layernorm.weight, cfg.rms_norm_eps, res=stream, wgrad=self.gview(layer.input_layernorm.weight))
             qkv = K.qkv_rope(x, at.qkv_weight, at.qkv_bias, cos, sin, pos, nh, nkv, hd, self.gview(at.qkv_weight), self.gview(at.qkv_bias))
-            if cache is not None:
+            if ragged:
+                K.kv_append_rows(qkv, B, T, nh, nkv, hd, cache.k[li], cache.v[li], pad[0], pad[1], cache.len)
+            elif cache is not None:
                 K.kv_append(qkv, B, T, nh, nkv, hd, cache.k[li], cache.v[li], cache.len)
             attn = K.attention(qkv, B, T, nh, nkv, hd, True, None, pad)
             if K.residual_fusable(attn, stream, self.gview(at.o_proj.weight), self.gview(layer.post_attention_layernorm.weight)):
@@ -335,14 +353,18 @@ class Qwen2Model(nn.Module):
             out, _ = K.rmsnorm(stream, self.norm.weight, cfg.rms_norm_eps, wgrad=self.gview(self.norm.weight))
         else:
             out, _ = K.rmsnorm(branch, self.norm.weight, cfg.rms_norm_eps, res=stream, wgrad=self.gview(self.norm.weight))
-        if cache is not None:
+        if ragged:
+            cache.len.add_(pad[1] - pad[0])
+            cache.advance(lengths)
+        elif cache is not None:
             cache.len.add_(T)
-            cache.length += T
+            cache.advance(T)
         return out.view(B, T, H), l_auxes, records
 
     def _decode_step(self, inputs_embeds, moe_noise, training_moe, cache):
         """One cached step: each sequence's new token sits at position len[b] (the reference's rule for a cached step,
-        llava_arch.py:162-172, on unpadded prompts), its k / v are appended at row len[b], and its query attends to rows [0, len[b] + 1).
+        llava_arch.py:162-172, on unpadded prompts; for a padded prompt len[b] = n_b + s counts its real rows only), its k / v are appended
+        at row len[b], and its query attends to rows [0, len[b] + 1).
         Everything the step reads about the position is on the device, so the step can be captured once and replayed.  MoE layers route
         the B new tokens alone (top2gating with S = B, as MoEQwen1_5Model_forward does with a cache, llava_qwen1_5_moe.py:223-236).
         The layer body is forward's no-grad layer body with the attention swapped for append + decode attention: the same norm and
@@ -398,18 +420,20 @@ class Qwen2Model(nn.Module):
         else:
             out, _ = K.rmsnorm(branch, self.norm.weight, cfg.rms_norm_eps, res=stream)
         cache.len.copy_(cache.end)
-        cache.length += 1
+        cache.advance(1)
         return out.view(B, 1, H), l_auxes, records
 
 
 class KVCache:
-    """Decoding cache of a Qwen2Model for B equal-length sequences of up to max_len positions.
+    """Decoding cache of a Qwen2Model for B sequences of up to max_len positions each.
 
     Per layer one K and one V buffer [B, nkv, max_len, hp] bf16 (HF's legacy layout; hp = the head width the attention kernels run,
     head dims below 64 zero-padded), the valid length of every sequence on the device (``len`` int32 [B], which the kernels read, so a
-    captured decode step serves every position) and its host mirror ``length``: the host always knows how many rows a forward adds, so
-    every append is bounds-checked without a sync.  ``cache[i]`` gives layer i's (k, v) views [B, nkv, length, hd], the legacy tuple layout
-    llava_arch.py:165 indexes.  The RoPE tables cover max_len at allocation, so nothing is rebuilt inside a captured step."""
+    captured decode step serves every position and every mix of lengths) and its host mirror ``lengths`` (``length`` is their maximum):
+    the host always knows how many rows a forward adds, so every append is bounds-checked without a sync.  Sequence b holds its rows
+    packed at [0, lengths[b]), whatever padding its prompt had.  ``cache[i]`` gives layer i's (k, v) views [B, nkv, length, hd], the legacy
+    tuple layout llava_arch.py:165 indexes; rows at or past a sequence's own length are unspecified.  The RoPE tables cover max_len at
+    allocation, so nothing is rebuilt inside a captured step."""
 
     def __init__(self, model, batch, max_len):
         cfg = model.config
@@ -426,13 +450,29 @@ class KVCache:
         self.pos = torch.zeros(batch, dtype=torch.int64, device=dev)          # RoPE positions of a decode step
         self.ws = torch.empty(max(1, K.attn_decode_ws_elems(batch, nh, nkv, self.head_dim, max_len)), dtype=torch.float32, device=dev)
         self.rope = model.rope(max_len, dev, dt)
-        self.length = 0
+        self.lengths = [0] * self.batch
+
+    @property
+    def length(self):
+        return max(self.lengths)
+
+    def _per_seq(self, n_new):
+        return [int(n) for n in n_new] if isinstance(n_new, (list, tuple)) else [int(n_new)] * self.batch
 
     def check(self, batch, n_new):
+        """n_new: positions each sequence adds (an int for all, or one per sequence)."""
         if batch != self.batch:
             raise ValueError("KVCache holds %d sequences, got a batch of %d" % (self.batch, batch))
-        if self.length + n_new > self.max_len:
-            raise ValueError("KVCache is full: %d cached + %d new positions > max_len %d" % (self.length, n_new, self.max_len))
+        for b, (n, a) in enumerate(zip(self.lengths, self._per_seq(n_new))):
+            if n + a > self.max_len:
+                raise ValueError("KVCache is full: sequence %d has %d cached + %d new positions > max_len %d" % (b, n, a, self.max_len))
+
+    def advance(self, n_new):
+        self.lengths = [n + a for n, a in zip(self.lengths, self._per_seq(n_new))]
+
+    def reset(self):
+        self.len.zero_()
+        self.lengths = [0] * self.batch
 
     def get_seq_length(self, layer_idx=0):
         return self.length

@@ -75,11 +75,13 @@ def embed_grad_order(src):
 
 class MaskInfo:
     """Attention mask + the host-side knowledge whether it contains padding, so the decoder never has to ask the device
-    (``bool(mask.all())`` would be a host sync and would break CUDA-graph capture)."""
+    (``bool(mask.all())`` would be a host sync and would break CUDA-graph capture), and each row's count of real positions
+    (``lengths``, a host list, or None) for the KV-cache prefill."""
 
-    def __init__(self, mask, all_true):
+    def __init__(self, mask, all_true, lengths=None):
         self.mask = mask
         self.all_true = bool(all_true)
+        self.lengths = lengths
 
     def all(self):
         return self.all_true
@@ -173,7 +175,8 @@ class LlavaMetaForCausalLM(ABC):
         plan = host.to(dev, non_blocking=True)
         return dict(src=plan[0].contiguous(), labels=plan[1], pos=plan[2], img=plan[3].contiguous(), mask=plan[4].bool(),
                     order=plan[5] if embed_trains else None,
-                    all_true=bool(nm.all()), has_labels=labels is not None, has_mask=attention_mask is not None, n_patches=n_patches)
+                    all_true=bool(nm.all()), lengths=nm.sum(1).tolist(), has_labels=labels is not None,
+                    has_mask=attention_mask is not None, n_patches=n_patches)
 
     def prepare_inputs_labels_for_multimodal(self, input_ids, position_ids, attention_mask, past_key_values, labels, images,
                                              tower_features=None, plan=None):
@@ -194,5 +197,5 @@ class LlavaMetaForCausalLM(ABC):
         if not plan["has_mask"]:
             new_mask = None
         else:       # "no padding" is known on the host, the decoder must not sync to find out
-            new_mask = MaskInfo(plan["mask"], plan["all_true"])
+            new_mask = MaskInfo(plan["mask"], plan["all_true"], plan.get("lengths"))
         return None, plan["pos"], new_mask, past_key_values, embeds, (plan["labels"] if plan["has_labels"] else None)

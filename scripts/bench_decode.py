@@ -1,7 +1,7 @@
 """Decoding benchmark: tokens/s of `generate` with and without the KV cache, decode-attention bandwidth, and the device time per
 kernel family of one cached decode step.
 
-    python scripts/bench_decode.py [--models student,teacher] [--new 128,512] [--batch 1,8] [--profile] [--out DIR]
+    python scripts/bench_decode.py [--models student,teacher] [--new 128,512] [--batch 1,8] [--profile] [--ragged] [--out DIR]
 
 * generate: the 0.5B-4E student and the 7B teacher (random weights, CLIP-L/336) on a prompt that splices to T' = 650 positions, greedy,
   use_cache False / True, CUDA graphs on / off (LLAVAMOD_CUDA_GRAPHS).  Tokens/s = B * new tokens / wall time of the call, which ends in
@@ -10,6 +10,9 @@ kernel family of one cached decode step.
 * attention: lmod_attn_decode alone, B = 1 and 8, lengths 1k to 32k, CUDA events over 50 launches; bytes = 2 * len * nkv * hd * 2 per
   sequence (K and V) plus q and out, against the 3.35 TB/s of the H100 SXM data sheet.
 * --profile: torch.profiler over 20 graph-less decode steps of the student at B = 1, device time summed per kernel family.
+* --ragged: B = 8 seeded prompts of different lengths (one image each, left-padded, spliced to 600-1100 positions), greedy, graphs on,
+  2 new tokens (a short-answer eval, dominated by the prefill) and 128: one padded B = 8 call, eight B = 1 calls on the same prompts,
+  and the equal-length B = 8 row (T' = 650), each as prompts/s and tokens/s (median of --repeat timed passes after one warm-up pass).
 The card's name and power limit are read in the same process and printed with the results (one JSON line per measurement)."""
 import argparse
 import json
@@ -61,6 +64,50 @@ def bench_generate(model, name, B, new, use_cache, graphs, out, info, repeat):
     rates.sort()
     emit(out, dict(kind="generate", model=name, B=B, new=res.shape[1] - ids.shape[1], use_cache=use_cache, graphs=graphs, runs=repeat,
                    tokens_per_s=round(rates[len(rates) // 2], 1), min=round(rates[0], 1), max=round(rates[-1], 1), card=info))
+
+
+def ragged_prompts(B=8, seed=7):
+    """B prompts of 24-524 text tokens plus one image (576 patches): 600-1100 spliced positions, left-padded with token 0."""
+    g = torch.Generator().manual_seed(seed)
+    lens = torch.randint(25, 526, (B,), generator=g).tolist()
+    T = max(lens)
+    ids = torch.zeros(B, T, dtype=torch.long)
+    mask = torch.zeros(B, T, dtype=torch.bool)
+    for b, n in enumerate(lens):
+        p = torch.randint(0, 150000, (n,), generator=g)
+        p[3] = -200
+        ids[b, T - n:], mask[b, T - n:] = p, True
+    imgs = [torch.randn(3, 336, 336, generator=g).to(torch.bfloat16) for _ in range(B)]
+    return ids, mask, imgs
+
+
+def bench_ragged(model, name, new, out, info, repeat):
+    """prompts/s and tokens/s of one padded B = 8 call, of eight B = 1 calls on the same prompts, and of the equal-length B = 8 call."""
+    os.environ["LLAVAMOD_CUDA_GRAPHS"] = "1"
+    ids, mask, imgs = ragged_prompts()
+    B = ids.shape[0]
+    eq_ids, eq_imgs = prompt(B)
+    runs = {
+        "padded_B8": lambda: [model.generate(ids, images=imgs, attention_mask=mask, max_new_tokens=new, use_cache=True, eos_token_id=-1)],
+        "eight_B1": lambda: [model.generate(ids[b:b + 1, mask[b]], images=imgs[b:b + 1], max_new_tokens=new, use_cache=True, eos_token_id=-1)
+                             for b in range(B)],
+        "equal_length_B8": lambda: [model.generate(eq_ids, images=eq_imgs, max_new_tokens=new, use_cache=True, eos_token_id=-1)],
+    }
+    n_b = model.spliced_length(ids, imgs, mask)
+    for row, fn in runs.items():
+        fn()                                                                     # warm-up (and graph capture)
+        secs = []
+        for _ in range(repeat):
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            fn()
+            torch.cuda.synchronize()
+            secs.append(time.perf_counter() - t0)
+        secs.sort()
+        t = secs[len(secs) // 2]
+        emit(out, dict(kind="ragged", model=name, row=row, B=B, new=new, spliced=(min(n_b), max(n_b)) if row != "equal_length_B8" else (650, 650),
+                       runs=repeat, seconds=round(t, 4), prompts_per_s=round(B / t, 2), tokens_per_s=round(B * new / t, 1),
+                       min_s=round(secs[0], 4), max_s=round(secs[-1], 4), card=info))
 
 
 def bench_attention(out, info):
@@ -135,6 +182,7 @@ def main():
     ap.add_argument("--profile", action="store_true")
     ap.add_argument("--skip-generate", action="store_true")
     ap.add_argument("--skip-attention", action="store_true")
+    ap.add_argument("--ragged", action="store_true", help="padded batches of prompts of different lengths (see the module docstring)")
     ap.add_argument("--repeat", type=int, default=3, help="timed generate calls per setting (median, min and max are reported)")
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
@@ -143,13 +191,16 @@ def main():
         os.makedirs(a.out, exist_ok=True)
     info = card()
     from llavamod.model import synthetic as S
-    if not a.skip_attention and not a.profile:
+    if not a.skip_attention and not a.profile and not a.ragged:
         bench_attention(a.out, info)
     for name in a.models.split(","):
         model = (S.make_student("qwen1.5-0.5b", "clip-l-336", seed=1) if name == "student" else
                  S.make_teacher("qwen1.5-7b", "clip-l-336", seed=0)).eval()
         if a.profile:
             profile_step(model, name, a.out, info)
+        elif a.ragged:
+            for new in (2, 128):
+                bench_ragged(model, name, new, a.out, info, a.repeat)
         elif not a.skip_generate:
             for B in [int(x) for x in a.batch.split(",")]:
                 for new in [int(x) for x in a.new.split(",")]:
