@@ -282,6 +282,30 @@ int64_t lmod_attn_decode_ws_elems(int64_t batch, int nh, int nkv, int hd, int64_
 int lmod_attn_decode(const void* q, int64_t ld_q, const void* k_cache, const void* v_cache, const int32_t* len, int64_t batch, int nh,
                      int nkv, int hd, int64_t max_len, float softmax_scale, void* out, int64_t ld_o, float* lse, float* ws,
                      int64_t ws_elems, void* stream);
+/* lmod_attn_decode_chunk: the past_key_value path of Qwen2SdpaAttention.forward for T >= 1 new queries per sequence (the verify step of
+ *   assisted decoding, HF generate(assistant_model=...)): q [batch*T, ld_q] (row b*T + t), their k / v already appended by lmod_kv_append
+ *   (n_new = T), len int32 [batch] the lengths after the append.  Row t attends to cache rows [0, len[b] - T + t + 1).  out [batch*T, nh*hd]
+ *   (row stride ld_o), lse [batch*T, nh] or NULL.  Row t gives the same bytes, in out and lse, as lmod_attn_decode on that row alone with
+ *   len = len[b] - T + t + 1.  hd in {64,128}, nh/nkv <= 8.  ws: fp32 workspace of at least lmod_attn_decode_chunk_ws_elems(...). */
+int64_t lmod_attn_decode_chunk_ws_elems(int64_t batch, int64_t T, int nh, int nkv, int hd, int64_t max_len);
+int lmod_attn_decode_chunk(const void* q, int64_t ld_q, const void* k_cache, const void* v_cache, const int32_t* len, int64_t batch,
+                           int64_t T, int nh, int nkv, int hd, int64_t max_len, float softmax_scale, void* out, int64_t ld_o, float* lse,
+                           float* ws, int64_t ws_elems, void* stream);
+
+/* ------------------------------------------------------------------------------------------
+ * Assisted decoding (csrc/spec.cu).
+ * lmod_spec_accept: HF's assisted-generation acceptance (generation/utils.py: the greedy candidate match of _assisted_decoding, and
+ *   _speculative_sampling) for one round of k drafted tokens.  target_logits fp32 [batch, k+1, V_t]: row j holds the target's logits after
+ *   the inputs [last, d_1 .. d_j], so it scores d_{j+1}; row k gives the bonus token.  draft_tokens int64 [batch, k].
+ *   u == NULL (greedy): n_acc = the largest n with d_{j+1} == argmax(row j) (first index on ties) for every j < n; next = argmax(row n_acc).
+ *   u fp32 [batch, k+1] (sampling; draft_logits fp32 [batch, k, V_d], both logit sets after the logits processors, -inf = probability 0,
+ *   draft probability 0 for ids >= V_d): accept d_{j+1} while u_j * q_j(d_{j+1}) <= p_j(d_{j+1}) (fp32 softmaxes); at the first rejection
+ *   next ~ normalize(max(0, p_j - q_j)), after k acceptances next ~ p_k, by inverse CDF with u_k over a fixed-order scan.
+ *   Writes n_acc int32 [batch] and next int64 [batch]; len_target / len_draft int32 [batch] (either may be NULL) -= k - n_acc[b].  No host
+ *   sync. */
+int lmod_spec_accept(const float* target_logits, int64_t V_t, const float* draft_logits, int64_t V_d, const int64_t* draft_tokens,
+                     const float* u, int64_t batch, int k, int32_t* n_acc, int64_t* next, int32_t* len_target, int32_t* len_draft,
+                     void* stream);
 
 
 #ifdef __cplusplus

@@ -16,6 +16,12 @@
 // The split writes its unnormalised fp32 output and (m, l) to the workspace; lmod_attn_decode's second launch merges the splits.
 // The split length depends on max_len, nkv and the SM count only -- not on len or B -- so one captured graph serves every step and a
 // sequence gives the same bits whatever batch it is decoded in.
+//
+// lmod_attn_decode_chunk: T new query rows per sequence (the verify step of assisted decoding), row t attending to keys
+// [0, len[b] - T + t + 1).  The same kernel body with CHUNK = true: a CTA serves G "virtual heads" (row t, query head g) of one KV head, and
+// each virtual head has its own key limit.  A key at or past the limit scores -inf and is skipped by P.V, and a split wholly past a row's
+// limit leaves (m, l) = (-inf, 0), so row t runs the single-query kernel's arithmetic at len = len[b] - T + t + 1 operation for operation:
+// the same splits, 64-key blocks, lane-to-key mapping and merge.  Its out and lse are the bytes lmod_attn_decode gives for that row alone.
 #include "sm90.cuh"
 
 namespace {
@@ -45,6 +51,7 @@ struct DecParams {
   float* ws_ml;             // [B, nh, nsplit, 2]  (running max in log2 units, sum of exp2)
   int nh, nkv, max_len, nsplit, split_blocks;
   float scale_log2;
+  int T, g, rows;           // chunk only: query rows per sequence (q / ws rows are b*T + t), query heads per KV head, rows per CTA
 };
 
 template <int HD>
@@ -59,7 +66,9 @@ __device__ __forceinline__ void dec_issue(uint8_t* sK, uint8_t* sV, uint64_t* fu
   bulk_g2s(sV + s * C::KV_BYTES, vg + (size_t)k0 * HD, bytes, &full[s]);
 }
 
-template <int HD, int G>
+// CHUNK = false: G query heads of one row per CTA.  CHUNK = true: G virtual heads v = (row t0 + v / p.g, head v % p.g), the rows of
+// blockIdx.y / nkv's row group; virtual heads past row T - 1 have limit 0 and write nothing.
+template <int HD, int G, bool CHUNK = false>
 __global__ void __launch_bounds__(DEC_THREADS) attn_decode_kernel(const DecParams p) {
   using C = DecCfg<HD>;
   constexpr int NST = C::NST, LANES = C::LANES, GROUPS = C::GROUPS, PAIRS = C::PAIRS, KSUB = C::KSUB;
@@ -71,9 +80,20 @@ __global__ void __launch_bounds__(DEC_THREADS) attn_decode_kernel(const DecParam
   uint8_t* sK = dec_smem;
   uint8_t* sV = dec_smem + NST * C::KV_BYTES;
 
-  const int split = blockIdx.x, hk = blockIdx.y, b = blockIdx.z;
+  const int split = blockIdx.x, hk = CHUNK ? blockIdx.y % p.nkv : blockIdx.y, b = blockIdx.z;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int len = min(p.len[b], p.max_len);
+  int len = min(p.len[b], p.max_len);
+  int lim[G];                                           // chunk: key limit of each virtual head
+  const int t0 = CHUNK ? (int)(blockIdx.y / p.nkv) * p.rows : 0;
+  if constexpr (CHUNK) {
+    const int base = p.len[b] - p.T;                    // cached rows before this step's T
+#pragma unroll
+    for (int g = 0; g < G; ++g) {
+      const int t = t0 + g / p.g;
+      lim[g] = t < p.T ? max(0, min(base + t + 1, p.max_len)) : 0;
+    }
+    len = max(0, min(base + min(t0 + p.rows, p.T), p.max_len));     // the row group's largest limit
+  }
   const int kbeg = split * p.split_blocks * DEC_BK;
   const int kend = min(len, kbeg + p.split_blocks * DEC_BK);
   const int nblk = kend > kbeg ? (kend - kbeg + DEC_BK - 1) / DEC_BK : 0;     // a split at or past len[b] contributes nothing
@@ -95,7 +115,14 @@ __global__ void __launch_bounds__(DEC_THREADS) attn_decode_kernel(const DecParam
   float qf[G][8];
 #pragma unroll
   for (int g = 0; g < G; ++g) {
-    const uint4 w = *reinterpret_cast<const uint4*>(p.q + (int64_t)b * p.ld_q + (int64_t)(hk * G + g) * HD + li * 8);
+    uint4 w;
+    if constexpr (CHUNK) {
+      const int t = t0 + g / p.g;
+      w = t < p.T ? *reinterpret_cast<const uint4*>(p.q + ((int64_t)b * p.T + t) * p.ld_q + (int64_t)(hk * p.g + g % p.g) * HD + li * 8)
+                  : make_uint4(0u, 0u, 0u, 0u);
+    } else {
+      w = *reinterpret_cast<const uint4*>(p.q + (int64_t)b * p.ld_q + (int64_t)(hk * G + g) * HD + li * 8);
+    }
     qf[g][0] = bf16lo(w.x); qf[g][1] = bf16hi(w.x); qf[g][2] = bf16lo(w.y); qf[g][3] = bf16hi(w.y);
     qf[g][4] = bf16lo(w.z); qf[g][5] = bf16hi(w.z); qf[g][6] = bf16lo(w.w); qf[g][7] = bf16hi(w.w);
   }
@@ -106,7 +133,8 @@ __global__ void __launch_bounds__(DEC_THREADS) attn_decode_kernel(const DecParam
 
   for (int j = 0; j < nblk; ++j) {
     const int s = j % NST;
-    const int n = min(DEC_BK, kend - (kbeg + j * DEC_BK));
+    const int kb = kbeg + j * DEC_BK;
+    const int n = min(DEC_BK, kend - kb);
     mbar_wait_bounded(&full[s], (j / NST) & 1);
     // ---- scores: every lane group runs the same trip count (the shuffles need the whole warp); rows >= n are discarded ----
     const uint8_t* Ks = sK + s * C::KV_BYTES;
@@ -129,20 +157,22 @@ __global__ void __launch_bounds__(DEC_THREADS) attn_decode_kernel(const DecParam
         for (int g = 0; g < G; ++g) sc[g] += __shfl_xor_sync(0xffffffffu, sc[g], off);
       if (li == 0)
 #pragma unroll
-        for (int g = 0; g < G; ++g) s_p[t][g] = t < n ? sc[g] * p.scale_log2 : -INFINITY;
+        for (int g = 0; g < G; ++g) s_p[t][g] = t < n && (!CHUNK || kb + t < lim[g]) ? sc[g] * p.scale_log2 : -INFINITY;
     }
     __syncthreads();
-    // ---- online softmax, one warp per head (key 0 of the block is always valid, so the block max is finite) ----
+    // ---- online softmax, one warp per head (key 0 of the block is always valid, so the block max is finite; in a chunk a virtual head
+    //      may have seen no valid key yet: m stays -inf, and exponents are taken against 0 so p = alpha = l = 0 instead of NaN) ----
     for (int g = warp; g < G; g += DEC_THREADS / 32) {
       const float a = s_p[lane][g], c = s_p[lane + 32][g];
       const float m_old = s_m[g];
       const float m_new = fmaxf(m_old, warp_max(fmaxf(a, c)));
-      const float pa = ex2f(a - m_new), pc = ex2f(c - m_new);
+      const float m_ref = CHUNK && m_new == -INFINITY ? 0.f : m_new;
+      const float pa = ex2f(a - m_ref), pc = ex2f(c - m_ref);
       s_p[lane][g] = pa;
       s_p[lane + 32][g] = pc;
       const float sum = warp_sum(pa + pc);
       if (lane == 0) {
-        const float alpha = ex2f(m_old - m_new);        // m_old = -inf -> 0
+        const float alpha = ex2f(m_old - m_ref);        // m_old = -inf -> 0
         s_alpha[g] = alpha;
         s_l[g] = fmaf(s_l[g], alpha, sum);
         s_m[g] = m_new;
@@ -158,6 +188,7 @@ __global__ void __launch_bounds__(DEC_THREADS) attn_decode_kernel(const DecParam
       const float v0 = bf16lo(w), v1 = bf16hi(w);
 #pragma unroll
       for (int g = 0; g < G; ++g) {
+        if (CHUNK && kb + t >= lim[g]) continue;        // past this row's limit: not visited, as the single-query kernel does not
         const float pg = s_p[t][g];
         o[g][0] = fmaf(pg, v0, o[g][0]);
         o[g][1] = fmaf(pg, v1, o[g][1]);
@@ -176,11 +207,23 @@ __global__ void __launch_bounds__(DEC_THREADS) attn_decode_kernel(const DecParam
     float a = 0.f;
 #pragma unroll
     for (int q = 0; q < KSUB; ++q) a += s_red[q][g][d];
-    const int h = hk * G + g;
-    p.ws_o[(((size_t)b * p.nh + h) * p.nsplit + split) * HD + d] = a;
+    if constexpr (CHUNK) {
+      const int t = t0 + g / p.g;
+      if (t < p.T) p.ws_o[((((size_t)b * p.T + t) * p.nh + hk * p.g + g % p.g) * p.nsplit + split) * HD + d] = a;
+    } else {
+      const int h = hk * G + g;
+      p.ws_o[(((size_t)b * p.nh + h) * p.nsplit + split) * HD + d] = a;
+    }
   }
   if (tid < G) {
-    float* ml = p.ws_ml + (((size_t)b * p.nh + hk * G + tid) * p.nsplit + split) * 2;
+    float* ml;
+    if constexpr (CHUNK) {
+      const int t = t0 + tid / p.g;
+      if (t >= p.T) return;
+      ml = p.ws_ml + ((((size_t)b * p.T + t) * p.nh + hk * p.g + tid % p.g) * p.nsplit + split) * 2;
+    } else {
+      ml = p.ws_ml + (((size_t)b * p.nh + hk * G + tid) * p.nsplit + split) * 2;
+    }
     ml[0] = s_m[tid];
     ml[1] = s_l[tid];
   }
@@ -289,6 +332,35 @@ int launch_decode_g(const DecParams& p, int64_t batch, int G, cudaStream_t st) {
   }
 }
 
+// chunk: G = virtual heads per CTA (rows per CTA * query heads per KV head); grid y = KV head + nkv * row group
+template <int HD, int G>
+int launch_decode_chunk(const DecParams& p, int64_t batch, cudaStream_t st) {
+  constexpr int SMEM = DecCfg<HD>::SMEM;
+  static bool attr = false;
+  if (!attr) {
+    LMOD_CUDA_OK(cudaFuncSetAttribute(attn_decode_kernel<HD, G, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
+    attr = true;
+  }
+  const unsigned groups = (unsigned)((p.T + p.rows - 1) / p.rows);
+  attn_decode_kernel<HD, G, true><<<dim3(p.nsplit, p.nkv * groups, (unsigned)batch), DEC_THREADS, SMEM, st>>>(p);
+  LMOD_LAUNCH_OK();
+  return LMOD_OK;
+}
+
+template <int HD>
+int launch_decode_chunk_g(const DecParams& p, int64_t batch, int VG, cudaStream_t st) {
+  switch (VG) {
+    case 1: return launch_decode_chunk<HD, 1>(p, batch, st);
+    case 2: return launch_decode_chunk<HD, 2>(p, batch, st);
+    case 3: return launch_decode_chunk<HD, 3>(p, batch, st);
+    case 4: return launch_decode_chunk<HD, 4>(p, batch, st);
+    case 5: return launch_decode_chunk<HD, 5>(p, batch, st);
+    case 6: return launch_decode_chunk<HD, 6>(p, batch, st);
+    case 7: return launch_decode_chunk<HD, 7>(p, batch, st);
+    default: return launch_decode_chunk<HD, 8>(p, batch, st);
+  }
+}
+
 }  // namespace
 
 extern "C" int lmod_kv_append(const void* qkv, int64_t ld_qkv, int64_t batch, int64_t n_new, int nh, int nkv, int hd,
@@ -351,6 +423,44 @@ extern "C" int lmod_attn_decode(const void* q, int64_t ld_q, const void* k_cache
   int rc = hd == 128 ? launch_decode_g<128>(p, batch, G, st) : launch_decode_g<64>(p, batch, G, st);
   if (rc) return rc;
   const dim3 grid(nh, (unsigned)batch);
+  if (hd == 128) attn_decode_merge_kernel<128><<<grid, 128, 0, st>>>(p.ws_o, p.ws_ml, nh, p.nsplit, (__nv_bfloat16*)out, ld_o, lse);
+  else attn_decode_merge_kernel<64><<<grid, 64, 0, st>>>(p.ws_o, p.ws_ml, nh, p.nsplit, (__nv_bfloat16*)out, ld_o, lse);
+  LMOD_LAUNCH_OK();
+  return LMOD_OK;
+}
+
+extern "C" int64_t lmod_attn_decode_chunk_ws_elems(int64_t batch, int64_t T, int nh, int nkv, int hd, int64_t max_len) {
+  if (T <= 0) return 0;
+  return lmod_attn_decode_ws_elems(batch * T, nh, nkv, hd, max_len);
+}
+
+extern "C" int lmod_attn_decode_chunk(const void* q, int64_t ld_q, const void* k_cache, const void* v_cache, const int32_t* len,
+                                      int64_t batch, int64_t T, int nh, int nkv, int hd, int64_t max_len, float softmax_scale, void* out,
+                                      int64_t ld_o, float* lse, float* ws, int64_t ws_elems, void* stream) {
+  LMOD_CHECK_ARG(q && k_cache && v_cache && len && out && ws && batch > 0 && T > 0 && T <= 4096 && nh > 0 && nkv > 0 && nh % nkv == 0 &&
+                 max_len > 0 && max_len < (1 << 30), "lmod_attn_decode_chunk: bad arguments");
+  LMOD_CHECK_ARG(hd == 64 || hd == 128, "lmod_attn_decode_chunk: head_dim %d not built (64 and 128 are)", hd);
+  LMOD_CHECK_ARG(nh / nkv <= DEC_MAX_G, "lmod_attn_decode_chunk: %d query heads per KV head (at most %d are built)", nh / nkv, DEC_MAX_G);
+  LMOD_CHECK_ARG(ld_q % 8 == 0 && (uintptr_t)q % 16 == 0 && (uintptr_t)k_cache % 16 == 0 && (uintptr_t)v_cache % 16 == 0,
+                 "lmod_attn_decode_chunk: alignment");
+  LMOD_CHECK_ARG(ws_elems >= lmod_attn_decode_chunk_ws_elems(batch, T, nh, nkv, hd, max_len), "lmod_attn_decode_chunk: workspace too small");
+  DecParams p;
+  p.q = (const __nv_bfloat16*)q; p.ld_q = ld_q;
+  p.k = (const __nv_bfloat16*)k_cache; p.v = (const __nv_bfloat16*)v_cache; p.len = len;
+  p.nh = nh; p.nkv = nkv; p.max_len = (int)max_len;
+  p.nsplit = decode_splits(max_len, nkv, &p.split_blocks);
+  p.ws_o = ws;
+  p.ws_ml = ws + batch * T * nh * (int64_t)p.nsplit * hd;
+  p.scale_log2 = softmax_scale * LOG2E_F;
+  p.T = (int)T;
+  p.g = nh / nkv;
+  p.rows = (int)std::min<int64_t>(T, DEC_MAX_G / p.g);
+  cudaStream_t st = (cudaStream_t)stream;
+  const int VG = p.rows * p.g;
+  int rc = hd == 128 ? launch_decode_chunk_g<128>(p, batch, VG, st) : launch_decode_chunk_g<64>(p, batch, VG, st);
+  if (rc) return rc;
+  // the merge is lmod_attn_decode's, over batch * T rows
+  const dim3 grid(nh, (unsigned)(batch * T));
   if (hd == 128) attn_decode_merge_kernel<128><<<grid, 128, 0, st>>>(p.ws_o, p.ws_ml, nh, p.nsplit, (__nv_bfloat16*)out, ld_o, lse);
   else attn_decode_merge_kernel<64><<<grid, 64, 0, st>>>(p.ws_o, p.ws_ml, nh, p.nsplit, (__nv_bfloat16*)out, ld_o, lse);
   LMOD_LAUNCH_OK();

@@ -486,6 +486,68 @@ def attn_decode(q, nh, nkv, hd, k_cache, v_cache, lens, ws, scale=None, need_lse
     return out, lse
 
 
+
+def attn_decode_chunk_ws_elems(B, T, nh, nkv, hd, max_len):
+    return int(_C.lib().lmod_attn_decode_chunk_ws_elems(B, T, nh, nkv, attn_head_dim(hd), max_len))
+
+
+def attn_decode_chunk(q, B, T, nh, nkv, hd, k_cache, v_cache, lens, ws, scale=None, need_lse=False):
+    """T new query rows per sequence over the cache (lmod_attn_decode_chunk): row t of sequence b attends to keys
+    [0, lens[b] - T + t + 1), where lens is the length after the T rows' k / v were appended.  q: [B*T, >= nh*hd] rows (row b*T + t);
+    k_cache / v_cache [B, nkv, max_len, hp]; lens int32 [B] on the device; ws fp32 of at least attn_decode_chunk_ws_elems(...).
+    Row t gives the bytes attn_decode gives for that row alone at lens[b] - T + t + 1.  -> (out [B*T, nh*hd] bf16, lse [B*T, nh] or None)."""
+    _need_cuda(q, k_cache, v_cache, lens, ws)
+    _check_cache(k_cache, v_cache, B, nkv, hd)
+    _check_i32(lens, B, "lens")
+    if T < 1 or q.dim() != 2 or q.shape[0] != B * T or q.shape[1] < nh * hd or q.stride(1) != 1 or q.dtype != BF16:
+        raise _C.LmodError("attn_decode_chunk: q must be bf16 [B*T, >= nh*hd] with unit column stride, got %s %s" % (q.dtype, tuple(q.shape)))
+    if ws.dtype != torch.float32 or not ws.is_contiguous():
+        raise _C.LmodError("attn_decode_chunk: ws must be a contiguous fp32 tensor")
+    hp, max_len = k_cache.shape[-1], k_cache.shape[2]
+    scale = float(scale if scale is not None else hd ** -0.5)
+    if hp != hd:
+        q = _pad_heads(q[:, :nh * hd], nh, hd, hp)
+    out = torch.empty(B * T, nh * hp, dtype=q.dtype, device=q.device)
+    lse = torch.empty(B * T, nh, dtype=torch.float32, device=q.device) if need_lse else None
+    call("lmod_attn_decode_chunk", ptr(q), q.stride(0), ptr(k_cache), ptr(v_cache), ptr(lens), B, T, nh, nkv, hp, max_len, scale, ptr(out),
+         out.stride(0), ptr(lse), ptr(ws), ws.numel())
+    if hp != hd:
+        out = out.view(B * T, nh, hp)[:, :, :hd].reshape(B * T, nh * hd)
+    return out, lse
+
+
+def spec_accept(target_logits, draft_tokens, draft_logits=None, u=None, len_target=None, len_draft=None):
+    """Acceptance of one assisted-decoding round (lmod_spec_accept).  target_logits fp32 [B, k+1, V_t]: row j scores draft token j+1 (row k
+    the bonus token); draft_tokens int64 [B, k].  Greedy (u None): accept while the draft equals the target's argmax.  Sampling: u fp32
+    [B, k+1] uniforms and draft_logits fp32 [B, k, V_d], both after the logits processors (-inf = probability 0).  len_target / len_draft:
+    int32 [B] cache lengths, rolled back on the device by k - n_acc.  -> (n_acc int32 [B], next int64 [B]) on the device."""
+    if target_logits.dim() != 3 or target_logits.dtype != torch.float32:
+        raise _C.LmodError("spec_accept: target_logits must be fp32 [B, k+1, V], got %s %s" % (target_logits.dtype, tuple(target_logits.shape)))
+    B, k1, V_t = target_logits.shape
+    k = k1 - 1
+    if k < 1 or draft_tokens.dtype != torch.int64 or tuple(draft_tokens.shape) != (B, k):
+        raise _C.LmodError("spec_accept: draft_tokens must be int64 [B, k] with k >= 1, got %s %s" % (draft_tokens.dtype, tuple(draft_tokens.shape)))
+    V_d = 0
+    if u is not None:
+        if draft_logits is None or draft_logits.dim() != 3 or draft_logits.dtype != torch.float32 or tuple(draft_logits.shape[:2]) != (B, k):
+            raise _C.LmodError("spec_accept: sampling needs fp32 draft_logits [B, k, V_d]")
+        if u.dtype != torch.float32 or tuple(u.shape) != (B, k + 1):
+            raise _C.LmodError("spec_accept: u must be fp32 [B, k+1], got %s %s" % (u.dtype, tuple(u.shape)))
+        V_d = draft_logits.shape[2]
+        draft_logits, u = draft_logits.contiguous(), u.contiguous()
+        _need_cuda(draft_logits, u)
+    for t, name in ((len_target, "len_target"), (len_draft, "len_draft")):
+        if t is not None:
+            _need_cuda(t)
+            _check_i32(t, B, name)
+    target_logits, draft_tokens = target_logits.contiguous(), draft_tokens.contiguous()
+    _need_cuda(target_logits, draft_tokens)
+    n_acc = torch.empty(B, dtype=torch.int32, device=target_logits.device)
+    nxt = torch.empty(B, dtype=torch.int64, device=target_logits.device)
+    call("lmod_spec_accept", ptr(target_logits), V_t, ptr(draft_logits) if u is not None else None, V_d, ptr(draft_tokens), ptr(u), B, k,
+         ptr(n_acc), ptr(nxt), ptr(len_target), ptr(len_draft))
+    return n_acc, nxt
+
 def pad_ranges(attention_mask):
     """[B,T] bool mask (contiguous real tokens, right or left padded -- what the collators and the multimodal splice produce) ->
     (kv_lo, kv_hi) int32 [B] on the device, no host sync."""

@@ -25,7 +25,18 @@ The result is HF's layout: the input ids as given, pads included, followed by th
 unpadded path unchanged.  (The reference's own batched decoding differs from this for padded image batches and right-padded batches,
 DESIGN section 8.)
 
-Supported: greedy, temperature / top-p sampling, num_beams == 1, EOS and `stopping_criteria` callables, padded or unpadded batches."""
+Assisted (speculative) decoding, generate(..., assistant_model=draft, num_assistant_tokens=k), HF's names with k fixed per call: the
+draft (dense or sparse, e.g. the distilled student) proposes k tokens with k + 1 of its own one-token cached steps, the target (dense)
+scores all of them in one cached step of k + 1 tokens per sequence, and lmod_spec_accept (csrc/spec.cu) decides on the device how many
+are kept, picks the next token and rolls both caches back; the host reads (n_acc, next) once per round.  Greedy: the target's argmax
+is kept wherever it differs from the draft, and the verify step gives each row the bytes of a one-token step, so the tokens are exactly
+those of generate(use_cache=True) on the target.  Sampling follows Leviathan et al. (HF _speculative_sampling): the tokens have the
+target's distribution.  Both models prefill the prompt with their own tower; padded batches work as in plain cached decoding and
+sequences accept different counts.  EOS and max_new_tokens are applied to each round's tokens and stopping_criteria is called once per
+round, as HF does.  The per-call counts are kept in `last_assisted_stats`.
+
+Supported: greedy, temperature / top-p sampling, num_beams == 1, EOS and `stopping_criteria` callables, padded or unpadded batches,
+assisted decoding with a dense target."""
 import collections
 import os
 import weakref
@@ -35,8 +46,9 @@ import torch
 from .. import kernels as K
 
 CACHE_BUCKET = 512
-_STEP_GRAPHS = collections.OrderedDict()     # (model id, B, max_len, weight pointers) -> dict(model, cache, graph, ids, logits)
+_STEP_GRAPHS = collections.OrderedDict()     # (model id, B, max_len, T, weight pointers) -> dict(model, cache, graph, ids, logits)
 _GRAPH_POOL = None
+last_assisted_stats = None                   # counts of the last assisted generate call: rounds, drafted and accepted per sequence
 
 
 @torch.no_grad()
@@ -69,8 +81,9 @@ def _graphs_enabled():
     return bool(int(os.environ.get("LLAVAMOD_CUDA_GRAPHS", "1")))
 
 
-def _decoder_entry(model, B, max_len):
-    """(cache, graph slot) for B sequences of up to max_len positions, reused across calls while graphs are on.  A captured step holds
+def _decoder_entry(model, B, max_len, T=1):
+    """(cache, graph slot) for B sequences of up to max_len positions and steps of T tokens per sequence, reused across calls while graphs
+    are on (T > 1: the verify step of assisted decoding; a model that is its own assistant gets one entry per width).  A captured step holds
     the addresses of the cache buffers and of the weights, and the host decisions made while it was captured: the MoE capacity rule of
     every sparse layer and the epilogue-fusion switches.  All of them are part of the key."""
     if not _graphs_enabled():
@@ -79,7 +92,7 @@ def _decoder_entry(model, B, max_len):
         del _STEP_GRAPHS[k]
     moe = tuple((l.mlp.num_experts, l.mlp.capacity_factor, l.mlp.eval_capacity_factor, l.mlp.min_capacity)
                 for l in model.model.layers if hasattr(l.mlp, "deepspeed_moe"))
-    key = (id(model), B, max_len, model.training, moe, K.FUSE_SWIGLU, K.FUSE_ROPE, K.FUSE_RESIDUAL,
+    key = (id(model), B, max_len, T, model.training, moe, K.FUSE_SWIGLU, K.FUSE_ROPE, K.FUSE_RESIDUAL,
            tuple(p.data_ptr() for p in model.parameters()))
     ent = _STEP_GRAPHS.pop(key, None)
     if ent is None or ent["model"]() is not model:
@@ -91,12 +104,22 @@ def _decoder_entry(model, B, max_len):
     return ent
 
 
+@torch.no_grad()
+def chunk_logits(model, input_ids, cache):
+    """fp32 logits [B, T, V] of every position of a cached step of input_ids [B, T]."""
+    h = model.forward_hidden(input_ids=input_ids, cache=cache)["hidden"]
+    B, T, H = h.shape
+    return K.mm_nt(h.reshape(B * T, H), model.lm_head.weight).float().view(B, T, -1)
+
+
 def _decode_step(model, ent, tok, eager):
-    """fp32 logits [B, V] of the next position after feeding tok [B] at the cache's current length."""
+    """fp32 logits [B, V] of the next position after feeding tok [B] at the cache's current length; tok [B, T]: logits [B, T, V] of
+    the T positions (one cached step of T tokens per sequence)."""
     global _GRAPH_POOL
     cache = ent["cache"]
+    step = (lambda ids: next_token_logits(model, ids[:, None], cache=cache)) if tok.dim() == 1 else (lambda ids: chunk_logits(model, ids, cache))
     if eager:
-        return next_token_logits(model, tok[:, None], cache=cache)
+        return step(tok)
     if ent["graph"] is None:
         ent["ids"] = tok.clone()
         n0 = list(cache.lengths)
@@ -104,23 +127,52 @@ def _decode_step(model, ent, tok, eager):
         if _GRAPH_POOL is None:
             _GRAPH_POOL = torch.cuda.graph_pool_handle()
         with torch.cuda.graph(g, pool=_GRAPH_POOL):
-            ent["logits"] = next_token_logits(model, ent["ids"][:, None], cache=cache)
+            ent["logits"] = step(ent["ids"])
         cache.lengths = n0                      # the capture ran the host code of a step; nothing ran on the device
         ent["graph"] = g
-    cache.check(tok.shape[0], 1)
+    T = 1 if tok.dim() == 1 else tok.shape[1]
+    cache.check(tok.shape[0], T)
     ent["ids"].copy_(tok)
     ent["graph"].replay()
-    cache.advance(1)
+    cache.advance(T)
     return ent["logits"].clone()
+
+
+def _process(logits, n_vocab, do_sample, temperature, top_p):
+    """The logits processors of a step: the narrowed vocabulary, then (sampling) temperature and top-p.  In place where possible."""
+    if n_vocab is not None and n_vocab < logits.shape[-1]:
+        logits[..., n_vocab:] = float("-inf")
+    if do_sample:
+        if temperature is not None and temperature != 1.0:
+            logits = logits / float(temperature)
+        if top_p is not None and top_p < 1.0:
+            logits = _top_p_filter(logits, float(top_p))
+    return logits
+
+
+def _pick(logits, do_sample, generator):
+    if do_sample:
+        return torch.multinomial(logits.softmax(dim=-1), 1, generator=generator).squeeze(1)
+    return logits.argmax(dim=-1)
 
 
 @torch.no_grad()
 def generate(model, inputs=None, images=None, attention_mask=None, max_new_tokens=20, do_sample=False, temperature=1.0, top_p=None,
-             num_beams=1, use_cache=False, stopping_criteria=None, eos_token_id=None, pad_token_id=None, generator=None, **unused):
+             num_beams=1, use_cache=False, stopping_criteria=None, eos_token_id=None, pad_token_id=None, generator=None,
+             assistant_model=None, num_assistant_tokens=5, **unused):
     """-> [B, T_in + n_new] int64: the prompt ids (image placeholders -200 included, pads included, as HF returns them) followed by the
-    new tokens."""
+    new tokens.  assistant_model: a draft model for assisted decoding (use_cache=True, dense target), num_assistant_tokens = k drafted
+    tokens per round."""
     if num_beams != 1:
         raise NotImplementedError("beam search is not built (the reference's eval shells run num_beams=1)")
+    if assistant_model is not None:
+        if not use_cache:
+            raise ValueError("generate: assisted decoding needs use_cache=True (the draft and the verify step decode against KV caches)")
+        if getattr(model, "is_moe", False):
+            raise ValueError("generate: assisted decoding needs a dense target; a sparse model cannot verify k + 1 tokens in one step "
+                             "(it would route them together)")
+        if int(num_assistant_tokens) < 1:
+            raise ValueError("generate: num_assistant_tokens must be >= 1, got %r" % (num_assistant_tokens,))
     dev = model.device
     ids = inputs.to(dev)
     mask = None
@@ -149,6 +201,12 @@ def generate(model, inputs=None, images=None, attention_mask=None, max_new_token
     done = torch.zeros(B, dtype=torch.bool, device=dev)
     ent = None
     ragged = mask is not None
+    if assistant_model is not None and int(max_new_tokens) > 0:
+        ids = _assisted(model, assistant_model, ids, images, feats, mask, int(max_new_tokens), int(num_assistant_tokens), do_sample,
+                        temperature, top_p, stopping_criteria, eos, pad, generator, n_vocab)
+        if was_training:
+            model.train()
+        return ids
     if use_cache and int(max_new_tokens) > 0:
         need = max(model.spliced_length(ids, images, mask)) + int(max_new_tokens)
         ent = _decoder_entry(model, B, (need + CACHE_BUCKET - 1) // CACHE_BUCKET * CACHE_BUCKET)
@@ -168,16 +226,8 @@ def generate(model, inputs=None, images=None, attention_mask=None, max_new_token
         elif step > 0:
             eager = not _graphs_enabled() or (step == 1 and ent["graph"] is None)      # one eager step before the capture
             logits = _decode_step(model, ent, nxt, eager)
-        if n_vocab is not None and n_vocab < logits.shape[-1]:
-            logits[:, n_vocab:] = float("-inf")
-        if do_sample:
-            if temperature is not None and temperature != 1.0:
-                logits = logits / float(temperature)
-            if top_p is not None and top_p < 1.0:
-                logits = _top_p_filter(logits, float(top_p))
-            nxt = torch.multinomial(logits.softmax(dim=-1), 1, generator=generator).squeeze(1)
-        else:
-            nxt = logits.argmax(dim=-1)
+        logits = _process(logits, n_vocab, do_sample, temperature, top_p)
+        nxt = _pick(logits, do_sample, generator)
         nxt = torch.where(done, torch.full_like(nxt, pad), nxt)
         ids = torch.cat([ids, nxt[:, None]], dim=1)
         if ent is None and ragged:
@@ -193,3 +243,115 @@ def generate(model, inputs=None, images=None, attention_mask=None, max_new_token
     if was_training:
         model.train()
     return ids
+
+
+def _bucket(n):
+    return (n + CACHE_BUCKET - 1) // CACHE_BUCKET * CACHE_BUCKET
+
+
+def _assisted(model, draft, ids, images, feats, mask, max_new, k, do_sample, temperature, top_p, stopping_criteria, eos, pad, generator,
+              n_vocab):
+    """Assisted decoding (module docstring).  Each round ends with both caches at base + n_acc + 1 rows: the draft's k + 1 steps and the
+    verify step add k + 1, lmod_spec_accept takes back the k - n_acc rejected ones.  A sequence that is finished (EOS or max_new tokens)
+    keeps running with the batch, but its cache rows are taken back after every round, so no cache grows past what it was sized for."""
+    global last_assisted_stats
+    dev = model.device
+    B = ids.shape[0]
+    ragged = mask is not None
+    dmask = mask.to(dev) if ragged else None
+    was_training = draft.training
+    draft.eval()
+    dfeats = None
+    if images is not None and draft.get_image_tower() is not None:
+        dfeats = draft.get_image_tower()(images.to(draft.dtype))
+    d_vocab = [v for v in (getattr(draft, "_active_vocab", None), n_vocab) if v is not None]
+    d_vocab = min(d_vocab) if d_vocab else None
+    ent_t = _decoder_entry(model, B, _bucket(max(model.spliced_length(ids, images, mask)) + max_new + k + 1), T=k + 1)
+    ent_d = _decoder_entry(draft, B, _bucket(max(draft.spliced_length(ids, images, mask)) + max_new + k + 1))
+    ct, cd = ent_t["cache"], ent_d["cache"]
+    logits = next_token_logits(model, ids, images=images, tower_features=feats, attention_mask=dmask, cache=ct, ragged=ragged)
+    draft.forward_hidden(input_ids=ids, attention_mask=dmask, images=images, tower_features=dfeats, cache=cd)
+    logits = _process(logits, n_vocab, do_sample, temperature, top_p)
+    first = _pick(logits, do_sample, generator)
+    out = [[t] for t in first.tolist()]
+    done = [bool(eos) and row[0] in eos for row in out]
+    last = first
+    rounds, drafted, accepted = 0, [0] * B, [0] * B
+    graphs = _graphs_enabled()
+    warm = set()
+
+    def step(ent, tok):
+        eager = not graphs or (ent["graph"] is None and id(ent) not in warm)       # one eager step of each entry before its capture
+        warm.add(id(ent))
+        return _decode_step(draft if ent is ent_d else model, ent, tok, eager)
+
+    def complete(b):
+        return done[b] or len(out[b]) >= max_new
+
+    stop = all(complete(b) for b in range(B))
+    if not stop and stopping_criteria:
+        stop = any(bool(c(_assemble(ids, out, pad, max_new), logits)) for c in stopping_criteria)
+    while not stop:
+        active = [not complete(b) for b in range(B)]
+        base_t, base_d = list(ct.lengths), list(cd.lengths)
+        tok, dtoks, dlogits = last, [], []
+        for j in range(k + 1):
+            lg = step(ent_d, tok)
+            if j == k:
+                break                                # the last draft step only puts d_k into the draft's cache
+            lg = _process(lg, d_vocab, do_sample, temperature, top_p)
+            tok = _pick(lg, do_sample, generator)
+            dtoks.append(tok)
+            if do_sample:
+                dlogits.append(lg)
+        dtoks = torch.stack(dtoks, 1)
+        vlogits = step(ent_t, torch.cat([last[:, None], dtoks], 1))
+        vlogits = _process(vlogits, n_vocab, do_sample, temperature, top_p)
+        if do_sample:
+            u = torch.rand(B, k + 1, device=dev, dtype=torch.float32, generator=generator)
+            n_acc, nxt = K.spec_accept(vlogits, dtoks, torch.stack(dlogits, 1), u, ct.len, cd.len)
+        else:
+            n_acc, nxt = K.spec_accept(vlogits, dtoks, None, None, ct.len, cd.len)
+        host = torch.cat([n_acc.to(torch.int64), nxt, dtoks.reshape(-1)]).tolist()      # the round's one device-to-host read
+        n_acc, nxt, dt = host[:B], host[B:2 * B], host[2 * B:]
+        ct.rollback([k - n for n in n_acc])
+        cd.rollback([k - n for n in n_acc])
+        rounds += 1
+        for b in range(B):
+            if not active[b]:
+                continue
+            drafted[b] += k
+            accepted[b] += n_acc[b]
+            for t in dt[b * k:b * k + n_acc[b]] + [nxt[b]]:
+                out[b].append(t)
+                if t in eos:
+                    done[b] = True
+                    break
+        # finished sequences: back to where they were, so their caches stay within their size
+        drop = [0 if active[b] and not complete(b) else ct.lengths[b] - base_t[b] for b in range(B)]
+        if any(drop):
+            dd = torch.tensor(drop, dtype=torch.int32, device=dev)
+            ct.len.sub_(dd)
+            ct.rollback(drop)
+            dd = torch.tensor([cd.lengths[b] - base_d[b] if drop[b] else 0 for b in range(B)], dtype=torch.int32, device=dev)
+            cd.len.sub_(dd)
+            cd.rollback(dd.tolist())
+        last = torch.tensor([pad if done[b] else out[b][-1] for b in range(B)], dtype=torch.int64, device=dev)
+        stop = all(complete(b) for b in range(B))
+        if not stop and stopping_criteria:
+            rows = torch.tensor(n_acc, dtype=torch.int64, device=dev)
+            stop = any(bool(c(_assemble(ids, out, pad, max_new), vlogits[torch.arange(B, device=dev), rows])) for c in stopping_criteria)
+    last_assisted_stats = dict(rounds=rounds, drafted=drafted, accepted=accepted)
+    if was_training:
+        draft.train()
+    return _assemble(ids, out, pad, max_new)
+
+
+def _assemble(ids, out, pad, max_new):
+    """The prompt ids followed by each sequence's new tokens, as many columns as the longest (at most max_new), finished rows padded."""
+    W = min(max_new, max(len(r) for r in out))
+    new = torch.full((len(out), W), pad, dtype=torch.int64)
+    for b, r in enumerate(out):
+        r = r[:W]
+        new[b, :len(r)] = torch.tensor(r, dtype=torch.int64)
+    return torch.cat([ids, new.to(ids.device)], dim=1)

@@ -137,11 +137,10 @@ class LlavaQwenForCausalLMBase(nn.Module, LlavaMetaForCausalLM):
     def forward_hidden(self, input_ids=None, attention_mask=None, position_ids=None, inputs_embeds=None, labels=None,
                        images=None, moe_noise=None, tower_features=None, plan=None, cache=None):
         """Splice + decoder.  Returns dict(hidden [B,T',H], labels [B,T'], attention_mask, l_aux list).
-        cache: a KVCache -- empty: prefill into it; holding a prefix: input_ids [B,1] is one decode step (no splice, as llava_arch.py:162)."""
+        cache: a KVCache -- empty: prefill into it; holding a prefix: input_ids [B,T] is one cached step of T tokens per sequence (no
+        splice, as llava_arch.py:162); T > 1 for dense models only."""
         if cache is not None and cache.length > 0 and inputs_embeds is None:
             ids = input_ids.to(self.device)
-            if ids.shape[1] != 1:
-                raise NotImplementedError("a cached step decodes one token per sequence (got %d)" % ids.shape[1])
             inputs_embeds = torch.nn.functional.embedding(ids, self.model.embed_tokens.weight)
             attention_mask = None
         if inputs_embeds is None:

@@ -258,8 +258,9 @@ class Qwen2Model(nn.Module):
     # -- forward -------------------------------------------------------------------------------------
     def forward(self, inputs_embeds, attention_mask=None, position_ids=None, moe_noise=None, training_moe=True, cache=None):
         """inputs_embeds [B,T,H] bf16; attention_mask [B,T] bool or None; position_ids [B,T] int64 or None.
-        cache: a KVCache.  Empty: the prefill -- this forward, plus the K / V of every layer appended to the cache.  Holding a prefix and
-        T == 1: one decode step at position len (modeling_qwen2.py:652-728 with past_key_value), attention over the cached keys.
+        cache: a KVCache.  Empty: the prefill -- this forward, plus the K / V of every layer appended to the cache.  Holding a prefix: one
+        cached step of T tokens per sequence at positions len .. len + T - 1 (modeling_qwen2.py:652-728 with past_key_value), attention
+        over the cached keys; T > 1 for dense models only.
         A padded prefill (attention_mask with zeros; real tokens contiguous, either side) is this same padded forward, with positions
         0 .. n_b - 1 over sequence b's real rows when position_ids is None; only the real rows go to the cache, packed at [0, n_b).
         Returns (final-normed hidden [B,T,H], [l_aux per MoE layer], routing records)."""
@@ -365,6 +366,10 @@ class Qwen2Model(nn.Module):
         """One cached step: each sequence's new token sits at position len[b] (the reference's rule for a cached step,
         llava_arch.py:162-172, on unpadded prompts; for a padded prompt len[b] = n_b + s counts its real rows only), its k / v are appended
         at row len[b], and its query attends to rows [0, len[b] + 1).
+        T > 1 tokens per sequence (the verify step of assisted decoding): token t sits at position len[b] + t, the T rows are appended at
+        once and token t attends to rows [0, len[b] + t + 1) (lmod_attn_decode_chunk).  Every kernel of the step works row by row, and
+        the chunked attention gives each row the bytes of the single-query kernel, so for a dense model this is T one-token steps, bit for
+        bit.
         Everything the step reads about the position is on the device, so the step can be captured once and replayed.  MoE layers route
         the B new tokens alone (top2gating with S = B, as MoEQwen1_5Model_forward does with a cache, llava_qwen1_5_moe.py:223-236).
         The layer body is forward's no-grad layer body with the attention swapped for append + decode attention: the same norm and
@@ -372,14 +377,21 @@ class Qwen2Model(nn.Module):
         tests/test_decode_gpu.py checks that the two give the same K / V, bit for bit."""
         cfg = self.config
         B, T, H = inputs_embeds.shape
-        if T != 1:
-            raise NotImplementedError("a cached step decodes one token per sequence (got %d)" % T)
-        cache.check(B, 1)
+        if T != 1 and any(isinstance(l.mlp, MoE) for l in self.layers):
+            raise NotImplementedError("a cached step of the sparse model decodes one token per sequence (got %d): a step of T tokens would "
+                                      "route its B*T tokens together (top2gating with S = B*T), which is not what T one-token steps "
+                                      "compute" % T)
+        cache.check(B, T)
         dev = inputs_embeds.device
         cos, sin = cache.rope
-        torch.add(cache.len, 1, out=cache.end)
-        cache.pos.copy_(cache.len)
-        stream = inputs_embeds.reshape(B, H)
+        torch.add(cache.len, T, out=cache.end)
+        if T == 1:
+            pos = cache.pos
+            pos.copy_(cache.len)
+        else:
+            pos = (cache.len.to(torch.int64)[:, None] + torch.arange(T, device=dev, dtype=torch.int64)[None, :]).reshape(B * T)
+            ws = cache.chunk_workspace(T)
+        stream = inputs_embeds.reshape(B * T, H)
         branch = None
         l_auxes, records = [], []
         moe_i = 0
@@ -390,9 +402,12 @@ class Qwen2Model(nn.Module):
                 x, stream = K.rmsnorm(stream, layer.input_layernorm.weight, cfg.rms_norm_eps)
             else:
                 x, stream = K.rmsnorm(branch, layer.input_layernorm.weight, cfg.rms_norm_eps, res=stream)
-            qkv = K.qkv_rope(x, at.qkv_weight, at.qkv_bias, cos, sin, cache.pos, nh, nkv, hd)
-            K.kv_append(qkv, B, 1, nh, nkv, hd, cache.k[li], cache.v[li], cache.len)
-            attn, _ = K.attn_decode(qkv, nh, nkv, hd, cache.k[li], cache.v[li], cache.end, cache.ws)
+            qkv = K.qkv_rope(x, at.qkv_weight, at.qkv_bias, cos, sin, pos, nh, nkv, hd)
+            K.kv_append(qkv, B, T, nh, nkv, hd, cache.k[li], cache.v[li], cache.len)
+            if T == 1:
+                attn, _ = K.attn_decode(qkv, nh, nkv, hd, cache.k[li], cache.v[li], cache.end, cache.ws)
+            else:
+                attn, _ = K.attn_decode_chunk(qkv, B, T, nh, nkv, hd, cache.k[li], cache.v[li], cache.end, ws)
             if K.residual_fusable(attn, stream):
                 stream = K.gemm_residual(attn, at.o_proj.weight, None, stream)
                 x, stream = K.rmsnorm(stream, layer.post_attention_layernorm.weight, cfg.rms_norm_eps)
@@ -420,8 +435,8 @@ class Qwen2Model(nn.Module):
         else:
             out, _ = K.rmsnorm(branch, self.norm.weight, cfg.rms_norm_eps, res=stream)
         cache.len.copy_(cache.end)
-        cache.advance(1)
-        return out.view(B, 1, H), l_auxes, records
+        cache.advance(T)
+        return out.view(B, T, H), l_auxes, records
 
 
 class KVCache:
@@ -449,6 +464,8 @@ class KVCache:
         self.end = torch.zeros(batch, dtype=torch.int32, device=dev)          # len + 1 during a decode step
         self.pos = torch.zeros(batch, dtype=torch.int64, device=dev)          # RoPE positions of a decode step
         self.ws = torch.empty(max(1, K.attn_decode_ws_elems(batch, nh, nkv, self.head_dim, max_len)), dtype=torch.float32, device=dev)
+        self._chunk_ws = {}                                                   # T -> workspace of a T-token step
+        self._shape = (nh, nkv)
         self.rope = model.rope(max_len, dev, dt)
         self.lengths = [0] * self.batch
 
@@ -473,6 +490,23 @@ class KVCache:
     def reset(self):
         self.len.zero_()
         self.lengths = [0] * self.batch
+
+    def rollback(self, n_drop):
+        """Forget the last n_drop[b] rows of every sequence (an int for all, or one per sequence) in the host mirror ``lengths``; the caller
+        has applied the same rollback to the device ``len`` (lmod_spec_accept does it on the device)."""
+        drop = self._per_seq(n_drop)
+        if any(d < 0 or d > n for d, n in zip(drop, self.lengths)):
+            raise ValueError("KVCache.rollback: cannot drop %s rows from lengths %s" % (drop, self.lengths))
+        self.lengths = [n - d for n, d in zip(self.lengths, drop)]
+
+    def chunk_workspace(self, T):
+        """The decode-attention workspace of a step of T tokens per sequence (kept, so a captured step keeps its address)."""
+        ws = self._chunk_ws.get(T)
+        if ws is None:
+            nh, nkv = self._shape
+            n = K.attn_decode_chunk_ws_elems(self.batch, T, nh, nkv, self.head_dim, self.max_len)
+            ws = self._chunk_ws[T] = torch.empty(max(1, n), dtype=torch.float32, device=self.len.device)
+        return ws
 
     def get_seq_length(self, layer_idx=0):
         return self.length

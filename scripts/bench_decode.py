@@ -1,7 +1,7 @@
 """Decoding benchmark: tokens/s of `generate` with and without the KV cache, decode-attention bandwidth, and the device time per
 kernel family of one cached decode step.
 
-    python scripts/bench_decode.py [--models student,teacher] [--new 128,512] [--batch 1,8] [--profile] [--ragged] [--out DIR]
+    python scripts/bench_decode.py [--models student,teacher] [--new 128,512] [--batch 1,8] [--profile] [--ragged] [--assisted] [--out DIR]
 
 * generate: the 0.5B-4E student and the 7B teacher (random weights, CLIP-L/336) on a prompt that splices to T' = 650 positions, greedy,
   use_cache False / True, CUDA graphs on / off (LLAVAMOD_CUDA_GRAPHS).  Tokens/s = B * new tokens / wall time of the call, which ends in
@@ -13,6 +13,12 @@ kernel family of one cached decode step.
 * --ragged: B = 8 seeded prompts of different lengths (one image each, left-padded, spliced to 600-1100 positions), greedy, graphs on,
   2 new tokens (a short-answer eval, dominated by the prefill) and 128: one padded B = 8 call, eight B = 1 calls on the same prompts,
   and the equal-length B = 8 row (T' = 650), each as prompts/s and tokens/s (median of --repeat timed passes after one warm-up pass).
+* --assisted: the 7B teacher with the 0.5B-4E student as draft (random weights, T' = 650, greedy, graphs on, the first --new value of new
+  tokens), B from --batch, k = 2 and 4: tokens/s of the teacher alone, of assisted decoding with the teacher as its own assistant (every
+  draft kept: the pure overhead of the scheme) and with the random student (almost every draft rejected: the worst case); and the device
+  time (CUDA events over 20 graph replays / launches) of one draft step, one verify step of k + 1 tokens, one teacher step and one accept
+  launch, with the per-token acceptance alpha at which a round breaks even with the teacher alone.  alpha of a trained pair is not
+  measured here (random weights).
 The card's name and power limit are read in the same process and printed with the results (one JSON line per measurement)."""
 import argparse
 import json
@@ -110,6 +116,88 @@ def bench_ragged(model, name, new, out, info, repeat):
                        min_s=round(secs[0], 4), max_s=round(secs[-1], 4), card=info))
 
 
+def _timed_generate(fn, repeat):
+    fn()                                                                         # warm-up (and graph capture)
+    secs = []
+    for _ in range(repeat):
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        fn()
+        torch.cuda.synchronize()
+        secs.append(time.perf_counter() - t0)
+    return sorted(secs)
+
+
+def _replay_ms(fn, n=20):
+    for _ in range(3):
+        fn()
+    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    a.record()
+    for _ in range(n):
+        fn()
+    b.record()
+    torch.cuda.synchronize()
+    return a.elapsed_time(b) / n
+
+
+def _step_graph(model, B, T, ids, imgs):
+    """A captured cached step of T tokens per sequence after the prompt, on its own cache (replays move the device lengths only)."""
+    from llavamod.model import generation as Gm
+    ent = dict(cache=model.new_kv_cache(B, 2048), graph=None)
+    with torch.no_grad():
+        Gm.next_token_logits(model, ids, images=imgs, cache=ent["cache"])
+        tok = torch.zeros((B,) if T == 1 else (B, T), dtype=torch.int64, device="cuda")
+        Gm._decode_step(model, ent, tok, eager=True)
+        Gm._decode_step(model, ent, tok, eager=False)
+    return ent["graph"]
+
+
+def _break_even(ratio, k):
+    """alpha with (1 - alpha^(k+1)) / (1 - alpha) = ratio (tokens per round needed to match the teacher alone); None past k + 1."""
+    if ratio >= k + 1:
+        return None
+    lo, hi = 0.0, 1.0
+    for _ in range(60):
+        mid = (lo + hi) / 2
+        if sum(mid ** i for i in range(k + 1)) < ratio:
+            lo = mid
+        else:
+            hi = mid
+    return round(lo, 3)
+
+
+def bench_assisted(teacher, student, batches, new, out, info, repeat):
+    from llavamod import kernels as K
+    from llavamod.model import generation as Gm
+    os.environ["LLAVAMOD_CUDA_GRAPHS"] = "1"
+    for B in batches:
+        ids, imgs = prompt(B)
+        kw = dict(images=imgs, max_new_tokens=new, use_cache=True, eos_token_id=-1)
+        rows = [("teacher_alone", None, 0)] + [(n, d, k) for k in (2, 4) for n, d in (("self_assisted", teacher), ("student_assisted", student))]
+        for row, draft, k in rows:
+            extra = dict(assistant_model=draft, num_assistant_tokens=k) if draft is not None else {}
+            secs = _timed_generate(lambda: teacher.generate(ids, **kw, **extra), repeat)
+            st = Gm.last_assisted_stats if draft is not None else None
+            rec = dict(kind="assisted", row=row, B=B, k=k, new=new, runs=repeat, tokens_per_s=round(B * new / secs[len(secs) // 2], 1),
+                       min=round(B * new / secs[-1], 1), max=round(B * new / secs[0], 1), card=info)
+            if st:
+                rec.update(rounds=st["rounds"], acceptance=round(sum(st["accepted"]) / max(1, sum(st["drafted"])), 3))
+            emit(out, rec)
+        t_step = _replay_ms(_step_graph(teacher, B, 1, ids, imgs).replay)
+        t_draft = _replay_ms(_step_graph(student, B, 1, ids, imgs).replay)
+        V = teacher.config.vocab_size
+        for k in (2, 4):
+            t_verify = _replay_ms(_step_graph(teacher, B, k + 1, ids, imgs).replay)
+            P = torch.randn(B, k + 1, V, device="cuda")
+            d = torch.randint(0, V, (B, k), device="cuda")
+            t_accept = _replay_ms(lambda: K.spec_accept(P, d))
+            round_ms = (k + 1) * t_draft + t_verify + t_accept
+            emit(out, dict(kind="assisted_step_ms", B=B, k=k, teacher_step=round(t_step, 3), draft_step=round(t_draft, 3),
+                           verify_step=round(t_verify, 3), accept=round(t_accept, 4), round=round(round_ms, 3),
+                           break_even_alpha=_break_even(round_ms / t_step, k), card=info))
+        torch.cuda.empty_cache()
+
+
 def bench_attention(out, info):
     from llavamod import kernels as K
     for hd, nh, nkv in [(64, 16, 16), (64, 14, 2), (128, 28, 4), (128, 32, 32)]:
@@ -183,6 +271,7 @@ def main():
     ap.add_argument("--skip-generate", action="store_true")
     ap.add_argument("--skip-attention", action="store_true")
     ap.add_argument("--ragged", action="store_true", help="padded batches of prompts of different lengths (see the module docstring)")
+    ap.add_argument("--assisted", action="store_true", help="assisted decoding, teacher with the student as draft (module docstring)")
     ap.add_argument("--repeat", type=int, default=3, help="timed generate calls per setting (median, min and max are reported)")
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
@@ -191,6 +280,11 @@ def main():
         os.makedirs(a.out, exist_ok=True)
     info = card()
     from llavamod.model import synthetic as S
+    if a.assisted:
+        teacher = S.make_teacher("qwen1.5-7b", "clip-l-336", seed=0).eval()
+        student = S.make_student("qwen1.5-0.5b", "clip-l-336", seed=1, share_tower_with=teacher).eval()
+        bench_assisted(teacher, student, [int(x) for x in a.batch.split(",")], int(a.new.split(",")[0]), a.out, info, a.repeat)
+        return
     if not a.skip_attention and not a.profile and not a.ragged:
         bench_attention(a.out, info)
     for name in a.models.split(","):
