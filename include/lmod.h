@@ -118,6 +118,20 @@ int lmod_moe_route_scatter(const void* x, const float* wg, const float* noise, i
                            float* logits, float* gates, int32_t* idx, int32_t* row, float* w,
                            int32_t* offsets, float* meta, void* xp, int32_t* ws, void* stream);
 int64_t lmod_moe_route_ws_elems(int64_t S, int E);
+/* Top-1 form (DeepSpeed-0.9.5 top1gating with random token selection, --top_k_experts 1): the same arguments and outputs, with
+ *   uniform [S,E] fp32 in [0,1) in place of the noise: among the tokens routed to expert e, the C with the largest uniform[s, e] keep
+ *   their seat (ties: the lower token index), seated in token order.  C = lmod_moe_capacity_top1 = ceil(S/E * cf) raised to
+ *   min_capacity.  idx[:,1] = row[:,1] = -1, w[:,1] = 0, w[:,0] = the raw gate of a kept token (not renormalised), 0 if dropped.
+ *   meta and offsets as for top-2, rows per expert min(n_e, C).  Three plain launches (gate, selection, seat+scatter).
+ *   Fails before any launch if S < min_capacity or C > S (top1gating's own failure cases).
+ *   ws: lmod_moe_route_top1_ws_elems(S, E) int32 elements.  The combine, scatter-backward and router-gradient entry points below serve
+ *   the top-1 record unchanged; its gate backward is lmod_moe_gate_bwd_top1. */
+int lmod_moe_capacity_top1(int64_t S, int E, double capacity_factor, int64_t min_capacity);
+int lmod_moe_route_scatter_top1(const void* x, const float* wg, const float* uniform, int64_t S, int64_t H,
+                                int E, double capacity_factor, int64_t min_capacity, int layout,
+                                float* logits, float* gates, int32_t* idx, int32_t* row, float* w,
+                                int32_t* offsets, float* meta, void* xp, int32_t* ws, void* stream);
+int64_t lmod_moe_route_top1_ws_elems(int64_t S, int E);
 /* combine einsum("sec,ecm->sm") with bf16-rounded weights + optional residual add (Appendix A step 11,
  * llava_qwen1_5_moe.py:167) */
 int lmod_moe_gather_combine(const void* y, const int32_t* row, const float* w, const void* residual,
@@ -129,6 +143,10 @@ int lmod_moe_combine_bwd(const void* dout, const void* y, const int32_t* row, co
 int lmod_moe_gate_bwd(const float* gates, const int32_t* idx, const int32_t* row, const float* dw,
                       const float* meta, const float* g_laux, int64_t S, int E, float* dlogits,
                       void* stream);
+/* top-1 gate backward: dgates[s, idx1] += dw1 for a kept token (no renormalisation), plus the l_aux term, through the softmax */
+int lmod_moe_gate_bwd_top1(const float* gates, const int32_t* idx, const int32_t* row, const float* dw,
+                           const float* meta, const float* g_laux, int64_t S, int E, float* dlogits,
+                           void* stream);
 /* dx[s] = dxp[row1] + dxp[row2] + sum_e dlogits[s,e]*wg[e] (+ dres) ; and dwg partial sums */
 int lmod_moe_scatter_bwd(const void* dxp, const int32_t* row, const float* dlogits, const float* wg,
                          const void* dres, int64_t S, int64_t H, int E, void* dx, void* stream);

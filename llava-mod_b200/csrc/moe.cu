@@ -1,5 +1,7 @@
 // moe.cu -- DeepSpeed-0.9.5 top-2 MoE routing on H100: gate (GEMV + softmax + top-2) and seat+scatter (stable capacity positions by
 // warp ballots, token copy) as two ordinary launches of small CTAs; weighted gather/combine; and their backward kernels.
+// Top-1 (top1gating with random token selection) reuses the gate and seat+scatter kernels through a template flag, with a selection
+// launch between them that finds, per expert, which routed tokens keep a seat (the C largest uniforms).
 //
 // Replaces (third-party, call site llavamod/model/language_model/llava_qwen1_5_moe.py:536-546)
 // deepspeed.moe.sharded_moe.TopKGate / top2gating / MOELayer dispatch+combine einsums
@@ -32,13 +34,15 @@ struct RouteParams {
   int tpb, ntiles;       // tokens per CTA (multiple of 16), number of CTAs
   float* logits; float* gates; int32_t* idx; int32_t* row; float* w;
   int32_t* offsets; float* meta; __nv_bfloat16* xp;
-  int32_t* tile_cnt;     // [ntiles][2*MAXE]: first-choice counts per expert, then second-choice counts
+  int32_t* tile_cnt;     // [ntiles][2*MAXE]: first-choice counts per expert, then second-choice counts (top-1: kept counts)
   float* tile_gsum;      // [ntiles][MAXE]: sum of gates per expert over the tile's tokens (token order)
+  int32_t* sel;          // top-1 only, [2*MAXE]: per expert the threshold key's bits, then the last token index kept at the threshold
 };
 
 // ---- kernel 1 of 2: gate.  fp32 GEMV against wg (staged in shared memory), softmax, top-1, Gumbel top-2; per-tile expert counts ----
 // An ordinary launch of ceil(S/16) small CTAs (no cooperative launch, no grid barrier): it shares the machine with whatever else is
-// running (the frozen teacher's GEMMs on the side stream).
+// running (the frozen teacher's GEMMs on the side stream).  K = 1: no second choice (idx[:,1] = -1, second-choice counts 0).
+template <int K>
 __global__ void __launch_bounds__(RT_THREADS) moe_gate_kernel(const RouteParams p) {
   extern __shared__ __align__(16) uint8_t smem[];
   float* s_wg = reinterpret_cast<float*>(smem);                           // [E,H] fp32
@@ -103,13 +107,16 @@ __global__ void __launch_bounds__(RT_THREADS) moe_gate_kernel(const RouteParams 
         g[e] = ex[e] / den;
         if (e < E && g[e] > gmx) { gmx = g[e]; i1 = e; }
       }
-      float best = -INFINITY;
-      int i2 = (i1 == 0) ? 1 : 0;
+      int i2 = -1;
+      if (K == 2) {
+        float best = -INFINITY;
+        i2 = (i1 == 0) ? 1 : 0;
 #pragma unroll
-      for (int e = 0; e < MAXE; ++e) {
-        if (e < E && e != i1) {
-          const float v = acc0[e] + p.noise[(size_t)tok * E + e];
-          if (v > best) { best = v; i2 = e; }
+        for (int e = 0; e < MAXE; ++e) {
+          if (e < E && e != i1) {
+            const float v = acc0[e] + p.noise[(size_t)tok * E + e];
+            if (v > best) { best = v; i2 = e; }
+          }
         }
       }
 #pragma unroll
@@ -119,7 +126,7 @@ __global__ void __launch_bounds__(RT_THREADS) moe_gate_kernel(const RouteParams 
       }
       p.idx[2 * tok] = i1; p.idx[2 * tok + 1] = i2;
       atomicAdd(&s_cnt[i1], 1);
-      atomicAdd(&s_cnt[MAXE + i2], 1);
+      if (K == 2) atomicAdd(&s_cnt[MAXE + i2], 1);
     }
   }
   __syncthreads();
@@ -132,9 +139,98 @@ __global__ void __launch_bounds__(RT_THREADS) moe_gate_kernel(const RouteParams 
   }
 }
 
+// ---- top-1 only, between the gate and seat+scatter: random token selection.  One CTA per expert.  top1gating keeps, per expert, the
+// routed tokens with the C largest uniforms u[s, idx1[s]] (topk over mask1 * u along the tokens).  A uniform in [0, 1) is a non-negative
+// float, so its bit pattern orders like its value: an MSB-first radix select over the 32 key bits (four 8-bit digits) finds the C-th
+// largest key T.  Keys above T are kept; among keys equal to T the lowest token indices are kept, up to the count still missing
+// (torch.topk leaves that order unspecified; this is the build's rule).  An expert with n_e <= C keeps every routed token (T = 0, every
+// index).  Writes sel = {T bits, last kept index at T} and each tile's kept count into tile_cnt[tile][MAXE + e]. ----
+constexpr int SEL_THREADS = 1024;
+constexpr int SEL_WARPS = SEL_THREADS / 32;
+__global__ void __launch_bounds__(SEL_THREADS) moe_top1_select_kernel(const RouteParams p) {
+  __shared__ int s_hist[256];
+  __shared__ int s_wt[SEL_WARPS];
+  __shared__ int s_n, s_need, s_lim;
+  __shared__ unsigned s_prefix;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int e = blockIdx.x, E = p.E, S = p.S;
+  if (tid == 0) { s_n = 0; s_lim = S - 1; s_prefix = 0u; s_need = 0; }
+  __syncthreads();
+  {
+    int n = 0;
+    for (int t = tid; t < p.ntiles; t += SEL_THREADS) n += __ldg(p.tile_cnt + (size_t)t * 2 * MAXE + e);
+    n = warp_sum(n);
+    if (lane == 0) atomicAdd(&s_n, n);
+  }
+  __syncthreads();
+  if (s_n > p.capacity) {                         // block-uniform
+    unsigned mask = 0u;
+    if (tid == 0) s_need = p.capacity;            // rank of the threshold from the top, 1-based
+    for (int shift = 24; shift >= 0; shift -= 8) {
+      if (tid < 256) s_hist[tid] = 0;
+      __syncthreads();
+      const unsigned prefix = s_prefix;
+      for (int t = tid; t < S; t += SEL_THREADS) {
+        if (__ldg(p.idx + 2 * t) != e) continue;
+        const unsigned key = __float_as_uint(__ldg(p.noise + (size_t)t * E + e));
+        if ((key & mask) == prefix) atomicAdd(&s_hist[(key >> shift) & 255u], 1);
+      }
+      __syncthreads();
+      if (tid == 0) {
+        int above = 0, d = 255;
+        for (; d > 0; --d) {
+          if (above + s_hist[d] >= s_need) break;
+          above += s_hist[d];
+        }
+        s_need -= above;
+        s_prefix = prefix | ((unsigned)d << shift);
+      }
+      mask |= 255u << shift;
+      __syncthreads();
+    }
+    // the s_need-th token (in token order) of this expert whose key equals the threshold is the last one kept at the threshold
+    const unsigned thr = s_prefix;
+    const int need = s_need;
+    const unsigned lt = (1u << lane) - 1u;
+    int run = 0;
+    for (int base = 0; base < S; base += SEL_THREADS) {
+      const int t = base + tid;
+      const bool tie = t < S && __ldg(p.idx + 2 * t) == e && __float_as_uint(__ldg(p.noise + (size_t)t * E + e)) == thr;
+      const unsigned b = __ballot_sync(0xffffffffu, tie);
+      if (lane == 0) s_wt[warp] = __popc(b);
+      __syncthreads();
+      int pre = run, tot = run;
+      for (int w = 0; w < SEL_WARPS; ++w) { const int c = s_wt[w]; tot += c; if (w < warp) pre += c; }
+      if (tie && pre + __popc(b & lt) + 1 == need) s_lim = t;
+      run = tot;
+      __syncthreads();
+      if (run >= need) break;                     // block-uniform
+    }
+  }
+  __syncthreads();
+  const unsigned thr = s_prefix;
+  const int lim = s_lim;
+  if (tid == 0) { p.sel[e] = (int)thr; p.sel[MAXE + e] = lim; }
+  // kept tokens per tile, for the seat kernel's token-order prefix
+  for (int t = warp; t < p.ntiles; t += SEL_WARPS) {
+    const int b0 = t * p.tpb, b1 = min(S, b0 + p.tpb);
+    int c = 0;
+    for (int s = b0 + lane; s < b1; s += 32) {
+      if (__ldg(p.idx + 2 * s) != e) continue;
+      const unsigned key = __float_as_uint(__ldg(p.noise + (size_t)s * E + e));
+      c += (key > thr || (key == thr && s <= lim)) ? 1 : 0;
+    }
+    c = warp_sum(c);
+    if (lane == 0) p.tile_cnt[(size_t)t * 2 * MAXE + MAXE + e] = c;
+  }
+}
+
 // ---- kernel 2 of 2: seat + scatter.  Every CTA rebuilds the global per-expert totals and its own exclusive prefix from the tile
 // counts (a few KB, L2 resident), seats its tokens in token order with warp ballots + popc (all first choices before any second
-// choice, drop at position >= capacity), renormalises the two gate weights, and copies its token rows to their expert rows. ----
+// choice, drop at position >= capacity), renormalises the two gate weights, and copies its token rows to their expert rows.
+// K = 1: the tokens the selection kept are seated in token order from the per-tile kept counts; w[:,0] is the raw gate of a kept token
+// (top1gating does not renormalise), row[:,1] = -1 and w[:,1] = 0. ----
+template <int K>
 __global__ void __launch_bounds__(RT_THREADS) moe_seat_scatter_kernel(const RouteParams p) {
   __shared__ int s_tot[2 * MAXE], s_pre[2 * MAXE], s_off[MAXE + 1], s_used[MAXE];
   __shared__ int s_row[2 * 32 * 64];                  // rows of this CTA's tokens (tpb <= 1024... see launch: tpb*2 <= 4096)
@@ -162,7 +258,7 @@ __global__ void __launch_bounds__(RT_THREADS) moe_seat_scatter_kernel(const Rout
     int o = 0, used = 0;
     for (int e = 0; e < E; ++e) {
       s_off[e] = (p.layout == 1) ? e * p.capacity : o;
-      const int rows_e = min(s_tot[e] + s_tot[MAXE + e], p.capacity);
+      const int rows_e = (K == 2) ? min(s_tot[e] + s_tot[MAXE + e], p.capacity) : s_tot[MAXE + e];    // top-1: kept = min(n_e, C)
       s_used[e] = rows_e;
       used += rows_e;
       o += (p.layout == 2) ? ((rows_e + 127) & ~127) : rows_e;
@@ -190,7 +286,48 @@ __global__ void __launch_bounds__(RT_THREADS) moe_seat_scatter_kernel(const Rout
   }
   __syncthreads();
   // warp 0 seats this CTA's tokens in order (32 at a time, ballot + popc prefix)
-  if (warp == 0) {
+  if (K == 1 && warp == 0) {
+    int c[MAXE];
+    unsigned thr[MAXE];
+    int lim[MAXE];
+#pragma unroll
+    for (int e = 0; e < MAXE; ++e) {
+      c[e] = s_pre[MAXE + e];
+      thr[e] = (e < E) ? (unsigned)__ldg(p.sel + e) : 0u;
+      lim[e] = (e < E) ? __ldg(p.sel + MAXE + e) : 0;
+    }
+    const unsigned lt = (1u << lane) - 1u;
+    for (int base = b0; base < b1; base += 32) {
+      const int tok = base + lane;
+      const bool valid = tok < b1;
+      int e1 = -1;
+      bool kept = false;
+      if (valid) {
+        e1 = __ldg(p.idx + 2 * tok);
+        unsigned t_e = 0u; int l_e = 0;
+#pragma unroll
+        for (int e = 0; e < MAXE; ++e) if (e == e1) { t_e = thr[e]; l_e = lim[e]; }
+        const unsigned key = __float_as_uint(__ldg(p.noise + (size_t)tok * E + e1));
+        kept = key > t_e || (key == t_e && tok <= l_e);
+      }
+      int loc = 0;
+#pragma unroll
+      for (int e = 0; e < MAXE; ++e) {
+        if (e < E) {
+          const unsigned a = __ballot_sync(0xffffffffu, kept && e1 == e);
+          if (kept && e1 == e) loc = c[e] + __popc(a & lt);
+          c[e] += __popc(a);
+        }
+      }
+      if (valid) {
+        const int r1 = kept ? s_off[e1] + loc : -1;
+        p.row[2 * tok] = r1; p.row[2 * tok + 1] = -1;
+        p.w[2 * tok] = kept ? __ldg(p.gates + (size_t)tok * E + e1) : 0.f; p.w[2 * tok + 1] = 0.f;
+        s_row[2 * (tok - b0)] = r1; s_row[2 * (tok - b0) + 1] = -1;
+      }
+    }
+  }
+  if (K == 2 && warp == 0) {
     int c1[MAXE], c2[MAXE];
 #pragma unroll
     for (int e = 0; e < MAXE; ++e) { c1[e] = s_pre[e]; c2[e] = s_pre[MAXE + e]; }
@@ -329,7 +466,8 @@ __global__ void __launch_bounds__(256) moe_combine_bwd_kernel(const __nv_bfloat1
   if (lane == 0) { dw[2 * warp] = (r1 >= 0) ? d1 : 0.f; dw[2 * warp + 1] = (r2 >= 0) ? d2 : 0.f; }
 }
 
-// gate backward: (dw1, dw2, d l_aux) -> dlogits through renormalisation + softmax
+// gate backward: (dw1, dw2, d l_aux) -> dlogits through renormalisation + softmax.  K = 1: w1 is the raw gate, dgates[s, e1] += dw1
+template <int K>
 __global__ void moe_gate_bwd_kernel(const float* __restrict__ gates, const int32_t* __restrict__ idx, const int32_t* __restrict__ row,
                                     const float* __restrict__ dw, const float* __restrict__ meta, const float* __restrict__ g_laux,
                                     int S, int E, float* __restrict__ dlogits) {
@@ -345,6 +483,11 @@ __global__ void moe_gate_bwd_kernel(const float* __restrict__ gates, const int32
   }
   const int e1 = idx[2 * s], e2 = idx[2 * s + 1];
   const bool k1 = row[2 * s] >= 0, k2 = row[2 * s + 1] >= 0;
+  if (K == 1) {
+    const float d1 = dw[2 * s];
+#pragma unroll
+    for (int e = 0; e < MAXE; ++e) if (e == e1 && k1) dg[e] += d1;
+  } else {
   float a = 0.f, b = 0.f;
 #pragma unroll
   for (int e = 0; e < MAXE; ++e) { if (e == e1 && k1) a = g[e]; if (e == e2 && k2) b = g[e]; }
@@ -360,6 +503,7 @@ __global__ void moe_gate_bwd_kernel(const float* __restrict__ gates, const int32
       if (e == e1 && k1) dg[e] += dw[2 * s] / FLT_EPSILON;
       if (e == e2 && k2) dg[e] += dw[2 * s + 1] / FLT_EPSILON;
     }
+  }
   }
   float dot = 0.f;
 #pragma unroll
@@ -455,6 +599,14 @@ extern "C" int lmod_moe_capacity(int64_t S, int E, double capacity_factor, int64
   return (int)ci;
 }
 
+// top1gating's _capacity: ceil(S/E * cf) (no factor 2), in double like lmod_moe_capacity, raised to min_capacity
+extern "C" int lmod_moe_capacity_top1(int64_t S, int E, double capacity_factor, int64_t min_capacity) {
+  double c = ceil(((double)S / (double)E) * capacity_factor);
+  int64_t ci = (int64_t)c;
+  if (ci < min_capacity) ci = min_capacity;
+  return (int)ci;
+}
+
 static int route_tpb(int64_t S) {
   int64_t tpb = TILE_MIN;
   while ((S + tpb - 1) / tpb > MAX_TILES) tpb += TILE_MIN;
@@ -469,36 +621,82 @@ extern "C" int64_t lmod_moe_route_ws_elems(int64_t S, int E) {
   return ntiles * (2 * MAXE + MAXE);
 }
 
-extern "C" int lmod_moe_route_scatter(const void* x, const float* wg, const float* noise, int64_t S, int64_t H, int E,
-                                      double capacity_factor, int64_t min_capacity, int layout, float* logits, float* gates,
-                                      int32_t* idx, int32_t* row, float* w, int32_t* offsets, float* meta, void* xp,
-                                      int32_t* ws, void* stream) {
-  LMOD_CHECK_ARG(x && wg && noise && logits && gates && idx && row && w && offsets && meta && xp && ws,
-                 "lmod_moe_route_scatter: null pointer");
-  LMOD_CHECK_ARG(E >= 2 && E <= MAXE, "lmod_moe_route_scatter: 2 <= E <= %d required (got %d)", MAXE, E);
-  LMOD_CHECK_ARG(S > 0 && H > 0 && H % 8 == 0, "lmod_moe_route_scatter: H must be a multiple of 8");
-  LMOD_CHECK_ARG(layout >= 0 && layout <= 2, "lmod_moe_route_scatter: layout must be 0 (compact), 1 (capacity slabs) or 2 (compact, 128-aligned)");
-  RouteParams p;
+extern "C" int64_t lmod_moe_route_top1_ws_elems(int64_t S, int E) {
+  return lmod_moe_route_ws_elems(S, E) + 2 * MAXE;
+}
+
+// the checks and the launch plan both routers share; the capacity is the caller's (top-2 or top-1 rule)
+static int route_params(RouteParams& p, const char* fn, const void* x, const float* wg, const float* noise, int64_t S, int64_t H, int E,
+                        int capacity, int layout, float* logits, float* gates, int32_t* idx, int32_t* row, float* w, int32_t* offsets,
+                        float* meta, void* xp, int32_t* ws) {
+  LMOD_CHECK_ARG(x && wg && noise && logits && gates && idx && row && w && offsets && meta && xp && ws, "%s: null pointer", fn);
+  LMOD_CHECK_ARG(E >= 2 && E <= MAXE, "%s: 2 <= E <= %d required (got %d)", fn, MAXE, E);
+  LMOD_CHECK_ARG(S > 0 && H > 0 && H % 8 == 0, "%s: H must be a multiple of 8", fn);
+  LMOD_CHECK_ARG(layout >= 0 && layout <= 2, "%s: layout must be 0 (compact), 1 (capacity slabs) or 2 (compact, 128-aligned)", fn);
   p.x = (const __nv_bfloat16*)x; p.wg = wg; p.noise = noise; p.S = (int)S; p.H = (int)H; p.E = E;
-  p.capacity = lmod_moe_capacity(S, E, capacity_factor, min_capacity);
+  p.capacity = capacity;
   p.layout = layout;
   p.logits = logits; p.gates = gates; p.idx = idx; p.row = row; p.w = w; p.offsets = offsets; p.meta = meta;
   p.xp = (__nv_bfloat16*)xp;
   p.tpb = route_tpb(S);
   p.ntiles = (int)((S + p.tpb - 1) / p.tpb);
-  LMOD_CHECK_ARG(p.tpb <= 2048, "lmod_moe_route_scatter: S = %lld is beyond the tile plan", (long long)S);
+  LMOD_CHECK_ARG(p.tpb <= 2048, "%s: S = %lld is beyond the tile plan", fn, (long long)S);
   p.tile_cnt = ws;
   p.tile_gsum = reinterpret_cast<float*>(ws + (size_t)p.ntiles * 2 * MAXE);
+  p.sel = ws + (size_t)p.ntiles * 3 * MAXE;
   const size_t smem = (size_t)E * H * 4 + (size_t)p.tpb * MAXE * 4;
-  LMOD_CHECK_ARG(smem <= 200 * 1024, "lmod_moe_route_scatter: E*H*4 exceeds the shared-memory budget");
+  LMOD_CHECK_ARG(smem <= 200 * 1024, "%s: E*H*4 exceeds the shared-memory budget", fn);
+  return LMOD_OK;
+}
+
+template <int K>
+static int launch_gate(const RouteParams& p, cudaStream_t stream) {
+  const size_t smem = (size_t)p.E * p.H * 4 + (size_t)p.tpb * MAXE * 4;
   static size_t smem_set = 0;
   if (smem > 48 * 1024 && smem > smem_set) {
-    LMOD_CUDA_OK(cudaFuncSetAttribute(moe_gate_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    LMOD_CUDA_OK(cudaFuncSetAttribute(moe_gate_kernel<K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     smem_set = smem;
   }
-  moe_gate_kernel<<<p.ntiles, RT_THREADS, smem, (cudaStream_t)stream>>>(p);
+  moe_gate_kernel<K><<<p.ntiles, RT_THREADS, smem, stream>>>(p);
   LMOD_LAUNCH_OK();
-  moe_seat_scatter_kernel<<<p.ntiles, RT_THREADS, 0, (cudaStream_t)stream>>>(p);
+  return LMOD_OK;
+}
+
+extern "C" int lmod_moe_route_scatter(const void* x, const float* wg, const float* noise, int64_t S, int64_t H, int E,
+                                      double capacity_factor, int64_t min_capacity, int layout, float* logits, float* gates,
+                                      int32_t* idx, int32_t* row, float* w, int32_t* offsets, float* meta, void* xp,
+                                      int32_t* ws, void* stream) {
+  RouteParams p;
+  const int rc = route_params(p, "lmod_moe_route_scatter", x, wg, noise, S, H, E, lmod_moe_capacity(S, E, capacity_factor, min_capacity),
+                              layout, logits, gates, idx, row, w, offsets, meta, xp, ws);
+  if (rc != LMOD_OK) return rc;
+  p.sel = nullptr;
+  const int rg = launch_gate<2>(p, (cudaStream_t)stream);
+  if (rg != LMOD_OK) return rg;
+  moe_seat_scatter_kernel<2><<<p.ntiles, RT_THREADS, 0, (cudaStream_t)stream>>>(p);
+  LMOD_LAUNCH_OK();
+  return LMOD_OK;
+}
+
+extern "C" int lmod_moe_route_scatter_top1(const void* x, const float* wg, const float* uniform, int64_t S, int64_t H, int E,
+                                           double capacity_factor, int64_t min_capacity, int layout, float* logits, float* gates,
+                                           int32_t* idx, int32_t* row, float* w, int32_t* offsets, float* meta, void* xp,
+                                           int32_t* ws, void* stream) {
+  // top1gating fails in these two cases (an assert on the batch size, torch.topk with k > S); say so before any launch
+  LMOD_CHECK_ARG(S >= min_capacity, "lmod_moe_route_scatter_top1: %lld tokens < min_capacity %lld (top1gating requires S >= min_capacity)",
+                 (long long)S, (long long)min_capacity);
+  const int C = lmod_moe_capacity_top1(S, E, capacity_factor, min_capacity);
+  LMOD_CHECK_ARG(C <= S, "lmod_moe_route_scatter_top1: capacity %d > %lld tokens (top1gating's topk over the tokens needs C <= S)",
+                 C, (long long)S);
+  RouteParams p;
+  const int rc = route_params(p, "lmod_moe_route_scatter_top1", x, wg, uniform, S, H, E, C, layout, logits, gates, idx, row, w, offsets,
+                              meta, xp, ws);
+  if (rc != LMOD_OK) return rc;
+  const int rg = launch_gate<1>(p, (cudaStream_t)stream);
+  if (rg != LMOD_OK) return rg;
+  moe_top1_select_kernel<<<E, SEL_THREADS, 0, (cudaStream_t)stream>>>(p);
+  LMOD_LAUNCH_OK();
+  moe_seat_scatter_kernel<1><<<p.ntiles, RT_THREADS, 0, (cudaStream_t)stream>>>(p);
   LMOD_LAUNCH_OK();
   return LMOD_OK;
 }
@@ -526,7 +724,17 @@ extern "C" int lmod_moe_combine_bwd(const void* dout, const void* y, const int32
 extern "C" int lmod_moe_gate_bwd(const float* gates, const int32_t* idx, const int32_t* row, const float* dw, const float* meta,
                                  const float* g_laux, int64_t S, int E, float* dlogits, void* stream) {
   LMOD_CHECK_ARG(gates && idx && row && dw && meta && dlogits && S > 0 && E >= 2 && E <= MAXE, "lmod_moe_gate_bwd: bad arguments");
-  moe_gate_bwd_kernel<<<(unsigned)((S + 127) / 128), 128, 0, (cudaStream_t)stream>>>(gates, idx, row, dw, meta, g_laux, (int)S, E, dlogits);
+  moe_gate_bwd_kernel<2><<<(unsigned)((S + 127) / 128), 128, 0, (cudaStream_t)stream>>>(gates, idx, row, dw, meta, g_laux, (int)S, E,
+                                                                                        dlogits);
+  LMOD_LAUNCH_OK();
+  return LMOD_OK;
+}
+
+extern "C" int lmod_moe_gate_bwd_top1(const float* gates, const int32_t* idx, const int32_t* row, const float* dw, const float* meta,
+                                      const float* g_laux, int64_t S, int E, float* dlogits, void* stream) {
+  LMOD_CHECK_ARG(gates && idx && row && dw && meta && dlogits && S > 0 && E >= 2 && E <= MAXE, "lmod_moe_gate_bwd_top1: bad arguments");
+  moe_gate_bwd_kernel<1><<<(unsigned)((S + 127) / 128), 128, 0, (cudaStream_t)stream>>>(gates, idx, row, dw, meta, g_laux, (int)S, E,
+                                                                                        dlogits);
   LMOD_LAUNCH_OK();
   return LMOD_OK;
 }

@@ -33,6 +33,10 @@ SIGNATURES = {
     "lmod_moe_capacity": [_L, _I, _D, _L],
     "lmod_moe_route_ws_elems": [_L, _I],
     "lmod_moe_route_scatter": [_P, _P, _P, _L, _L, _I, _D, _L, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P],
+    "lmod_moe_capacity_top1": [_L, _I, _D, _L],
+    "lmod_moe_route_top1_ws_elems": [_L, _I],
+    "lmod_moe_route_scatter_top1": [_P, _P, _P, _L, _L, _I, _D, _L, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P],
+    "lmod_moe_gate_bwd_top1": [_P, _P, _P, _P, _P, _P, _L, _I, _P, _P],
     "lmod_moe_gather_combine": [_P, _P, _P, _P, _L, _L, _P, _P],
     "lmod_moe_combine_bwd": [_P, _P, _P, _P, _L, _L, _P, _P, _P],
     "lmod_moe_gate_bwd": [_P, _P, _P, _P, _P, _P, _L, _I, _P, _P],
@@ -75,7 +79,7 @@ SIGNATURES = {
     "lmod_launch_count_reset": [],
 }
 _RESTYPES = {"lmod_last_error": ctypes.c_char_p, "lmod_launch_count": c_int64, "lmod_launch_count_reset": None,
-             "lmod_moe_route_ws_elems": c_int64, "lmod_attn_decode_ws_elems": c_int64,
+             "lmod_moe_route_ws_elems": c_int64, "lmod_moe_route_top1_ws_elems": c_int64, "lmod_attn_decode_ws_elems": c_int64,
              "lmod_attn_decode_chunk_ws_elems": c_int64}
 
 

@@ -849,35 +849,52 @@ def splice_embed(feats, embed_w, src, img_index, n_patches, embed_grad=None, ord
 # ---------------------------------------------------------------------------------------------------
 # MoE layer (DeepSpeed 0.9.5 MoE; call site llava_qwen1_5_moe.py:536-546, SURVEY.md Appendix A)
 # ---------------------------------------------------------------------------------------------------
-def moe_capacity(S, E, capacity_factor, min_capacity):
-    """DeepSpeed's _capacity, ceil(S/E * cf * 2) raised to min_capacity, with cf as the Python double the user set."""
-    return int(_C.lib().lmod_moe_capacity(S, E, float(capacity_factor), int(min_capacity)))
+def moe_capacity(S, E, capacity_factor, min_capacity, k=2):
+    """DeepSpeed's _capacity, ceil(S/E * cf * 2) for top-2 and ceil(S/E * cf) for top-1, raised to min_capacity, with cf as the Python
+    double the user set."""
+    fn = _C.lib().lmod_moe_capacity if k == 2 else _C.lib().lmod_moe_capacity_top1
+    return int(fn(S, E, float(capacity_factor), int(min_capacity)))
+
+
+def _check_k(k):
+    if k not in (1, 2):
+        raise ValueError("Only top-1 and top-2 gatings are supported (k = %r)" % (k,))
 
 
 LAYOUT_COMPACT, LAYOUT_SLABS, LAYOUT_ALIGNED = 0, 1, 2
 
 
-def moe_route_scatter(x, wg, noise, capacity_factor, min_capacity, layout=LAYOUT_ALIGNED, padded=None):
+def moe_route_scatter(x, wg, noise, capacity_factor, min_capacity, layout=LAYOUT_ALIGNED, padded=None, k=2):
     """Two ordinary launches (gate, seat+scatter): fp32 gate GEMV, softmax, top-1 / Gumbel top-2, stable capacity positions,
     renormalised weights, l_aux, expert offsets and the token scatter.  Returns a dict of device tensors.
-    layout: 0 compact rows, 1 capacity-padded [E,C] slabs, 2 compact with 128-row aligned groups (grouped GEMM input)."""
+    layout: 0 compact rows, 1 capacity-padded [E,C] slabs, 2 compact with 128-row aligned groups (grouped GEMM input).
+    k = 1: top1gating with random token selection, noise being the uniform [S,E] in [0, 1); a selection launch runs between the two
+    (the C routed tokens with the largest uniform keep their seat), w[:,0] is the raw gate and the second choice is empty (-1 / 0)."""
     _need_cuda(x, wg, noise)
+    _check_k(k)
     if padded is not None:
         layout = LAYOUT_SLABS if padded else LAYOUT_COMPACT
     S, H = x.shape
     E = wg.shape[0]
-    C = moe_capacity(S, E, capacity_factor, min_capacity)
+    if k == 1 and S < min_capacity:
+        raise ValueError("top-1 routing of %d tokens with min_capacity %d: top1gating requires at least min_capacity tokens" % (S, min_capacity))
+    C = moe_capacity(S, E, capacity_factor, min_capacity, k)
+    if k == 1 and C > S:
+        raise ValueError("top-1 routing of %d tokens: capacity %d exceeds the token count (top1gating's topk over the tokens needs C <= S)"
+                         % (S, C))
     dev = x.device
     r = dict(
         logits=torch.empty(S, E, dtype=torch.float32, device=dev), gates=torch.empty(S, E, dtype=torch.float32, device=dev),
         idx=torch.empty(S, 2, dtype=torch.int32, device=dev), row=torch.empty(S, 2, dtype=torch.int32, device=dev),
         w=torch.empty(S, 2, dtype=torch.float32, device=dev), offsets=torch.empty(E + 1, dtype=torch.int32, device=dev),
         meta=torch.empty(4 + E, dtype=torch.float32, device=dev), capacity=C)
-    rows = E * C if layout == LAYOUT_SLABS else (min(2 * S, E * C) + (128 * E if layout == LAYOUT_ALIGNED else 0))
+    rows = E * C if layout == LAYOUT_SLABS else (min(k * S, E * C) + (128 * E if layout == LAYOUT_ALIGNED else 0))
     r["max_rows"] = rows
+    r["k"] = k
     r["xp"] = torch.empty(rows, H, dtype=x.dtype, device=dev)      # the op zeroes the padding rows itself (inert for the wgrad reduction)
-    ws = torch.empty(int(_C.lib().lmod_moe_route_ws_elems(S, E)), dtype=torch.int32, device=dev)       # per call: safe across streams
-    call("lmod_moe_route_scatter", ptr(x), ptr(wg), ptr(noise), S, H, E, float(capacity_factor), int(min_capacity), int(layout),
+    top1 = "_top1" if k == 1 else ""
+    ws = torch.empty(int(getattr(_C.lib(), "lmod_moe_route%s_ws_elems" % top1)(S, E)), dtype=torch.int32, device=dev)   # per call
+    call("lmod_moe_route_scatter" + top1, ptr(x), ptr(wg), ptr(noise), S, H, E, float(capacity_factor), int(min_capacity), int(layout),
          ptr(r["logits"]), ptr(r["gates"]), ptr(r["idx"]), ptr(r["row"]), ptr(r["w"]), ptr(r["offsets"]), ptr(r["meta"]), ptr(r["xp"]),
          ptr(ws))
     return r
@@ -891,11 +908,11 @@ def moe_gather_combine(y, row, w, residual=None):
     return out
 
 
-def moe_forward_stages(x, res, wg, w_gu, w_dn, noise, cf, min_cap, fused):
+def moe_forward_stages(x, res, wg, w_gu, w_dn, noise, cf, min_cap, fused, k=2):
     """The MoE forward as MoEFn runs it, returning every intermediate (the router's record, xp, h1, act, y, out).  fused: SwiGLU in the
-    grouped GEMM's epilogue instead of GEMM + silu_mul (bit-identical)."""
+    grouped GEMM's epilogue instead of GEMM + silu_mul (bit-identical).  k: routing width (1: noise is the uniform of top-1's selection)."""
     E, I2, H = w_gu.shape
-    r = moe_route_scatter(x, wg, noise, cf, min_cap, LAYOUT_ALIGNED)
+    r = moe_route_scatter(x, wg, noise, cf, min_cap, LAYOUT_ALIGNED, k=k)
     R = r["max_rows"]
     xp, offs = r["xp"], r["offsets"]
     # only xp (and dy in the backward) are zero-filled: in the 128-aligned layout the grouped GEMM writes EVERY row below offsets[E],
@@ -941,7 +958,8 @@ def moe_backward_stages(st, x, wg, w_gu, w_dn, dout, dlaux, grads):
     gl = None
     if dlaux is not None:
         gl = dlaux.to(torch.float32).reshape(1).contiguous()
-    call("lmod_moe_gate_bwd", ptr(gates), ptr(idx), ptr(row), ptr(dw), ptr(meta), ptr(gl) if gl is not None else None, S, E, ptr(dlogits))
+    call("lmod_moe_gate_bwd_top1" if st.get("k", 2) == 1 else "lmod_moe_gate_bwd", ptr(gates), ptr(idx), ptr(row), ptr(dw), ptr(meta),
+         ptr(gl) if gl is not None else None, S, E, ptr(dlogits))
     dx = torch.empty_like(x)
     call("lmod_moe_scatter_bwd", ptr(dxp), ptr(row), ptr(dlogits), ptr(wg), None, S, H, E, ptr(dx))
     if g is not None and g.get("wg") is not None:
@@ -957,30 +975,31 @@ class MoEFn(Function):
     padding; the reference computes E*C = 1.5x the routed rows).  Returns (res + moe_out, l_aux)."""
 
     @staticmethod
-    def forward(ctx, x, res, wg, w_gu, w_dn, noise, cf, min_cap, grads):
+    def forward(ctx, x, res, wg, w_gu, w_dn, noise, cf, min_cap, grads, k=2):
         x = _c(x)
         res = _c(res)
         E, I2, H = w_gu.shape
-        st = moe_forward_stages(x, res, wg, w_gu, w_dn, noise, cf, min_cap, swiglu_fusable(I2 // 2, H, training=True))
-        ctx.save_for_backward(x, wg, w_gu, w_dn, *(st[k] for k in _MOE_SAVED))
+        st = moe_forward_stages(x, res, wg, w_gu, w_dn, noise, cf, min_cap, swiglu_fusable(I2 // 2, H, training=True), k)
+        ctx.save_for_backward(x, wg, w_gu, w_dn, *(st[n] for n in _MOE_SAVED))
         ctx.fused = st["fused"]
+        ctx.k = k
         ctx.grads = grads
         return st["out"], st["meta"][0].clone()
 
     @staticmethod
     def backward(ctx, dout, dlaux):
         x, wg, w_gu, w_dn, *saved = ctx.saved_tensors
-        st = dict(zip(_MOE_SAVED, saved), fused=ctx.fused)
+        st = dict(zip(_MOE_SAVED, saved), fused=ctx.fused, k=ctx.k)
         dx = moe_backward_stages(st, x, wg, w_gu, w_dn, _c(dout), dlaux, ctx.grads)["dx"]
-        return dx, dout, None, None, None, None, None, None, None
+        return dx, dout, None, None, None, None, None, None, None, None
 
 
 _MOE_SAVED = ("xp", "h1", "act", "y", "row", "w", "gates", "idx", "meta", "offsets")
 
 
-def moe_forward_nograd(x, res, wg, w_gu, w_dn, noise, cf, min_cap):
+def moe_forward_nograd(x, res, wg, w_gu, w_dn, noise, cf, min_cap, k=2):
     E, I2, H = w_gu.shape
-    r = moe_route_scatter(_c(x), wg, noise, cf, min_cap, LAYOUT_ALIGNED)
+    r = moe_route_scatter(_c(x), wg, noise, cf, min_cap, LAYOUT_ALIGNED, k=k)
     R = r["max_rows"]
     if swiglu_fusable(I2 // 2, H):
         act, _ = grouped_gemm_swiglu(r["xp"], w_gu, r["offsets"], R, False)

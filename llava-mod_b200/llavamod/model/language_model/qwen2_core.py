@@ -187,13 +187,14 @@ class MOELayer(nn.Module):
 
 class MoE(nn.Module):
     """Parameter layout of deepspeed.moe.layer.MoE (call site llava_qwen1_5_moe.py:536-546): ``deepspeed_moe.gate.wg``
-    and ``deepspeed_moe.experts.deepspeed_experts.{e}``.  k=2 only (the distillation shells use top-2)."""
+    and ``deepspeed_moe.experts.deepspeed_experts.{e}``.  k = 2 (top2gating, the distillation shells' default) or k = 1 (top1gating
+    with random token selection), the two widths DeepSpeed's TopKGate accepts."""
 
     def __init__(self, cfg, expert: Qwen2MLP, num_experts=4, ep_size=1, k=2, capacity_factor=1.0,
                  eval_capacity_factor=1.0, min_capacity=4, use_residual=False):
         super().__init__()
-        if k != 2:
-            raise NotImplementedError("only top-2 gating is built (the reference's distillation recipes use --top_k_experts 2)")
+        if k not in (1, 2):
+            raise ValueError("Only top-1 and top-2 gatings are supported (got k = %r)" % (k,))
         if ep_size != 1:
             raise NotImplementedError("expert parallelism is size 1 in the reference's recipes (SURVEY.md 2.3)")
         if use_residual:
@@ -301,11 +302,11 @@ class Qwen2Model(nn.Module):
         l_auxes, records = [], []
         moe_i = 0
         if moe_noise is None:
-            # DeepSpeed draws fresh Gumbel noise in every MoE layer; one draw for all layers of this forward is the same distribution
-            # with 5 launches instead of 5 per layer
+            # DeepSpeed draws fresh Gumbel noise (top-2) or uniforms (top-1's token selection) in every MoE layer; one draw for all layers
+            # of this forward is the same distribution with 5 launches instead of 5 per layer
             moes = [l.mlp for l in self.layers if isinstance(l.mlp, MoE)]
-            if moes and len({m.num_experts for m in moes}) == 1:
-                moe_noise = gumbel_noise((len(moes), B * T, moes[0].num_experts), dev).unbind(0)
+            if moes and len({(m.num_experts, m.k) for m in moes}) == 1:
+                moe_noise = moe_draw((len(moes), B * T, moes[0].num_experts), moes[0].k, dev).unbind(0)
         for li, layer in enumerate(self.layers):
             at = layer.self_attn
             nh, nkv, hd = at.num_heads, at.num_key_value_heads, at.head_dim
@@ -331,17 +332,17 @@ class Qwen2Model(nn.Module):
             if isinstance(mlp, MoE):
                 ds = mlp.deepspeed_moe
                 E = mlp.num_experts
-                noise = moe_noise[moe_i] if moe_noise is not None else gumbel_noise((B * T, E), dev)
+                noise = moe_noise[moe_i] if moe_noise is not None else moe_draw((B * T, E), mlp.k, dev)
                 moe_i += 1
                 cf = mlp.capacity_factor if training_moe else mlp.eval_capacity_factor
                 wg = ds.gate.wg.weight
                 if torch.is_grad_enabled() and (x.requires_grad or wg.requires_grad or ds.experts.deepspeed_experts[0].down_proj.weight.requires_grad):
                     grads = dict(wg=self.gview(wg), w_gu=self.gview(ds.experts.gu_weight), w_dn=self.gview(ds.experts.dn_weight))
                     stream, l_aux = K.MoEFn.apply(x, stream, wg, ds.experts.gu_weight, ds.experts.dn_weight, noise, cf,
-                                                  mlp.min_capacity, grads)
+                                                  mlp.min_capacity, grads, mlp.k)
                 else:
                     stream, l_aux, rec = K.moe_forward_nograd(x, stream, wg, ds.experts.gu_weight, ds.experts.dn_weight, noise,
-                                                              cf, mlp.min_capacity)
+                                                              cf, mlp.min_capacity, mlp.k)
                     records.append(rec)
                 l_auxes.append(l_aux)
                 branch = None
@@ -371,7 +372,8 @@ class Qwen2Model(nn.Module):
         the chunked attention gives each row the bytes of the single-query kernel, so for a dense model this is T one-token steps, bit for
         bit.
         Everything the step reads about the position is on the device, so the step can be captured once and replayed.  MoE layers route
-        the B new tokens alone (top2gating with S = B, as MoEQwen1_5Model_forward does with a cache, llava_qwen1_5_moe.py:223-236).
+        the B new tokens alone (top2gating / top1gating with S = B, as MoEQwen1_5Model_forward does with a cache,
+        llava_qwen1_5_moe.py:223-236).
         The layer body is forward's no-grad layer body with the attention swapped for append + decode attention: the same norm and
         residual-fusion choices, the same MoE call and final norm.  A change to one loop must be made to the other;
         tests/test_decode_gpu.py checks that the two give the same K / V, bit for bit."""
@@ -417,11 +419,11 @@ class Qwen2Model(nn.Module):
             mlp = layer.mlp
             if isinstance(mlp, MoE):
                 ds = mlp.deepspeed_moe
-                noise = moe_noise[moe_i] if moe_noise is not None else gumbel_noise((B, mlp.num_experts), dev)
+                noise = moe_noise[moe_i] if moe_noise is not None else moe_draw((B, mlp.num_experts), mlp.k, dev)
                 moe_i += 1
                 cf = mlp.capacity_factor if training_moe else mlp.eval_capacity_factor
                 stream, l_aux, rec = K.moe_forward_nograd(x, stream, ds.gate.wg.weight, ds.experts.gu_weight, ds.experts.dn_weight, noise,
-                                                          cf, mlp.min_capacity)
+                                                          cf, mlp.min_capacity, mlp.k)
                 records.append(rec)
                 l_auxes.append(l_aux)
                 branch = None
@@ -523,3 +525,11 @@ def gumbel_noise(shape, device):
     """deepspeed gumbel_rsample (Gumbel(0,1) via -log(-log U)); Philox stream of the current device generator."""
     u = torch.rand(shape, device=device, dtype=torch.float32).clamp_(min=1e-20, max=1.0 - 1e-7)
     return -torch.log(-torch.log(u))
+
+
+def moe_draw(shape, k, device):
+    """The random input of a k-wide MoE layer: Gumbel noise for top-2's second choice, Uniform(0, 1) for top-1's random token selection
+    (top1gating draws it on every call, training and eval alike)."""
+    if k == 1:
+        return torch.rand(shape, device=device, dtype=torch.float32)
+    return gumbel_noise(shape, device)
