@@ -260,6 +260,31 @@ int lmod_grouped_gemm_bf16(const void* A, int64_t lda, const void* B, int64_t ld
                            int mode, int epilogue, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * FP8 (e4m3) frozen teacher: the decoder linears of a model that is never differentiated, on e4m3 wgmma (csrc/gemm_fp8.cu, csrc/quant.cu).
+ * Quantiser (fp32; stated in full at the top of csrc/quant.cu): scale = amax > 0 ? amax / 448 : 1 per row, q = e4m3_rn(clamp(x / scale,
+ * +-448)).  Weights [N,K] are quantised per output channel with the same function, once; activations per token by the kernel that
+ * produces the GEMM input.  GEMM: D[m,n] = (acc[m,n] * s_a[m]) * s_w[n] in fp32 (acc = the wgmma fp32 sum of the e4m3 products), then bias
+ * / RoPE / SwiGLU with the expressions and bf16 roundings of the bf16 forms above.  Forward only, K-major operands only.
+ * lmod_quant_rows_e4m3: x [M,K] bf16 (row stride ld) -> q [M,K] bytes + scale [M]; in front of o_proj (modeling_qwen2.py:726) and down_proj
+ *   (:200), and for the weights.  K %% 16 == 0.
+ * lmod_rmsnorm_quant_e4m3: lmod_rmsnorm_fwd (Qwen2RMSNorm :105-110 with the residual add of :796,808) writing q / scale instead of the bf16
+ *   row -- bit-equal to lmod_quant_rows_e4m3 of lmod_rmsnorm_fwd's y; x_out as there.  In front of q|k|v (:678-680) and gate|up (:199).
+ * lmod_gemm_e4m3: nn.Linear forward (o_proj :726, down_proj :200).  lda / ldb: row strides of the e4m3 operands in bytes (multiples of 16).
+ * lmod_gemm_e4m3_qkv_rope: lmod_gemm_qkv_rope (:678-691,159-184) on e4m3 operands; bit-identical to lmod_gemm_e4m3 + lmod_rope.
+ * lmod_gemm_e4m3_swiglu: lmod_gemm_swiglu (:199-200) on e4m3 operands, W8_gu [2I,K] / s_w [2I] the fused gate|up weight; no pre-activations
+ *   are kept; bit-identical to lmod_gemm_e4m3 + lmod_silu_mul_fwd.  I %% 128 == 0. */
+int lmod_quant_rows_e4m3(const void* x, int64_t ld, void* q, float* scale, int64_t M, int64_t K, void* stream);
+int lmod_rmsnorm_quant_e4m3(const void* x, const void* res, const void* w, int64_t rows, int64_t H, float eps, void* q, float* scale,
+                            void* x_out, void* stream);
+int lmod_gemm_e4m3(const void* A8, int64_t lda, const float* s_a, const void* W8, int64_t ldb, const float* s_w, const void* bias, void* D,
+                   int64_t ldd, int64_t M, int64_t N, int64_t K, void* stream);
+int lmod_gemm_e4m3_qkv_rope(const void* A8, int64_t lda, const float* s_a, const void* W8, int64_t ldb, const float* s_w, const void* bias,
+                            void* D, int64_t ldd, int64_t M, int64_t K, int nh, int nkv, int hd, const void* cos_table,
+                            const void* sin_table, const int64_t* position_ids, void* stream);
+int lmod_gemm_e4m3_swiglu(const void* A8, int64_t lda, const float* s_a, const void* W8_gu, int64_t ldb, const float* s_w, void* act,
+                          int64_t ld_act, int64_t M, int64_t I, int64_t K, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * K7: flash-attention FORWARD on wgmma/TMA (modeling_qwen2.py:713-721 causal; CLIP non-causal), reading the fused RoPE'd
  * QKV buffer [batch*seq, (nh+2*nkv)*hd] in place (GQA by index).  hd in {64,128}.  out [batch*seq, nh*hd];
  * lse [batch, nh, seq] fp32 (natural-log LSE of the scaled scores, consumed by lmod_attn_bwd) or NULL.

@@ -127,6 +127,7 @@ class AlignArguments:
     ref_model_name_or_path: Optional[str] = None
     ref_pretrain_mm_mlp_adapter: Optional[str] = None
     moe_loss_enable: bool = False
+    ref_fp8: bool = False            # run the frozen teacher's decoder linears in FP8 (e4m3): ref_model.quantize_fp8_()
 
 
 @dataclass
@@ -137,6 +138,7 @@ class DPOArguments:
     policy_model_name_or_path: Optional[str] = None
     ref_model_name_or_path: Optional[str] = None
     moe_loss_enable: bool = False
+    ref_fp8: bool = False            # as AlignArguments.ref_fp8
 
 
 def _str2bool(v):

@@ -321,6 +321,89 @@ def gemm_residual(x, w, bias, res, inplace=False):
 
 
 # ---------------------------------------------------------------------------------------------------
+# FP8 (e4m3) frozen decoder linears: csrc/quant.cu (row-wise quantisers) + csrc/gemm_fp8.cu (e4m3 wgmma GEMM).  Forward only.
+# ---------------------------------------------------------------------------------------------------
+class Fp8Rows:
+    """Rows quantised to e4m3: ``q`` uint8 [M,K] (the e4m3 bytes), ``scale`` fp32 [M]; row m stands for scale[m] * e4m3(q[m]).  A weight
+    [N,K] quantised per output channel, or activations quantised per token."""
+    __slots__ = ("q", "scale")
+
+    def __init__(self, q, scale):
+        self.q, self.scale = q, scale
+
+    @property
+    def shape(self):
+        return self.q.shape
+
+    def dequant(self):
+        """fp32 [M,K] (exact: an e4m3 value times an fp32 scale is rounded once)."""
+        return self.q.view(torch.float8_e4m3fn).float() * self.scale[:, None]
+
+
+def quant_rows(x):
+    """lmod_quant_rows_e4m3 on the rows of a bf16 matrix (row stride free) -> Fp8Rows."""
+    _need_cuda(x)
+    x2 = x if x.dim() == 2 and x.stride(1) == 1 else _rows(x)
+    M, Kd = x2.shape
+    out = Fp8Rows(torch.empty(M, Kd, dtype=torch.uint8, device=x.device), torch.empty(M, dtype=torch.float32, device=x.device))
+    call("lmod_quant_rows_e4m3", ptr(x2), x2.stride(0), ptr(out.q), ptr(out.scale), M, Kd)
+    return out
+
+
+def rmsnorm_quant(x, w, eps, res=None):
+    """K.rmsnorm (no autograd) whose normalised rows come back quantised: -> (Fp8Rows, stream).  lmod_rmsnorm_quant_e4m3."""
+    _need_cuda(x, w)
+    if torch.is_grad_enabled() and (x.requires_grad or (res is not None and res.requires_grad)):
+        raise RuntimeError("an FP8 (e4m3) decoder is forward-only: its input requires grad, run it under torch.no_grad()")
+    x = _c(x)
+    H = x.shape[-1]
+    rows = x.numel() // H
+    out = Fp8Rows(torch.empty(rows, H, dtype=torch.uint8, device=x.device), torch.empty(rows, dtype=torch.float32, device=x.device))
+    s = torch.empty_like(x) if res is not None else None
+    call("lmod_rmsnorm_quant_e4m3", ptr(x), ptr(_c(res)) if res is not None else None, ptr(w), rows, H, eps, ptr(out.q), ptr(out.scale), ptr(s))
+    return out, (s if res is not None else x)
+
+
+def gemm_fp8(a, w, bias=None):
+    """bf16 [M,N] = a (Fp8Rows [M,K]) x w (Fp8Rows [N,K])^T (+bias) on the e4m3 wgmma GEMM (lmod_gemm_e4m3)."""
+    M, Kd = a.shape
+    out = torch.empty(M, w.shape[0], dtype=BF16, device=a.q.device)
+    call("lmod_gemm_e4m3", ptr(a.q), a.q.stride(0), ptr(a.scale), ptr(w.q), w.q.stride(0), ptr(w.scale), ptr(bias) if bias is not None else None,
+         ptr(out), out.stride(0), M, w.shape[0], Kd)
+    return out
+
+
+def qkv_rope_fp8(a, w, bias, cos, sin, pos, nh, nkv, hd):
+    """K.qkv_rope of a frozen FP8 layer: a = the quantised normalised rows (rmsnorm_quant), w = the quantised fused q|k|v weight."""
+    if hd not in ATTN_HEAD_DIMS or FUSE_ROPE == "0":
+        return rope_(gemm_fp8(a, w, bias), cos, sin, pos, nh, nkv, hd)
+    M, Kd = a.shape
+    out = torch.empty(M, w.shape[0], dtype=BF16, device=a.q.device)
+    call("lmod_gemm_e4m3_qkv_rope", ptr(a.q), a.q.stride(0), ptr(a.scale), ptr(w.q), w.q.stride(0), ptr(w.scale), ptr(bias) if bias is not None else None,
+         ptr(out), out.stride(0), M, Kd, nh, nkv, hd, ptr(cos), ptr(sin), ptr(pos))
+    return out
+
+
+def linear_fp8(x, w):
+    """K.linear of a frozen FP8 layer for a bf16 input (o_proj on the attention output): quantise the rows, then the e4m3 GEMM."""
+    y = gemm_fp8(quant_rows(x), w)
+    return y if x.dim() == 2 else y.view(*x.shape[:-1], w.shape[0])
+
+
+def mlp_fp8(a, w_gu, w_dn):
+    """K.mlp of a frozen FP8 layer: a = the quantised normalised rows; gate|up with the SwiGLU epilogue where K.mlp fuses it, the
+    activation quantised per token, down_proj."""
+    I = w_gu.shape[0] // 2
+    if swiglu_fusable(I, w_gu.shape[1]):
+        act = torch.empty(a.shape[0], I, dtype=BF16, device=a.q.device)
+        call("lmod_gemm_e4m3_swiglu", ptr(a.q), a.q.stride(0), ptr(a.scale), ptr(w_gu.q), w_gu.q.stride(0), ptr(w_gu.scale), ptr(act), I,
+             a.shape[0], I, a.shape[1])
+    else:
+        act = silu_mul(gemm_fp8(a, w_gu))
+    return gemm_fp8(quant_rows(act), w_dn)
+
+
+# ---------------------------------------------------------------------------------------------------
 # attention (K7)
 # ---------------------------------------------------------------------------------------------------
 ATTN_HEAD_DIMS = (64, 128)

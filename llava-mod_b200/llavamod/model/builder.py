@@ -32,7 +32,8 @@ def pick_eval_class(model_name):
 def load_pretrained_model(model_path, model_base, model_name, load_8bit=False, load_4bit=False, device_map="auto", device="cuda",
                           padding_side="right", merge=False, tokenizer=None, **kwargs):
     if load_8bit or load_4bit:
-        raise NotImplementedError("4/8-bit loading is not built")
+        raise NotImplementedError("4/8-bit loading is not built; a frozen dense model runs in 8 bits on the H100 as FP8 (e4m3): "
+                                  "model.quantize_fp8_() after loading, or --ref_fp8 for the teacher of the distillation recipes")
     if "lora" in model_name.lower() or model_base is not None:
         raise NotImplementedError("LoRA / base+projector loading is not built (the distillation recipes save full state dicts)")
     if "llava" not in model_name.lower():

@@ -85,15 +85,18 @@ def _decoder_entry(model, B, max_len, T=1):
     """(cache, graph slot) for B sequences of up to max_len positions and steps of T tokens per sequence, reused across calls while graphs
     are on (T > 1: the verify step of assisted decoding; a model that is its own assistant gets one entry per width).  A captured step holds
     the addresses of the cache buffers and of the weights, and the host decisions made while it was captured: the MoE capacity rule of
-    every sparse layer and the epilogue-fusion switches.  All of them are part of the key."""
+    every sparse layer and the epilogue-fusion switches.  All of them are part of the key; the e4m3 buffers of a quantize_fp8_ model are not
+    Parameters, so they are listed beside them (a step captured before the quantisation is never replayed after it)."""
     if not _graphs_enabled():
         return dict(cache=model.new_kv_cache(B, max_len), graph=None)
     for k in [k for k, v in _STEP_GRAPHS.items() if v["model"]() is None]:       # the model is gone: free its cache and graph
         del _STEP_GRAPHS[k]
     moe = tuple((l.mlp.num_experts, l.mlp.capacity_factor, l.mlp.eval_capacity_factor, l.mlp.min_capacity)
                 for l in model.model.layers if hasattr(l.mlp, "deepspeed_moe"))
+    fp8 = tuple(t.data_ptr() for l in model.model.layers if isinstance(l.self_attn.qkv_weight, K.Fp8Rows)
+                for w in (l.self_attn.qkv_weight, l.self_attn.o_fp8, l.mlp.gu_weight, l.mlp.down_fp8) for t in (w.q, w.scale))
     key = (id(model), B, max_len, T, model.training, moe, K.FUSE_SWIGLU, K.FUSE_ROPE, K.FUSE_RESIDUAL,
-           tuple(p.data_ptr() for p in model.parameters()))
+           tuple(p.data_ptr() for p in model.parameters()), fp8)
     ent = _STEP_GRAPHS.pop(key, None)
     if ent is None or ent["model"]() is not model:
         ent = dict(model=weakref.ref(model), cache=model.new_kv_cache(B, max_len), graph=None)

@@ -55,6 +55,7 @@ class LlavaQwenForCausalLMBase(nn.Module, LlavaMetaForCausalLM):
     config_class = Qwen2Config
     model_class = LlavaQwenModelBase
     is_moe = False
+    is_fp8 = False            # quantize_fp8_ has run: the decoder linears hold e4m3 weights, the model is forward-only
 
     def __init__(self, config, device="cuda", dtype=torch.bfloat16):
         nn.Module.__init__(self)
@@ -89,7 +90,43 @@ class LlavaQwenForCausalLMBase(nn.Module, LlavaMetaForCausalLM):
         """state_dict with tied lm_head de-duplicated the way HF saves it."""
         return {k: v for k, v in self.state_dict().items()}
 
+    _FP8_NO_SAVE = ("this model's decoder weights were quantised to e4m3 in place (quantize_fp8_): their bf16 values are gone and there is "
+                    "no e4m3 checkpoint format -- save the model before quantising it, or reload the bf16 checkpoint")
+
+    def quantize_fp8_(self):
+        """Run the decoder linears (q|k|v, o_proj, gate|up, down_proj of every layer) of this frozen dense model in FP8 from now on: e4m3
+        weights with one scale per output channel, activations quantised per token on the fly, fp32 accumulation (csrc/gemm_fp8.cu,
+        csrc/quant.cu).  Embeddings, norms, RoPE, attention, the residual stream, lm_head, the CLIP tower and the projector stay bf16.
+        In place and one-way: the bf16 decoder weights are released.  Afterwards the model is forward-only -- labels, autograd through
+        the decoder and saving raise.  The counterpart of the reference's 8-bit loading of a frozen model (align_train.py:536-553)."""
+        if self.is_moe or any(isinstance(l.mlp, MoE) for l in self.model.layers):
+            raise ValueError("quantize_fp8_ is for frozen dense models (the teacher); %s has trainable sparse-MoE experts" % type(self).__name__)
+        if self.is_fp8:
+            raise ValueError("this model is already quantised to e4m3")
+        for n, p in self.model.layers.named_parameters():
+            if p.requires_grad:
+                raise ValueError("quantize_fp8_ needs a frozen decoder: model.layers.%s requires grad (an e4m3 weight cannot be trained)" % n)
+        if self.training:
+            raise ValueError("quantize_fp8_ needs the model in eval mode (call .eval() first): an FP8 model is forward-only")
+        if self.device.type != "cuda":
+            raise ValueError("quantize_fp8_ needs the model on the GPU (the weights are quantised by a CUDA kernel); it is on %s" % self.device)
+        self.model.quantize_fp8_()
+        self.is_fp8 = True
+        return self
+
+    def state_dict(self, *args, **kwargs):
+        if self.is_fp8:
+            raise RuntimeError(self._FP8_NO_SAVE)
+        return super().state_dict(*args, **kwargs)
+
+    def train(self, mode=True):
+        if mode and self.is_fp8:
+            raise RuntimeError("an e4m3-quantised model is forward-only and stays in eval mode")
+        return super().train(mode)
+
     def save_pretrained(self, path, state_dict=None):
+        if self.is_fp8:
+            raise RuntimeError(self._FP8_NO_SAVE)
         os.makedirs(path, exist_ok=True)
         cfg = self.config
         cfg.architectures = [type(self).__name__]
@@ -167,6 +204,8 @@ class LlavaQwenForCausalLMBase(nn.Module, LlavaMetaForCausalLM):
     def forward_train_loss(self, input_ids=None, attention_mask=None, labels=None, images=None, moe_noise=None, plan=None):
         """Training-time `.loss` of `forward` without materialising the fp32 logits the reference returns (llava_qwen1_5_moe.py:408-434;
         dense: modeling_qwen2.py:1195-1207): shifted CE (+ moe_loss).  -> (loss, ce.detach(), moe_loss or None)"""
+        if self.is_fp8:
+            raise RuntimeError("an e4m3-quantised model is forward-only: it has no training loss")
         r = self.forward_hidden(input_ids, attention_mask, None, None, labels, images, moe_noise, plan=plan)
         hidden = r["hidden"]
         B, T, H = hidden.shape
@@ -179,6 +218,8 @@ class LlavaQwenForCausalLMBase(nn.Module, LlavaMetaForCausalLM):
                 labels=None, use_cache=None, output_attentions=None, output_hidden_states=None, images=None,
                 return_dict=None, moe_noise=None):
         cache = None
+        if self.is_fp8 and labels is not None:
+            raise RuntimeError("an e4m3-quantised model is forward-only: call it without labels")
         if past_key_values is not None or use_cache:
             # KV-cache path (modeling_qwen2.py:1110-1217 with past_key_values; llava_arch.py:162-172 for the cached multimodal step).
             # Without a cache one is allocated for the prompt plus CACHE_ROOM positions; pass new_kv_cache(B, max_len) for longer runs.

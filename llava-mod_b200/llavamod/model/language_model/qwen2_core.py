@@ -256,6 +256,19 @@ class Qwen2Model(nn.Module):
     def gview(self, t):
         return self.grad_views.get(id(t))
 
+    def quantize_fp8_(self):
+        """Turn the decoder linears of every (dense, frozen) layer into e4m3 weights with one fp32 scale per output channel
+        (K.quant_rows on the device; the fused q|k|v and gate|up buffers as the single buffers they are) and release the bf16 copies:
+        ``qkv_weight`` / ``gu_weight`` become K.Fp8Rows, o_proj / down_proj are held as ``o_fp8`` / ``down_fp8``, and the per-projection
+        ``weight`` Parameters are gone.  Biases, norms, embeddings stay bf16.  The callers (quantize_fp8_ of the causal-LM classes) have
+        checked that nothing here trains."""
+        for layer in self.layers:
+            at, mlp = layer.self_attn, layer.mlp
+            at.o_fp8, mlp.down_fp8 = K.quant_rows(at.o_proj.weight.detach()), K.quant_rows(mlp.down_proj.weight.detach())
+            at.qkv_weight, mlp.gu_weight = K.quant_rows(at.qkv_weight), K.quant_rows(mlp.gu_weight)
+            for lin in (at.q_proj, at.k_proj, at.v_proj, at.o_proj, mlp.gate_proj, mlp.up_proj, mlp.down_proj):
+                lin.weight = None
+
     # -- forward -------------------------------------------------------------------------------------
     def forward(self, inputs_embeds, attention_mask=None, position_ids=None, moe_noise=None, training_moe=True, cache=None):
         """inputs_embeds [B,T,H] bf16; attention_mask [B,T] bool or None; position_ids [B,T] int64 or None.
@@ -310,17 +323,26 @@ class Qwen2Model(nn.Module):
         for li, layer in enumerate(self.layers):
             at = layer.self_attn
             nh, nkv, hd = at.num_heads, at.num_key_value_heads, at.head_dim
-            if branch is None:
-                x, stream = K.rmsnorm(stream, layer.input_layernorm.weight, cfg.rms_norm_eps, wgrad=self.gview(layer.input_layernorm.weight))
+            fp8 = isinstance(at.qkv_weight, K.Fp8Rows)      # a layer of quantize_fp8_: the norms hand e4m3 rows to e4m3 projections
+            if fp8:
+                x, stream = K.rmsnorm_quant(stream if branch is None else branch, layer.input_layernorm.weight, cfg.rms_norm_eps,
+                                            res=None if branch is None else stream)
+                qkv = K.qkv_rope_fp8(x, at.qkv_weight, at.qkv_bias, cos, sin, pos, nh, nkv, hd)
             else:
-                x, stream = K.rmsnorm(branch, layer.input_layernorm.weight, cfg.rms_norm_eps, res=stream, wgrad=self.gview(layer.input_layernorm.weight))
-            qkv = K.qkv_rope(x, at.qkv_weight, at.qkv_bias, cos, sin, pos, nh, nkv, hd, self.gview(at.qkv_weight), self.gview(at.qkv_bias))
+                if branch is None:
+                    x, stream = K.rmsnorm(stream, layer.input_layernorm.weight, cfg.rms_norm_eps, wgrad=self.gview(layer.input_layernorm.weight))
+                else:
+                    x, stream = K.rmsnorm(branch, layer.input_layernorm.weight, cfg.rms_norm_eps, res=stream, wgrad=self.gview(layer.input_layernorm.weight))
+                qkv = K.qkv_rope(x, at.qkv_weight, at.qkv_bias, cos, sin, pos, nh, nkv, hd, self.gview(at.qkv_weight), self.gview(at.qkv_bias))
             if ragged:
                 K.kv_append_rows(qkv, B, T, nh, nkv, hd, cache.k[li], cache.v[li], pad[0], pad[1], cache.len)
             elif cache is not None:
                 K.kv_append(qkv, B, T, nh, nkv, hd, cache.k[li], cache.v[li], cache.len)
             attn = K.attention(qkv, B, T, nh, nkv, hd, True, None, pad)
-            if K.residual_fusable(attn, stream, self.gview(at.o_proj.weight), self.gview(layer.post_attention_layernorm.weight)):
+            if fp8:                                     # the add stays in the norm's kernel (the same bytes as the fused epilogue)
+                branch = K.linear_fp8(attn, at.o_fp8)
+                x, stream = K.rmsnorm_quant(branch, layer.post_attention_layernorm.weight, cfg.rms_norm_eps, res=stream)
+            elif K.residual_fusable(attn, stream, self.gview(at.o_proj.weight), self.gview(layer.post_attention_layernorm.weight)):
                 # frozen / no-grad forward: o_proj's epilogue writes residual + branch (modeling_qwen2.py:796), the norm reads one tensor
                 stream = K.gemm_residual(attn, at.o_proj.weight, None, stream)
                 x, stream = K.rmsnorm(stream, layer.post_attention_layernorm.weight, cfg.rms_norm_eps)
@@ -346,6 +368,8 @@ class Qwen2Model(nn.Module):
                     records.append(rec)
                 l_auxes.append(l_aux)
                 branch = None
+            elif fp8:
+                branch = K.mlp_fp8(x, mlp.gu_weight, mlp.down_fp8)
             elif K.residual_fusable(x, stream, self.gview(mlp.gu_weight), self.gview(mlp.down_proj.weight)):
                 stream = K.mlp(x, mlp.gu_weight, mlp.down_proj.weight, res=stream)      # down_proj epilogue adds the stream (:808)
                 branch = None
@@ -400,17 +424,22 @@ class Qwen2Model(nn.Module):
         for li, layer in enumerate(self.layers):
             at = layer.self_attn
             nh, nkv, hd = at.num_heads, at.num_key_value_heads, at.head_dim
+            fp8 = isinstance(at.qkv_weight, K.Fp8Rows)
+            norm = K.rmsnorm_quant if fp8 else K.rmsnorm
             if branch is None:
-                x, stream = K.rmsnorm(stream, layer.input_layernorm.weight, cfg.rms_norm_eps)
+                x, stream = norm(stream, layer.input_layernorm.weight, cfg.rms_norm_eps)
             else:
-                x, stream = K.rmsnorm(branch, layer.input_layernorm.weight, cfg.rms_norm_eps, res=stream)
-            qkv = K.qkv_rope(x, at.qkv_weight, at.qkv_bias, cos, sin, pos, nh, nkv, hd)
+                x, stream = norm(branch, layer.input_layernorm.weight, cfg.rms_norm_eps, res=stream)
+            qkv = (K.qkv_rope_fp8 if fp8 else K.qkv_rope)(x, at.qkv_weight, at.qkv_bias, cos, sin, pos, nh, nkv, hd)
             K.kv_append(qkv, B, T, nh, nkv, hd, cache.k[li], cache.v[li], cache.len)
             if T == 1:
                 attn, _ = K.attn_decode(qkv, nh, nkv, hd, cache.k[li], cache.v[li], cache.end, cache.ws)
             else:
                 attn, _ = K.attn_decode_chunk(qkv, B, T, nh, nkv, hd, cache.k[li], cache.v[li], cache.end, ws)
-            if K.residual_fusable(attn, stream):
+            if fp8:
+                branch = K.linear_fp8(attn, at.o_fp8)
+                x, stream = K.rmsnorm_quant(branch, layer.post_attention_layernorm.weight, cfg.rms_norm_eps, res=stream)
+            elif K.residual_fusable(attn, stream):
                 stream = K.gemm_residual(attn, at.o_proj.weight, None, stream)
                 x, stream = K.rmsnorm(stream, layer.post_attention_layernorm.weight, cfg.rms_norm_eps)
             else:
@@ -427,6 +456,8 @@ class Qwen2Model(nn.Module):
                 records.append(rec)
                 l_auxes.append(l_aux)
                 branch = None
+            elif fp8:
+                branch = K.mlp_fp8(x, mlp.gu_weight, mlp.down_fp8)
             elif K.residual_fusable(x, stream):
                 stream = K.mlp(x, mlp.gu_weight, mlp.down_proj.weight, res=stream)
                 branch = None

@@ -181,7 +181,7 @@ def train(argv=None):
         model.config.pad_token_id = tokenizer.pad_token_id                               # align_train.py:437
     data_module = make_supervised_data_module(data_args, training_args, model, tokenizer)
     trainer = AlignTrainer(model=model, ref_model=ref_model, args=training_args, loss_type=align_args.loss_type,
-                           moe_loss_enable=align_args.moe_loss_enable, tokenizer=tokenizer, **data_module)
+                           moe_loss_enable=align_args.moe_loss_enable, ref_fp8=align_args.ref_fp8, tokenizer=tokenizer, **data_module)
     resume = bool(glob.glob(os.path.join(training_args.output_dir, "checkpoint-*")))     # align_train.py:601-604
     trainer.train(resume_from_checkpoint=resume)
     model.config.use_cache = True

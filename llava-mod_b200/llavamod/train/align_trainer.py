@@ -46,12 +46,21 @@ def same_frozen_tower(a, b):
     return ta.select_layer == tb.select_layer and all(torch.equal(sa[k], sb[k]) for k in sa)
 
 
+def quantize_ref_fp8(ref, ref_fp8):
+    """--ref_fp8 / LLAVAMOD_REF_FP8=1: the frozen teacher's decoder linears run in FP8 (e4m3) from here on (quantize_fp8_ of the dense
+    causal-LM classes).  Opt-in: it changes the teacher's logits.  The quantisers and the e4m3 GEMM are plain stream-ordered launches, so
+    the teacher keeps its side stream, its one-micro-batch lead and its place in the captured step."""
+    import os
+    if (ref_fp8 or bool(int(os.environ.get("LLAVAMOD_REF_FP8", "0")))) and not ref.is_fp8:
+        ref.quantize_fp8_()
+
+
 class AlignTrainer(BaseTrainer):
     def __init__(self, model=None, ref_model=None, args=None, data_collator=None, train_dataset=None, eval_dataset=None,
                  tokenizer=None, label_pad_token_id: int = -100, padding_value: int = 0, beta: float = 0.1,
                  label_smoothing: float = 0, loss_type: str = "sigmoid", moe_loss_enable: bool = False,
                  disable_dropout: bool = True, model_init=None, compute_metrics=None, callbacks=None,
-                 optimizers=(None, None), preprocess_logits_for_metrics=None):
+                 optimizers=(None, None), preprocess_logits_for_metrics=None, ref_fp8: bool = False):
         if ref_model:
             self.ref_model = ref_model
         else:
@@ -78,6 +87,7 @@ class AlignTrainer(BaseTrainer):
         self.share_tower = same_frozen_tower(self.model, self.ref_model.module)
         self.kd_vocab = KD_VOCAB_SIZE
         import os
+        quantize_ref_fp8(self.ref_model.module, ref_fp8)
         self.overlap_teacher = bool(int(os.environ.get("LLAVAMOD_OVERLAP_TEACHER", "1"))) and next(model.parameters()).is_cuda
         self._teacher_stream = torch.cuda.Stream() if self.overlap_teacher else None
         self.pipeline_teacher = bool(int(os.environ.get("LLAVAMOD_PIPELINE_TEACHER", "1")))

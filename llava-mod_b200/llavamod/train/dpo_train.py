@@ -70,7 +70,7 @@ def train(argv=None):
                                  training_args.seed)
         data_module = dict(train_dataset=ds, eval_dataset=None, data_collator=collate_dpo)
     trainer = DPOTrainer(model=model, ref_model=ref_model, args=training_args, loss_type=dpo_args.loss_type,
-                         moe_loss_enable=dpo_args.moe_loss_enable, tokenizer=tokenizer, **data_module)
+                         moe_loss_enable=dpo_args.moe_loss_enable, ref_fp8=dpo_args.ref_fp8, tokenizer=tokenizer, **data_module)
     trainer.train(resume_from_checkpoint=bool(glob.glob(os.path.join(training_args.output_dir, "checkpoint-*"))))
     if not dist.is_initialized() or dist.get_rank() == 0:
         model.config.save_pretrained(training_args.output_dir)

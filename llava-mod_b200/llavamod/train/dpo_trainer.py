@@ -16,7 +16,7 @@ import torch.nn.functional as F
 
 from .. import kernels as K
 from ..model.utils import create_reference_model, disable_dropout_in_model
-from .align_trainer import _Wrapped, same_frozen_tower
+from .align_trainer import _Wrapped, quantize_ref_fp8, same_frozen_tower
 from .trainer_base import BaseTrainer
 
 
@@ -25,7 +25,7 @@ class DPOTrainer(BaseTrainer):
                  tokenizer=None, label_pad_token_id: int = -100, padding_value: int = 0, beta: float = 0.1,
                  label_smoothing: float = 0, loss_type: str = "sigmoid", moe_loss_enable: bool = False,
                  disable_dropout: bool = True, model_init=None, compute_metrics=None, callbacks=None,
-                 optimizers=(None, None), preprocess_logits_for_metrics=None):
+                 optimizers=(None, None), preprocess_logits_for_metrics=None, ref_fp8: bool = False):
         self.ref_model = ref_model if ref_model else create_reference_model(model)
         if disable_dropout:
             disable_dropout_in_model(model)
@@ -46,6 +46,7 @@ class DPOTrainer(BaseTrainer):
         for p in self.ref_model.module.parameters():
             p.requires_grad = False
         self.share_tower = same_frozen_tower(self.model, self.ref_model.module)
+        quantize_ref_fp8(self.ref_model.module, ref_fp8)
         import os
         self.overlap_teacher = bool(int(os.environ.get("LLAVAMOD_OVERLAP_TEACHER", "1"))) and next(model.parameters()).is_cuda
         self._teacher_stream = torch.cuda.Stream() if self.overlap_teacher else None
