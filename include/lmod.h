@@ -224,8 +224,10 @@ int lmod_gemm_bf16(const void* A, int64_t lda, int a_mn_major, const void* B, in
                    float* d_f32_accum, void* stream);
 /* lmod_gemm_bf16 with extents read from DEVICE memory at kernel start (dense problems only): M_eff = min(M, *m_rows_dev),
  * K_eff = min(K, round_up(*k_rows_dev, 64)); either pointer may be NULL (static extent).  Tensor maps and the launch grid are sized for the
- * static M / K; tiles beyond the effective extent are skipped, an empty reduction contributes zero.  Rows of A (or of both MN-major
- * operands, for a dynamic K) between the count and the next tile boundary must hold finite values (lmod_gather_rows zero-fills them). */
+ * static M / K; tiles beyond the effective extent are skipped, an empty reduction contributes zero.  Dynamic M: the last tile stores
+ * all its rows, up to min(M, round_up(M_eff, 128)) (A's rows there times B; rows at or past that are untouched).  Dynamic K: rows
+ * [*k_rows_dev, round_up(*k_rows_dev, 64)) of both MN-major operands are read, must be finite, and one of the two must be zero there
+ * (lmod_gather_rows zero-fills the hidden rows; an m_rows_dev GEMM of them writes zero rows); rows past that are never read. */
 int lmod_gemm_bf16_dyn(const void* A, int64_t lda, int a_mn_major, const void* B, int64_t ldb, int b_mn_major,
                        void* D, int64_t ldd, int64_t M, int64_t N, int64_t K, const void* bias, int epilogue,
                        float* d_f32_accum, const int32_t* m_rows_dev, const int32_t* k_rows_dev, void* stream);

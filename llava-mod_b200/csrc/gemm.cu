@@ -72,14 +72,25 @@ struct GemmParams {
   int64_t d_group_stride;          // wgrad grouped: element stride of D per group
   int wgrad_grouped;               // 1: groups split the REDUCTION (K) range via offsets; M,N dense per group
   // dense only: extents read from DEVICE memory at kernel start (the loss head works on the batch's supervised rows, whose count is
-  // data-dependent, inside a CUDA graph): M_eff = min(M, *m_dev), K_eff = min(K, round_up(*k_dev, BK)); null = static
+  // data-dependent, inside a CUDA graph): null = static.
+  //   m_dev: M_eff = min(M, *m_dev).  Only the tiles holding rows < M_eff run, and they store their WHOLE 128-row tile (up to
+  //          min(M, round_up(M_eff, 128))), not just the rows < M_eff: the rows past M_eff then hold A's rows times B (exact zeros
+  //          for the zero-padded rows of lmod_gather_rows) instead of whatever the buffer held, so that a k_dev reduction over them
+  //          (the lm_head wgrad after an m_dev forward) never meets unwritten memory.
+  //   k_dev: K_eff = min(K, round_up(*k_dev, BK)).  Rows [*k_dev, round_up(*k_dev, 64)) of BOTH operands are read and must be
+  //          finite, with at least one of the two zero there; rows at or past round_up(*k_dev, 64) are never read.
   const int32_t* m_dev;
   const int32_t* k_dev;
+  int m_store;                     // set by effective_extents: rows of D the dense tiles store below (M, or the m_dev tile end)
 };
 
 __device__ __forceinline__ GemmParams effective_extents(const GemmParams& in) {
   GemmParams p = in;
-  if (in.m_dev) p.M = min(in.M, max(0, *in.m_dev));
+  p.m_store = in.M;
+  if (in.m_dev) {
+    p.M = min(in.M, max(0, *in.m_dev));
+    p.m_store = min(in.M, (p.M + BM - 1) / BM * BM);
+  }
   if (in.k_dev) p.K = min(in.K, (max(0, *in.k_dev) + BK - 1) / BK * BK);
   return p;
 }
@@ -115,7 +126,7 @@ __device__ __forceinline__ bool get_tile(const GemmParams& p, int t, Tile& o) {
     if (t >= mn * p.splits) return false;
     const int ks = t / mn, r = t % mn;                       // output tiles fastest: concurrent CTAs hit different D tiles
     const int per = (nk + p.splits - 1) / p.splits;
-    o.m0 = (r % num_m) * BM; o.n0 = (r / num_m) * BN; o.kb0 = ks * per; o.kb1 = min(nk, o.kb0 + per); o.group = 0; o.m_end = p.M;
+    o.m0 = (r % num_m) * BM; o.n0 = (r / num_m) * BN; o.kb0 = ks * per; o.kb1 = min(nk, o.kb0 + per); o.group = 0; o.m_end = p.m_store;
     return true;
   }
   if (p.wgrad_grouped) {

@@ -5,8 +5,11 @@
 // data ~40-60 % of the positions (system prompt, image patches, the question) carry neither a KD mask nor a CE target, so here the
 // student / teacher lm_head GEMMs, the fused KL+CE kernel and the lm_head backward GEMMs run on the batch's ACTIVE rows only:
 //   lmod_active_rows  -> perm[j] = original row of the j-th active row, count (device scalars, no host sync, CUDA-graph friendly)
-//   lmod_gather_rows  -> compact copy of the hidden states (rows count..round_up(count,pad) zero-filled so partial GEMM tiles and the
-//                        wgrad reduction tail stay exact zeros)
+//   lmod_gather_rows  -> compact copy of the hidden states (rows count..round_up(count,pad) zero-filled, so the rows past count that
+//                        a partial GEMM tile computes are exact zeros)
+//   The lm_head wgrad reduces over rows [0, round_up(count, 64)) of BOTH the hidden rows and dlogits, and 0 * NaN is NaN: dlogits rows
+//   [count, round_up(count, 64)) must be finite too.  The KL kernel writes rows < count only; the m_dev logits GEMM stores its whole
+//   last 128-row tile (gemm.cu), which puts exact zeros (zero hidden rows times W) into those rows before the KL kernel runs.
 //   lmod_scatter_rows -> d hidden back to its original rows
 // The GEMMs read the dynamic extents from device memory (lmod_gemm_bf16_dyn).  Results are identical: a row that contributes
 // exactly zero to the loss contributes exactly zero gradient.

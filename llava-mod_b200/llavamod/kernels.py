@@ -69,7 +69,7 @@ def mm_nn(dy, w, m_dev=None):
         gemm(dy2, w, b_mn=True, out_f32=acc, split_k=split, m_dev=m_dev)
         return acc.to(dy.dtype)
     if m_dev is not None:
-        out = torch.zeros(M, Kout, dtype=dy.dtype, device=dy.device)         # rows past the dynamic extent stay zero
+        out = torch.zeros(M, Kout, dtype=dy.dtype, device=dy.device)         # rows past the extent's last 128-row tile stay zero
         return gemm(dy2, w, b_mn=True, out=out, m_dev=m_dev)
     return gemm(dy2, w, b_mn=True)
 

@@ -1,5 +1,6 @@
 """Shared fixtures for the GPU parity tests, smoke() and bench.py: tiny config-1 models, seeded batches, and the
 oracle-side evaluation of the same step."""
+import contextlib
 import math
 import types
 
@@ -1092,3 +1093,23 @@ def check_moe_stages(k, ref, E, old, report=None):
         for e in range(E):
             if int(rec["used"][e]) == 0:                       # an expert without rows leaves its pre-filled gradient untouched
                 check_moe(f"g_{gname}[{e}] (empty expert)", k["g_" + gname][e], old[gname][e], None)
+
+
+# ---------------------------------------------------------------------------------------------------
+# reads of memory nobody wrote
+# ---------------------------------------------------------------------------------------------------
+@contextlib.contextmanager
+def poisoned_uninitialised_memory():
+    """Inside: every torch.empty / empty_like (and every allocation torch makes for an op's output) is filled at allocation, floats with
+    NaN and integers with their largest value (torch's deterministic mode with fill_uninitialized_memory).  A kernel that reads memory
+    nobody wrote then reads NaN every time, instead of whatever an earlier tensor left there.  Both settings are restored on exit."""
+    import torch.utils.deterministic as det
+    was_det, was_warn, was_fill = torch.are_deterministic_algorithms_enabled(), torch.is_deterministic_algorithms_warn_only_enabled(), \
+        det.fill_uninitialized_memory
+    torch.use_deterministic_algorithms(True, warn_only=True)
+    det.fill_uninitialized_memory = True
+    try:
+        yield
+    finally:
+        det.fill_uninitialized_memory = was_fill
+        torch.use_deterministic_algorithms(was_det, warn_only=was_warn)

@@ -1,6 +1,8 @@
 """Active-row compaction of the loss head (csrc/rows.cu, lmod_gemm_bf16_dyn, lmod_kl_fwd_bwd_rows): integer index work bit-exact
 against numpy/torch, the compact KL kernel bit-identical to the dense one on the rows that matter, dynamic-extent GEMMs equal to the
 static GEMM on the effective sub-problem, and the whole compact head equal to the dense head."""
+import contextlib
+
 import pytest
 import torch
 
@@ -76,39 +78,71 @@ def test_compact_kl_equals_dense_kl(N, V, frac, w_ce):
     assert bool((d_dense[inactive] == 0).all())             # what the compact path never has to write
 
 
-@pytest.mark.parametrize("count", [0, 1, 255, 256, 700, 2048])
+COUNTS = [0, 1, 255, 256, 700, 2048]
+
+
+@pytest.mark.parametrize("count", COUNTS)
 def test_dynamic_extent_gemms_match_static_subproblem(count):
-    """M from device memory (forward / dgrad) and K from device memory (wgrad), incl. the empty problem."""
+    """M from device memory (forward / dgrad) and K from device memory (wgrad), incl. the empty problem.  A is zero from row `count` on,
+    what gather_rows guarantees up to the tile boundary; the m_dev GEMM stores exactly its last 128-row tile."""
+    _dynamic_extent_case(count, "zero")
+
+
+@pytest.mark.parametrize("count", COUNTS)
+def test_dynamic_extent_gemms_keep_nan_past_the_extent_out(count):
+    """As above, but A is zero only on [count, round_up(count, 64)) -- the rows the wgrad reads past the count, which must be finite with
+    one operand zero -- and NaN from there on: no NaN may reach a valid output row or the wgrad."""
+    _dynamic_extent_case(count, "nan")
+
+
+def _dynamic_extent_case(count, tail):
     from llavamod import kernels as K
     g = torch.Generator().manual_seed(count)
     M, Kd, N = 2048, 256, 2048 + 512
+    r64 = min(M, (count + 63) // 64 * 64)
     a = torch.randn(M, Kd, generator=g).to(torch.bfloat16).cuda()
-    a[count:] = 0                                                           # what gather_rows guarantees up to the tile boundary
+    a[count:] = 0
+    if tail == "nan":
+        a[r64:] = float("nan")
     w = torch.randn(N, Kd, generator=g).to(torch.bfloat16).cuda()
     cnt = torch.tensor([count], dtype=torch.int32, device="cuda")
     full = K.gemm(a, w)
     out = torch.full((M, N), 3.0, dtype=torch.bfloat16, device="cuda")
     K.gemm(a, w, out=out, m_dev=cnt)
     assert torch.equal(out[:count], full[:count])
-    tile_end = (count + 255) // 256 * 256
-    assert bool((out[tile_end:] == 3.0).all())                              # tiles past the extent are not touched
+    m_store = min(M, (count + 127) // 128 * 128)                            # the whole last tile is stored, NaN rows of A included
+    assert torch.equal(out[:m_store].view(torch.int16), full[:m_store].view(torch.int16))
+    assert bool((out[m_store:] == 3.0).all())                              # tiles past the extent are not touched
     # dgrad form (B MN-major); N = 2560 stays below mm_nn's split-K threshold (N >= 16384), which test_loss_head_gpu.py covers
     dx = K.mm_nn(full, w, m_dev=cnt)
-    ref = K.mm_nn(full, w)
-    assert torch.allclose(dx[:count].float(), ref[:count].float(), rtol=2e-2, atol=2e-2 * ref.float().abs().max().item())
-    # wgrad form: reduction over the first `count` rows only
+    ref = K.mm_nn(full[:max(count, 1)], w)[:count]
+    assert bool(torch.isfinite(dx[:count]).all())
+    assert torch.allclose(dx[:count].float(), ref.float(), rtol=2e-2, atol=2e-2 * max(1.0, ref.float().abs().max().item() if count else 0.0))
+    # wgrad form: reduction over the first round_up(count, 64) rows only (rows [count, r64) of `full` are zero rows of `a` times w)
     gacc = torch.zeros(N, Kd, dtype=torch.bfloat16, device="cuda")
     K.mm_tn_acc(full, a, gacc, k_dev=cnt)
     gref = torch.zeros(N, Kd, dtype=torch.bfloat16, device="cuda")
     if count:
-        K.mm_tn_acc(full[:tile_end if tile_end <= M else M], a[:tile_end if tile_end <= M else M], gref)
+        K.mm_tn_acc(full[:r64], a[:r64], gref)
+    assert bool(torch.isfinite(gacc).all())
     err = (gacc.float() - gref.float()).abs().max().item()
     assert err <= 2e-2 * max(1.0, gref.float().abs().max().item()), err
 
 
 def test_compact_head_equals_dense_head():
-    """DistillHeadFn with and without row compaction: same losses, same d hidden, same lm_head gradient."""
+    """DistillHeadFn with and without row compaction: same losses, same d hidden, same lm_head gradient.  The active-row count is not a
+    multiple of 64, so the lm_head wgrad reads dlogits rows past the count."""
+    _compact_vs_dense_head(poisoned=False)
+
+
+def test_compact_head_equals_dense_head_with_poisoned_allocations():
+    """The same with every torch.empty NaN-filled: a dlogits row nobody wrote would turn the lm_head gradient into NaN."""
+    _compact_vs_dense_head(poisoned=True)
+
+
+def _compact_vs_dense_head(poisoned):
     from llavamod import kernels as K
+    from tests.helpers import poisoned_uninitialised_memory
     g = torch.Generator().manual_seed(5)
     B, T, H, V = 2, 96, 128, 4096
     hid = torch.randn(B, T, H, generator=g).to(torch.bfloat16).cuda()
@@ -116,16 +150,22 @@ def test_compact_head_equals_dense_head():
     th = torch.randn(B * T, H, generator=g).to(torch.bfloat16).cuda()
     wt = (torch.randn(V, H, generator=g) * 0.05).to(torch.bfloat16).cuda()
     lab = _labels(B, T, V, 0.55, seed=9, tail_pad=4).cuda()
+    n_active = int(_active_ref(lab.cpu()).sum())
+    assert n_active % 64 != 0, n_active
     res = []
-    for compact in (False, True):
-        h = hid.clone().requires_grad_(True)
-        hg = torch.zeros(V, H, dtype=torch.bfloat16, device="cuda")
-        rows = K.active_rows(lab.reshape(-1), T) if compact else None
-        t_logits = K.gemm(K.gather_rows(th, *rows) if compact else th, wt, m_dev=rows[1] if compact else None)
-        total, align, ce = K.distill_head(h, w, t_logits, lab, V, 1.0, 1.0, False, hg, rows=rows)
-        (total * 0.5).backward()
-        res.append((float(total), float(align), float(ce), h.grad.clone(), hg))
+    with poisoned_uninitialised_memory() if poisoned else contextlib.nullcontext():
+        for compact in (False, True):
+            h = hid.clone().requires_grad_(True)
+            hg = torch.zeros(V, H, dtype=torch.bfloat16, device="cuda")
+            rows = K.active_rows(lab.reshape(-1), T) if compact else None
+            t_logits = K.gemm(K.gather_rows(th, *rows) if compact else th, wt, m_dev=rows[1] if compact else None)
+            total, align, ce = K.distill_head(h, w, t_logits, lab, V, 1.0, 1.0, False, hg, rows=rows)
+            (total * 0.5).backward()
+            torch.cuda.synchronize()
+            res.append((float(total), float(align), float(ce), h.grad.clone(), hg))
     a, b = res
+    for name, t in (("d hidden", b[3]), ("lm_head gradient", b[4])):
+        assert bool(torch.isfinite(t).all()), f"compact head: non-finite {name} ({int((~torch.isfinite(t)).sum())} elements)"
     assert a[:3] == b[:3]
     assert torch.allclose(a[3].float(), b[3].float(), rtol=2e-2, atol=1e-5)
     assert torch.allclose(a[4].float(), b[4].float(), rtol=2e-2, atol=2e-2 * a[4].float().abs().max().item())
