@@ -18,13 +18,15 @@ struct OnlineLse {
     float x[8] = {bf16lo(v.x), bf16hi(v.x), bf16lo(v.y), bf16hi(v.y), bf16lo(v.z), bf16hi(v.z), bf16lo(v.w), bf16hi(v.w)};
     float vm = fmaxf(fmaxf(fmaxf(x[0], x[1]), fmaxf(x[2], x[3])), fmaxf(fmaxf(x[4], x[5]), fmaxf(x[6], x[7])));
     if (vm > m) { z *= ex2f((m - vm) * LOG2E_F); m = vm; }     // m == -inf: z is 0 and stays 0 (ex2(-inf)=0)
-    const float nm = -m * LOG2E_F;
+    // While m is still -inf (every element so far -inf) the exponent is taken against 0, so a -inf element adds ex2(-inf) = 0;
+    // against m it would be -inf - (-inf) = NaN, which no later rescale clears (the same guard as kl.cu).
+    const float nm = isinf(m) ? 0.f : -m * LOG2E_F;
 #pragma unroll
     for (int j = 0; j < 8; ++j) z += ex2f(fmaf(x[j], LOG2E_F, nm));
   }
   __device__ __forceinline__ void add1(float x) {
     if (x > m) { z *= ex2f((m - x) * LOG2E_F); m = x; }
-    z += ex2f((x - m) * LOG2E_F);
+    z += ex2f((x - (isinf(m) ? 0.f : m)) * LOG2E_F);
   }
 };
 

@@ -200,6 +200,186 @@ def check_out4(out4, ref, msg="out4"):
 
 
 # ---------------------------------------------------------------------------------------------------
+# log-prob gather and the dense compat forms (csrc/logp.cu): float64 references and element-wise bounds
+# ---------------------------------------------------------------------------------------------------
+# Every kernel of logp.cu gives a row to one CTA of 256 threads.  The lse is an online (m, z) per thread over the thread's columns
+# (16-byte vectors i, i + 256, ... then the tail; softmax_rows strides single columns by 256), then block_max / block_sum and
+# lse = M + lg2(Z) ln2.  Bounds in the regime |x| < 128 for every finite logit (so |lse| < 128 + ln V; every case tested), with
+# A = max(|lse|, max |finite x|) of the row:
+#   lse:  KL_LSE_ATOL + KL_LSE_RTOL A + (ceil(V/256) + 20) 2^-24
+#           KL_LSE_*: -m log2e rounded once per thread (2^-24 |m| nats, |m| <= A), the fma x log2e - m log2e rounded (2^-24 |x - m| log2e
+#           on a term of weight e^-|x - m|, at most 2^-24 in all), fp32 log2e (2^-26 |x - m|), ex2.approx per term and per rescale of z
+#           (2^-22 each; a thread's running max rises about ln(n) times on rows in random order), lg2.approx and the roundings of
+#           M + lg2(Z) ln2 -- far below 1e-5 + 2e-6 A.
+#           The fp32 sum Z: a thread adds at most 8 ceil(V/2048) + 1 <= ceil(V/256) + 9 positive terms in order, block_sum 10 more levels
+#           (5 shuffles, 5 over the warps' partials): relative (ceil(V/256) + 20) 2^-24, the same in nats.
+#   tok = x[label] - lse:  the lse bound + 2^-24 |tok|.
+#   seq (logp_seq_sum_kernel):  the sum of the active rows' tok bounds + (ceil((T-1)/256) + 10) 2^-24 sum|tok| (a thread adds
+#           ceil((T-1)/256) rows in order, then block_sum); the average form divides by the exact count: that / n + 2^-24 |avg|.
+#   d logits = bf16(-g q + g onehot), q = ex2(fma(x, log2e, -lse_k log2e)) from the forward's fp32 lse_k:
+#           2^-8 |d| + eps |g| (q + onehot) + 2^-126 (1 + |g|), eps = LOGP_GRAD_EPS per element:
+#             the lse bound (lse_k - lse) + 2^-24 |lse| (-lse_k log2e rounded) + 2^-23 |x - lse| (the fma rounded, fp32 log2e)
+#             + 2^-21 (ex2.approx 2^-22, the product -g q and the add of g, and the fp32 g its caller formed, 2^-24 each);
+#           as in KL_GRAD_EPS the cancellation of g onehot - g q on the label column turns the relative error of q into an absolute one.
+#           2^-126 (1 + |g|): ex2.approx.ftz flushes q below 2^-126 to zero.
+#   softmax_rows:  log mode  x - lse_k:  the lse bound + 2^-24 |x - lse|;
+#                  prob mode ex2((x - lse_k) log2e):  p (the lse bound + 3 2^-24 |x - lse| + 2^-22) + 2^-126  (the difference, fp32
+#                  log2e and the product rounded, ex2.approx).
+#   align_loss_dense, from the kernel's own fp32 logp and probs (only the reductions are under test):
+#           row_x = sum p l over the finite l:  (ceil(V/256) + 12) 2^-24 sum|p l|  (a product and an add per term, block_sum);
+#           loss = -sum(row_x m) / sum(m):  (sum of the masked row_x bounds + (ceil(n/1024) + 10) 2^-24 sum|row_x m|) / sum(m)
+#           + 2^-24 |loss|  (1024 threads, block_sum; the count is exact).
+# Values that are not finite in the reference (tok = -inf at a -inf label, the 0/0 average) must match exactly: see check_exact_bound.
+LOGP_ABS_FLOOR = 2.0 ** -126
+
+
+def logp_lse_tol(lse, amax, V):
+    return KL_LSE_ATOL + KL_LSE_RTOL * torch.maximum(lse.abs(), amax) + (math.ceil(V / 256) + 20) * FP32_U
+
+
+def _finite_absmax(x):
+    return torch.where(torch.isfinite(x), x.abs(), torch.zeros_like(x)).amax(-1)
+
+
+def _seq_chain(T):
+    return math.ceil(max(T - 1, 0) / 256) + 10
+
+
+def logp_reference_fp64(logits, labels, T, V, g_seq=None, g_dtype=torch.float64, block_bytes=1 << 30):
+    """Float64 restatement of lmod_logp_gather_fwd / _bwd (R.dpo_get_logp and its gradient) on [N, >= V] bf16 logits (the first V columns)
+    and the flat [N] labels of B = N / T sequences.  Row r = b T + t predicts labels[r + 1]; the last position of a sequence has no next
+    label.  Works on the tensors' device in blocks of rows so that the float64 temporaries stay near `block_bytes`.  Returns a dict:
+      nxt, active [N]     the next label (-100 when none) and whether it is set
+      lse, tok [N]        float64, 0 on masked rows (as the kernel writes them); tok = x[next label] - lse
+      lse_tol, tok_tol    the bounds above
+      seq, seq_tol [B]    the masked sum of tok; avg, avg_tol the average form (0/0 gives NaN, as R.dpo_get_logp); n [B] the counts
+    With g_seq [B] (the upstream gradient of seq):
+      g [N, V]            g_b (onehot(next label) - q) on active rows, 0 on masked rows (g_dtype)
+      gscale [N, V]       |g_b| (q + onehot), the size of the two terms the kernel combines
+      g_tol [N, V]        the element-wise bound of the bf16 d logits
+    One input differs from R.dpo_get_logp on purpose: a -inf at column 0 of a masked row.  R.dpo_get_logp gathers column 0 there (the
+    label is replaced by 0) and multiplies -inf by 0, which is NaN in its sum; the kernel skips masked rows and writes 0, as this does."""
+    x_all = logits[:, :V]
+    dev = x_all.device
+    labels = labels.reshape(-1).to(dev)
+    N = labels.numel()
+    B = N // T
+    _, active, nxt = kl_row_masks(labels, T)
+    lab = torch.where(active, nxt, torch.zeros_like(nxt))
+    f64 = torch.float64
+    lse = torch.zeros(N, dtype=f64, device=dev)
+    tok = torch.zeros_like(lse)
+    amax = torch.zeros_like(lse)
+    grads = g_seq is not None
+    if grads:
+        gb_row = g_seq.to(dev, f64).repeat_interleave(T) * active.to(f64)
+        g = torch.zeros(N, V, dtype=g_dtype, device=dev)
+        gscale = torch.zeros_like(g)
+        g_tol = torch.zeros_like(g)
+    step = max(1, block_bytes // (8 * 8 * V))
+    for r0 in range(0, N, step):
+        r1 = min(N, r0 + step)
+        x = x_all[r0:r1].to(f64)
+        l_b = torch.logsumexp(x, -1)
+        a_b = _finite_absmax(x)
+        t_b = x.gather(1, lab[r0:r1, None])[:, 0] - l_b
+        act = active[r0:r1]
+        lse[r0:r1] = torch.where(act, l_b, torch.zeros_like(l_b))
+        tok[r0:r1] = torch.where(act, t_b, torch.zeros_like(t_b))
+        amax[r0:r1] = torch.where(act, a_b, torch.zeros_like(a_b))
+        if grads:
+            gr = gb_row[r0:r1, None]
+            q = (x - l_b[:, None]).exp()
+            oh = torch.zeros_like(q).scatter_(1, lab[r0:r1, None], 1.0)
+            gg = gr * (oh - q)
+            sc = gr.abs() * (q + oh)
+            dx = torch.where(torch.isfinite(x), (x - l_b[:, None]).abs(), torch.zeros_like(x))
+            eps = logp_lse_tol(l_b, a_b, V)[:, None] + FP32_U * l_b.abs()[:, None] + 2 * FP32_U * dx + 2.0 ** -21
+            gt = BF16_U * gg.abs() + eps * sc + LOGP_ABS_FLOOR * (1 + gr.abs())
+            g[r0:r1] = torch.where(act[:, None], gg, torch.zeros_like(gg)).to(g_dtype)
+            gscale[r0:r1] = torch.where(act[:, None], sc, torch.zeros_like(sc)).to(g_dtype)
+            g_tol[r0:r1] = torch.where(act[:, None], gt, torch.zeros_like(gt)).to(g_dtype)
+            del q, oh, gg, sc, dx, eps, gt
+        del x
+    lse_tol = torch.where(active, logp_lse_tol(lse, amax, V), torch.zeros_like(lse))
+    tok_tol = torch.where(active, lse_tol + FP32_U * tok.abs(), torch.zeros_like(lse))
+    m = active.to(f64).view(B, T)
+    tk = tok.view(B, T)
+    seq = (tk * m).sum(-1)
+    n = m.sum(-1)
+    seq_tol = (tok_tol.view(B, T) * m).sum(-1) + _seq_chain(T) * FP32_U * (tk.abs() * m).sum(-1)
+    avg = seq / n
+    avg_tol = seq_tol / n + FP32_U * avg.abs()
+    out = dict(nxt=nxt, active=active, lse=lse, tok=tok, lse_tol=lse_tol, tok_tol=tok_tol, seq=seq, seq_tol=seq_tol, avg=avg,
+               avg_tol=avg_tol, n=n)
+    if grads:
+        out.update(g=g, gscale=gscale, g_tol=g_tol)
+    return out
+
+
+def softmax_rows_reference_fp64(logits, V, log_mode):
+    """lmod_softmax_rows on [N, >= V] bf16 logits (the first V columns): log_softmax (log_mode) or softmax of each row in float64, with the
+    bound above.  Returns (out [N, V], tol [N, V]) float64 on the logits' device; -inf logits give -inf (log mode) or 0."""
+    x = logits[:, :V].to(torch.float64)
+    lse = torch.logsumexp(x, -1, keepdim=True)
+    lt = logp_lse_tol(lse, _finite_absmax(x)[:, None], V)
+    y = x - lse
+    dx = torch.where(torch.isfinite(y), y.abs(), torch.zeros_like(y))
+    if log_mode:
+        return y, lt + FP32_U * dx
+    p = y.exp()
+    return p, p * (lt + 3 * FP32_U * dx + 2.0 ** -22) + LOGP_ABS_FLOOR
+
+
+def align_dense_reference_fp64(logp, probs, labels, distill_all=False):
+    """lmod_align_loss_dense (R.compute_align_loss) in float64 on the kernel's own fp32 inputs logp, probs [N, V] and the flat [N] labels
+    (not shifted; distill_all counts every row).  row_x = sum p l over the finite l; loss = -sum(row_x m) / sum(m), NaN when no row
+    counts.  Returns dict(row_x, row_x_tol [N], loss, loss_tol) with the bounds above."""
+    l, p = logp.to(torch.float64), probs.to(torch.float64)
+    n, V = l.shape
+    fin = torch.isfinite(l)
+    pl = torch.where(fin, p * torch.where(fin, l, torch.zeros_like(l)), torch.zeros_like(l))
+    row_x = pl.sum(-1)
+    row_tol = (math.ceil(V / 256) + 12) * FP32_U * pl.abs().sum(-1)
+    labels = labels.reshape(-1).to(l.device)
+    m = torch.ones_like(row_x) if distill_all else (labels != IGNORE_INDEX).to(torch.float64)
+    c = m.sum()
+    loss = -(row_x * m).sum() / c
+    loss_tol = ((row_tol * m).sum() + (math.ceil(n / 1024) + 10) * FP32_U * (row_x.abs() * m).sum()) / c + FP32_U * loss.abs()
+    return dict(row_x=row_x, row_x_tol=row_tol, loss=loss, loss_tol=loss_tol)
+
+
+def check_exact_bound(name, got, want, tol, report=None, block=256):
+    """Element-wise |got - want| <= tol for the logp.cu outputs ([N] or [N, V]; compared in blocks of rows).  An element equal to the
+    reference passes (-inf = -inf, and a NaN where the reference has NaN: the 0/0 average); where the reference is not finite nothing else
+    does.  On failure names the first element out of bound and the worst err / bound.  Returns the worst err / bound; `report`, a dict,
+    keeps the largest under `name`."""
+    got = got.detach().reshape(-1) if got.dim() == 0 else got.detach()
+    want, tol = torch.as_tensor(want).to(got.device).reshape(got.shape), torch.as_tensor(tol).to(got.device).reshape(got.shape)
+    nbad, first, worst = 0, None, 0.0
+    for r0 in range(0, max(1, got.shape[0]), block):
+        g, w = got[r0:r0 + block].to(torch.float64), want[r0:r0 + block].to(torch.float64)
+        t = tol[r0:r0 + block].to(torch.float64)
+        same = (g == w) | (torch.isnan(g) & torch.isnan(w))
+        t = torch.where(torch.isfinite(w), t, torch.zeros_like(t))
+        err = torch.where(same, torch.zeros_like(g), (g - w).abs().nan_to_num(float("inf")))
+        ok = same | (err <= t)
+        ratio = torch.where(same, torch.zeros_like(err), (err / t).nan_to_num(float("inf"), float("inf"), float("inf")))
+        if ratio.numel():
+            worst = max(worst, float(ratio.max()))
+        if not bool(ok.all()):
+            nbad += int((~ok).sum())
+            if first is None:
+                i = tuple(int(v) for v in torch.nonzero(~ok)[0])
+                first = ((r0 + i[0],) + i[1:], g[i].item(), w[i].item(), t[i].item())
+    if report is not None:
+        report[name] = max(worst, report.get(name, 0.0))
+    assert nbad == 0, (f"{name}: {nbad} / {got.numel()} elements out of bound, max err/bound {worst:.3g}; first (index, got, want, bound) "
+                       f"= {first}")
+    return worst
+
+
+# ---------------------------------------------------------------------------------------------------
 # flash attention (csrc/attn.cu, csrc/attn_bwd.cu): float64 reference and element-wise bounds
 # ---------------------------------------------------------------------------------------------------
 def attn_visible(B, T, causal, keep=None, device="cpu"):
