@@ -152,6 +152,23 @@ int lmod_moe_scatter_bwd(const void* dxp, const int32_t* row, const float* dlogi
                          const void* dres, int64_t S, int64_t H, int E, void* dx, void* stream);
 int lmod_moe_wg_grad(const void* x, const float* dlogits, int64_t S, int64_t H, int E,
                      float* ws /* [32,E,H] */, float* dwg /* [E,H], accumulated (+=) */, void* stream);
+/* Residual-MoE (DeepSpeed MoE(use_residual=True), SURVEY.md Appendix A "Residual"): the routed output moe [S,H] (gather_combine without
+ * residual) and the dense MLP's output mlp [S,H] mixed per token by a two-way softmax of the coefficient Linear, plus the residual add.
+ * All bf16; one warp per token, 16-byte loads, no host sync.
+ *   z = bf16(x Wc^T + bc) (fp32 accumulate; bc may be NULL), coef = bf16(softmax_fp32(z)) [S,2],
+ *   out = bf16(res + bf16(bf16(moe*c0) + bf16(mlp*c1))).  wc [2,H], bc [2]. */
+int lmod_moe_residual_mix(const void* x, const void* moe, const void* mlp, const void* res, const void* wc, const void* bc,
+                          int64_t S, int64_t H, void* out, void* coef, void* stream);
+/* fp32 elements of the workspace lmod_moe_residual_mix_bwd needs for the coefficient's gradient (no initialisation needed) */
+int64_t lmod_moe_residual_ws_elems(int64_t H);
+/* Backward of the mix for upstream g (the residual's gradient is g itself):
+ *   d_moe = bf16(g*c0), d_mlp = bf16(g*c1) [S,H]; dz [S,2] fp32 = c (dc - <c,dc>) with dc_j = sum_h g*{moe,mlp} (fp32);
+ *   dx_coef = bf16(dz Wc) [S,H], the coefficient's share of dx (callers accumulate the other addends onto it).
+ *   dwc [2,H] / dbc [2] bf16 gradient views, accumulated (+=) by a fixed-partition two-stage reduction (bit-reproducible); either may
+ *   be NULL (frozen), and with both NULL x and ws are not read.  ws: lmod_moe_residual_ws_elems(H) fp32 elements. */
+int lmod_moe_residual_mix_bwd(const void* g, const void* x, const void* moe, const void* mlp, const void* coef, const void* wc,
+                              int64_t S, int64_t H, void* d_moe, void* d_mlp, float* dz, void* dx_coef, float* ws, void* dwc,
+                              void* dbc, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * K4/K6/K9/K2/K1 element-wise + norm kernels (modeling_qwen2.py:105-110,159-184,199-200;

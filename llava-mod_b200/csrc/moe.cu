@@ -588,6 +588,147 @@ __global__ void moe_wg_grad_reduce_kernel(const float* __restrict__ ws, int H, i
   dwg[i] += a;
 }
 
+// ---- Residual-MoE (DeepSpeed MoE(use_residual=True)): the routed output and a dense MLP mixed per token by softmax(coefficient(x)).
+// One warp per token.  Forward, all bf16 tensors as the reference rounds them:
+//   z = bf16(x Wc^T + b) (fp32 accumulate), c = bf16(softmax_fp32(z)), out = bf16(bf16(moe*c0) + bf16(mlp*c1)), stream = bf16(res + out)
+__global__ void __launch_bounds__(256) moe_residual_mix_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ moe,
+                                                              const __nv_bfloat16* __restrict__ mlp, const __nv_bfloat16* __restrict__ res,
+                                                              const __nv_bfloat16* __restrict__ wc, const __nv_bfloat16* __restrict__ bc,
+                                                              int S, int H, __nv_bfloat16* __restrict__ out, __nv_bfloat16* __restrict__ coef) {
+  const int s = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (s >= S) return;
+  const int hv = H >> 3;
+  const size_t o = (size_t)s * H;
+  float z0 = 0.f, z1 = 0.f;
+  for (int v = lane; v < hv; v += 32) {
+    const uint4 u = ldg_nc_v4(reinterpret_cast<const uint4*>(x + o) + v);
+    const uint4 a = ldg_nc_v4(reinterpret_cast<const uint4*>(wc) + v), b = ldg_nc_v4(reinterpret_cast<const uint4*>(wc + H) + v);
+    const float xf[8] = {bf16lo(u.x), bf16hi(u.x), bf16lo(u.y), bf16hi(u.y), bf16lo(u.z), bf16hi(u.z), bf16lo(u.w), bf16hi(u.w)};
+    const float af[8] = {bf16lo(a.x), bf16hi(a.x), bf16lo(a.y), bf16hi(a.y), bf16lo(a.z), bf16hi(a.z), bf16lo(a.w), bf16hi(a.w)};
+    const float bf[8] = {bf16lo(b.x), bf16hi(b.x), bf16lo(b.y), bf16hi(b.y), bf16lo(b.z), bf16hi(b.z), bf16lo(b.w), bf16hi(b.w)};
+#pragma unroll
+    for (int j = 0; j < 8; ++j) { z0 = fmaf(xf[j], af[j], z0); z1 = fmaf(xf[j], bf[j], z1); }
+  }
+  z0 = warp_sum(z0); z1 = warp_sum(z1);
+  if (bc) { z0 += __bfloat162float(bc[0]); z1 += __bfloat162float(bc[1]); }
+  z0 = bf16_round(z0); z1 = bf16_round(z1);
+  const float m = fmaxf(z0, z1), e0 = expf(z0 - m), e1 = expf(z1 - m), den = e0 + e1;
+  const float c0 = bf16_round(e0 / den), c1 = bf16_round(e1 / den);
+  if (lane == 0) *reinterpret_cast<uint32_t*>(coef + 2 * (size_t)s) = pack_bf16x2(c0, c1);
+  for (int v = lane; v < hv; v += 32) {
+    const uint4 a = ldg_nc_v4(reinterpret_cast<const uint4*>(moe + o) + v), b = ldg_nc_v4(reinterpret_cast<const uint4*>(mlp + o) + v);
+    const uint4 r = ldg_nc_v4(reinterpret_cast<const uint4*>(res + o) + v);
+    const float af[8] = {bf16lo(a.x), bf16hi(a.x), bf16lo(a.y), bf16hi(a.y), bf16lo(a.z), bf16hi(a.z), bf16lo(a.w), bf16hi(a.w)};
+    const float bf[8] = {bf16lo(b.x), bf16hi(b.x), bf16lo(b.y), bf16hi(b.y), bf16lo(b.z), bf16hi(b.z), bf16lo(b.w), bf16hi(b.w)};
+    const float rf[8] = {bf16lo(r.x), bf16hi(r.x), bf16lo(r.y), bf16hi(r.y), bf16lo(r.z), bf16hi(r.z), bf16lo(r.w), bf16hi(r.w)};
+    float y[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) y[j] = rf[j] + bf16_round(bf16_round(af[j] * c0) + bf16_round(bf[j] * c1));
+    uint4 w;
+    w.x = pack_bf16x2(y[0], y[1]); w.y = pack_bf16x2(y[2], y[3]); w.z = pack_bf16x2(y[4], y[5]); w.w = pack_bf16x2(y[6], y[7]);
+    stg_v4(reinterpret_cast<uint4*>(out + o) + v, w);
+  }
+}
+
+// Backward of the mix for upstream g (the residual's own gradient is g itself and is not touched here).  One warp per token:
+//   d_moe = bf16(g*c0), d_mlp = bf16(g*c1), dc_j = sum_h g*{moe,mlp}_j (fp32), dz = c (dc - <c, dc>),
+//   dx_coef = bf16(dz0*Wc[0] + dz1*Wc[1]) (the coefficient's input-gradient term).  dz [S,2] fp32 feeds the Wc / b reduction.
+__global__ void __launch_bounds__(256) moe_residual_mix_bwd_kernel(const __nv_bfloat16* __restrict__ g, const __nv_bfloat16* __restrict__ moe,
+                                                                  const __nv_bfloat16* __restrict__ mlp, const __nv_bfloat16* __restrict__ coef,
+                                                                  const __nv_bfloat16* __restrict__ wc, int S, int H,
+                                                                  __nv_bfloat16* __restrict__ d_moe, __nv_bfloat16* __restrict__ d_mlp,
+                                                                  float* __restrict__ dz, __nv_bfloat16* __restrict__ dx) {
+  const int s = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (s >= S) return;
+  const int hv = H >> 3;
+  const size_t o = (size_t)s * H;
+  const uint32_t cw = __ldg(reinterpret_cast<const unsigned int*>(coef) + s);
+  const float c0 = bf16lo(cw), c1 = bf16hi(cw);
+  float d0 = 0.f, d1 = 0.f;
+  for (int v = lane; v < hv; v += 32) {
+    const uint4 q = ldg_nc_v4(reinterpret_cast<const uint4*>(g + o) + v);
+    const uint4 a = ldg_nc_v4(reinterpret_cast<const uint4*>(moe + o) + v), b = ldg_nc_v4(reinterpret_cast<const uint4*>(mlp + o) + v);
+    const float gf[8] = {bf16lo(q.x), bf16hi(q.x), bf16lo(q.y), bf16hi(q.y), bf16lo(q.z), bf16hi(q.z), bf16lo(q.w), bf16hi(q.w)};
+    const float af[8] = {bf16lo(a.x), bf16hi(a.x), bf16lo(a.y), bf16hi(a.y), bf16lo(a.z), bf16hi(a.z), bf16lo(a.w), bf16hi(a.w)};
+    const float bf[8] = {bf16lo(b.x), bf16hi(b.x), bf16lo(b.y), bf16hi(b.y), bf16lo(b.z), bf16hi(b.z), bf16lo(b.w), bf16hi(b.w)};
+#pragma unroll
+    for (int j = 0; j < 8; ++j) { d0 = fmaf(gf[j], af[j], d0); d1 = fmaf(gf[j], bf[j], d1); }
+    uint4 w;
+    w.x = pack_bf16x2(gf[0] * c0, gf[1] * c0); w.y = pack_bf16x2(gf[2] * c0, gf[3] * c0);
+    w.z = pack_bf16x2(gf[4] * c0, gf[5] * c0); w.w = pack_bf16x2(gf[6] * c0, gf[7] * c0);
+    stg_v4(reinterpret_cast<uint4*>(d_moe + o) + v, w);
+    w.x = pack_bf16x2(gf[0] * c1, gf[1] * c1); w.y = pack_bf16x2(gf[2] * c1, gf[3] * c1);
+    w.z = pack_bf16x2(gf[4] * c1, gf[5] * c1); w.w = pack_bf16x2(gf[6] * c1, gf[7] * c1);
+    stg_v4(reinterpret_cast<uint4*>(d_mlp + o) + v, w);
+  }
+  d0 = warp_sum(d0); d1 = warp_sum(d1);
+  const float dot = c0 * d0 + c1 * d1;
+  const float z0 = c0 * (d0 - dot), z1 = c1 * (d1 - dot);
+  if (lane == 0) { dz[2 * (size_t)s] = z0; dz[2 * (size_t)s + 1] = z1; }
+  for (int v = lane; v < hv; v += 32) {
+    const uint4 a = ldg_nc_v4(reinterpret_cast<const uint4*>(wc) + v), b = ldg_nc_v4(reinterpret_cast<const uint4*>(wc + H) + v);
+    const float af[8] = {bf16lo(a.x), bf16hi(a.x), bf16lo(a.y), bf16hi(a.y), bf16lo(a.z), bf16hi(a.z), bf16lo(a.w), bf16hi(a.w)};
+    const float bf[8] = {bf16lo(b.x), bf16hi(b.x), bf16lo(b.y), bf16hi(b.y), bf16lo(b.z), bf16hi(b.z), bf16lo(b.w), bf16hi(b.w)};
+    float y[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) y[j] = fmaf(z1, bf[j], z0 * af[j]);
+    uint4 w;
+    w.x = pack_bf16x2(y[0], y[1]); w.y = pack_bf16x2(y[2], y[3]); w.z = pack_bf16x2(y[4], y[5]); w.w = pack_bf16x2(y[6], y[7]);
+    stg_v4(reinterpret_cast<uint4*>(dx + o) + v, w);
+  }
+}
+
+// dWc / db of the coefficient, deterministic: a fixed partition of the tokens into RM_SPLITS contiguous ranges (a function of S only),
+// per-range partial sums in token order, then one pass adding the ranges in range order into the bf16 gradient.
+constexpr int RM_SPLITS = 128;
+constexpr int RM_COLS = 1024;                         // columns per CTA of the partial kernel: 128 threads x 8
+// ws[(split*2 + j)*H + h] = sum_{s in split} dz[s,j] * x[s,h] ; ws[RM_SPLITS*2*H + split*2 + j] = sum_{s in split} dz[s,j]
+__global__ void __launch_bounds__(128) moe_residual_coef_grad_partial_kernel(const __nv_bfloat16* __restrict__ x, const float* __restrict__ dz,
+                                                                            int S, int H, float* __restrict__ ws) {
+  const int split = blockIdx.y;
+  const int per = (S + RM_SPLITS - 1) / RM_SPLITS;
+  const int s0 = min(S, split * per), s1 = min(S, s0 + per);
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    float b0 = 0.f, b1 = 0.f;
+    for (int s = s0; s < s1; ++s) { b0 += __ldg(dz + 2 * s); b1 += __ldg(dz + 2 * s + 1); }
+    ws[(size_t)RM_SPLITS * 2 * H + 2 * split] = b0;
+    ws[(size_t)RM_SPLITS * 2 * H + 2 * split + 1] = b1;
+  }
+  const int h0 = (blockIdx.x * RM_COLS) + threadIdx.x * 8;
+  if (h0 >= H) return;
+  float a0[8], a1[8];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) { a0[j] = 0.f; a1[j] = 0.f; }
+  for (int s = s0; s < s1; ++s) {
+    const float z0 = __ldg(dz + 2 * s), z1 = __ldg(dz + 2 * s + 1);
+    const uint4 u = ldg_nc_v4(x + (size_t)s * H + h0);
+    const float xf[8] = {bf16lo(u.x), bf16hi(u.x), bf16lo(u.y), bf16hi(u.y), bf16lo(u.z), bf16hi(u.z), bf16lo(u.w), bf16hi(u.w)};
+#pragma unroll
+    for (int j = 0; j < 8; ++j) { a0[j] = fmaf(z0, xf[j], a0[j]); a1[j] = fmaf(z1, xf[j], a1[j]); }
+  }
+  float* w0 = ws + (size_t)(split * 2) * H + h0;
+  float* w1 = w0 + H;
+#pragma unroll
+  for (int j = 0; j < 8; j += 4) {
+    *reinterpret_cast<float4*>(w0 + j) = make_float4(a0[j], a0[j + 1], a0[j + 2], a0[j + 3]);
+    *reinterpret_cast<float4*>(w1 + j) = make_float4(a1[j], a1[j + 1], a1[j + 2], a1[j + 3]);
+  }
+}
+// dwc[i] = bf16(dwc[i] + sum_split ws[split][i]) for i < 2H, dbc[j] likewise (either pointer null: that parameter is frozen)
+__global__ void moe_residual_coef_grad_reduce_kernel(const float* __restrict__ ws, int H, __nv_bfloat16* __restrict__ dwc,
+                                                     __nv_bfloat16* __restrict__ dbc) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= 2 * H + 2) return;
+  const bool bias = i >= 2 * H;
+  __nv_bfloat16* dst = bias ? (dbc ? dbc + (i - 2 * H) : nullptr) : (dwc ? dwc + i : nullptr);
+  if (!dst) return;
+  const size_t stride = bias ? 2 : (size_t)2 * H;
+  const float* src = bias ? ws + (size_t)RM_SPLITS * 2 * H + (i - 2 * H) : ws + i;
+  float a = 0.f;
+  for (int sp = 0; sp < RM_SPLITS; ++sp) a += src[(size_t)sp * stride];
+  *dst = __float2bfloat16_rn(__bfloat162float(*dst) + a);
+}
+
 }  // namespace
 
 extern "C" int lmod_moe_capacity(int64_t S, int E, double capacity_factor, int64_t min_capacity) {
@@ -757,5 +898,48 @@ extern "C" int lmod_moe_wg_grad(const void* x, const float* dlogits, int64_t S, 
   LMOD_LAUNCH_OK();
   moe_wg_grad_reduce_kernel<<<(unsigned)((E * H + 255) / 256), 256, 0, (cudaStream_t)stream>>>(ws, (int)H, E, dwg);
   LMOD_LAUNCH_OK();
+  return LMOD_OK;
+}
+
+static bool aligned16(const void* p) { return ((uintptr_t)p & 15u) == 0; }
+
+extern "C" int lmod_moe_residual_mix(const void* x, const void* moe, const void* mlp, const void* res, const void* wc, const void* bc,
+                                     int64_t S, int64_t H, void* out, void* coef, void* stream) {
+  LMOD_CHECK_ARG(x && moe && mlp && res && wc && out && coef && S > 0 && H > 0 && H % 8 == 0,
+                 "lmod_moe_residual_mix: bad arguments (H must be a multiple of 8)");
+  LMOD_CHECK_ARG(aligned16(x) && aligned16(moe) && aligned16(mlp) && aligned16(res) && aligned16(wc) && aligned16(out) && aligned16(coef),
+                 "lmod_moe_residual_mix: every tensor must be 16-byte aligned");
+  const unsigned blocks = (unsigned)((S * 32 + 255) / 256);
+  moe_residual_mix_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(
+      (const __nv_bfloat16*)x, (const __nv_bfloat16*)moe, (const __nv_bfloat16*)mlp, (const __nv_bfloat16*)res, (const __nv_bfloat16*)wc,
+      (const __nv_bfloat16*)bc, (int)S, (int)H, (__nv_bfloat16*)out, (__nv_bfloat16*)coef);
+  LMOD_LAUNCH_OK();
+  return LMOD_OK;
+}
+
+extern "C" int64_t lmod_moe_residual_ws_elems(int64_t H) { return (int64_t)RM_SPLITS * (2 * H + 2); }
+
+extern "C" int lmod_moe_residual_mix_bwd(const void* g, const void* x, const void* moe, const void* mlp, const void* coef, const void* wc,
+                                         int64_t S, int64_t H, void* d_moe, void* d_mlp, float* dz, void* dx_coef, float* ws, void* dwc,
+                                         void* dbc, void* stream) {
+  LMOD_CHECK_ARG(g && moe && mlp && coef && wc && d_moe && d_mlp && dz && dx_coef && S > 0 && H > 0 && H % 8 == 0,
+                 "lmod_moe_residual_mix_bwd: bad arguments (H must be a multiple of 8)");
+  LMOD_CHECK_ARG(!(dwc || dbc) || (x && ws), "lmod_moe_residual_mix_bwd: x and ws are required for the coefficient's gradient");
+  LMOD_CHECK_ARG(aligned16(g) && aligned16(moe) && aligned16(mlp) && aligned16(wc) && aligned16(d_moe) && aligned16(d_mlp) &&
+                 aligned16(dx_coef) && (!x || aligned16(x)) && (!ws || aligned16(ws)) && ((uintptr_t)coef & 3u) == 0,
+                 "lmod_moe_residual_mix_bwd: every [S,H] tensor must be 16-byte aligned");
+  const unsigned blocks = (unsigned)((S * 32 + 255) / 256);
+  moe_residual_mix_bwd_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(
+      (const __nv_bfloat16*)g, (const __nv_bfloat16*)moe, (const __nv_bfloat16*)mlp, (const __nv_bfloat16*)coef, (const __nv_bfloat16*)wc,
+      (int)S, (int)H, (__nv_bfloat16*)d_moe, (__nv_bfloat16*)d_mlp, dz, (__nv_bfloat16*)dx_coef);
+  LMOD_LAUNCH_OK();
+  if (dwc || dbc) {
+    dim3 grid((unsigned)((H + RM_COLS - 1) / RM_COLS), RM_SPLITS);
+    moe_residual_coef_grad_partial_kernel<<<grid, 128, 0, (cudaStream_t)stream>>>((const __nv_bfloat16*)x, dz, (int)S, (int)H, ws);
+    LMOD_LAUNCH_OK();
+    moe_residual_coef_grad_reduce_kernel<<<(unsigned)((2 * H + 2 + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
+        ws, (int)H, (__nv_bfloat16*)dwc, (__nv_bfloat16*)dbc);
+    LMOD_LAUNCH_OK();
+  }
   return LMOD_OK;
 }

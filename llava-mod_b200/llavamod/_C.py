@@ -42,6 +42,9 @@ SIGNATURES = {
     "lmod_moe_gate_bwd": [_P, _P, _P, _P, _P, _P, _L, _I, _P, _P],
     "lmod_moe_scatter_bwd": [_P, _P, _P, _P, _P, _L, _L, _I, _P, _P],
     "lmod_moe_wg_grad": [_P, _P, _L, _L, _I, _P, _P, _P],
+    "lmod_moe_residual_mix": [_P, _P, _P, _P, _P, _P, _L, _L, _P, _P, _P],
+    "lmod_moe_residual_ws_elems": [_L],
+    "lmod_moe_residual_mix_bwd": [_P, _P, _P, _P, _P, _P, _L, _L, _P, _P, _P, _P, _P, _P, _P, _P],
     "lmod_rmsnorm_fwd": [_P, _P, _P, _L, _L, _F, _P, _P, _P, _P],
     "lmod_rmsnorm_bwd": [_P, _P, _P, _P, _P, _L, _L, _P, _P],
     "lmod_rmsnorm_wgrad": [_P, _P, _P, _L, _L, _P, _P, _P],
@@ -84,7 +87,8 @@ SIGNATURES = {
     "lmod_launch_count_reset": [],
 }
 _RESTYPES = {"lmod_last_error": ctypes.c_char_p, "lmod_launch_count": c_int64, "lmod_launch_count_reset": None,
-             "lmod_moe_route_ws_elems": c_int64, "lmod_moe_route_top1_ws_elems": c_int64, "lmod_attn_decode_ws_elems": c_int64,
+             "lmod_moe_route_ws_elems": c_int64, "lmod_moe_route_top1_ws_elems": c_int64, "lmod_moe_residual_ws_elems": c_int64,
+             "lmod_attn_decode_ws_elems": c_int64,
              "lmod_attn_decode_chunk_ws_elems": c_int64}
 
 

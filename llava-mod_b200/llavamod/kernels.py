@@ -1012,9 +1012,10 @@ def moe_forward_stages(x, res, wg, w_gu, w_dn, noise, cf, min_cap, fused, k=2):
     return r
 
 
-def moe_backward_stages(st, x, wg, w_gu, w_dn, dout, dlaux, grads):
+def moe_backward_stages(st, x, wg, w_gu, w_dn, dout, dlaux, grads, dres=None):
     """The MoE backward as MoEFn runs it, from moe_forward_stages' record; returns every intermediate (dy, dw, dact on the unfused
-    path, dh1, dxp, dlogits, dx).  Weight gradients accumulate in place into grads['wg'|'w_gu'|'w_dn'] (None or a missing key = frozen)."""
+    path, dh1, dxp, dlogits, dx).  Weight gradients accumulate in place into grads['wg'|'w_gu'|'w_dn'] (None or a missing key = frozen).
+    dres: another addend of dx [S,H], summed in the scatter-backward kernel."""
     E, I2, H = w_gu.shape
     xp, h1, act, y, row, w, gates, idx, meta, offs = (st[k] for k in ("xp", "h1", "act", "y", "row", "w", "gates", "idx", "meta", "offsets"))
     R = xp.shape[0]
@@ -1044,7 +1045,7 @@ def moe_backward_stages(st, x, wg, w_gu, w_dn, dout, dlaux, grads):
     call("lmod_moe_gate_bwd_top1" if st.get("k", 2) == 1 else "lmod_moe_gate_bwd", ptr(gates), ptr(idx), ptr(row), ptr(dw), ptr(meta),
          ptr(gl) if gl is not None else None, S, E, ptr(dlogits))
     dx = torch.empty_like(x)
-    call("lmod_moe_scatter_bwd", ptr(dxp), ptr(row), ptr(dlogits), ptr(wg), None, S, H, E, ptr(dx))
+    call("lmod_moe_scatter_bwd", ptr(dxp), ptr(row), ptr(dlogits), ptr(wg), ptr(dres), S, H, E, ptr(dx))
     if g is not None and g.get("wg") is not None:
         ws = torch.empty(32, E, H, dtype=torch.float32, device=dout.device)
         call("lmod_moe_wg_grad", ptr(x), ptr(dlogits), S, H, E, ptr(ws), ptr(g["wg"]))
@@ -1092,7 +1093,109 @@ def moe_forward_nograd(x, res, wg, w_gu, w_dn, noise, cf, min_cap, k=2):
         act = silu_mul(h1)
     y = torch.empty(R, H, dtype=x.dtype, device=x.device)
     grouped_gemm(act, w_dn, y, r["offsets"], 0)
-    return moe_gather_combine(y, r["row"], r["w"], _c(res)), r["meta"][0].clone(), r
+    return moe_gather_combine(y, r["row"], r["w"], _c(res) if res is not None else None), r["meta"][0].clone(), r
+
+
+# ---- Residual-MoE (DeepSpeed MoE(use_residual=True), SURVEY.md Appendix A "Residual"): the routed output and the dense MLP on every token,
+# mixed per token by softmax(coefficient(x)) [S,2] (csrc/moe.cu lmod_moe_residual_mix / _bwd); the routed part runs with no residual.
+def moe_residual_mix(x, moe, mlp_out, res, wc, bc):
+    """-> (bf16(res + bf16(bf16(moe*c0) + bf16(mlp*c1))) [S,H], coef [S,2] bf16), c = bf16(softmax(bf16(x Wc^T + bc)))."""
+    _need_cuda(x, moe, mlp_out, res, wc)
+    S, H = x.shape
+    out = torch.empty(S, H, dtype=x.dtype, device=x.device)
+    coef = torch.empty(S, 2, dtype=x.dtype, device=x.device)
+    call("lmod_moe_residual_mix", ptr(x), ptr(moe), ptr(mlp_out), ptr(_c(res)), ptr(wc), ptr(bc), S, H, ptr(out), ptr(coef))
+    return out, coef
+
+
+def moe_residual_mix_bwd(g, x, moe, mlp_out, coef, wc, dwc=None, dbc=None):
+    """Backward of moe_residual_mix for upstream g: returns dict(d_moe, d_mlp [S,H] bf16, dz [S,2] fp32, dx [S,H] bf16 = the
+    coefficient's term of dx, which callers accumulate the other addends onto).  dwc / dbc: gradient views accumulated in place
+    (deterministic two-stage reduction); None = frozen."""
+    S, H = g.shape
+    dev = g.device
+    d = dict(d_moe=torch.empty(S, H, dtype=g.dtype, device=dev), d_mlp=torch.empty(S, H, dtype=g.dtype, device=dev),
+             dz=torch.empty(S, 2, dtype=torch.float32, device=dev), dx=torch.empty(S, H, dtype=g.dtype, device=dev))
+    ws = None
+    if dwc is not None or dbc is not None:
+        ws = torch.empty(int(_C.lib().lmod_moe_residual_ws_elems(H)), dtype=torch.float32, device=dev)
+    call("lmod_moe_residual_mix_bwd", ptr(g), ptr(x), ptr(moe), ptr(mlp_out), ptr(coef), ptr(wc), S, H, ptr(d["d_moe"]), ptr(d["d_mlp"]),
+         ptr(d["dz"]), ptr(d["dx"]), ptr(ws), ptr(dwc), ptr(dbc))
+    return d
+
+
+def moe_residual_forward_stages(x, res, wg, w_gu, w_dn, noise, cf, min_cap, r_gu, r_dn, wc, bc, fused, k=2):
+    """The Residual-MoE forward as ResidualMoEFn runs it: moe_forward_stages with no residual (its 'out' is kept as 'moe'), the dense
+    SwiGLU MLP (r_gu [2I,H], r_dn [H,I]; pre-activations kept) and the mix.  Returns every intermediate; 'out' is the new stream."""
+    st = moe_forward_stages(x, None, wg, w_gu, w_dn, noise, cf, min_cap, fused, k)
+    if fused:
+        m_act, m_h1 = gemm_swiglu(x, r_gu, True)
+    else:
+        m_h1 = gemm(x, r_gu)
+        m_act = silu_mul(m_h1)
+    m_y = gemm(m_act, r_dn)
+    out, coef = moe_residual_mix(x, st["out"], m_y, res, wc, bc)
+    st.update(moe=st["out"], mlp_h1=m_h1, mlp_act=m_act, mlp=m_y, coef=coef, out=out)
+    return st
+
+
+def moe_residual_backward_stages(st, x, wg, w_gu, w_dn, r_gu, r_dn, wc, dout, dlaux, grads):
+    """Backward of moe_residual_forward_stages.  The mix backward splits dout into the routed and dense branches and writes the
+    coefficient's dx term; the dense dgrad GEMM accumulates onto that term, and the routed scatter-backward adds the sum (its dres), so dx
+    takes no extra pass.  grads: the keys of moe_backward_stages plus 'r_gu', 'r_dn', 'wc', 'bc' (None or missing = frozen)."""
+    g = grads or {}
+    mix = moe_residual_mix_bwd(dout, x, st["moe"], st["mlp"], st["coef"], wc, g.get("wc"), g.get("bc"))
+    d_mlp = mix["d_mlp"]
+    if st["fused"]:
+        m_dh1 = gemm_silu_bwd(d_mlp, r_dn, st["mlp_h1"])
+    else:
+        m_dh1 = silu_mul_bwd(mm_nn(d_mlp, r_dn), st["mlp_h1"])
+    if g.get("r_dn") is not None:
+        mm_tn_acc(d_mlp, st["mlp_act"], g["r_dn"])
+    dres = mix["dx"]
+    gemm(m_dh1, r_gu, b_mn=True, out=dres, accumulate=True)            # dx_coef + dh1 @ W_gu
+    if g.get("r_gu") is not None:
+        mm_tn_acc(m_dh1, x, g["r_gu"])
+    out = moe_backward_stages(st, x, wg, w_gu, w_dn, mix["d_moe"], dlaux, g, dres=dres)
+    out.update(mix=mix, mlp_dh1=m_dh1, dres=dres)
+    return out
+
+
+class ResidualMoEFn(Function):
+    """MoEFn with DeepSpeed's use_residual=True: (res + bf16(moe*c0) + bf16(mlp*c1), l_aux), the dense MLP r_gu / r_dn (the module the
+    experts were up-cycled from) run on every token, c = softmax(coefficient(x)).  grads: MoEFn's keys plus 'r_gu', 'r_dn', 'wc', 'bc'."""
+
+    @staticmethod
+    def forward(ctx, x, res, wg, w_gu, w_dn, noise, cf, min_cap, r_gu, r_dn, wc, bc, grads, k=2):
+        x = _c(x)
+        res = _c(res)
+        E, I2, H = w_gu.shape
+        st = moe_residual_forward_stages(x, res, wg, w_gu, w_dn, noise, cf, min_cap, r_gu, r_dn, wc, bc,
+                                         swiglu_fusable(I2 // 2, H, training=True), k)
+        ctx.save_for_backward(x, wg, w_gu, w_dn, r_gu, r_dn, wc, *(st[n] for n in _MOE_SAVED + _RES_SAVED))
+        ctx.fused = st["fused"]
+        ctx.k = k
+        ctx.grads = grads
+        return st["out"], st["meta"][0].clone()
+
+    @staticmethod
+    def backward(ctx, dout, dlaux):
+        x, wg, w_gu, w_dn, r_gu, r_dn, wc, *saved = ctx.saved_tensors
+        st = dict(zip(_MOE_SAVED + _RES_SAVED, saved), fused=ctx.fused, k=ctx.k)
+        dx = moe_residual_backward_stages(st, x, wg, w_gu, w_dn, r_gu, r_dn, wc, _c(dout), dlaux, ctx.grads)["dx"]
+        return (dx, dout) + (None,) * 12
+
+
+_RES_SAVED = ("moe", "mlp_h1", "mlp_act", "mlp", "coef")
+
+
+def moe_residual_forward_nograd(x, res, wg, w_gu, w_dn, noise, cf, min_cap, r_gu, r_dn, wc, bc, k=2):
+    """moe_forward_nograd with use_residual=True -> (new stream, l_aux, routing record with 'coef')."""
+    x = _c(x)
+    moe, l_aux, r = moe_forward_nograd(x, None, wg, w_gu, w_dn, noise, cf, min_cap, k)
+    out, coef = moe_residual_mix(x, moe, mlp(x, r_gu, r_dn), res, wc, bc)
+    r["coef"] = coef
+    return out, l_aux, r
 
 
 # ---------------------------------------------------------------------------------------------------

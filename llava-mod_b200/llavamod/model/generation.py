@@ -91,7 +91,7 @@ def _decoder_entry(model, B, max_len, T=1):
         return dict(cache=model.new_kv_cache(B, max_len), graph=None)
     for k in [k for k, v in _STEP_GRAPHS.items() if v["model"]() is None]:       # the model is gone: free its cache and graph
         del _STEP_GRAPHS[k]
-    moe = tuple((l.mlp.num_experts, l.mlp.capacity_factor, l.mlp.eval_capacity_factor, l.mlp.min_capacity)
+    moe = tuple((l.mlp.num_experts, l.mlp.k, l.mlp.use_residual, l.mlp.capacity_factor, l.mlp.eval_capacity_factor, l.mlp.min_capacity)
                 for l in model.model.layers if hasattr(l.mlp, "deepspeed_moe"))
     fp8 = tuple(t.data_ptr() for l in model.model.layers if isinstance(l.self_attn.qkv_weight, K.Fp8Rows)
                 for w in (l.self_attn.qkv_weight, l.self_attn.o_fp8, l.mlp.gu_weight, l.mlp.down_fp8) for t in (w.q, w.scale))

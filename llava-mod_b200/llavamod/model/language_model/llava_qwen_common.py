@@ -316,6 +316,8 @@ class LLaVAMoDForCausalLMBase(LlavaQwenForCausalLMBase):
                       eval_capacity_factor=ecf, min_capacity=min_cap, use_residual=use_residual)
             for e in moe.deepspeed_moe.experts.deepspeed_experts:             # same sanity check as the reference (:547-550)
                 assert torch.equal(e.gate_proj.weight, dense.gate_proj.weight) and torch.equal(e.down_proj.weight, dense.down_proj.weight)
+            if use_residual:                                                  # MoE(use_residual=True) keeps the dense module itself
+                assert moe.mlp is dense
             self.model.layers[li].mlp = moe
 
 

@@ -188,7 +188,9 @@ class MOELayer(nn.Module):
 class MoE(nn.Module):
     """Parameter layout of deepspeed.moe.layer.MoE (call site llava_qwen1_5_moe.py:536-546): ``deepspeed_moe.gate.wg``
     and ``deepspeed_moe.experts.deepspeed_experts.{e}``.  k = 2 (top2gating, the distillation shells' default) or k = 1 (top1gating
-    with random token selection), the two widths DeepSpeed's TopKGate accepts."""
+    with random token selection), the two widths DeepSpeed's TopKGate accepts.
+    use_residual=True (Residual-MoE): ``mlp`` is the dense module passed in (the very object, not a copy) and ``coefficient`` a bf16
+    Linear(H, 2) with a bias; the layer returns bf16(moe*c0) + bf16(mlp*c1), c = softmax(coefficient(x)) (SURVEY.md Appendix A)."""
 
     def __init__(self, cfg, expert: Qwen2MLP, num_experts=4, ep_size=1, k=2, capacity_factor=1.0,
                  eval_capacity_factor=1.0, min_capacity=4, use_residual=False):
@@ -197,12 +199,50 @@ class MoE(nn.Module):
             raise ValueError("Only top-1 and top-2 gatings are supported (got k = %r)" % (k,))
         if ep_size != 1:
             raise NotImplementedError("expert parallelism is size 1 in the reference's recipes (SURVEY.md 2.3)")
-        if use_residual:
-            raise NotImplementedError("use_residual=True (Residual-MoE) is not on the hot path")
         dev, dt = expert.down_proj.weight.device, expert.down_proj.weight.dtype
         self.num_experts, self.k = num_experts, k
         self.capacity_factor, self.eval_capacity_factor, self.min_capacity = capacity_factor, eval_capacity_factor, min_capacity
+        self.use_residual = bool(use_residual)
         self.deepspeed_moe = MOELayer(cfg, num_experts, dev, dt, expert)
+        if self.use_residual:
+            # module order = DeepSpeed's (deepspeed_moe, mlp, coefficient), hence the state-dict order; nn.Linear's default init drawn
+            # in fp32 and cast, as the bf16 engine cast leaves the coefficient bf16
+            H = cfg.hidden_size
+            self.mlp = expert
+            w = torch.empty(2, H, device=dev, dtype=torch.float32)
+            nn.init.kaiming_uniform_(w, a=math.sqrt(5))
+            b = torch.empty(2, device=dev, dtype=torch.float32).uniform_(-1.0 / math.sqrt(H), 1.0 / math.sqrt(H))
+            self.coefficient = ParamLinear(w.to(dt), b.to(dt))
+
+    def trainable(self):
+        """Whether any parameter of the layer trains (the routed path's test, plus the dense MLP and coefficient of a residual layer)."""
+        ds = self.deepspeed_moe
+        if ds.gate.wg.weight.requires_grad or ds.experts.deepspeed_experts[0].down_proj.weight.requires_grad:
+            return True
+        if not self.use_residual:
+            return False
+        return any(p.requires_grad for p in (self.mlp.gate_proj.weight, self.mlp.up_proj.weight, self.mlp.down_proj.weight,
+                                             self.coefficient.weight, self.coefficient.bias))
+
+    def run(self, x, stream, noise, cf, gview):
+        """The layer on post-norm x [S,H] with the residual stream: -> (new stream, l_aux, routing record or None).  Autograd path when
+        anything is differentiated (gradients go to the arena views gview returns), the no-grad path otherwise."""
+        ds = self.deepspeed_moe
+        wg, gu, dn = ds.gate.wg.weight, ds.experts.gu_weight, ds.experts.dn_weight
+        grad = torch.is_grad_enabled() and (x.requires_grad or self.trainable())
+        if not self.use_residual:
+            if grad:
+                grads = dict(wg=gview(wg), w_gu=gview(gu), w_dn=gview(dn))
+                return K.MoEFn.apply(x, stream, wg, gu, dn, noise, cf, self.min_capacity, grads, self.k) + (None,)
+            return K.moe_forward_nograd(x, stream, wg, gu, dn, noise, cf, self.min_capacity, self.k)
+        rm, cw = self.mlp, self.coefficient
+        if grad:
+            grads = dict(wg=gview(wg), w_gu=gview(gu), w_dn=gview(dn), r_gu=gview(rm.gu_weight), r_dn=gview(rm.down_proj.weight),
+                         wc=gview(cw.weight), bc=gview(cw.bias))
+            return K.ResidualMoEFn.apply(x, stream, wg, gu, dn, noise, cf, self.min_capacity, rm.gu_weight, rm.down_proj.weight,
+                                         cw.weight, cw.bias, grads, self.k) + (None,)
+        return K.moe_residual_forward_nograd(x, stream, wg, gu, dn, noise, cf, self.min_capacity, rm.gu_weight, rm.down_proj.weight,
+                                             cw.weight, cw.bias, self.k)
 
 
 class Qwen2DecoderLayer(nn.Module):
@@ -352,19 +392,12 @@ class Qwen2Model(nn.Module):
                                       wgrad=self.gview(layer.post_attention_layernorm.weight))
             mlp = layer.mlp
             if isinstance(mlp, MoE):
-                ds = mlp.deepspeed_moe
                 E = mlp.num_experts
                 noise = moe_noise[moe_i] if moe_noise is not None else moe_draw((B * T, E), mlp.k, dev)
                 moe_i += 1
                 cf = mlp.capacity_factor if training_moe else mlp.eval_capacity_factor
-                wg = ds.gate.wg.weight
-                if torch.is_grad_enabled() and (x.requires_grad or wg.requires_grad or ds.experts.deepspeed_experts[0].down_proj.weight.requires_grad):
-                    grads = dict(wg=self.gview(wg), w_gu=self.gview(ds.experts.gu_weight), w_dn=self.gview(ds.experts.dn_weight))
-                    stream, l_aux = K.MoEFn.apply(x, stream, wg, ds.experts.gu_weight, ds.experts.dn_weight, noise, cf,
-                                                  mlp.min_capacity, grads, mlp.k)
-                else:
-                    stream, l_aux, rec = K.moe_forward_nograd(x, stream, wg, ds.experts.gu_weight, ds.experts.dn_weight, noise,
-                                                              cf, mlp.min_capacity, mlp.k)
+                stream, l_aux, rec = mlp.run(x, stream, noise, cf, self.gview)
+                if rec is not None:
                     records.append(rec)
                 l_auxes.append(l_aux)
                 branch = None
@@ -447,12 +480,11 @@ class Qwen2Model(nn.Module):
                 x, stream = K.rmsnorm(branch, layer.post_attention_layernorm.weight, cfg.rms_norm_eps, res=stream)
             mlp = layer.mlp
             if isinstance(mlp, MoE):
-                ds = mlp.deepspeed_moe
                 noise = moe_noise[moe_i] if moe_noise is not None else moe_draw((B, mlp.num_experts), mlp.k, dev)
                 moe_i += 1
                 cf = mlp.capacity_factor if training_moe else mlp.eval_capacity_factor
-                stream, l_aux, rec = K.moe_forward_nograd(x, stream, ds.gate.wg.weight, ds.experts.gu_weight, ds.experts.dn_weight, noise,
-                                                          cf, mlp.min_capacity, mlp.k)
+                with torch.no_grad():
+                    stream, l_aux, rec = mlp.run(x, stream, noise, cf, self.gview)
                 records.append(rec)
                 l_auxes.append(l_aux)
                 branch = None

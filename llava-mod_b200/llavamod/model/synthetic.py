@@ -35,10 +35,11 @@ def vision_args(clip):
                                  image_projector_type="mlp2x_gelu")
 
 
-def moe_args(num_experts=4, capacity_factor=1.5, moe_mode="sparse", train_modules=TRAIN_MODULES, aux=0.01, min_capacity=0, top_k=2):
+def moe_args(num_experts=4, capacity_factor=1.5, moe_mode="sparse", train_modules=TRAIN_MODULES, aux=0.01, min_capacity=0, top_k=2,
+             use_residual=False):
     return types.SimpleNamespace(moe_enable=True, train_modules=list(train_modules) if train_modules else None, moe_mode=moe_mode,
                                  moe_layers_idx=None, ep_size=1, top_k_experts=top_k, capacity_factor=capacity_factor,
-                                 eval_capacity_factor=2.0, min_capacity=min_capacity, use_residual=False,
+                                 eval_capacity_factor=2.0, min_capacity=min_capacity, use_residual=use_residual,
                                  router_aux_loss_coef=aux, num_experts=[num_experts])
 
 
