@@ -280,15 +280,21 @@ int lmod_grouped_gemm_bf16(const void* A, int64_t lda, const void* B, int64_t ld
 
 /* ------------------------------------------------------------------------------------------
  * FP8 (e4m3) frozen teacher: the decoder linears of a model that is never differentiated, on e4m3 wgmma (csrc/gemm_fp8.cu, csrc/quant.cu).
- * Quantiser (fp32; stated in full at the top of csrc/quant.cu): scale = amax > 0 ? amax / 448 : 1 per row, q = e4m3_rn(clamp(x / scale,
- * +-448)).  Weights [N,K] are quantised per output channel with the same function, once; activations per token by the kernel that
- * produces the GEMM input.  GEMM: D[m,n] = (acc[m,n] * s_a[m]) * s_w[n] in fp32 (acc = the wgmma fp32 sum of the e4m3 products), then bias
+ * Quantiser (fp32, per row; stated in full at the top of csrc/quant.cu):
+ *     amax  = max_k |x[k]|, NaN-propagating (any NaN -> NaN; +-inf -> inf)
+ *     scale = amax == 0 ? 1 : amax / 448          (NaN -> NaN, inf -> inf)
+ *     q[k]  = e4m3_rn(clamp(x[k] / scale, +-448)), the clamp passing NaN through
+ * A row holding a NaN gets scale NaN and NaN bytes; a row holding an inf gets scale inf, NaN bytes at its infinite elements and +-0
+ * elsewhere; either way that row of every e4m3 GEMM output is NaN and no other row changes.  e4m3 subnormal operands (2^-9 .. 0.875 *
+ * 2^-6) are exact on the tensor core, not flushed.  Weights [N,K] are quantised per output channel with the same function, once;
+ * activations per token by the kernel that produces the GEMM input.  GEMM: D[m,n] = (acc[m,n] * s_a[m]) * s_w[n] in fp32 (acc = the wgmma fp32 sum of the e4m3 products), then bias
  * / RoPE / SwiGLU with the expressions and bf16 roundings of the bf16 forms above.  Forward only, K-major operands only.
  * lmod_quant_rows_e4m3: x [M,K] bf16 (row stride ld) -> q [M,K] bytes + scale [M]; in front of o_proj (modeling_qwen2.py:726) and down_proj
  *   (:200), and for the weights.  K %% 16 == 0.
  * lmod_rmsnorm_quant_e4m3: lmod_rmsnorm_fwd (Qwen2RMSNorm :105-110 with the residual add of :796,808) writing q / scale instead of the bf16
  *   row -- bit-equal to lmod_quant_rows_e4m3 of lmod_rmsnorm_fwd's y; x_out as there.  In front of q|k|v (:678-680) and gate|up (:199).
- * lmod_gemm_e4m3: nn.Linear forward (o_proj :726, down_proj :200).  lda / ldb: row strides of the e4m3 operands in bytes (multiples of 16).
+ * lmod_gemm_e4m3: nn.Linear forward (o_proj :726, down_proj :200).  lda / ldb: row strides of the e4m3 operands in bytes (multiples of 16);
+ *   bias (and cos / sin of the q|k|v form) 4-byte aligned.
  * lmod_gemm_e4m3_qkv_rope: lmod_gemm_qkv_rope (:678-691,159-184) on e4m3 operands; bit-identical to lmod_gemm_e4m3 + lmod_rope.
  * lmod_gemm_e4m3_swiglu: lmod_gemm_swiglu (:199-200) on e4m3 operands, W8_gu [2I,K] / s_w [2I] the fused gate|up weight; no pre-activations
  *   are kept; bit-identical to lmod_gemm_e4m3 + lmod_silu_mul_fwd.  I %% 128 == 0. */

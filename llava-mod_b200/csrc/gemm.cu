@@ -392,6 +392,8 @@ static int gemm_dense(const void* A, int64_t lda, int a_mn_major, const void* B,
   LMOD_CHECK_ARG(A && B && (D || d_f32_accum) && M > 0 && N > 0 && K > 0, "lmod_gemm_bf16: null pointer or empty problem");
   LMOD_CHECK_ARG(lda % 8 == 0 && ldb % 8 == 0 && ldd % 8 == 0 && N % 8 == 0 && ((uintptr_t)A % 16 == 0) && ((uintptr_t)B % 16 == 0) &&
                  (!D || (uintptr_t)D % 16 == 0), "lmod_gemm_bf16: strides / N must be multiples of 8 elements and pointers 16-byte aligned (TMA)");
+  LMOD_CHECK_ARG((uintptr_t)bias % 4 == 0 && (!rope || ((uintptr_t)rope->cos % 4 == 0 && (uintptr_t)rope->sin % 4 == 0)),
+                 "lmod_gemm_bf16: bias, cos and sin must be 4-byte aligned (the epilogue reads them two bf16 at a time)");
   CUtensorMap ta, tb;
   int rc;
   const int splits_req = (epilogue >> 8) > 1 ? (epilogue >> 8) : 1;

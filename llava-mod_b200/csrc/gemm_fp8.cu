@@ -269,6 +269,8 @@ int gemm8(const char* who, const void* A, int64_t lda, const float* sa, const vo
   LMOD_CHECK_ARG(K % 16 == 0 && lda % 16 == 0 && ldb % 16 == 0 && ldd % 8 == 0 && N % 8 == 0 && (uintptr_t)A % 16 == 0 && (uintptr_t)W % 16 == 0 &&
                  (uintptr_t)D % 16 == 0 && (uintptr_t)sw % 8 == 0,
                  "%s: K and the e4m3 row strides must be multiples of 16, N and ldd of 8, pointers 16-byte aligned (TMA, 16-byte stores)", who);
+  LMOD_CHECK_ARG((uintptr_t)bias % 4 == 0 && (!rope || ((uintptr_t)rope->cos % 4 == 0 && (uintptr_t)rope->sin % 4 == 0)),
+                 "%s: bias, cos and sin must be 4-byte aligned (the epilogue reads them two bf16 at a time)", who);
   Fp8Params p = {};
   p.D = (__nv_bfloat16*)D; p.ldd = ldd; p.bias = (const __nv_bfloat16*)bias; p.sa = sa; p.sw = sw;
   p.M = (int)M; p.N = (int)N; p.K = (int)K; p.swiglu_I = (int)swiglu_I;

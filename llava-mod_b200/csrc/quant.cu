@@ -1,12 +1,16 @@
 // quant.cu -- row-wise e4m3 quantisation of bf16 rows for the FP8 (e4m3) frozen teacher (gemm_fp8.cu consumes the bytes and the scales).
 //
 // The quantiser, in fp32, for one row x[0..K) (bf16 values are exact in fp32):
-//     amax  = max_k |x[k]|
-//     scale = amax > 0 ? amax / 448.0f : 1.0f                       one IEEE division, round to nearest
-//     q[k]  = e4m3_rn( min(max(x[k] / scale, -448.0f), 448.0f) )     an IEEE division per element (not a reciprocal multiply), the clamp
-//                                                                   after the division and before the conversion, conversion to e4m3 (the
-//                                                                   finite-only "fn" format, largest value 448) round-to-nearest-even
-// Subnormal scales are kept (no flush to zero); an all-zero row gets scale 1 and zero bytes.  x ~= scale * q.
+//     amax  = max_k |x[k]|, NaN-propagating (any NaN -> NaN; +-inf -> inf)
+//     scale = amax == 0 ? 1 : amax / 448          (NaN -> NaN, inf -> inf)
+//     q[k]  = e4m3_rn(clamp(x[k] / scale, +-448)), the clamp passing NaN through
+// with IEEE divisions, round to nearest (one for the scale, one per element: not a reciprocal multiply), the clamp after the division and
+// before the conversion to e4m3 (the "fn" format: largest finite value 448, NaN 0x7F / 0xFF) round-to-nearest-even.  Subnormal scales are
+// kept (no flush to zero); an all-zero row gets scale 1 and zero bytes.  x ~= scale * q.
+// Non-finite rows: a row holding a NaN gets scale NaN and NaN bytes; a row holding an inf gets scale inf, NaN bytes at its infinite
+// elements and +-0 elsewhere.  Either way every column of that row of an e4m3 GEMM is NaN, as in the bf16 teacher, and no other row
+// changes.  (fmaxf / fminf return the non-NaN operand, which would turn such a row into finite -448's: hence max_nan / clamp448 below,
+// kept local to this file.)
 // tests/fp8_oracle.py restates exactly this; lmod_quant_rows_e4m3 and lmod_rmsnorm_quant_e4m3 are bit-equal to it.
 //
 // One CTA of 128 threads per row.  The row is read from global memory once (16-byte loads), parked in shared memory while the block
@@ -28,24 +32,48 @@ __device__ __forceinline__ uint4 pack8(const float* f) {
   o.x = pack_bf16x2(f[0], f[1]); o.y = pack_bf16x2(f[2], f[3]); o.z = pack_bf16x2(f[4], f[5]); o.w = pack_bf16x2(f[6], f[7]);
   return o;
 }
+// max and clamp that return NaN when an operand is NaN (PTX max.NaN / min.NaN, sm_80+)
+__device__ __forceinline__ float max_nan(float a, float b) {
+  float r;
+  asm("max.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+  return r;
+}
+__device__ __forceinline__ float clamp448(float v) {
+  float r;
+  asm("max.NaN.f32 %0, %1, 0fC3E00000;\n\tmin.NaN.f32 %0, %0, 0f43E00000;" : "=f"(r) : "f"(v));     // -448, 448
+  return r;
+}
 __device__ __forceinline__ float amax8(const uint4& u, float m) {
   float f[8];
   unpack8(u, f);
 #pragma unroll
-  for (int j = 0; j < 8; ++j) m = fmaxf(m, fabsf(f[j]));
+  for (int j = 0; j < 8; ++j) m = max_nan(m, fabsf(f[j]));
   return m;
+}
+// block_max of common.cuh with max_nan: a NaN in any thread's amax reaches every thread
+__device__ __forceinline__ float block_max_nan(float v, float* red) {
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = max_nan(v, __shfl_xor_sync(0xffffffffu, v, o));
+  __syncthreads();
+  if (lane == 0) red[w] = v;
+  __syncthreads();
+  float r = lane < QUANT_THREADS / 32 ? red[lane] : 0.f;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) r = max_nan(r, __shfl_xor_sync(0xffffffffu, r, o));
+  return r;
 }
 __device__ __forceinline__ uint32_t e4m3x4(const float* f, float scale) {
   float v[4];
 #pragma unroll
-  for (int j = 0; j < 4; ++j) v[j] = fminf(fmaxf(__fdiv_rn(f[j], scale), -448.f), 448.f);
+  for (int j = 0; j < 4; ++j) v[j] = clamp448(__fdiv_rn(f[j], scale));
   const uint32_t lo = __nv_cvt_float2_to_fp8x2(make_float2(v[0], v[1]), __NV_SATFINITE, __NV_E4M3);
   const uint32_t hi = __nv_cvt_float2_to_fp8x2(make_float2(v[2], v[3]), __NV_SATFINITE, __NV_E4M3);
   return lo | (hi << 16);
 }
 // second pass: the bf16 row in shared memory (K % 16 == 0) -> e4m3 bytes, 16 per thread and store
 __device__ __forceinline__ void convert_row(const uint4* srow, int K, float amax, uint8_t* q, float* scale_out) {
-  const float scale = amax > 0.f ? __fdiv_rn(amax, 448.f) : 1.f;
+  const float scale = amax == 0.f ? 1.f : __fdiv_rn(amax, 448.f);
   if (threadIdx.x == 0) *scale_out = scale;
   uint4* qr = reinterpret_cast<uint4*>(q);
   for (int c = threadIdx.x; c < (K >> 4); c += QUANT_THREADS) {
@@ -68,7 +96,7 @@ __global__ void __launch_bounds__(QUANT_THREADS) quant_rows_e4m3_kernel(const __
     srow[v] = u;
     m = amax8(u, m);
   }
-  m = block_max(m, red);                     // its barriers also publish srow
+  m = block_max_nan(m, red);                 // its barriers also publish srow
   convert_row(srow, K, m, q + row * K, scale + row);
 }
 
@@ -117,7 +145,7 @@ __global__ void __launch_bounds__(QUANT_THREADS) rmsnorm_quant_e4m3_kernel(const
     srow[v] = y;
     m = amax8(y, m);
   }
-  m = block_max(m, red);
+  m = block_max_nan(m, red);
   convert_row(srow, H, m, q + row * H, scale + row);
 }
 

@@ -2,10 +2,13 @@
 fake-quantised dense decoder on top of oracle/restated.py.
 
 The quantiser, in fp32, for one row x (the expression csrc/quant.cu states in its header):
-    amax  = max |x|
-    scale = amax / 448 if amax > 0 else 1                      (one fp32 division)
-    q     = e4m3( clamp(x / scale, -448, 448) )                (an fp32 division per element, the clamp after it, round to nearest even)
-e4m3 is torch.float8_e4m3fn (finite only, largest value 448, smallest subnormal 2^-9)."""
+    amax  = max_k |x[k]|, NaN-propagating (any NaN -> NaN; +-inf -> inf)
+    scale = amax == 0 ? 1 : amax / 448          (NaN -> NaN, inf -> inf)
+    q[k]  = e4m3_rn(clamp(x[k] / scale, +-448)), the clamp passing NaN through
+(an fp32 division for the scale and one per element, the clamp after it, round to nearest even).  So a row holding a NaN gets scale NaN
+and NaN bytes; a row holding an inf gets scale inf, NaN bytes at its infinite elements and +-0 elsewhere; every e4m3 GEMM output of
+such a row is NaN.  torch's amax and clamp propagate NaN already.  e4m3 is torch.float8_e4m3fn (finite values up to 448, smallest
+subnormal 2^-9, NaN encoded as 0x7F or 0xFF)."""
 import contextlib
 import re
 
@@ -20,9 +23,14 @@ def quant_rows(x):
     """x [..., K] (bf16 or fp32 values) -> (q uint8 [..., K] holding the e4m3 bytes, scale fp32 [...])."""
     x = x.detach().to("cpu", torch.float32)
     amax = x.abs().amax(-1)
-    scale = torch.where(amax > 0, amax / torch.tensor(E4M3_MAX, dtype=torch.float32), torch.ones_like(amax))
+    scale = torch.where(amax == 0, torch.ones_like(amax), amax / torch.tensor(E4M3_MAX, dtype=torch.float32))
     q = (x / scale[..., None]).clamp(-E4M3_MAX, E4M3_MAX).to(torch.float8_e4m3fn)
     return q.view(torch.uint8), scale
+
+
+def is_nan_byte(q):
+    """The e4m3 NaN encodings, 0x7F and 0xFF (quantiser outputs are compared by NaN class there and bit for bit elsewhere)."""
+    return (q & 0x7F) == 0x7F
 
 
 def dequant(q, scale, dtype=torch.float64):

@@ -57,6 +57,45 @@ def test_row_of_one_repeated_value_and_a_subnormal_amax():
     assert s2.item() == 293 * 2.0 ** -149 and q2[0].tolist() == [0x7E, 0x76]     # 2^16 / 293 = 223.7 -> 224 = 0x76
 
 
+NAN, INF = float("nan"), float("inf")
+FINITE_ROW = [448.0, -448.0, 1.0, 17.0, 0.0, 2.0 ** -9, 2.0 ** -10, -19.0]
+FINITE_BYTES = [0x7E, 0xFE, 0x38, 0x58, 0x00, 0x01, 0x00, 0xDA]
+
+
+def test_non_finite_rows_propagate_and_leave_their_neighbours_alone():
+    x = torch.tensor([FINITE_ROW,
+                      [1.0, NAN, -2.0, 0.0, -0.0, 448.0, 3.0, -3.0],          # NaN: scale NaN, every byte NaN
+                      [1.0, INF, -2.0, 0.0, -0.0, 448.0, 3.0, -3.0],          # +inf: scale inf, NaN at the inf, +-0 elsewhere
+                      [-INF, 3.0, -3.0, 0.0, -0.0, 1e30, -1e-30, 7.0],        # -inf likewise
+                      [NAN, INF, -INF, 1.0, -1.0, 0.0, 2.0, 3.0],             # both: the NaN wins
+                      FINITE_ROW]).to(torch.bfloat16)
+    q, s = O.quant_rows(x)
+    assert q.dtype == torch.uint8 and s.dtype == torch.float32
+    assert s[0].item() == 1.0 and s[5].item() == 1.0 and q[0].tolist() == FINITE_BYTES and q[5].tolist() == FINITE_BYTES
+    assert torch.isnan(s[1]) and O.is_nan_byte(q[1]).all()
+    assert s[2].item() == INF and s[3].item() == INF
+    assert q[2].tolist() == [0x00, q[2, 1].item(), 0x80, 0x00, 0x80, 0x00, 0x00, 0x80] and O.is_nan_byte(q[2, 1])
+    assert q[3].tolist() == [q[3, 0].item(), 0x00, 0x80, 0x00, 0x80, 0x00, 0x80, 0x00] and O.is_nan_byte(q[3, 0])
+    assert torch.isnan(s[4]) and O.is_nan_byte(q[4]).all()
+    # a row is quantised on its own: without the non-finite rows the finite ones come out the same
+    q2, s2 = O.quant_rows(x[[0, 5]])
+    assert torch.equal(q2, q[[0, 5]]) and torch.equal(s2, s[[0, 5]])
+    # every product with a non-finite row is NaN in every column (an inf row dequantises to NaN at the inf and inf * 0 = NaN elsewhere);
+    # the finite rows keep their values
+    w = torch.tensor([[1.0] * 8, [0.0] * 8, [-1.0, 2.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.5]])
+    qw, sw = O.quant_rows(w)
+    d = O.gemm_dequant_fp64(q, s, qw, sw)
+    assert torch.isnan(d[1:5]).all() and torch.isfinite(d[[0, 5]]).all()
+    assert torch.equal(d[0], O.gemm_dequant_fp64(q[:1], s[:1], qw, sw)[0])
+
+
+def test_negative_values_that_underflow_keep_their_sign():
+    # amax 448 -> scale 1: -2^-11 rounds to -0 (0x80), -2^-10 (a tie with 0) to -0, -0.0 stays -0, -0.6 * 2^-9 to -2^-9 (0x81)
+    x = torch.tensor([[448.0, -(2.0 ** -11), -(2.0 ** -10), -0.0, -0.6 * 2.0 ** -9, 2.0 ** -11]])
+    q, s = O.quant_rows(x)
+    assert s.item() == 1.0 and q[0].tolist() == [0x7E, 0x80, 0x80, 0x80, 0x81, 0x00]
+
+
 def test_dequantised_gemm_is_the_float64_product():
     g = torch.Generator().manual_seed(0)
     a, w = torch.randn(5, 64, generator=g).to(torch.bfloat16), torch.randn(7, 64, generator=g).to(torch.bfloat16)
