@@ -14,6 +14,7 @@ import torch
 pytestmark = pytest.mark.gpu
 
 from llavamod import kernels as K  # noqa: E402
+from tests.decode_exact import decode_reference_fp64  # noqa: E402,F401  (the float64 attention with the kernel's bound)
 
 BK = 64                          # keys per ring stage (csrc/decode.cu)
 NST = {64: 4, 128: 3}            # ring stages per head width
@@ -26,42 +27,6 @@ def split_keys(max_len, nkv):
     ns = -(-2 * torch.cuda.get_device_properties(0).multi_processor_count // nkv)
     ns = max(1, min(ns, -(-blocks // 4)))
     return -(-blocks // ns) * BK
-
-
-def decode_reference_fp64(q, k, v, lens, nh, nkv, hd, scale):
-    """float64 attention of q [B, nh*hd] over cache rows [0, lens[b]) of k / v [B, nkv, max_len, hp], with the error bound of the kernel.
-
-    Kernel arithmetic and its error, per (b, h):
-      * score q.k: bf16 x bf16 products are exact in fp32; the fp32 sum of hd terms (fma chain over 8, then a shuffle tree) errs by at
-        most hd * 2^-24 * sum|q_i k_i|; the multiply by scale*log2(e) and the subtraction of the running max add 2^-24 relative each;
-      * p = ex2.approx(s - m): 2^-22 relative, plus the rescale factors 2^(m_old - m_new), applied once per block and once per split
-        merge (another 2^-22 each, at most len/64 + 2 of them);
-      * a relative error d on every weight p_t moves sum p_t v_t / sum p_t by at most 2 d max|v|;
-      * fp32 sums of p_t v_t and of p_t over len terms: len * 2^-24 relative to sum p |v| <= max|v| sum p;
-      * the output is rounded to bf16: 2^-9 |out|.
-    Bound: |out - ref| <= 2^-8 |ref| + max|v| (2 d + len 2^-23 + 2^-20), d = scale hd 2^-23 max_t sum|q k_t| + (len/64 + 4) 2^-21.
-    For the LSE (natural log): |lse - ref| <= d + len 2^-23 + 2^-20."""
-    B = q.shape[0]
-    G = nh // nkv
-    q64 = q[:, :nh * hd].double().reshape(B, nh, hd)
-    out = torch.zeros(B, nh, hd, dtype=torch.float64, device=q.device)
-    lse = torch.zeros(B, nh, dtype=torch.float64, device=q.device)
-    tol = torch.zeros(B, nh, hd, dtype=torch.float64, device=q.device)
-    tol_lse = torch.zeros(B, nh, dtype=torch.float64, device=q.device)
-    for b in range(B):
-        n = int(lens[b])
-        for h in range(nh):
-            kk = k[b, h // G, :n, :hd].double()
-            vv = v[b, h // G, :n, :hd].double()
-            s = (kk @ q64[b, h]) * scale
-            lse[b, h] = torch.logsumexp(s, 0)
-            p = torch.softmax(s, 0)
-            out[b, h] = p @ vv
-            d = scale * hd * 2.0 ** -23 * (kk.abs() @ q64[b, h].abs()).max() + (n / 64 + 4) * 2.0 ** -21
-            vmax = vv.abs().max()
-            tol[b, h] = 2.0 ** -8 * out[b, h].abs() + vmax * (2 * d + n * 2.0 ** -23 + 2.0 ** -20)
-            tol_lse[b, h] = d + n * 2.0 ** -23 + 2.0 ** -20
-    return out, lse, tol, tol_lse
 
 
 def make_cache(B, nh, nkv, hd, lens, max_len, seed, needles=()):
@@ -110,6 +75,7 @@ def check(name, q, k, v, lens, nh, nkv, hd):
 
 CASES = [   # hd, nh, nkv
     (64, 4, 4), (128, 4, 2), (64, 12, 2), (128, 14, 2), (128, 16, 2), (32, 4, 2), (80, 7, 1),
+    (64, 6, 2), (64, 8, 2), (64, 10, 2), (128, 2, 2), (128, 6, 2), (128, 8, 2), (128, 10, 2), (128, 12, 2), (128, 32, 32),
 ]
 
 
@@ -129,10 +95,11 @@ def test_decode_matches_fp64_at_split_and_ring_edges(hd, nh, nkv):
             needles.append((b, sk - 1, 20.0))
             needles.append((b, sk, 20.0))
     q, k, v = make_cache(B, nh, nkv, hd, lens, max_len, seed=hd * 100 + nh, needles=needles)
-    out, lse = check("hd%d_g%d" % (hd, nh // nkv), q, k, v, lens, nh, nkv, hd)
+    name = "hd%d_g%d" % (hd, nh // nkv) + ("_nkv%d" % nkv if nkv > 4 else "")
+    out, lse = check(name, q, k, v, lens, nh, nkv, hd)
     # no needles: the plain softmax average
     q2, k2, v2 = make_cache(B, nh, nkv, hd, lens, max_len, seed=hd * 100 + nh + 1)
-    check("hd%d_g%d_plain" % (hd, nh // nkv), q2, k2, v2, lens, nh, nkv, hd)
+    check(name + "_plain", q2, k2, v2, lens, nh, nkv, hd)
     # every sequence alone gives the same bits as inside the unequal-length batch; a second launch gives the same bytes
     for b in range(B):
         o1, l1 = run_decode(q[b:b + 1].contiguous(), k[b:b + 1].contiguous(), v[b:b + 1].contiguous(), lens[b:b + 1], nh, nkv, hd)
