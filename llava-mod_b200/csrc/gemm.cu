@@ -97,23 +97,6 @@ __device__ __forceinline__ GemmParams effective_extents(const GemmParams& in) {
 
 struct Tile { int m0, n0, kb0, kb1, group, m_end; };
 
-// d(gate), d(up) from dact (the fp32 accumulator rounded to bf16, as the unfused path materialises it) and the saved pre-activations:
-// the expression of silu_mul_bwd_kernel
-__device__ __forceinline__ void silu_bwd_store2(float a0, float a1, const __nv_bfloat16* gp, const __nv_bfloat16* up, __nv_bfloat16* dgp, __nv_bfloat16* dup) {
-  const uint32_t gv = __ldg(reinterpret_cast<const uint32_t*>(gp)), uv = __ldg(reinterpret_cast<const uint32_t*>(up));
-  const float g[2] = {bf16lo(gv), bf16hi(gv)}, u[2] = {bf16lo(uv), bf16hi(uv)}, dacc[2] = {a0, a1};
-  float dg[2], du[2];
-#pragma unroll
-  for (int j = 0; j < 2; ++j) {
-    const float d = bf16_round(dacc[j]);
-    const float sg = sigmoid_f(g[j]);
-    du[j] = d * g[j] * sg;
-    dg[j] = d * u[j] * sg * (1.f + g[j] * (1.f - sg));
-  }
-  *reinterpret_cast<uint32_t*>(dgp) = pack_bf16x2(dg[0], dg[1]);
-  *reinterpret_cast<uint32_t*>(dup) = pack_bf16x2(du[0], du[1]);
-}
-
 // tile index -> coordinates.  Dense: M fastest (consecutive CTAs share the B tile in L2).  Grouped forward/dgrad: per-group row
 // ranges [offsets[g], offsets[g+1]) (128-row aligned by the router), B rows offset by g*b_group_rows.  Grouped wgrad: each group owns
 // the reduction range [offsets[g], offsets[g+1]) and its own D.
@@ -247,32 +230,46 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_consta
     if (!empty_k && wg_leader) mbar_arrive(&empty_bar[prev]);
     reg_fence<BN / 2>(acc);
 
-    // accumulator fragment: register 4i + 2h + e holds row 16w + lane/4 + 8h, column 8i + 2(lane%4) + e of this warpgroup's 64 x BN block
+    // accumulator fragment: register 4i + 2h + e holds row 16w + lane/4 + 8h, column 8i + 2(lane%4) + e of this warpgroup's 64 x BN block.
+    // Every form works on transpose groups: the 4 blocks of 8 columns [32k, 32k + 32) of one row, whose packed column pairs the four
+    // lanes of a quad trade (quad_transpose) so that lane q ends up with the 8 columns of block 4k + q -- a quad writes 64 contiguous bytes
+    // of a row per instruction instead of 16, with a quarter of the store instructions.  N % 8 == 0: a block is in or out as a whole.
     const int row0 = t.m0 + c * 64 + w * 16 + (lane >> 2);
-    const int cq = 2 * (lane & 3);
+    const int cq = 2 * (lane & 3), q = lane & 3;
     const int64_t goff = p.wgrad_grouped ? t.group * p.d_group_stride : 0;
+    if (p.dbg_nostore) continue;
     if (BN == 256 && p.swiglu) {
-      // accumulator columns [0,128) = gate, [128,256) = up of the same 128 act columns
+      // accumulator columns [0,128) = gate, [128,256) = up of the same 128 act columns (I % 128 == 0: all in range)
 #pragma unroll
-      for (int i = 0; i < 16; ++i) {
-        const int col = t.n0 + 8 * i + cq;
-        if (col >= p.N) continue;
+      for (int k = 0; k < 4; ++k) {
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
-          const int row = row0 + 8 * h;
+          uint32_t wg[4], wu[4], wa[4];
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+            const int i = 4 * k + j;
+            wg[j] = pack_bf16x2(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
+            wu[j] = pack_bf16x2(acc[4 * (i + 16) + 2 * h], acc[4 * (i + 16) + 2 * h + 1]);
+            wa[j] = swiglu2(wg[j], wu[j]);
+          }
+          quad_transpose(wa, q);
+          const int row = row0 + 8 * h, col8 = t.n0 + 8 * (4 * k + q);
+          if (p.H1) { quad_transpose(wg, q); quad_transpose(wu, q); }
           if (row >= t.m_end) continue;
-          __nv_bfloat16* drow = p.D + (int64_t)row * p.ldd;
-          __nv_bfloat16* h1row = p.H1 ? p.H1 + (int64_t)row * p.ld_h1 : nullptr;
-          swiglu_store2(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1], acc[4 * (i + 16) + 2 * h], acc[4 * (i + 16) + 2 * h + 1], drow + col,
-                        h1row ? h1row + col : nullptr, h1row ? h1row + p.swiglu_I + col : nullptr);
+          st16(p.D + (int64_t)row * p.ldd + col8, make_uint4(wa[0], wa[1], wa[2], wa[3]));
+          if (p.H1) {
+            __nv_bfloat16* h1row = p.H1 + (int64_t)row * p.ld_h1;
+            st16(h1row + col8, make_uint4(wg[0], wg[1], wg[2], wg[3]));
+            st16(h1row + p.swiglu_I + col8, make_uint4(wu[0], wu[1], wu[2], wu[3]));
+          }
         }
       }
       continue;
     }
-    if (!p.rope_cos && !p.silu_bwd && !p.D32 && !p.beta && !p.R && !p.dbg_nostore && (reinterpret_cast<uintptr_t>(p.D) & 15) == 0) {
-      // plain bf16 output (+bias): the four lanes of a quad trade their packed column pairs so that each stores one 16-byte block of
-      // 8 columns -- a quad writes 64 contiguous bytes of a row per instruction instead of 16, with a quarter of the store instructions
-      const int q = lane & 3;
+    // plain (+bias), residual and SwiGLU-backward: x = bf16(acc + bias) traded across the quad, then the form's work on the 8 columns.
+    // Each form is its own straight-line pass over the groups (stores predicated, no branch between groups), so that the compiler can
+    // overlap the shuffles and loads of different groups.
+    auto bf16_groups = [&](auto&& finish) {
 #pragma unroll
       for (int k = 0; k < BN / 32; ++k) {
 #pragma unroll
@@ -287,59 +284,125 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_consta
           }
           quad_transpose(wd, q);
           const int row = row0 + 8 * h, col8 = t.n0 + 8 * (4 * k + q);
-          if (row < t.m_end && col8 < p.N)                 // N % 8 == 0: a block of 8 columns is in or out as a whole
-            *reinterpret_cast<uint4*>(p.D + goff + (int64_t)row * p.ldd + col8) = make_uint4(wd[0], wd[1], wd[2], wd[3]);
+          if (row < t.m_end && col8 < p.N) finish(wd, row, col8);
         }
       }
+    };
+    if (p.silu_bwd) {
+      bf16_groups([&](const uint32_t (&wd)[4], int row, int col8) {
+        const __nv_bfloat16* gu = p.GU + (int64_t)row * p.ld_gu + col8;
+        __nv_bfloat16* d = p.D + (int64_t)row * p.ldd + col8;
+        silu_bwd_store8(wd, gu, gu + p.N, d, d + p.N);
+      });
       continue;
     }
+    if (p.R) {
+      bf16_groups([&](const uint32_t (&wd)[4], int row, int col8) {
+        residual_store8(wd, p.R + (int64_t)row * p.ld_r + col8, p.D + (int64_t)row * p.ldd + col8);
+      });
+      continue;
+    }
+    if (!p.rope_cos && !p.D32 && !p.beta) {
+      bf16_groups([&](const uint32_t (&wd)[4], int row, int col8) {
+        st16(p.D + goff + (int64_t)row * p.ldd + col8, make_uint4(wd[0], wd[1], wd[2], wd[3]));
+      });
+      continue;
+    }
+    // RoPE (and the v columns of its output), split-K atomics, fp32 D32 += acc and D = bf16(D + acc)
+    int64_t pos[2] = {0, 0};                               // the rotary positions of the thread's two rows
+    if (p.rope_cos) {
 #pragma unroll
-    for (int i = 0; i < BN / 8; ++i) {
-      const int col8 = t.n0 + 8 * i, col = col8 + cq;
-      if (p.rope_cos && col8 < p.rope_cols) {
-        // q / k head columns: the first half of a head is processed together with its partner half a head further on (same thread)
-        const int hoff = col8 % p.rope_hd, half = p.rope_hd >> 1;
-        if (hoff >= half) continue;                                     // done with its partner
-        const int ip = (half == 32) ? i + 4 : i + 8;
-        if (ip >= BN / 8) continue;                                     // (a head never straddles a tile: tiles start at multiples of 128)
+      for (int h = 0; h < 2; ++h) if (row0 + 8 * h < t.m_end) pos[h] = __ldg(p.rope_pos + row0 + 8 * h);
+    }
+#pragma unroll
+    for (int k = 0; k < BN / 32; ++k) {
+      const int cg = t.n0 + 32 * k;                        // first column of the group (the same in every lane)
+      if (cg >= p.N) continue;
+      if (p.rope_cos && cg < p.rope_cols) {
+        // q / k head columns: a group of the first half of a head is rotated together with its partner group half a head further on
+        // (k + 2 for hd 128, k + 1 for hd 64; a head never straddles a tile: tiles start at multiples of 128); the partner is skipped
+        const int half = p.rope_hd >> 1, hoff = cg % p.rope_hd;
+        if (hoff >= half) continue;
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
-          const int row = row0 + 8 * h;
+          uint32_t w1[4], w2[4];
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+            const int i1 = 4 * k + j, col = t.n0 + 8 * i1 + cq;
+            const int i2a = (i1 + 4) % (BN / 8), i2b = (i1 + 8) % (BN / 8);
+            float x10 = acc[4 * i1 + 2 * h], x11 = acc[4 * i1 + 2 * h + 1];
+            float x20 = half == 32 ? acc[4 * i2a + 2 * h] : acc[4 * i2b + 2 * h];
+            float x21 = half == 32 ? acc[4 * i2a + 2 * h + 1] : acc[4 * i2b + 2 * h + 1];
+            if (p.bias) { bias2(p.bias + col, x10, x11); bias2(p.bias + col + half, x20, x21); }
+            w1[j] = pack_bf16x2(x10, x11);
+            w2[j] = pack_bf16x2(x20, x21);
+          }
+          quad_transpose(w1, q);
+          quad_transpose(w2, q);
+          const int row = row0 + 8 * h, col8 = cg + 8 * q;
           if (row >= t.m_end) continue;
-          float x20, x21;
-          if (half == 32) { x20 = acc[4 * ((i + 4) % (BN / 8)) + 2 * h]; x21 = acc[4 * ((i + 4) % (BN / 8)) + 2 * h + 1]; }
-          else { x20 = acc[4 * ((i + 8) % (BN / 8)) + 2 * h]; x21 = acc[4 * ((i + 8) % (BN / 8)) + 2 * h + 1]; }
-          const int64_t pp = __ldg(p.rope_pos + row);
-          __nv_bfloat16* drow = p.D + (int64_t)row * p.ldd;
-          rope_store2(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1], x20, x21, p.bias ? p.bias + col : nullptr, p.bias ? p.bias + col + half : nullptr,
-                      p.rope_cos + pp * p.rope_hd + hoff + cq, p.rope_sin + pp * p.rope_hd + hoff + cq, drow + col, drow + col + half);
+          const int64_t cs = pos[h] * p.rope_hd + hoff + 8 * q;
+          __nv_bfloat16* d = p.D + (int64_t)row * p.ldd + col8;
+          uint4 o1, o2;
+          rope8(w1, w2, p.rope_cos + cs, p.rope_sin + cs, o1, o2);
+          st16(d, o1);
+          st16(d + half, o2);
         }
         continue;
       }
-      if (col >= p.N || p.dbg_nostore) continue;
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        const int row = row0 + 8 * h;
-        if (row >= t.m_end) continue;
-        float f0 = empty_k ? 0.f : acc[4 * i + 2 * h], f1 = empty_k ? 0.f : acc[4 * i + 2 * h + 1];
-        if (p.bias) bias2(p.bias + col, f0, f1);
-        if (p.silu_bwd) {
-          const __nv_bfloat16* gurow = p.GU + (int64_t)row * p.ld_gu;
-          __nv_bfloat16* drow = p.D + (int64_t)row * p.ldd;
-          silu_bwd_store2(f0, f1, gurow + col, gurow + p.N + col, drow + col, drow + p.N + col);
-        } else if (p.D32) {
-          float* d32 = p.D32 + goff + (int64_t)row * p.ldd + col;
-          if (p.splits > 1) { atomicAdd(d32, f0); atomicAdd(d32 + 1, f1); }
-          else { float2 o = *reinterpret_cast<float2*>(d32); o.x += f0; o.y += f1; *reinterpret_cast<float2*>(d32) = o; }
-        } else {
-          uint32_t* o = reinterpret_cast<uint32_t*>(p.D + goff + (int64_t)row * p.ldd + col);
-          if (p.beta) { const uint32_t old = *o; f0 += bf16lo(old); f1 += bf16hi(old); }
-          if (p.R) {
-            const uint32_t rr = __ldg(reinterpret_cast<const uint32_t*>(p.R + (int64_t)row * p.ld_r + col));
-            f0 = bf16_round(f0) + bf16lo(rr); f1 = bf16_round(f1) + bf16hi(rr);
-          }
-          *o = pack_bf16x2(f0, f1);
+        const int row = row0 + 8 * h, col8 = cg + 8 * q;
+        float f[4][2];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const int i = 4 * k + j, col = cg + 8 * j + cq;
+          f[j][0] = empty_k ? 0.f : acc[4 * i + 2 * h];
+          f[j][1] = empty_k ? 0.f : acc[4 * i + 2 * h + 1];
+          if (p.bias && col < p.N) bias2(p.bias + col, f[j][0], f[j][1]);
         }
+        if (p.D32 && p.splits > 1) {                       // split-K: fp32 atomics on the accumulator's own column pairs
+          if (row >= t.m_end) continue;
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+            const int col = cg + 8 * j + cq;
+            if (col >= p.N) continue;
+            float* d32 = p.D32 + goff + (int64_t)row * p.ldd + col;
+            atomicAdd(d32, f[j][0]); atomicAdd(d32 + 1, f[j][1]);
+          }
+          continue;
+        }
+        if (p.D32 || p.beta) {
+          // fp32 D32 += acc, or D = bf16(D + acc): nothing is rounded before the add, so the fp32 words themselves are traded --
+          // e[j] / o[j] end up as columns 2j / 2j + 1 of the lane's block
+          uint32_t e[4], o[4];
+#pragma unroll
+          for (int j = 0; j < 4; ++j) { e[j] = __float_as_uint(f[j][0]); o[j] = __float_as_uint(f[j][1]); }
+          quad_transpose(e, q);
+          quad_transpose(o, q);
+          if (row >= t.m_end || col8 >= p.N) continue;
+          if (p.D32) {
+            float4* d32 = reinterpret_cast<float4*>(p.D32 + goff + (int64_t)row * p.ldd + col8);
+            float4 lo = d32[0], hi = d32[1];
+            lo.x += __uint_as_float(e[0]); lo.y += __uint_as_float(o[0]); lo.z += __uint_as_float(e[1]); lo.w += __uint_as_float(o[1]);
+            hi.x += __uint_as_float(e[2]); hi.y += __uint_as_float(o[2]); hi.z += __uint_as_float(e[3]); hi.w += __uint_as_float(o[3]);
+            d32[0] = lo; d32[1] = hi;
+          } else {
+            uint4* d = reinterpret_cast<uint4*>(p.D + goff + (int64_t)row * p.ldd + col8);
+            const uint4 old = *d;
+            const uint32_t ow[4] = {old.x, old.y, old.z, old.w};
+            uint32_t r[4];
+#pragma unroll
+            for (int j = 0; j < 4; ++j) r[j] = pack_bf16x2(__uint_as_float(e[j]) + bf16lo(ow[j]), __uint_as_float(o[j]) + bf16hi(ow[j]));
+            *d = make_uint4(r[0], r[1], r[2], r[3]);
+          }
+          continue;
+        }
+        uint32_t wd[4];                                    // the v columns of the RoPE form
+#pragma unroll
+        for (int j = 0; j < 4; ++j) wd[j] = pack_bf16x2(f[j][0], f[j][1]);
+        quad_transpose(wd, q);
+        if (row < t.m_end && col8 < p.N) st16(p.D + (int64_t)row * p.ldd + col8, make_uint4(wd[0], wd[1], wd[2], wd[3]));
       }
     }
   }
@@ -391,9 +454,12 @@ static int gemm_dense(const void* A, int64_t lda, int a_mn_major, const void* B,
                       const int32_t* m_rows_dev, const int32_t* k_rows_dev, void* stream, const RopeArgs* rope, const ResidArgs* resid = nullptr) {
   LMOD_CHECK_ARG(A && B && (D || d_f32_accum) && M > 0 && N > 0 && K > 0, "lmod_gemm_bf16: null pointer or empty problem");
   LMOD_CHECK_ARG(lda % 8 == 0 && ldb % 8 == 0 && ldd % 8 == 0 && N % 8 == 0 && ((uintptr_t)A % 16 == 0) && ((uintptr_t)B % 16 == 0) &&
-                 (!D || (uintptr_t)D % 16 == 0), "lmod_gemm_bf16: strides / N must be multiples of 8 elements and pointers 16-byte aligned (TMA)");
+                 (!D || (uintptr_t)D % 16 == 0) && ((uintptr_t)d_f32_accum % 16 == 0),
+                 "lmod_gemm_bf16: strides / N must be multiples of 8 elements and pointers 16-byte aligned (TMA, 16-byte epilogue stores)");
   LMOD_CHECK_ARG((uintptr_t)bias % 4 == 0 && (!rope || ((uintptr_t)rope->cos % 4 == 0 && (uintptr_t)rope->sin % 4 == 0)),
-                 "lmod_gemm_bf16: bias, cos and sin must be 4-byte aligned (the epilogue reads them two bf16 at a time)");
+                 "lmod_gemm_bf16: bias, cos and sin must be 4-byte aligned (the epilogue reads bias two bf16 at a time)");
+  LMOD_CHECK_ARG(!rope || ((uintptr_t)rope->cos % 16 == 0 && (uintptr_t)rope->sin % 16 == 0 && rope->hd % 8 == 0),
+                 "lmod_gemm_qkv_rope: cos and sin must be 16-byte aligned and head_dim a multiple of 8 (the epilogue reads them 8 bf16 at a time)");
   CUtensorMap ta, tb;
   int rc;
   const int splits_req = (epilogue >> 8) > 1 ? (epilogue >> 8) : 1;
@@ -538,7 +604,8 @@ extern "C" int lmod_grouped_gemm_silu_bwd(const void* dY, int64_t lda, const voi
 extern "C" int lmod_grouped_gemm_bf16(const void* A, int64_t lda, const void* B, int64_t ldb, void* D, int64_t ldd, const int32_t* offsets, int G,
                                       int64_t max_rows, int64_t M, int64_t N, int64_t K, int mode, int epilogue, void* stream) {
   LMOD_CHECK_ARG(A && B && D && offsets && G >= 1 && G <= MAX_GROUPS && max_rows > 0, "lmod_grouped_gemm_bf16: bad arguments");
-  LMOD_CHECK_ARG(lda % 8 == 0 && ldb % 8 == 0 && ldd % 8 == 0 && N % 8 == 0, "lmod_grouped_gemm_bf16: strides / N must be multiples of 8");
+  LMOD_CHECK_ARG(lda % 8 == 0 && ldb % 8 == 0 && ldd % 8 == 0 && N % 8 == 0 && (uintptr_t)D % 16 == 0,
+                 "lmod_grouped_gemm_bf16: strides / N must be multiples of 8 and D 16-byte aligned (16-byte epilogue stores)");
   CUtensorMap ta, tb;
   GemmParams p = {};
   p.D = (__nv_bfloat16*)D; p.ldd = ldd; p.beta = epilogue & 1; p.offsets = offsets; p.groups = G; p.splits = 1;

@@ -8,41 +8,81 @@ namespace {
 
 constexpr int BM = 128;
 
-// The epilogue works on what one thread holds of a wgmma accumulator: two adjacent columns (col, col + 1) of one row.
+// The epilogue starts from what one thread holds of a wgmma accumulator: two adjacent columns (col, col + 1) of one row.  Whatever is
+// rounded to bf16 first (or, where nothing is, the fp32 words) is traded across the quad with quad_transpose, after which each lane holds
+// 8 consecutive columns of the row; the functions below finish the element-wise work on such a block, loading their side inputs and
+// storing their outputs 16 bytes at a time.  Every operation after the first rounding is per element, so this is exact.
 __device__ __forceinline__ float sigmoid_f(float x) { return 1.f / (1.f + __expf(-x)); }
 __device__ __forceinline__ void bias2(const __nv_bfloat16* b, float& f0, float& f1) {
   const uint32_t w = __ldg(reinterpret_cast<const uint32_t*>(b));
   f0 += bf16lo(w); f1 += bf16hi(w);
 }
-// rotate one (x1, x2) pair of columns of a head: x = bf16(acc + bias); o1 = bf16(bf16(x1 c) + bf16(-x2 s)), o2 = bf16(bf16(x2 c) + bf16(x1 s))
-// (the expression of rope_vec_kernel).  a1 / a2: fp32 accumulators of the first-half / second-half columns, b1 / b2: their bias (or null).
-__device__ __forceinline__ void rope_store2(float a10, float a11, float a20, float a21, const __nv_bfloat16* b1, const __nv_bfloat16* b2,
-                                            const __nv_bfloat16* cs, const __nv_bfloat16* sn, __nv_bfloat16* d1, __nv_bfloat16* d2) {
-  float x1[2] = {a10, a11}, x2[2] = {a20, a21};
-  if (b1) { bias2(b1, x1[0], x1[1]); bias2(b2, x2[0], x2[1]); }
-  const uint32_t cw = __ldg(reinterpret_cast<const uint32_t*>(cs)), sw = __ldg(reinterpret_cast<const uint32_t*>(sn));
-  const float c[2] = {bf16lo(cw), bf16hi(cw)}, s[2] = {bf16lo(sw), bf16hi(sw)};
-  float o1[2], o2[2];
+__device__ __forceinline__ void unpack8w(const uint32_t (&w)[4], float (&f)[8]) {
 #pragma unroll
-  for (int j = 0; j < 2; ++j) {
-    const float y1 = bf16_round(x1[j]), y2 = bf16_round(x2[j]);
-    o1[j] = bf16_round(y1 * c[j]) + bf16_round(-y2 * s[j]);
-    o2[j] = bf16_round(y2 * c[j]) + bf16_round(y1 * s[j]);
-  }
-  *reinterpret_cast<uint32_t*>(d1) = pack_bf16x2(o1[0], o1[1]);
-  *reinterpret_cast<uint32_t*>(d2) = pack_bf16x2(o2[0], o2[1]);
+  for (int j = 0; j < 4; ++j) { f[2 * j] = bf16lo(w[j]); f[2 * j + 1] = bf16hi(w[j]); }
 }
-// act = bf16(bf16(silu(g)) * u) on bf16-rounded GEMM outputs: the expression of silu_mul_fwd_kernel (bit-identical to GEMM + that kernel)
-__device__ __forceinline__ void swiglu_store2(float g0, float g1, float u0, float u1, __nv_bfloat16* act, __nv_bfloat16* h1g, __nv_bfloat16* h1u) {
-  const float gb[2] = {bf16_round(g0), bf16_round(g1)}, ub[2] = {bf16_round(u0), bf16_round(u1)};
-  float f[2];
+__device__ __forceinline__ void unpack8v(const uint4 v, float (&f)[8]) {
+  const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+  unpack8w(w, f);
+}
+__device__ __forceinline__ uint4 pack8v(const float (&f)[8]) {
+  return make_uint4(pack_bf16x2(f[0], f[1]), pack_bf16x2(f[2], f[3]), pack_bf16x2(f[4], f[5]), pack_bf16x2(f[6], f[7]));
+}
+// 16-byte stores.  st16 is a plain C++ store, which leaves the compiler free to move the next block's loads (bias, cos / sin, side
+// inputs) ahead of it; st16_asm is one st.global.v4 whatever the compiler would make of the words -- the e4m3 kernel's compiler splits
+// the C++ store of its RoPE and SwiGLU blocks into four 32-bit ones.
+__device__ __forceinline__ void st16(__nv_bfloat16* d, const uint4 v) { *reinterpret_cast<uint4*>(d) = v; }
+__device__ __forceinline__ void st16_asm(__nv_bfloat16* d, const uint4 v) {
+  asm volatile("st.global.v4.b32 [%0], {%1,%2,%3,%4};" :: "l"(d), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w));
+}
+// rotate 8 (x1, x2) column pairs of a head, x1 / x2 = bf16(acc + bias) of the first-half / second-half block:
+// o1 = bf16(bf16(x1 c) + bf16(-x2 s)), o2 = bf16(bf16(x2 c) + bf16(x1 s)) (the expression of rope_vec_kernel).  cs / sn: the 8 first-half
+// columns of the cos / sin row of the position.
+__device__ __forceinline__ void rope8(const uint32_t (&w1)[4], const uint32_t (&w2)[4], const __nv_bfloat16* cs, const __nv_bfloat16* sn,
+                                      uint4& r1, uint4& r2) {
+  float x1[8], x2[8], c[8], s[8], o1[8], o2[8];
+  unpack8w(w1, x1); unpack8w(w2, x2);
+  unpack8v(__ldg(reinterpret_cast<const uint4*>(cs)), c);
+  unpack8v(__ldg(reinterpret_cast<const uint4*>(sn)), s);
 #pragma unroll
-  for (int j = 0; j < 2; ++j) f[j] = bf16_round(gb[j] * sigmoid_f(gb[j])) * ub[j];
-  *reinterpret_cast<uint32_t*>(act) = pack_bf16x2(f[0], f[1]);
-  if (h1g) {
-    *reinterpret_cast<uint32_t*>(h1g) = pack_bf16x2(gb[0], gb[1]);
-    *reinterpret_cast<uint32_t*>(h1u) = pack_bf16x2(ub[0], ub[1]);
+  for (int j = 0; j < 8; ++j) {
+    o1[j] = bf16_round(x1[j] * c[j]) + bf16_round(-x2[j] * s[j]);
+    o2[j] = bf16_round(x2[j] * c[j]) + bf16_round(x1[j] * s[j]);
   }
+  r1 = pack8v(o1);
+  r2 = pack8v(o2);
+}
+// act = bf16(bf16(silu(g)) * u) of one packed column pair of the bf16-rounded GEMM outputs: the expression of silu_mul_fwd_kernel
+// (bit-identical to GEMM + that kernel).  Computed before the transpose, so that only the activation has to be traded.
+__device__ __forceinline__ uint32_t swiglu2(const uint32_t wg, const uint32_t wu) {
+  const float g0 = bf16lo(wg), g1 = bf16hi(wg);
+  return pack_bf16x2(bf16_round(g0 * sigmoid_f(g0)) * bf16lo(wu), bf16_round(g1 * sigmoid_f(g1)) * bf16hi(wu));
+}
+// d(gate), d(up) from dact (the fp32 accumulator rounded to bf16, as the unfused path materialises it) and the saved pre-activations gp / up:
+// the expression of silu_mul_bwd_kernel
+__device__ __forceinline__ void silu_bwd_store8(const uint32_t (&wd)[4], const __nv_bfloat16* gp, const __nv_bfloat16* up, __nv_bfloat16* dgp,
+                                                __nv_bfloat16* dup) {
+  float d[8], g[8], u[8], dg[8], du[8];
+  unpack8w(wd, d);
+  unpack8v(__ldg(reinterpret_cast<const uint4*>(gp)), g);
+  unpack8v(__ldg(reinterpret_cast<const uint4*>(up)), u);
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const float sg = sigmoid_f(g[j]);
+    du[j] = d[j] * g[j] * sg;
+    dg[j] = d[j] * u[j] * sg * (1.f + g[j] * (1.f - sg));
+  }
+  st16(dgp, pack8v(dg));
+  st16(dup, pack8v(du));
+}
+// D = bf16(x + r), x = bf16(acc + bias): the residual add (the expression of add_kernel)
+__device__ __forceinline__ void residual_store8(const uint32_t (&wx)[4], const __nv_bfloat16* r, __nv_bfloat16* d) {
+  float x[8], y[8];
+  unpack8w(wx, x);
+  unpack8v(__ldg(reinterpret_cast<const uint4*>(r)), y);
+#pragma unroll
+  for (int j = 0; j < 8; ++j) y[j] += x[j];
+  st16(d, pack8v(y));
 }
 // 4 x 4 transpose within each quad of lanes: lane q holds w[j] = word j of its own; afterwards w[j] = word q of lane j (the lane index
 // within the quad is q).  The sender picks the word its receiver needs, so no register is indexed dynamically.

@@ -143,88 +143,98 @@ gemm_e4m3_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constan
       for (int i = 0; i < BN / 2; ++i) acc[i] += part[i];
     }
 
-    // accumulator fragment: register 4i + 2h + e holds row 16w + lane/4 + 8h, column 8i + 2(lane%4) + e of this warpgroup's 64 x BN block
+    // accumulator fragment: register 4i + 2h + e holds row 16w + lane/4 + 8h, column 8i + 2(lane%4) + e of this warpgroup's 64 x BN block.
+    // The forms are those of gemm_wgmma_kernel on the scaled accumulators (acc * s_a[m]) * s_w[n]: each rounds to bf16, trades the packed
+    // column pairs of a transpose group (4 blocks of 8 columns) across the quad, and stores 16-byte blocks.
     const int row0 = m0 + c * 64 + w * 16 + (lane >> 2);
-    const int cq = 2 * (lane & 3);
+    const int cq = 2 * (lane & 3), q = lane & 3;
     const float sar[2] = {row0 < p.M ? __ldg(p.sa + row0) : 0.f, row0 + 8 < p.M ? __ldg(p.sa + row0 + 8) : 0.f};
     if (p.swiglu_I) {
-      // accumulator columns [0,64) = gate, [64,128) = up of the same 64 act columns
+      // accumulator columns [0,64) = gate, [64,128) = up of the same 64 act columns (I % 128 == 0: all in range)
 #pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const int col = n0 + 8 * i + cq;
-        if (col >= p.N) continue;
-        const float2 sg = scale2(p.sw, col, p.N), su = scale2(p.sw + p.swiglu_I, col, p.N);
+      for (int k = 0; k < 2; ++k) {
+        float2 sg[4], su[4];
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int row = row0 + 8 * h;
-          if (row >= p.M) continue;
-          swiglu_store2(acc[4 * i + 2 * h] * sar[h] * sg.x, acc[4 * i + 2 * h + 1] * sar[h] * sg.y, acc[4 * (i + 8) + 2 * h] * sar[h] * su.x,
-                        acc[4 * (i + 8) + 2 * h + 1] * sar[h] * su.y, p.D + (int64_t)row * p.ldd + col, nullptr, nullptr);
+        for (int j = 0; j < 4; ++j) {
+          const int col = n0 + 8 * (4 * k + j) + cq;
+          sg[j] = scale2(p.sw, col, p.N); su[j] = scale2(p.sw + p.swiglu_I, col, p.N);
         }
-      }
-      continue;
-    }
-    if (!p.rope_cos) {
-      // plain bf16 output (+bias), 16-byte stores: see the same block of gemm_wgmma_kernel
-      const int q = lane & 3;
-#pragma unroll
-      for (int k = 0; k < BN / 32; ++k) {
-        float2 s[4];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) s[j] = scale2(p.sw, n0 + 8 * (4 * k + j) + cq, p.N);
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
-          uint32_t wd[4];
+          uint32_t wa[4];
 #pragma unroll
           for (int j = 0; j < 4; ++j) {
-            const int col = n0 + 8 * (4 * k + j) + cq;
-            float f0 = acc[4 * (4 * k + j) + 2 * h] * sar[h] * s[j].x, f1 = acc[4 * (4 * k + j) + 2 * h + 1] * sar[h] * s[j].y;
-            if (p.bias && col < p.N) bias2(p.bias + col, f0, f1);
-            wd[j] = pack_bf16x2(f0, f1);
+            const int i = 4 * k + j;
+            wa[j] = swiglu2(pack_bf16x2(acc[4 * i + 2 * h] * sar[h] * sg[j].x, acc[4 * i + 2 * h + 1] * sar[h] * sg[j].y),
+                            pack_bf16x2(acc[4 * (i + 8) + 2 * h] * sar[h] * su[j].x, acc[4 * (i + 8) + 2 * h + 1] * sar[h] * su[j].y));
           }
-          quad_transpose(wd, q);
-          const int row = row0 + 8 * h, col8 = n0 + 8 * (4 * k + q);
-          if (row < p.M && col8 < p.N)                     // N % 8 == 0: a block of 8 columns is in or out as a whole
-            *reinterpret_cast<uint4*>(p.D + (int64_t)row * p.ldd + col8) = make_uint4(wd[0], wd[1], wd[2], wd[3]);
+          quad_transpose(wa, q);
+          const int row = row0 + 8 * h;
+          if (row < p.M) st16_asm(p.D + (int64_t)row * p.ldd + n0 + 8 * (4 * k + q), make_uint4(wa[0], wa[1], wa[2], wa[3]));
         }
       }
       continue;
     }
-    // q|k|v + bias + RoPE: the loop of gemm_wgmma_kernel on the scaled accumulators
+    int64_t pos[2] = {0, 0};                               // the rotary positions of the thread's two rows
+    if (p.rope_cos) {
 #pragma unroll
-    for (int i = 0; i < BN / 8; ++i) {
-      const int col8 = n0 + 8 * i, col = col8 + cq;
-      if (col8 < p.rope_cols) {
-        // q / k head columns: the first half of a head is processed together with its partner half a head further on (same thread)
-        const int hoff = col8 % p.rope_hd, half = p.rope_hd >> 1;
-        if (hoff >= half) continue;                                     // done with its partner
-        const int ip = (half == 32) ? i + 4 : i + 8;
-        if (ip >= BN / 8) continue;                                     // (a head never straddles a tile: tiles start at multiples of 128)
-        const float2 s1 = scale2(p.sw, col, p.N), s2 = scale2(p.sw, col + half, p.N);
+      for (int h = 0; h < 2; ++h) if (row0 + 8 * h < p.M) pos[h] = __ldg(p.rope_pos + row0 + 8 * h);
+    }
+#pragma unroll
+    for (int k = 0; k < BN / 32; ++k) {
+      const int cg = n0 + 32 * k;                          // first column of the group (the same in every lane)
+      if (cg >= p.N) continue;
+      if (p.rope_cos && cg < p.rope_cols) {
+        // q / k head columns: a group of the first half of a head is rotated together with its partner group half a head further on
+        // (k + 2 for hd 128, k + 1 for hd 64; a head never straddles a tile); the partner is skipped
+        const int half = p.rope_hd >> 1, hoff = cg % p.rope_hd;
+        if (hoff >= half) continue;
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
+          uint32_t w1[4], w2[4];
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+            const int i1 = 4 * k + j, col = n0 + 8 * i1 + cq;
+            const int i2a = (i1 + 4) % (BN / 8), i2b = (i1 + 8) % (BN / 8);
+            const float2 s1 = scale2(p.sw, col, p.N), s2 = scale2(p.sw, col + half, p.N);
+            const float a20 = half == 32 ? acc[4 * i2a + 2 * h] : acc[4 * i2b + 2 * h];
+            const float a21 = half == 32 ? acc[4 * i2a + 2 * h + 1] : acc[4 * i2b + 2 * h + 1];
+            float x10 = acc[4 * i1 + 2 * h] * sar[h] * s1.x, x11 = acc[4 * i1 + 2 * h + 1] * sar[h] * s1.y;
+            float x20 = a20 * sar[h] * s2.x, x21 = a21 * sar[h] * s2.y;
+            if (p.bias) { bias2(p.bias + col, x10, x11); bias2(p.bias + col + half, x20, x21); }
+            w1[j] = pack_bf16x2(x10, x11);
+            w2[j] = pack_bf16x2(x20, x21);
+          }
+          quad_transpose(w1, q);
+          quad_transpose(w2, q);
           const int row = row0 + 8 * h;
           if (row >= p.M) continue;
-          float x20, x21;
-          if (half == 32) { x20 = acc[4 * ((i + 4) % (BN / 8)) + 2 * h]; x21 = acc[4 * ((i + 4) % (BN / 8)) + 2 * h + 1]; }
-          else { x20 = acc[4 * ((i + 8) % (BN / 8)) + 2 * h]; x21 = acc[4 * ((i + 8) % (BN / 8)) + 2 * h + 1]; }
-          const int64_t pp = __ldg(p.rope_pos + row);
-          __nv_bfloat16* drow = p.D + (int64_t)row * p.ldd;
-          rope_store2(acc[4 * i + 2 * h] * sar[h] * s1.x, acc[4 * i + 2 * h + 1] * sar[h] * s1.y, x20 * sar[h] * s2.x, x21 * sar[h] * s2.y,
-                      p.bias ? p.bias + col : nullptr, p.bias ? p.bias + col + half : nullptr,
-                      p.rope_cos + pp * p.rope_hd + hoff + cq, p.rope_sin + pp * p.rope_hd + hoff + cq, drow + col, drow + col + half);
+          const int64_t cs = pos[h] * p.rope_hd + hoff + 8 * q;
+          __nv_bfloat16* d = p.D + (int64_t)row * p.ldd + cg + 8 * q;
+          uint4 o1, o2;
+          rope8(w1, w2, p.rope_cos + cs, p.rope_sin + cs, o1, o2);
+          st16_asm(d, o1);
+          st16_asm(d + half, o2);
         }
         continue;
       }
-      if (col >= p.N) continue;
-      const float2 s = scale2(p.sw, col, p.N);
+      // plain bf16 output (+bias)
+      float2 s[4];
+#pragma unroll
+      for (int j = 0; j < 4; ++j) s[j] = scale2(p.sw, cg + 8 * j + cq, p.N);
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        const int row = row0 + 8 * h;
-        if (row >= p.M) continue;
-        float f0 = acc[4 * i + 2 * h] * sar[h] * s.x, f1 = acc[4 * i + 2 * h + 1] * sar[h] * s.y;
-        if (p.bias) bias2(p.bias + col, f0, f1);
-        *reinterpret_cast<uint32_t*>(p.D + (int64_t)row * p.ldd + col) = pack_bf16x2(f0, f1);
+        uint32_t wd[4];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const int col = cg + 8 * j + cq;
+          float f0 = acc[4 * (4 * k + j) + 2 * h] * sar[h] * s[j].x, f1 = acc[4 * (4 * k + j) + 2 * h + 1] * sar[h] * s[j].y;
+          if (p.bias && col < p.N) bias2(p.bias + col, f0, f1);
+          wd[j] = pack_bf16x2(f0, f1);
+        }
+        quad_transpose(wd, q);
+        const int row = row0 + 8 * h, col8 = cg + 8 * q;
+        if (row < p.M && col8 < p.N) st16(p.D + (int64_t)row * p.ldd + col8, make_uint4(wd[0], wd[1], wd[2], wd[3]));
       }
     }
   }
@@ -270,7 +280,9 @@ int gemm8(const char* who, const void* A, int64_t lda, const float* sa, const vo
                  (uintptr_t)D % 16 == 0 && (uintptr_t)sw % 8 == 0,
                  "%s: K and the e4m3 row strides must be multiples of 16, N and ldd of 8, pointers 16-byte aligned (TMA, 16-byte stores)", who);
   LMOD_CHECK_ARG((uintptr_t)bias % 4 == 0 && (!rope || ((uintptr_t)rope->cos % 4 == 0 && (uintptr_t)rope->sin % 4 == 0)),
-                 "%s: bias, cos and sin must be 4-byte aligned (the epilogue reads them two bf16 at a time)", who);
+                 "%s: bias, cos and sin must be 4-byte aligned (the epilogue reads bias two bf16 at a time)", who);
+  LMOD_CHECK_ARG(!rope || ((uintptr_t)rope->cos % 16 == 0 && (uintptr_t)rope->sin % 16 == 0 && rope->hd % 8 == 0),
+                 "%s: cos and sin must be 16-byte aligned and head_dim a multiple of 8 (the epilogue reads them 8 bf16 at a time)", who);
   Fp8Params p = {};
   p.D = (__nv_bfloat16*)D; p.ldd = ldd; p.bias = (const __nv_bfloat16*)bias; p.sa = sa; p.sw = sw;
   p.M = (int)M; p.N = (int)N; p.K = (int)K; p.swiglu_I = (int)swiglu_I;

@@ -136,7 +136,10 @@ def gemm(a, b, a_mn=False, b_mn=False, bias=None, out=None, accumulate=False, ou
 # length of FUSE_MIN_K on (the teacher's K = 4096); at the student's K = 1024 the element-wise kernels, which use every warp of the SM,
 # are preferred.  The (lighter) RoPE epilogue of the q|k|v projection is always fused.  LLAVAMOD_FUSE_SWIGLU: "auto" (by
 # reduction length), "1" always, "0" never; LLAVAMOD_FUSE_ROPE: "0" = GEMM + lmod_rope.  Measured again with asynchronous MMAs
-# (DESIGN.md section 4): "1" is within the step's run-to-run spread of "auto".
+# (DESIGN.md section 4): "1" is within the step's run-to-run spread of "auto".  Measured again once every fused epilogue stored 16-byte
+# blocks (DESIGN.md section 4; one H100 80GB HBM3 at 700 W, two alternating runs per arm, the same kernel outputs in every arm): the
+# defaults 14.14 samples/s (14.136-14.138), LLAVAMOD_FUSE_ROPE=0 14.11, LLAVAMOD_FUSE_SWIGLU=1 14.10, LLAVAMOD_FUSE_RESIDUAL=1 14.08 --
+# none beats the defaults, which stay.  The teacher's fused q|k|v + RoPE now takes about the time of GEMM + lmod_rope (0.331 / 0.323 ms).
 FUSE_SWIGLU = _os.environ.get("LLAVAMOD_FUSE_SWIGLU", "auto")
 FUSE_ROPE = _os.environ.get("LLAVAMOD_FUSE_ROPE", "auto")
 # residual add in the o_proj / down_proj (CLIP: out_proj / fc2) epilogue of no-grad forwards.  Bit-identical to the add inside the next norm's
