@@ -231,7 +231,7 @@ int lmod_adamw(float* master, float* m, float* v, const void* grad, int grad_is_
  *   a_mn_major / b_mn_major: 0 = operand stored K-major ([rows,K], "T"), 1 = stored MN-major ([K,rows], "N"), so that
  *   dgrad (B = W as stored) and wgrad (A = dY^T, B = X^T) need no transposed copies.
  *   epilogue bit0: D = bf16(D + acc).  bias [N] optional.  d_f32_accum != NULL: fp32 D32[M,ldd] += acc instead of D.
- *   epilogue bits 8..: split-K factor.  (The fused SwiGLU forms are lmod_gemm_swiglu / lmod_gemm_silu_bwd below.)
+ *   epilogue bits 8..: split-K factor.  (The fused SwiGLU forward is lmod_gemm_swiglu below.)
  * Grouped form = DeepSpeed Experts.forward on COMPACT rows (offsets from lmod_moe_route_scatter, 128-row aligned):
  *   mode 0 fwd  : D[rows_g,N] = A[rows_g,K] * B[g][N,K]^T     mode 1 dgrad: D[rows_g,N] = A[rows_g,K] * B[g][K,N]
  *   mode 2 wgrad: D[g][M,N] (+)= A[rows_g,M]^T * B[rows_g,N]
@@ -248,32 +248,21 @@ int lmod_gemm_bf16(const void* A, int64_t lda, int a_mn_major, const void* B, in
 int lmod_gemm_bf16_dyn(const void* A, int64_t lda, int a_mn_major, const void* B, int64_t ldb, int b_mn_major,
                        void* D, int64_t ldd, int64_t M, int64_t N, int64_t K, const void* bias, int epilogue,
                        float* d_f32_accum, const int32_t* m_rows_dev, const int32_t* k_rows_dev, void* stream);
-/* Fused SwiGLU MLP input (Qwen2MLP act_fn(gate_proj(x)) * up_proj(x), modeling_qwen2.py:199-200; DeepSpeed Experts.forward of the sparse
- * layers): ONE GEMM against the fused gate|up weight W_gu [2I, K] exactly as the checkpoint stores it (gate rows, then up rows; no
- * re-layout) whose epilogue applies SwiGLU: act[M, I] = bf16(bf16(silu(g)) * u), g / u = the bf16-rounded GEMM outputs (bit-identical to
- * lmod_gemm_bf16 + lmod_silu_mul_fwd).  h1 (optional, [M, 2I]) receives the pre-activations for the backward.  I %% 128 == 0.
- * Grouped form: compact expert rows, W_gu [G, 2I, K], offsets from lmod_moe_route_scatter (128-row aligned).
- * Backward: lmod_gemm_silu_bwd computes dh1[M, 2I] = silu_mul_bwd(dY W_dn, h1) in the epilogue of the down_proj dgrad GEMM
- * (dY [M, K], W_dn [K, I] as stored), so the [M, I] dact tensor is never written; grouped form W_dn [G, K, I]. */
-/* D[M,N] = bf16( bf16(A W^T + bias) + R ): a projection written straight into the residual stream -- o_proj / down_proj of
- * Qwen2DecoderLayer.forward (`hidden_states = residual + hidden_states`, modeling_qwen2.py:796,808) and out_proj / fc2 of the CLIP encoder
- * layers.  The GEMM output is rounded to bf16 before the add, as the reference materialises it: bit-identical to lmod_gemm_bf16 + lmod_add.
- * A [M,K], W [N,K] (both K-major), bias [N] or NULL, R [M,N] (row stride ld_r); D may alias R. */
-int lmod_gemm_residual(const void* A, int64_t lda, const void* W, int64_t ldb, const void* bias, const void* R, int64_t ld_r,
-                       void* D, int64_t ldd, int64_t M, int64_t N, int64_t K, void* stream);
 /* q|k|v projection with apply_rotary_pos_emb (modeling_qwen2.py:678-691,159-184) in the GEMM epilogue: D[M,(nh+2nkv)*hd] = A W^T + bias,
  * q and k heads rotated with cos/sin [max_pos, hd] (bf16) at position_ids[row], v untouched.  Bit-identical to lmod_gemm_bf16 followed by
  * lmod_rope (same bf16 roundings).  hd in {64,128}. */
 int lmod_gemm_qkv_rope(const void* A, int64_t lda, const void* W, int64_t ldb, const void* bias, void* D, int64_t ldd, int64_t M, int64_t K,
                        int nh, int nkv, int hd, const void* cos_table, const void* sin_table, const int64_t* position_ids, void* stream);
+/* Fused SwiGLU MLP input, forward only (Qwen2MLP act_fn(gate_proj(x)) * up_proj(x), modeling_qwen2.py:199-200; DeepSpeed Experts.forward
+ * of the sparse layers): ONE GEMM against the fused gate|up weight W_gu [2I, K] exactly as the checkpoint stores it (gate rows, then up
+ * rows; no re-layout) whose epilogue applies SwiGLU: act[M, I] = bf16(bf16(silu(g)) * u), g / u = the bf16-rounded GEMM outputs
+ * (bit-identical to lmod_gemm_bf16 + lmod_silu_mul_fwd).  I %% 128 == 0.  h1 must be NULL (ld_h1 is ignored): the pre-activations are
+ * not stored; a backward runs lmod_gemm_bf16 + lmod_silu_mul_fwd, which keeps them.
+ * Grouped form: compact expert rows, W_gu [G, 2I, K], offsets from lmod_moe_route_scatter (128-row aligned). */
 int lmod_gemm_swiglu(const void* A, int64_t lda, const void* W_gu, int64_t ldb, void* act, int64_t ld_act, void* h1, int64_t ld_h1,
                      int64_t M, int64_t I, int64_t K, void* stream);
 int lmod_grouped_gemm_swiglu(const void* A, int64_t lda, const void* W_gu, int64_t ldb, void* act, int64_t ld_act, void* h1, int64_t ld_h1,
                              const int32_t* offsets, int G, int64_t max_rows, int64_t I, int64_t K, void* stream);
-int lmod_gemm_silu_bwd(const void* dY, int64_t lda, const void* W_dn, int64_t ldb, const void* h1, int64_t ld_h1, void* dh1, int64_t ld_dh1,
-                       int64_t M, int64_t I, int64_t K, void* stream);
-int lmod_grouped_gemm_silu_bwd(const void* dY, int64_t lda, const void* W_dn, int64_t ldb, const void* h1, int64_t ld_h1, void* dh1,
-                               int64_t ld_dh1, const int32_t* offsets, int G, int64_t max_rows, int64_t I, int64_t K, void* stream);
 int lmod_grouped_gemm_bf16(const void* A, int64_t lda, const void* B, int64_t ldb, void* D, int64_t ldd,
                            const int32_t* offsets, int G, int64_t max_rows, int64_t M, int64_t N, int64_t K,
                            int mode, int epilogue, void* stream);

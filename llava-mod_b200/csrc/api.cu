@@ -25,6 +25,6 @@ int lmod_num_sms() {
 }
 
 extern "C" const char* lmod_last_error(void) { return g_err; }
-extern "C" int lmod_version(void) { return 100; }
+extern "C" int lmod_version(void) { return 101; }
 extern "C" int64_t lmod_launch_count(void) { return g_launches.load(); }
 extern "C" void lmod_launch_count_reset(void) { g_launches.store(0); }

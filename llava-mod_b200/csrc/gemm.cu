@@ -13,7 +13,6 @@
 //   mbarriers             : full[stage] (TMA complete_tx) / empty[stage] (one arrive per math warpgroup)
 // Operand "major-ness" is a template parameter, so dgrad (B = W as stored, MN-major) and wgrad (A = dY^T, B = X^T, both MN-major)
 // run without transposes: the wgmma transpose bits and descriptors and the TMA boxes change, the pipeline does not.
-#include <stdlib.h>
 #include "sm90.cuh"
 #include "gemm_epilogue.cuh"
 
@@ -42,17 +41,9 @@ struct GemmParams {
   int splits;                      // split-K factor (>1: fp32 atomic accumulation into D32)
   // fused SwiGLU forward (Qwen2MLP act_fn(gate_proj(x)) * up_proj(x), modeling_qwen2.py:199-200): B is the fused gate|up weight [2I, K]
   // as stored (gate rows, then up rows); N = I; an output tile = 128 act columns whose accumulator holds [128 gate | 128 up] columns (the
-  // two halves of the B stage are loaded from rows n0 and I + n0).  D[:, I] = bf16(bf16(silu(g)) * u); H1 (optional) keeps the bf16
-  // pre-activations [M, 2I] for the backward.
+  // two halves of the B stage are loaded from rows n0 and I + n0).  D[:, I] = bf16(bf16(silu(g)) * u).
   int swiglu;
   int swiglu_I;
-  __nv_bfloat16* H1;
-  int64_t ld_h1;
-  // fused SwiGLU backward in the epilogue of the down_proj dgrad (dact = dY W_dn, N = I): reads the saved pre-activations GU [M, 2I],
-  // writes d(gate) | d(up) into D [M, 2I] (columns col and I + col) -- the [M, I] dact tensor never exists
-  int silu_bwd;
-  const __nv_bfloat16* GU;
-  int64_t ld_gu;
   // fused rotary embedding in the epilogue of the q|k|v projection (apply_rotary_pos_emb, modeling_qwen2.py:159-184): columns below
   // rope_cols (the q and k heads) are rotated per head of rope_hd columns with cos / sin [max_pos, rope_hd] rows picked by rope_pos[row];
   // the v columns pass through.  Same bf16 roundings as GEMM(+bias) followed by lmod_rope (bit-identical).
@@ -60,11 +51,6 @@ struct GemmParams {
   const __nv_bfloat16* rope_sin;
   const int64_t* rope_pos;
   int rope_hd, rope_cols;
-  // fused residual add (Qwen2DecoderLayer `hidden_states = residual + hidden_states`, modeling_qwen2.py:796,808; CLIP encoder layers):
-  // D = bf16( bf16(acc + bias) + R ) -- the GEMM output is rounded to bf16 first, exactly as the reference materialises it before its add
-  const __nv_bfloat16* R;
-  int64_t ld_r;
-  int dbg_nostore;                 // timing experiments only (LMOD_GEMM_NOSTORE=1): the epilogue does not write D
   // grouped (experts): row ranges from `offsets` (device), B / D32 advance per group
   const int32_t* offsets;          // [groups+1] or null
   int groups;
@@ -237,38 +223,29 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_consta
     const int row0 = t.m0 + c * 64 + w * 16 + (lane >> 2);
     const int cq = 2 * (lane & 3), q = lane & 3;
     const int64_t goff = p.wgrad_grouped ? t.group * p.d_group_stride : 0;
-    if (p.dbg_nostore) continue;
     if (BN == 256 && p.swiglu) {
       // accumulator columns [0,128) = gate, [128,256) = up of the same 128 act columns (I % 128 == 0: all in range)
 #pragma unroll
       for (int k = 0; k < 4; ++k) {
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
-          uint32_t wg[4], wu[4], wa[4];
+          uint32_t wa[4];
 #pragma unroll
           for (int j = 0; j < 4; ++j) {
             const int i = 4 * k + j;
-            wg[j] = pack_bf16x2(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
-            wu[j] = pack_bf16x2(acc[4 * (i + 16) + 2 * h], acc[4 * (i + 16) + 2 * h + 1]);
-            wa[j] = swiglu2(wg[j], wu[j]);
+            wa[j] = swiglu2(pack_bf16x2(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]),
+                            pack_bf16x2(acc[4 * (i + 16) + 2 * h], acc[4 * (i + 16) + 2 * h + 1]));
           }
           quad_transpose(wa, q);
           const int row = row0 + 8 * h, col8 = t.n0 + 8 * (4 * k + q);
-          if (p.H1) { quad_transpose(wg, q); quad_transpose(wu, q); }
           if (row >= t.m_end) continue;
           st16(p.D + (int64_t)row * p.ldd + col8, make_uint4(wa[0], wa[1], wa[2], wa[3]));
-          if (p.H1) {
-            __nv_bfloat16* h1row = p.H1 + (int64_t)row * p.ld_h1;
-            st16(h1row + col8, make_uint4(wg[0], wg[1], wg[2], wg[3]));
-            st16(h1row + p.swiglu_I + col8, make_uint4(wu[0], wu[1], wu[2], wu[3]));
-          }
         }
       }
       continue;
     }
-    // plain (+bias), residual and SwiGLU-backward: x = bf16(acc + bias) traded across the quad, then the form's work on the 8 columns.
-    // Each form is its own straight-line pass over the groups (stores predicated, no branch between groups), so that the compiler can
-    // overlap the shuffles and loads of different groups.
+    // plain (+bias): x = bf16(acc + bias) traded across the quad, then stored 8 columns at a time.  A straight-line pass over the groups
+    // (stores predicated, no branch between groups), so that the compiler can overlap the shuffles and loads of different groups.
     auto bf16_groups = [&](auto&& finish) {
 #pragma unroll
       for (int k = 0; k < BN / 32; ++k) {
@@ -288,20 +265,6 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_consta
         }
       }
     };
-    if (p.silu_bwd) {
-      bf16_groups([&](const uint32_t (&wd)[4], int row, int col8) {
-        const __nv_bfloat16* gu = p.GU + (int64_t)row * p.ld_gu + col8;
-        __nv_bfloat16* d = p.D + (int64_t)row * p.ldd + col8;
-        silu_bwd_store8(wd, gu, gu + p.N, d, d + p.N);
-      });
-      continue;
-    }
-    if (p.R) {
-      bf16_groups([&](const uint32_t (&wd)[4], int row, int col8) {
-        residual_store8(wd, p.R + (int64_t)row * p.ld_r + col8, p.D + (int64_t)row * p.ldd + col8);
-      });
-      continue;
-    }
     if (!p.rope_cos && !p.D32 && !p.beta) {
       bf16_groups([&](const uint32_t (&wd)[4], int row, int col8) {
         st16(p.D + goff + (int64_t)row * p.ldd + col8, make_uint4(wd[0], wd[1], wd[2], wd[3]));
@@ -447,11 +410,10 @@ int pick_bn(int64_t m_tiles, int64_t N) {
 // epilogue bit 1: retired (the fused SwiGLU forward is lmod_gemm_swiglu);
 // epilogue bits 8..: split-K factor (fp32 atomic accumulation into D32, which the caller zero-initialises).
 struct RopeArgs { const void* cos; const void* sin; const int64_t* pos; int hd; int cols; };
-struct ResidArgs { const void* R; int64_t ld_r; };
 
 static int gemm_dense(const void* A, int64_t lda, int a_mn_major, const void* B, int64_t ldb, int b_mn_major, void* D, int64_t ldd,
                       int64_t M, int64_t N, int64_t K, const void* bias, int epilogue, float* d_f32_accum,
-                      const int32_t* m_rows_dev, const int32_t* k_rows_dev, void* stream, const RopeArgs* rope, const ResidArgs* resid = nullptr) {
+                      const int32_t* m_rows_dev, const int32_t* k_rows_dev, void* stream, const RopeArgs* rope) {
   LMOD_CHECK_ARG(A && B && (D || d_f32_accum) && M > 0 && N > 0 && K > 0, "lmod_gemm_bf16: null pointer or empty problem");
   LMOD_CHECK_ARG(lda % 8 == 0 && ldb % 8 == 0 && ldd % 8 == 0 && N % 8 == 0 && ((uintptr_t)A % 16 == 0) && ((uintptr_t)B % 16 == 0) &&
                  (!D || (uintptr_t)D % 16 == 0) && ((uintptr_t)d_f32_accum % 16 == 0),
@@ -474,10 +436,8 @@ static int gemm_dense(const void* A, int64_t lda, int a_mn_major, const void* B,
   GemmParams p = {};
   p.D = (__nv_bfloat16*)D; p.bias = (const __nv_bfloat16*)bias; p.D32 = d_f32_accum; p.ldd = ldd;
   p.M = (int)M; p.N = (int)N; p.K = (int)K; p.beta = epilogue & 1; p.offsets = nullptr; p.groups = 1; p.bn = BN;
-  p.dbg_nostore = getenv("LMOD_GEMM_NOSTORE") ? 1 : 0;
   p.splits = (epilogue >> 8) > 1 ? (epilogue >> 8) : 1;
   p.m_dev = m_rows_dev; p.k_dev = k_rows_dev;
-  if (resid) { p.R = (const __nv_bfloat16*)resid->R; p.ld_r = resid->ld_r; }
   if (rope) { p.rope_cos = (const __nv_bfloat16*)rope->cos; p.rope_sin = (const __nv_bfloat16*)rope->sin; p.rope_pos = rope->pos; p.rope_hd = rope->hd; p.rope_cols = rope->cols; }
   LMOD_CHECK_ARG(p.splits == 1 || d_f32_accum, "lmod_gemm_bf16: split-K needs the fp32 accumulate output");
   const int tiles = (int)(((M + BM - 1) / BM) * ((N + BN - 1) / BN)) * p.splits;
@@ -502,35 +462,26 @@ extern "C" int lmod_gemm_qkv_rope(const void* A, int64_t lda, const void* W, int
   return gemm_dense(A, lda, 0, W, ldb, 0, D, ldd, M, (int64_t)(nh + 2 * nkv) * hd, K, bias, 0, nullptr, nullptr, nullptr, stream, &r);
 }
 
-// D[M,N] = bf16( bf16(A W^T + bias) + R ): a projection whose output goes straight into the residual stream (o_proj / down_proj of
-// Qwen2DecoderLayer, modeling_qwen2.py:796,808; out_proj / fc2 of the CLIP encoder layers).  Bit-identical to lmod_gemm_bf16 followed by
-// lmod_add.  D may alias R (in-place update of the stream: every element is read and written by the same thread).
-extern "C" int lmod_gemm_residual(const void* A, int64_t lda, const void* W, int64_t ldb, const void* bias, const void* R, int64_t ld_r,
-                                  void* D, int64_t ldd, int64_t M, int64_t N, int64_t K, void* stream) {
-  LMOD_CHECK_ARG(R && D && ld_r % 8 == 0 && ((uintptr_t)R % 16 == 0), "lmod_gemm_residual: residual pointer / stride (16-byte rows)");
-  ResidArgs r = {R, ld_r};
-  return gemm_dense(A, lda, 0, W, ldb, 0, D, ldd, M, N, K, bias, 0, nullptr, nullptr, nullptr, stream, nullptr, &r);
-}
-
 extern "C" int lmod_gemm_bf16(const void* A, int64_t lda, int a_mn_major, const void* B, int64_t ldb, int b_mn_major, void* D, int64_t ldd,
                               int64_t M, int64_t N, int64_t K, const void* bias, int epilogue, float* d_f32_accum, void* stream) {
   return lmod_gemm_bf16_dyn(A, lda, a_mn_major, B, ldb, b_mn_major, D, ldd, M, N, K, bias, epilogue, d_f32_accum, nullptr, nullptr, stream);
 }
 
-// ---- fused SwiGLU forward / backward (Qwen2MLP, modeling_qwen2.py:199-200; DeepSpeed Experts of the sparse layers) ----------------------
-// act[M, I] = bf16(bf16(silu(A W_g^T)) * (A W_u^T)) with W_gu = [W_g ; W_u] stored [2I, K] exactly as the checkpoint holds it; h1 (optional,
-// [M, 2I]) receives the bf16 pre-activations for the backward.  I % 128 == 0.
-static int swiglu_common(const void* A, int64_t lda, const void* W, int64_t ldb, void* act, int64_t ld_act, void* h1, int64_t ld_h1,
+// ---- fused SwiGLU forward (Qwen2MLP, modeling_qwen2.py:199-200; DeepSpeed Experts of the sparse layers) ----------------------------------
+// act[M, I] = bf16(bf16(silu(A W_g^T)) * (A W_u^T)) with W_gu = [W_g ; W_u] stored [2I, K] exactly as the checkpoint holds it.  I % 128 == 0.
+// Forward only: h1 / ld_h1 are retired (h1 must be null); a training step runs GEMM + lmod_silu_mul_fwd, which keeps the pre-activations.
+static int swiglu_common(const void* A, int64_t lda, const void* W, int64_t ldb, void* act, int64_t ld_act, const void* h1,
                          const int32_t* offsets, int G, int64_t M, int64_t I, int64_t K, cudaStream_t st) {
+  LMOD_CHECK_ARG(!h1, "lmod_gemm_swiglu: h1 is retired -- the fused SwiGLU is forward-only (GEMM + lmod_silu_mul_fwd keeps the pre-activations)");
   LMOD_CHECK_ARG(A && W && act && M > 0 && I > 0 && K > 0, "lmod_gemm_swiglu: null pointer or empty problem");
   LMOD_CHECK_ARG(I % 128 == 0, "lmod_gemm_swiglu: intermediate size %lld is not a multiple of 128 (use GEMM + lmod_silu_mul_fwd)", (long long)I);
-  LMOD_CHECK_ARG(lda % 8 == 0 && ldb % 8 == 0 && ld_act % 8 == 0 && (!h1 || ld_h1 % 8 == 0) && ((uintptr_t)A % 16 == 0) && ((uintptr_t)W % 16 == 0) &&
-                 ((uintptr_t)act % 16 == 0) && (!h1 || (uintptr_t)h1 % 16 == 0), "lmod_gemm_swiglu: strides must be multiples of 8 elements, pointers 16-byte aligned");
+  LMOD_CHECK_ARG(lda % 8 == 0 && ldb % 8 == 0 && ld_act % 8 == 0 && ((uintptr_t)A % 16 == 0) && ((uintptr_t)W % 16 == 0) && ((uintptr_t)act % 16 == 0),
+                 "lmod_gemm_swiglu: strides must be multiples of 8 elements, pointers 16-byte aligned");
   CUtensorMap ta, tb;
   int rc;
   GemmParams p = {};
   p.D = (__nv_bfloat16*)act; p.ldd = ld_act; p.M = (int)M; p.N = (int)I; p.K = (int)K; p.splits = 1; p.groups = G > 0 ? G : 1;
-  p.swiglu = 1; p.swiglu_I = (int)I; p.H1 = (__nv_bfloat16*)h1; p.ld_h1 = ld_h1; p.bn = 128;     // tile enumeration: 128 act columns per tile
+  p.swiglu = 1; p.swiglu_I = (int)I; p.bn = 128;     // tile enumeration: 128 act columns per tile
   rc = make_map(&ta, A, (uint64_t)K, (uint64_t)M, (uint64_t)lda, BK, BM);
   if (rc) return rc;
   rc = make_map(&tb, W, (uint64_t)K, (uint64_t)((offsets ? G : 1) * 2 * I), (uint64_t)ldb, BK, 128);
@@ -547,53 +498,14 @@ static int swiglu_common(const void* A, int64_t lda, const void* W, int64_t ldb,
 
 extern "C" int lmod_gemm_swiglu(const void* A, int64_t lda, const void* W_gu, int64_t ldb, void* act, int64_t ld_act, void* h1, int64_t ld_h1,
                                 int64_t M, int64_t I, int64_t K, void* stream) {
-  return swiglu_common(A, lda, W_gu, ldb, act, ld_act, h1, ld_h1, nullptr, 0, M, I, K, (cudaStream_t)stream);
+  return swiglu_common(A, lda, W_gu, ldb, act, ld_act, h1, nullptr, 0, M, I, K, (cudaStream_t)stream);
 }
 
 // grouped form on compact expert rows: A [max_rows, K], W_gu [G, 2I, K], rows of group g = [offsets[g], offsets[g+1]) (128-aligned)
 extern "C" int lmod_grouped_gemm_swiglu(const void* A, int64_t lda, const void* W_gu, int64_t ldb, void* act, int64_t ld_act, void* h1,
                                         int64_t ld_h1, const int32_t* offsets, int G, int64_t max_rows, int64_t I, int64_t K, void* stream) {
   LMOD_CHECK_ARG(offsets && G >= 1 && G <= MAX_GROUPS, "lmod_grouped_gemm_swiglu: bad group arguments");
-  return swiglu_common(A, lda, W_gu, ldb, act, ld_act, h1, ld_h1, offsets, G, max_rows, I, K, (cudaStream_t)stream);
-}
-
-// backward of the fused MLP input: dh1[M, 2I] = silu_mul_bwd(dY W_dn, h1) computed in the epilogue of the dgrad GEMM dY [M, K=H] x W_dn [K, I]
-// (W_dn as stored: [H, I] = MN-major B).  Grouped form: W_dn [G, K, I].
-static int silu_bwd_common(const void* dY, int64_t lda, const void* W, int64_t ldb, const void* h1, int64_t ld_h1, void* dh1, int64_t ld_dh1,
-                           const int32_t* offsets, int G, int64_t M, int64_t I, int64_t K, cudaStream_t st) {
-  LMOD_CHECK_ARG(dY && W && h1 && dh1 && M > 0 && I > 0 && K > 0 && I % 8 == 0, "lmod_gemm_silu_bwd: bad arguments");
-  LMOD_CHECK_ARG(lda % 8 == 0 && ldb % 8 == 0 && ld_h1 % 8 == 0 && ld_dh1 % 8 == 0 && ((uintptr_t)dY % 16 == 0) && ((uintptr_t)W % 16 == 0) &&
-                 ((uintptr_t)h1 % 16 == 0) && ((uintptr_t)dh1 % 16 == 0), "lmod_gemm_silu_bwd: strides must be multiples of 8 elements, pointers 16-byte aligned");
-  CUtensorMap ta, tb;
-  int rc;
-  GemmParams p = {};
-  p.D = (__nv_bfloat16*)dh1; p.ldd = ld_dh1; p.M = (int)M; p.N = (int)I; p.K = (int)K; p.splits = 1; p.groups = G > 0 ? G : 1;
-  p.silu_bwd = 1; p.GU = (const __nv_bfloat16*)h1; p.ld_gu = ld_h1;
-  const int BN = pick_bn((M + BM - 1) / BM, I);
-  p.bn = BN;
-  rc = make_map(&ta, dY, (uint64_t)K, (uint64_t)M, (uint64_t)lda, BK, BM);
-  if (rc) return rc;
-  rc = make_map(&tb, W, (uint64_t)I, (uint64_t)((offsets ? G : 1) * K), (uint64_t)ldb, 64, BK);
-  if (rc) return rc;
-  int tiles;
-  if (offsets) {
-    p.offsets = offsets; p.b_group_rows = K;
-    tiles = (int)(((M + BM - 1) / BM + G) * ((I + BN - 1) / BN));
-  } else {
-    tiles = (int)(((M + BM - 1) / BM) * ((I + BN - 1) / BN));
-  }
-  return dispatch(false, true, ta, tb, p, tiles, st);
-}
-
-extern "C" int lmod_gemm_silu_bwd(const void* dY, int64_t lda, const void* W_dn, int64_t ldb, const void* h1, int64_t ld_h1, void* dh1,
-                                  int64_t ld_dh1, int64_t M, int64_t I, int64_t K, void* stream) {
-  return silu_bwd_common(dY, lda, W_dn, ldb, h1, ld_h1, dh1, ld_dh1, nullptr, 0, M, I, K, (cudaStream_t)stream);
-}
-
-extern "C" int lmod_grouped_gemm_silu_bwd(const void* dY, int64_t lda, const void* W_dn, int64_t ldb, const void* h1, int64_t ld_h1, void* dh1,
-                                          int64_t ld_dh1, const int32_t* offsets, int G, int64_t max_rows, int64_t I, int64_t K, void* stream) {
-  LMOD_CHECK_ARG(offsets && G >= 1 && G <= MAX_GROUPS, "lmod_grouped_gemm_silu_bwd: bad group arguments");
-  return silu_bwd_common(dY, lda, W_dn, ldb, h1, ld_h1, dh1, ld_dh1, offsets, G, max_rows, I, K, (cudaStream_t)stream);
+  return swiglu_common(A, lda, W_gu, ldb, act, ld_act, h1, offsets, G, max_rows, I, K, (cudaStream_t)stream);
 }
 
 // Grouped (per-expert) GEMM on rows [offsets[g], offsets[g+1]) (device array; boundaries must be multiples of 128 for mode 0/1, of 64 for

@@ -58,32 +58,6 @@ __device__ __forceinline__ uint32_t swiglu2(const uint32_t wg, const uint32_t wu
   const float g0 = bf16lo(wg), g1 = bf16hi(wg);
   return pack_bf16x2(bf16_round(g0 * sigmoid_f(g0)) * bf16lo(wu), bf16_round(g1 * sigmoid_f(g1)) * bf16hi(wu));
 }
-// d(gate), d(up) from dact (the fp32 accumulator rounded to bf16, as the unfused path materialises it) and the saved pre-activations gp / up:
-// the expression of silu_mul_bwd_kernel
-__device__ __forceinline__ void silu_bwd_store8(const uint32_t (&wd)[4], const __nv_bfloat16* gp, const __nv_bfloat16* up, __nv_bfloat16* dgp,
-                                                __nv_bfloat16* dup) {
-  float d[8], g[8], u[8], dg[8], du[8];
-  unpack8w(wd, d);
-  unpack8v(__ldg(reinterpret_cast<const uint4*>(gp)), g);
-  unpack8v(__ldg(reinterpret_cast<const uint4*>(up)), u);
-#pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    const float sg = sigmoid_f(g[j]);
-    du[j] = d[j] * g[j] * sg;
-    dg[j] = d[j] * u[j] * sg * (1.f + g[j] * (1.f - sg));
-  }
-  st16(dgp, pack8v(dg));
-  st16(dup, pack8v(du));
-}
-// D = bf16(x + r), x = bf16(acc + bias): the residual add (the expression of add_kernel)
-__device__ __forceinline__ void residual_store8(const uint32_t (&wx)[4], const __nv_bfloat16* r, __nv_bfloat16* d) {
-  float x[8], y[8];
-  unpack8w(wx, x);
-  unpack8v(__ldg(reinterpret_cast<const uint4*>(r)), y);
-#pragma unroll
-  for (int j = 0; j < 8; ++j) y[j] += x[j];
-  st16(d, pack8v(y));
-}
 // 4 x 4 transpose within each quad of lanes: lane q holds w[j] = word j of its own; afterwards w[j] = word q of lane j (the lane index
 // within the quad is q).  The sender picks the word its receiver needs, so no register is indexed dynamically.
 __device__ __forceinline__ uint32_t pick4(const uint32_t (&w)[4], int i) { return i == 0 ? w[0] : i == 1 ? w[1] : i == 2 ? w[2] : w[3]; }

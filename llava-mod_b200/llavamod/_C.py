@@ -65,10 +65,7 @@ SIGNATURES = {
     "lmod_gemm_qkv_rope": [_P, _L, _P, _L, _P, _P, _L, _L, _L, _I, _I, _I, _P, _P, _P, _P],
     "lmod_gemm_swiglu": [_P, _L, _P, _L, _P, _L, _P, _L, _L, _L, _L, _P],
     "lmod_grouped_gemm_swiglu": [_P, _L, _P, _L, _P, _L, _P, _L, _P, _I, _L, _L, _L, _P],
-    "lmod_gemm_silu_bwd": [_P, _L, _P, _L, _P, _L, _P, _L, _L, _L, _L, _P],
-    "lmod_grouped_gemm_silu_bwd": [_P, _L, _P, _L, _P, _L, _P, _L, _P, _I, _L, _L, _L, _P],
     "lmod_grouped_gemm_bf16": [_P, _L, _P, _L, _P, _L, _P, _I, _L, _L, _L, _L, _I, _I, _P],
-    "lmod_gemm_residual": [_P, _L, _P, _L, _P, _P, _L, _P, _L, _L, _L, _L, _P],
     "lmod_quant_rows_e4m3": [_P, _L, _P, _P, _L, _L, _P],
     "lmod_rmsnorm_quant_e4m3": [_P, _P, _P, _L, _L, _F, _P, _P, _P, _P],
     "lmod_gemm_e4m3": [_P, _L, _P, _P, _L, _P, _P, _P, _L, _L, _L, _L, _P],

@@ -132,123 +132,46 @@ def gemm(a, b, a_mn=False, b_mn=False, bias=None, out=None, accumulate=False, ou
     return out
 
 
-# Epilogue fusions pay off only when the GEMM's main loop is long enough to hide them: the fused SwiGLU forward is used from a reduction
-# length of FUSE_MIN_K on (the teacher's K = 4096); at the student's K = 1024 the element-wise kernels, which use every warp of the SM,
-# are preferred.  The (lighter) RoPE epilogue of the q|k|v projection is always fused.  LLAVAMOD_FUSE_SWIGLU: "auto" (by
-# reduction length), "1" always, "0" never; LLAVAMOD_FUSE_ROPE: "0" = GEMM + lmod_rope.  Measured again with asynchronous MMAs
-# (DESIGN.md section 4): "1" is within the step's run-to-run spread of "auto".  Measured again once every fused epilogue stored 16-byte
-# blocks (DESIGN.md section 4; one H100 80GB HBM3 at 700 W, two alternating runs per arm, the same kernel outputs in every arm): the
-# defaults 14.14 samples/s (14.136-14.138), LLAVAMOD_FUSE_ROPE=0 14.11, LLAVAMOD_FUSE_SWIGLU=1 14.10, LLAVAMOD_FUSE_RESIDUAL=1 14.08 --
-# none beats the defaults, which stay.  The teacher's fused q|k|v + RoPE now takes about the time of GEMM + lmod_rope (0.331 / 0.323 ms).
-FUSE_SWIGLU = _os.environ.get("LLAVAMOD_FUSE_SWIGLU", "auto")
-FUSE_ROPE = _os.environ.get("LLAVAMOD_FUSE_ROPE", "auto")
-# residual add in the o_proj / down_proj (CLIP: out_proj / fc2) epilogue of no-grad forwards.  Bit-identical to the add inside the next norm's
-# kernel; opt-in: the add is cheap inside the norm kernel, and the fused form measures within the step's spread (DESIGN.md section 4)
-FUSE_RESIDUAL = _os.environ.get("LLAVAMOD_FUSE_RESIDUAL", "0")
+# The fused SwiGLU forward pays off only when the GEMM's main loop is long enough to hide its epilogue: it is used from a reduction
+# length of FUSE_MIN_K on (the teacher's K = 4096); at the student's K = 1024 the element-wise kernel, which uses every warp of the SM,
+# is faster (DESIGN.md section 4).
 FUSE_MIN_K = 2048
 
 
-def _fuse(mode, K):
-    return mode == "1" or (mode == "auto" and K >= FUSE_MIN_K)
+def swiglu_fusable(I, K=None):
+    """The fused SwiGLU GEMM tiles the intermediate dimension by 128 (the reference's tiny test shapes with I = 320 take GEMM + silu_mul).
+    It is forward-only: a differentiated MLP keeps its pre-activations and runs GEMM + silu_mul."""
+    return I % 128 == 0 and (K is None or K >= FUSE_MIN_K)
 
 
-def swiglu_fusable(I, K=None, training=False):
-    """The fused SwiGLU GEMM tiles the intermediate dimension by 128 (the reference's tiny test shapes with I = 320 take GEMM + silu_mul);
-    training keeps the pre-activations, which makes the epilogue heavier still: fused only on request."""
-    if I % 128 != 0:
-        return False
-    if K is None:
-        return True
-    if training:
-        return FUSE_SWIGLU == "1"
-    return _fuse(FUSE_SWIGLU, K)
-
-
-def gemm_swiglu(x2, w_gu, save_h1):
-    """act[M,I] (, h1[M,2I]) = SwiGLU(x2 @ w_gu^T) in ONE GEMM (lmod_gemm_swiglu): w_gu is the fused gate|up weight [2I,H] as stored."""
+def gemm_swiglu(x2, w_gu):
+    """act[M,I] = SwiGLU(x2 @ w_gu^T) in ONE GEMM (lmod_gemm_swiglu): w_gu is the fused gate|up weight [2I,H] as stored."""
     _need_cuda(x2, w_gu)
     M, H = x2.shape
     I = w_gu.shape[0] // 2
     act = torch.empty(M, I, dtype=x2.dtype, device=x2.device)
-    h1 = torch.empty(M, 2 * I, dtype=x2.dtype, device=x2.device) if save_h1 else None
-    call("lmod_gemm_swiglu", ptr(x2), x2.stride(0), ptr(w_gu), w_gu.stride(0), ptr(act), I, ptr(h1), 2 * I, M, I, H)
-    return act, h1
+    call("lmod_gemm_swiglu", ptr(x2), x2.stride(0), ptr(w_gu), w_gu.stride(0), ptr(act), I, None, 0, M, I, H)
+    return act
 
 
-def gemm_silu_bwd(dy2, w_dn, h1):
-    """dh1[M,2I] = silu_mul_bwd(dy2 @ w_dn, h1) in the epilogue of the down_proj dgrad (lmod_gemm_silu_bwd); w_dn [H,I] as stored."""
-    M, H = dy2.shape
-    I = w_dn.shape[1]
-    dh1 = torch.empty(M, 2 * I, dtype=dy2.dtype, device=dy2.device)
-    call("lmod_gemm_silu_bwd", ptr(dy2), dy2.stride(0), ptr(w_dn), w_dn.stride(0), ptr(h1), h1.stride(0), ptr(dh1), 2 * I, M, I, H)
-    return dh1
-
-
-def grouped_gemm_swiglu(xp, w_gu, offsets, max_rows, save_h1):
-    """Experts' gate|up + SwiGLU on compact expert rows: w_gu [E,2I,H]; returns (act [R,I], h1 [R,2I] or None)."""
+def grouped_gemm_swiglu(xp, w_gu, offsets, max_rows):
+    """Experts' gate|up + SwiGLU on compact expert rows: w_gu [E,2I,H]; returns act [R,I]."""
     E, I2, H = w_gu.shape
     I = I2 // 2
     act = torch.empty(max_rows, I, dtype=xp.dtype, device=xp.device)
-    h1 = torch.empty(max_rows, I2, dtype=xp.dtype, device=xp.device) if save_h1 else None
-    call("lmod_grouped_gemm_swiglu", ptr(xp), xp.stride(0), ptr(w_gu), w_gu.stride(1), ptr(act), I, ptr(h1), I2, ptr(offsets), E, max_rows, I, H)
-    return act, h1
+    call("lmod_grouped_gemm_swiglu", ptr(xp), xp.stride(0), ptr(w_gu), w_gu.stride(1), ptr(act), I, None, 0, ptr(offsets), E, max_rows, I, H)
+    return act
 
 
-def grouped_gemm_silu_bwd(dy, w_dn, h1, offsets, max_rows):
-    """dh1 [R,2I] = silu_mul_bwd(dy @ w_dn[e], h1) per expert group; w_dn [E,H,I]."""
-    E, H, I = w_dn.shape
-    dh1 = torch.empty(max_rows, 2 * I, dtype=dy.dtype, device=dy.device)
-    call("lmod_grouped_gemm_silu_bwd", ptr(dy), dy.stride(0), ptr(w_dn), w_dn.stride(1), ptr(h1), h1.stride(0), ptr(dh1), 2 * I, ptr(offsets), E,
-         max_rows, I, H)
-    return dh1
-
-
-class MLPFn(Function):
-    """Qwen2MLP (modeling_qwen2.py:188-200) as two GEMMs: gate|up with the SwiGLU epilogue (pre-activations kept for the backward), then
-    down_proj.  Backward: the down_proj dgrad GEMM turns dY straight into d(gate)|d(up) in its epilogue; wgrads accumulate in place into
-    the flat gradient buffer views ``g_gu`` / ``g_dn`` (None = frozen)."""
-
-    @staticmethod
-    def forward(ctx, x, w_gu, w_dn, g_gu, g_dn):
-        x2 = _rows(x)
-        act, h1 = gemm_swiglu(x2, w_gu, True)
-        y = gemm(act, w_dn)
-        ctx.save_for_backward(x2, w_gu, w_dn, h1, act)
-        ctx.g = (g_gu, g_dn)
-        ctx.xshape = x.shape
-        return y.view(*x.shape[:-1], w_dn.shape[0])
-
-    @staticmethod
-    def backward(ctx, dy):
-        x2, w_gu, w_dn, h1, act = ctx.saved_tensors
-        g_gu, g_dn = ctx.g
-        dy2 = _c(dy).reshape(-1, dy.shape[-1])
-        dh1 = gemm_silu_bwd(dy2, w_dn, h1)
-        if g_dn is not None:
-            mm_tn_acc(dy2, act, g_dn)
-        dx = mm_nn(dh1, w_gu).reshape(ctx.xshape) if ctx.needs_input_grad[0] else None
-        if g_gu is not None:
-            mm_tn_acc(dh1, x2, g_gu)
-        return dx, None, None, None, None
-
-
-def mlp(x, w_gu, w_dn, g_gu=None, g_dn=None, res=None):
-    """Dense SwiGLU MLP.  Fused SwiGLU epilogues whenever the intermediate size allows; frozen / no-grad calls keep nothing.
-    res (no-grad calls only, see residual_fusable): the residual stream, added in the down_proj epilogue -- the return value is the new stream."""
+def mlp(x, w_gu, w_dn, g_gu=None, g_dn=None):
+    """Dense SwiGLU MLP.  No-grad calls take the fused SwiGLU epilogue where swiglu_fusable allows and keep nothing; differentiated
+    calls run GEMM + silu_mul, whose backward needs the pre-activations."""
     I = w_gu.shape[0] // 2
     grad = torch.is_grad_enabled() and (x.requires_grad or g_gu is not None or g_dn is not None)
-    assert res is None or not grad
-    if swiglu_fusable(I, w_gu.shape[1], training=grad):
-        if grad:
-            return MLPFn.apply(x, w_gu, w_dn, g_gu, g_dn)
-        act, _ = gemm_swiglu(_rows(x), w_gu, False)
-        if res is not None:
-            return gemm_residual(act, w_dn, None, res)
-        y = gemm(act, w_dn)
+    if not grad and swiglu_fusable(I, w_gu.shape[1]):
+        y = gemm(gemm_swiglu(_rows(x), w_gu), w_dn)
         return y if x.dim() == 2 else y.view(*x.shape[:-1], w_dn.shape[0])
     gu = linear(x, w_gu, None, g_gu, None)
-    if res is not None:
-        return gemm_residual(silu_mul(gu), w_dn, None, res)
     return linear(silu_mul(gu), w_dn, None, g_dn, None)
 
 
@@ -299,28 +222,6 @@ def linear(x, w, bias=None, wgrad=None, bgrad=None):
     if torch.is_grad_enabled() and (x.requires_grad or wgrad is not None):
         return LinearFn.apply(x, w, bias, wgrad, bgrad)
     return mm_nt(x, w, bias)
-
-
-def residual_fusable(x, res, *grads):
-    """The projection's epilogue may add the residual stream itself when nothing of the call is differentiated (frozen teacher, CLIP tower,
-    eval): the trainable students keep the add inside the next norm's kernel, whose backward needs the un-added branch anyway."""
-    if FUSE_RESIDUAL != "1" or res is None:
-        return False
-    if not torch.is_grad_enabled():
-        return True
-    return not (x.requires_grad or res.requires_grad or any(g is not None for g in grads))
-
-
-def gemm_residual(x, w, bias, res, inplace=False):
-    """bf16( bf16(x @ w^T + bias) + res ) in one GEMM (lmod_gemm_residual): the output IS the new residual stream (inplace: written over res)."""
-    _need_cuda(x, w, res)
-    x2, r2 = _rows(x), _rows(res)
-    M, Kd = x2.shape
-    N = w.shape[0]
-    out = r2 if inplace else torch.empty(M, N, dtype=x2.dtype, device=x2.device)
-    call("lmod_gemm_residual", ptr(x2), x2.stride(0), ptr(w), w.stride(0), ptr(bias) if bias is not None else None, ptr(r2), r2.stride(0),
-         ptr(out), out.stride(0), M, N, Kd)
-    return out if res.dim() == 2 else out.view(res.shape)
 
 
 # ---------------------------------------------------------------------------------------------------
@@ -378,7 +279,7 @@ def gemm_fp8(a, w, bias=None):
 
 def qkv_rope_fp8(a, w, bias, cos, sin, pos, nh, nkv, hd):
     """K.qkv_rope of a frozen FP8 layer: a = the quantised normalised rows (rmsnorm_quant), w = the quantised fused q|k|v weight."""
-    if hd not in ATTN_HEAD_DIMS or FUSE_ROPE == "0":
+    if hd not in ATTN_HEAD_DIMS:
         return rope_(gemm_fp8(a, w, bias), cos, sin, pos, nh, nkv, hd)
     M, Kd = a.shape
     out = torch.empty(M, w.shape[0], dtype=BF16, device=a.q.device)
@@ -787,7 +688,7 @@ class QKVRopeFn(Function):
 
 def qkv_rope(x, w, bias, cos, sin, pos, nh, nkv, hd, wgrad=None, bgrad=None):
     """Fused q|k|v projection + RoPE for the head dims the epilogue is built for; other head dims (tiny test shapes) take GEMM + lmod_rope."""
-    if hd not in ATTN_HEAD_DIMS or FUSE_ROPE == "0":
+    if hd not in ATTN_HEAD_DIMS:
         return rope_(linear(x, w, bias, wgrad, bgrad), cos, sin, pos, nh, nkv, hd)
     if torch.is_grad_enabled() and (x.requires_grad or wgrad is not None):
         return QKVRopeFn.apply(x, w, bias, cos, sin, pos, nh, nkv, hd, wgrad, bgrad)
@@ -994,30 +895,27 @@ def moe_gather_combine(y, row, w, residual=None):
     return out
 
 
-def moe_forward_stages(x, res, wg, w_gu, w_dn, noise, cf, min_cap, fused, k=2):
-    """The MoE forward as MoEFn runs it, returning every intermediate (the router's record, xp, h1, act, y, out).  fused: SwiGLU in the
-    grouped GEMM's epilogue instead of GEMM + silu_mul (bit-identical).  k: routing width (1: noise is the uniform of top-1's selection)."""
+def moe_forward_stages(x, res, wg, w_gu, w_dn, noise, cf, min_cap, k=2):
+    """The MoE forward as MoEFn runs it, returning every intermediate (the router's record, xp, h1, act, y, out).  k: routing width (1: noise
+    is the uniform of top-1's selection)."""
     E, I2, H = w_gu.shape
     r = moe_route_scatter(x, wg, noise, cf, min_cap, LAYOUT_ALIGNED, k=k)
     R = r["max_rows"]
     xp, offs = r["xp"], r["offsets"]
     # only xp (and dy in the backward) are zero-filled: in the 128-aligned layout the grouped GEMM writes EVERY row below offsets[E],
     # so the padding rows of h1 / act / y come out as exact zeros (0 @ W); rows past offsets[E] are never read by a GEMM
-    if fused:
-        act, h1 = grouped_gemm_swiglu(xp, w_gu, offs, R, True)         # act [R,I], pre-activations [R,2I]: SwiGLU in the GEMM epilogue
-    else:
-        h1 = torch.empty(R, I2, dtype=x.dtype, device=x.device)
-        grouped_gemm(xp, w_gu, h1, offs, 0)                            # [R,2I] = xp @ w_gu[e]^T
-        act = silu_mul(h1)                                             # [R,I]
+    h1 = torch.empty(R, I2, dtype=x.dtype, device=x.device)
+    grouped_gemm(xp, w_gu, h1, offs, 0)                                # [R,2I] = xp @ w_gu[e]^T
+    act = silu_mul(h1)                                                 # [R,I]
     y = torch.empty(R, H, dtype=x.dtype, device=x.device)
     grouped_gemm(act, w_dn, y, offs, 0)                                # [R,H] = act @ w_dn[e]^T
-    r.update(h1=h1, act=act, y=y, out=moe_gather_combine(y, r["row"], r["w"], res), fused=fused)
+    r.update(h1=h1, act=act, y=y, out=moe_gather_combine(y, r["row"], r["w"], res))
     return r
 
 
 def moe_backward_stages(st, x, wg, w_gu, w_dn, dout, dlaux, grads, dres=None):
-    """The MoE backward as MoEFn runs it, from moe_forward_stages' record; returns every intermediate (dy, dw, dact on the unfused
-    path, dh1, dxp, dlogits, dx).  Weight gradients accumulate in place into grads['wg'|'w_gu'|'w_dn'] (None or a missing key = frozen).
+    """The MoE backward as MoEFn runs it, from moe_forward_stages' record; returns every intermediate (dy, dw, dact, dh1, dxp, dlogits,
+    dx).  Weight gradients accumulate in place into grads['wg'|'w_gu'|'w_dn'] (None or a missing key = frozen).
     dres: another addend of dx [S,H], summed in the scatter-backward kernel."""
     E, I2, H = w_gu.shape
     xp, h1, act, y, row, w, gates, idx, meta, offs = (st[k] for k in ("xp", "h1", "act", "y", "row", "w", "gates", "idx", "meta", "offsets"))
@@ -1027,14 +925,10 @@ def moe_backward_stages(st, x, wg, w_gu, w_dn, dout, dlaux, grads, dres=None):
     dw = torch.empty(S, 2, dtype=torch.float32, device=dout.device)
     call("lmod_moe_combine_bwd", ptr(dout), ptr(y), ptr(row), ptr(w), S, H, ptr(dy), ptr(dw))
     g = grads
-    out = dict(dy=dy, dw=dw, dact=None)
-    if st["fused"]:
-        dh1 = grouped_gemm_silu_bwd(dy, w_dn, h1, offs, R)             # d(gate)|d(up) straight from the dgrad GEMM's epilogue
-    else:
-        dact = torch.empty(R, I2 // 2, dtype=dout.dtype, device=dout.device)
-        grouped_gemm(dy, w_dn, dact, offs, 1)                          # dact = dy @ w_dn[e]
-        dh1 = silu_mul_bwd(dact, h1)
-        out["dact"] = dact
+    dact = torch.empty(R, I2 // 2, dtype=dout.dtype, device=dout.device)
+    grouped_gemm(dy, w_dn, dact, offs, 1)                              # dact = dy @ w_dn[e]
+    dh1 = silu_mul_bwd(dact, h1)
+    out = dict(dy=dy, dw=dw, dact=dact)
     if g is not None and g.get("w_dn") is not None:
         grouped_gemm(dy, act, g["w_dn"], offs, 2, accumulate=True)      # dW_dn[e] += dy_e^T @ act_e
     dxp = torch.empty(R, H, dtype=dout.dtype, device=dout.device)
@@ -1065,10 +959,8 @@ class MoEFn(Function):
     def forward(ctx, x, res, wg, w_gu, w_dn, noise, cf, min_cap, grads, k=2):
         x = _c(x)
         res = _c(res)
-        E, I2, H = w_gu.shape
-        st = moe_forward_stages(x, res, wg, w_gu, w_dn, noise, cf, min_cap, swiglu_fusable(I2 // 2, H, training=True), k)
+        st = moe_forward_stages(x, res, wg, w_gu, w_dn, noise, cf, min_cap, k)
         ctx.save_for_backward(x, wg, w_gu, w_dn, *(st[n] for n in _MOE_SAVED))
-        ctx.fused = st["fused"]
         ctx.k = k
         ctx.grads = grads
         return st["out"], st["meta"][0].clone()
@@ -1076,7 +968,7 @@ class MoEFn(Function):
     @staticmethod
     def backward(ctx, dout, dlaux):
         x, wg, w_gu, w_dn, *saved = ctx.saved_tensors
-        st = dict(zip(_MOE_SAVED, saved), fused=ctx.fused, k=ctx.k)
+        st = dict(zip(_MOE_SAVED, saved), k=ctx.k)
         dx = moe_backward_stages(st, x, wg, w_gu, w_dn, _c(dout), dlaux, ctx.grads)["dx"]
         return dx, dout, None, None, None, None, None, None, None, None
 
@@ -1089,7 +981,7 @@ def moe_forward_nograd(x, res, wg, w_gu, w_dn, noise, cf, min_cap, k=2):
     r = moe_route_scatter(_c(x), wg, noise, cf, min_cap, LAYOUT_ALIGNED, k=k)
     R = r["max_rows"]
     if swiglu_fusable(I2 // 2, H):
-        act, _ = grouped_gemm_swiglu(r["xp"], w_gu, r["offsets"], R, False)
+        act = grouped_gemm_swiglu(r["xp"], w_gu, r["offsets"], R)
     else:
         h1 = torch.empty(R, I2, dtype=x.dtype, device=x.device)
         grouped_gemm(r["xp"], w_gu, h1, r["offsets"], 0)
@@ -1127,15 +1019,12 @@ def moe_residual_mix_bwd(g, x, moe, mlp_out, coef, wc, dwc=None, dbc=None):
     return d
 
 
-def moe_residual_forward_stages(x, res, wg, w_gu, w_dn, noise, cf, min_cap, r_gu, r_dn, wc, bc, fused, k=2):
+def moe_residual_forward_stages(x, res, wg, w_gu, w_dn, noise, cf, min_cap, r_gu, r_dn, wc, bc, k=2):
     """The Residual-MoE forward as ResidualMoEFn runs it: moe_forward_stages with no residual (its 'out' is kept as 'moe'), the dense
     SwiGLU MLP (r_gu [2I,H], r_dn [H,I]; pre-activations kept) and the mix.  Returns every intermediate; 'out' is the new stream."""
-    st = moe_forward_stages(x, None, wg, w_gu, w_dn, noise, cf, min_cap, fused, k)
-    if fused:
-        m_act, m_h1 = gemm_swiglu(x, r_gu, True)
-    else:
-        m_h1 = gemm(x, r_gu)
-        m_act = silu_mul(m_h1)
+    st = moe_forward_stages(x, None, wg, w_gu, w_dn, noise, cf, min_cap, k)
+    m_h1 = gemm(x, r_gu)
+    m_act = silu_mul(m_h1)
     m_y = gemm(m_act, r_dn)
     out, coef = moe_residual_mix(x, st["out"], m_y, res, wc, bc)
     st.update(moe=st["out"], mlp_h1=m_h1, mlp_act=m_act, mlp=m_y, coef=coef, out=out)
@@ -1149,10 +1038,7 @@ def moe_residual_backward_stages(st, x, wg, w_gu, w_dn, r_gu, r_dn, wc, dout, dl
     g = grads or {}
     mix = moe_residual_mix_bwd(dout, x, st["moe"], st["mlp"], st["coef"], wc, g.get("wc"), g.get("bc"))
     d_mlp = mix["d_mlp"]
-    if st["fused"]:
-        m_dh1 = gemm_silu_bwd(d_mlp, r_dn, st["mlp_h1"])
-    else:
-        m_dh1 = silu_mul_bwd(mm_nn(d_mlp, r_dn), st["mlp_h1"])
+    m_dh1 = silu_mul_bwd(mm_nn(d_mlp, r_dn), st["mlp_h1"])
     if g.get("r_dn") is not None:
         mm_tn_acc(d_mlp, st["mlp_act"], g["r_dn"])
     dres = mix["dx"]
@@ -1172,11 +1058,8 @@ class ResidualMoEFn(Function):
     def forward(ctx, x, res, wg, w_gu, w_dn, noise, cf, min_cap, r_gu, r_dn, wc, bc, grads, k=2):
         x = _c(x)
         res = _c(res)
-        E, I2, H = w_gu.shape
-        st = moe_residual_forward_stages(x, res, wg, w_gu, w_dn, noise, cf, min_cap, r_gu, r_dn, wc, bc,
-                                         swiglu_fusable(I2 // 2, H, training=True), k)
+        st = moe_residual_forward_stages(x, res, wg, w_gu, w_dn, noise, cf, min_cap, r_gu, r_dn, wc, bc, k)
         ctx.save_for_backward(x, wg, w_gu, w_dn, r_gu, r_dn, wc, *(st[n] for n in _MOE_SAVED + _RES_SAVED))
-        ctx.fused = st["fused"]
         ctx.k = k
         ctx.grads = grads
         return st["out"], st["meta"][0].clone()
@@ -1184,7 +1067,7 @@ class ResidualMoEFn(Function):
     @staticmethod
     def backward(ctx, dout, dlaux):
         x, wg, w_gu, w_dn, r_gu, r_dn, wc, *saved = ctx.saved_tensors
-        st = dict(zip(_MOE_SAVED + _RES_SAVED, saved), fused=ctx.fused, k=ctx.k)
+        st = dict(zip(_MOE_SAVED + _RES_SAVED, saved), k=ctx.k)
         dx = moe_residual_backward_stages(st, x, wg, w_gu, w_dn, r_gu, r_dn, wc, _c(dout), dlaux, ctx.grads)["dx"]
         return (dx, dout) + (None,) * 12
 

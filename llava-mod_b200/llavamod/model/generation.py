@@ -95,8 +95,7 @@ def _decoder_entry(model, B, max_len, T=1):
                 for l in model.model.layers if hasattr(l.mlp, "deepspeed_moe"))
     fp8 = tuple(t.data_ptr() for l in model.model.layers if isinstance(l.self_attn.qkv_weight, K.Fp8Rows)
                 for w in (l.self_attn.qkv_weight, l.self_attn.o_fp8, l.mlp.gu_weight, l.mlp.down_fp8) for t in (w.q, w.scale))
-    key = (id(model), B, max_len, T, model.training, moe, K.FUSE_SWIGLU, K.FUSE_ROPE, K.FUSE_RESIDUAL,
-           tuple(p.data_ptr() for p in model.parameters()), fp8)
+    key = (id(model), B, max_len, T, model.training, moe, tuple(p.data_ptr() for p in model.parameters()), fp8)
     ent = _STEP_GRAPHS.pop(key, None)
     if ent is None or ent["model"]() is not model:
         ent = dict(model=weakref.ref(model), cache=model.new_kv_cache(B, max_len), graph=None)

@@ -379,13 +379,9 @@ class Qwen2Model(nn.Module):
             elif cache is not None:
                 K.kv_append(qkv, B, T, nh, nkv, hd, cache.k[li], cache.v[li], cache.len)
             attn = K.attention(qkv, B, T, nh, nkv, hd, True, None, pad)
-            if fp8:                                     # the add stays in the norm's kernel (the same bytes as the fused epilogue)
+            if fp8:
                 branch = K.linear_fp8(attn, at.o_fp8)
                 x, stream = K.rmsnorm_quant(branch, layer.post_attention_layernorm.weight, cfg.rms_norm_eps, res=stream)
-            elif K.residual_fusable(attn, stream, self.gview(at.o_proj.weight), self.gview(layer.post_attention_layernorm.weight)):
-                # frozen / no-grad forward: o_proj's epilogue writes residual + branch (modeling_qwen2.py:796), the norm reads one tensor
-                stream = K.gemm_residual(attn, at.o_proj.weight, None, stream)
-                x, stream = K.rmsnorm(stream, layer.post_attention_layernorm.weight, cfg.rms_norm_eps)
             else:
                 branch = K.linear(attn, at.o_proj.weight, None, self.gview(at.o_proj.weight), None)
                 x, stream = K.rmsnorm(branch, layer.post_attention_layernorm.weight, cfg.rms_norm_eps, res=stream,
@@ -403,9 +399,6 @@ class Qwen2Model(nn.Module):
                 branch = None
             elif fp8:
                 branch = K.mlp_fp8(x, mlp.gu_weight, mlp.down_fp8)
-            elif K.residual_fusable(x, stream, self.gview(mlp.gu_weight), self.gview(mlp.down_proj.weight)):
-                stream = K.mlp(x, mlp.gu_weight, mlp.down_proj.weight, res=stream)      # down_proj epilogue adds the stream (:808)
-                branch = None
             else:
                 branch = K.mlp(x, mlp.gu_weight, mlp.down_proj.weight, self.gview(mlp.gu_weight), self.gview(mlp.down_proj.weight))
         if branch is None:
@@ -431,8 +424,8 @@ class Qwen2Model(nn.Module):
         Everything the step reads about the position is on the device, so the step can be captured once and replayed.  MoE layers route
         the B new tokens alone (top2gating / top1gating with S = B, as MoEQwen1_5Model_forward does with a cache,
         llava_qwen1_5_moe.py:223-236).
-        The layer body is forward's no-grad layer body with the attention swapped for append + decode attention: the same norm and
-        residual-fusion choices, the same MoE call and final norm.  A change to one loop must be made to the other;
+        The layer body is forward's no-grad layer body with the attention swapped for append + decode attention: the same norm
+        choices, the same MoE call and final norm.  A change to one loop must be made to the other;
         tests/test_decode_gpu.py checks that the two give the same K / V, bit for bit."""
         cfg = self.config
         B, T, H = inputs_embeds.shape
@@ -472,9 +465,6 @@ class Qwen2Model(nn.Module):
             if fp8:
                 branch = K.linear_fp8(attn, at.o_fp8)
                 x, stream = K.rmsnorm_quant(branch, layer.post_attention_layernorm.weight, cfg.rms_norm_eps, res=stream)
-            elif K.residual_fusable(attn, stream):
-                stream = K.gemm_residual(attn, at.o_proj.weight, None, stream)
-                x, stream = K.rmsnorm(stream, layer.post_attention_layernorm.weight, cfg.rms_norm_eps)
             else:
                 branch = K.linear(attn, at.o_proj.weight)
                 x, stream = K.rmsnorm(branch, layer.post_attention_layernorm.weight, cfg.rms_norm_eps, res=stream)
@@ -490,9 +480,6 @@ class Qwen2Model(nn.Module):
                 branch = None
             elif fp8:
                 branch = K.mlp_fp8(x, mlp.gu_weight, mlp.down_fp8)
-            elif K.residual_fusable(x, stream):
-                stream = K.mlp(x, mlp.gu_weight, mlp.down_proj.weight, res=stream)
-                branch = None
             else:
                 branch = K.mlp(x, mlp.gu_weight, mlp.down_proj.weight)
         if branch is None:

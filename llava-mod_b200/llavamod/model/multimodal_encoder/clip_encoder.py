@@ -162,25 +162,18 @@ class CLIPVisionModel(nn.Module):
         h = K.layernorm(seq.view(n * T, H), vm.pre_layrnorm.weight, vm.pre_layrnorm.bias, c.layer_norm_eps)
         n_run = c.num_hidden_layers + 1 + select_layer if select_layer < 0 else select_layer
         hd = H // nh
-        fuse = K.FUSE_RESIDUAL == "1"                   # frozen tower: the residual adds ride in the out_proj / fc2 epilogues
         for layer in vm.encoder.layers[:n_run]:
             a = layer.self_attn
             y = K.layernorm(h, layer.layer_norm1.weight, layer.layer_norm1.bias, c.layer_norm_eps)
             qkv = K.mm_nt(y, a.qkv_weight, a.qkv_bias)
             o = K.attention(qkv, n, T, nh, nh, hd, causal=False, scale=hd ** -0.5)
-            if fuse:
-                K.gemm_residual(o, a.out_proj.weight, a.out_proj.bias, h, inplace=True)      # h += out_proj(o) in the GEMM epilogue
-            else:
-                o = K.mm_nt(o, a.out_proj.weight, a.out_proj.bias)
-                K.call("lmod_add", K.ptr(h), K.ptr(o), h.numel(), K.ptr(h))
+            o = K.mm_nt(o, a.out_proj.weight, a.out_proj.bias)
+            K.call("lmod_add", K.ptr(h), K.ptr(o), h.numel(), K.ptr(h))
             y = K.layernorm(h, layer.layer_norm2.weight, layer.layer_norm2.bias, c.layer_norm_eps)
             f = K.mm_nt(y, layer.mlp.fc1.weight)
             f = K.bias_act(f, layer.mlp.fc1.bias, K.ACT_QUICK_GELU)
-            if fuse:
-                K.gemm_residual(f, layer.mlp.fc2.weight, layer.mlp.fc2.bias, h, inplace=True)
-            else:
-                f = K.mm_nt(f, layer.mlp.fc2.weight, layer.mlp.fc2.bias)
-                K.call("lmod_add", K.ptr(h), K.ptr(f), h.numel(), K.ptr(h))
+            f = K.mm_nt(f, layer.mlp.fc2.weight, layer.mlp.fc2.bias)
+            K.call("lmod_add", K.ptr(h), K.ptr(f), h.numel(), K.ptr(h))
         return h.view(n, T, H)
 
 

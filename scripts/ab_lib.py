@@ -2,7 +2,7 @@
 """A/B two or more prebuilt kernel libraries in one process tree on one GPU.
 
     python scripts/ab_lib.py --arm parent=ab_libs/parent.so --arm branch=ab_libs/branch.so \
-        [--arm fuse1=ab_libs/branch.so,LLAVAMOD_FUSE_SWIGLU=1 ...] [--runs 3] [--detail parent,branch [--reports] [--full]] --out DIR
+        [--runs 3] [--detail parent,branch [--reports] [--full]] --out DIR
 
 An arm is NAME=LIB[,VAR=VALUE...]: the library is copied over llavamod/liblmod_b200.so while the arm runs (the original is put back at
 the end), and the variables are set in the arm's child processes.  Build each library beforehand with llava-mod_b200/build_ext.py from
@@ -100,16 +100,13 @@ def dump_kernels(out_dir):
     ang = torch.cat([ang, ang], 1)
     cos, sin = ang.cos().to(torch.bfloat16), ang.sin().to(torch.bfloat16)
     w_o, w_gu, w_dn = rnd(H, H, scale=H ** -0.5), rnd(2 * I, H, scale=H ** -0.5), rnd(H, I, scale=I ** -0.5)
-    res, act = rnd(M, H), rnd(M, I)
-    dy, h1 = rnd(M, H), rnd(M, 2 * I)
+    act, dy = rnd(M, I), rnd(M, H)
     with torch.no_grad():
         case("teacher_plain_MxNxK_2048x4096x4096", lambda: K.gemm(x, w_o), mm=lambda: torch.mm(x, w_o.t()))
         case("teacher_bias_2048x12288x4096", lambda: K.gemm(x, w_qkv, bias=b_qkv), mm=lambda: torch.mm(x, w_qkv.t()))
         case("teacher_qkv_rope_2048x12288x4096", lambda: K.qkv_rope(x, w_qkv, b_qkv, cos, sin, pos, nh, nh, hd))
-        case("teacher_swiglu_2048x22016x4096", lambda: K.gemm_swiglu(x, w_gu, True), mm=lambda: torch.mm(x, w_gu.t()))
-        case("teacher_residual_2048x4096x11008", lambda: K.gemm_residual(act, w_dn, None, res))
+        case("teacher_swiglu_2048x22016x4096", lambda: K.gemm_swiglu(x, w_gu), mm=lambda: torch.mm(x, w_gu.t()))
         case("teacher_down_2048x4096x11008", lambda: K.gemm(act, w_dn), mm=lambda: torch.mm(act, w_dn.t()))
-        case("teacher_silu_bwd_2048x11008x4096", lambda: K.gemm_silu_bwd(dy, w_dn, h1), mm=lambda: torch.mm(dy, w_dn))
         case("teacher_dgrad_2048x4096x4096", lambda: K.mm_nn(dy, w_o), mm=lambda: torch.mm(dy, w_o))
         case("teacher_wgrad_4096x4096x2048", lambda: K.gemm(dy, x, a_mn=True, b_mn=True), mm=lambda: torch.mm(dy.t(), x))
         # a ragged M: an odd number of 128-row tiles, the last one partial
@@ -130,7 +127,7 @@ def dump_kernels(out_dir):
         dys = rnd(M, 3 * Hs)
         case("student_plain_2048x3072x1024", lambda: K.gemm(xs, w_s), mm=lambda: torch.mm(xs, w_s.t()))
         case("student_plain_2048x1024x1024", lambda: K.gemm(xs, w_s[:Hs]), mm=lambda: torch.mm(xs, w_s[:Hs].t()))
-        case("student_swiglu_2048x5632x1024", lambda: K.gemm_swiglu(xs, w_gus, True), mm=lambda: torch.mm(xs, w_gus.t()))
+        case("student_swiglu_2048x5632x1024", lambda: K.gemm_swiglu(xs, w_gus), mm=lambda: torch.mm(xs, w_gus.t()))
         case("student_wgrad_3072x1024x2048", lambda: K.gemm(dys, xs, a_mn=True, b_mn=True), mm=lambda: torch.mm(dys.t(), xs))
         w_lm = rnd(151936, Hs, scale=0.02)
         case("student_lm_head_2048x151936x1024", lambda: K.gemm(xs, w_lm), dump=False,    # timed only: a 622 MB output
@@ -146,7 +143,7 @@ def dump_kernels(out_dir):
         case("grouped_wgrad_4x1024x2816", lambda: K.grouped_gemm(dye, acte, torch.zeros(E, Hs, Is, device=dev, dtype=torch.bfloat16), offsets, 2))
         dwe = torch.zeros(E, Hs, Is, device=dev, dtype=torch.bfloat16)
         case("grouped_wgrad_accumulate_4x1024x2816", lambda: K.grouped_gemm(dye, acte, dwe, offsets, 2, accumulate=True), dump=False)
-        case("grouped_swiglu_4x5632x1024", lambda: K.grouped_gemm_swiglu(xe, w_gue, offsets, R, True))
+        case("grouped_swiglu_4x5632x1024", lambda: K.grouped_gemm_swiglu(xe, w_gue, offsets, R))
         # attention forward: teacher heads (hd 128) and student heads (hd 64), causal; a padded batch of two
         for hdx, nhx in ((128, 32), (64, 16)):
             qkv = rnd(M, 3 * nhx * hdx)

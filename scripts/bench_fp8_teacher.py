@@ -70,7 +70,7 @@ def gemm_rows(iters):
             f16 = lambda: K.qkv_rope(x, w, bias, cos, sin, pos, nh, nkv, hd)          # noqa: E731
             f8 = lambda: K.qkv_rope_fp8(xq, wq, bias, cos, sin, pos, nh, nkv, hd)      # noqa: E731
         elif form == "swiglu":
-            f16 = lambda: K.gemm_swiglu(x, w, False)                                   # noqa: E731
+            f16 = lambda: K.gemm_swiglu(x, w)                                          # noqa: E731
             act = torch.empty(M, N // 2, dtype=torch.bfloat16, device="cuda")
             f8 = lambda: K.call("lmod_gemm_e4m3_swiglu", K.ptr(xq.q), Kd, K.ptr(xq.scale), K.ptr(wq.q), Kd, K.ptr(wq.scale), K.ptr(act), N // 2, M, N // 2, Kd)  # noqa: E731
         else:

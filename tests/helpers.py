@@ -588,8 +588,8 @@ def make_trainer(student, teacher, loss_type="kd_lm", accum=1, lr=2e-5, max_step
 #   gates: softmax of the kernel's fp32 logits with expf (<= 2 ulp), the rounded shift l - max, an E-term sum and a division:
 #       |got - ref| <= 2^-22 (E + 4 + max_e |l - max|) g
 #   act / dh1: SwiGLU of the kernel's bf16 h1.  bf16(silu(g)) and the bf16 store are 2^-8 each; the sigmoid (__expf: relative error
-#     about 2^-22 (2 + |g|)) and the fp32 products are covered by 2^-16.  dh1 also carries the error of dact (bf16 of a GEMM accumulator,
-#     never materialised on the fused path): 2^-8 |dact| + the GEMM term above, times |d dh1 / d dact|.
+#     about 2^-22 (2 + |g|)) and the fp32 products are covered by 2^-16.  dh1 also carries the error of dact (bf16 of a GEMM
+#     accumulator): 2^-8 |dact| + the GEMM term above, times |d dh1 / d dact|.
 #   dlogits: gate_bwd's fp32 arithmetic.  dg_e (l_aux term + renormalisation term) is off by at most 16 2^-24 D_e (D_e the sum of the
 #     terms' magnitudes), the dot sum_j g_j dg_j by sum_j g_j (16 2^-24 D_j + E 2^-24 |dg_j|), the final g (dg - dot) by 2 2^-24 of itself.
 #   l_aux: E sum_e mean(g_e) count_e / S over the tiles' fp32 sums (tpb + ntiles + E + 8 roundings of positive terms).
@@ -1232,12 +1232,12 @@ def moe_force_pairs(pairs, rows):
     return pairs
 
 
-def moe_run_stages(x, res, wg, w_gu, w_dn, noise, cf, mc, dout, g_laux, old, fused):
+def moe_run_stages(x, res, wg, w_gu, w_dn, noise, cf, mc, dout, g_laux, old):
     """kernels.moe_forward_stages + moe_backward_stages with weight gradients accumulated into copies of `old`; one dict of every
     intermediate, the gradients under 'g_wg', 'g_w_gu', 'g_w_dn'."""
     from llavamod import kernels as K
     grads = {k: v.clone() for k, v in old.items()}
-    st = K.moe_forward_stages(x, res, wg, w_gu, w_dn, noise, cf, mc, fused)
+    st = K.moe_forward_stages(x, res, wg, w_gu, w_dn, noise, cf, mc)
     bw = K.moe_backward_stages(st, x, wg, w_gu, w_dn, dout, torch.tensor(g_laux, device="cuda"), grads)
     k = {**st, **bw, **{"g_" + n: v for n, v in grads.items()}}
     return k
@@ -1260,7 +1260,7 @@ def check_moe_stages(k, ref, E, old, report=None):
     la_want, la_tol = ref["l_aux"]
     assert abs(float(k["meta"][0]) - float(la_want)) <= float(la_tol), ("l_aux", float(k["meta"][0]), float(la_want))
     check_moe("xp", k["xp"][:n_rows], ref["xp"][0], None, report)
-    for name in ("h1", "act", "y", "dh1", "dxp") + (("dact",) if k["dact"] is not None else ()):
+    for name in ("h1", "act", "y", "dh1", "dxp", "dact"):
         check_moe(name, k[name][:n_rows], *ref[name], report=report, rows=routed)
         if name in ("h1", "act", "y"):                           # padding rows below offsets[E] are exact zeros
             assert int(k[name][:n_rows][pad].ne(0).sum()) == 0, f"{name}: non-zero padding row"

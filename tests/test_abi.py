@@ -65,3 +65,15 @@ def test_cpu_tensor_is_rejected_not_silently_computed():
     from llavamod import _C, kernels as K
     with pytest.raises(_C.LmodError):
         K.kl_fused(torch.zeros(4, 8, dtype=torch.bfloat16), torch.zeros(4, 8, dtype=torch.bfloat16), torch.zeros(4, dtype=torch.int64), 4, 8, 1.0, 1.0)
+
+
+def test_fused_swiglu_refuses_h1():
+    """lmod_gemm_swiglu / lmod_grouped_gemm_swiglu are forward-only: a non-NULL h1 (the retired pre-activation output) is refused before
+    any operand is read or anything is launched."""
+    from llavamod import _C
+    L = _C.lib()
+    p = 1 << 20                                # never dereferenced: the call must return before
+    assert L.lmod_gemm_swiglu(p, 64, p, 64, p, 128, p, 256, 128, 128, 64, None) == -1
+    assert b"h1" in L.lmod_last_error()
+    assert L.lmod_grouped_gemm_swiglu(p, 64, p, 64, p, 128, p, 256, p, 1, 128, 128, 64, None) == -1
+    assert b"h1" in L.lmod_last_error()

@@ -368,40 +368,17 @@ def _bits_equal(name, got, want):
     assert n == 0, f"{name}: {n} / {got.numel()} elements differ in bits; first at {tuple(int(t) for t in torch.nonzero(diff)[0])}"
 
 
-@pytest.mark.parametrize("save_h1", [False, True])
-@pytest.mark.parametrize("M", [1, 127, 129, 300])
-def test_fused_swiglu_tails(M, save_h1):
+@pytest.mark.parametrize("M", [1, 127, 128, 129, 255, 256, 257, 300])
+def test_fused_swiglu_tails(M):
     from llavamod import kernels as Kk
     H, I = 200, 128
     g = _gen(M)
     x, w = _rnd(g, M, H), _rnd(g, 2 * I, H, scale=0.1)
     with poisoned_uninitialised_memory():
-        act, h1 = Kk.gemm_swiglu(x, w, save_h1)
-        h1_ref = Kk.gemm(x, w)
-        act_ref = Kk.silu_mul(h1_ref)
+        act = Kk.gemm_swiglu(x, w)
+        act_ref = Kk.silu_mul(Kk.gemm(x, w))
     _bits_equal("act", act, act_ref)
-    if save_h1:
-        _bits_equal("h1", h1, h1_ref)
     assert bool(torch.isfinite(act).all())
-
-
-@pytest.mark.parametrize("M,I", [(300, 384), (129, 136), (257, 128), (3 * 128 * 67, 256)])
-def test_fused_silu_bwd_both_widths(M, I):
-    """M = 3 * 128 * 67, I = 256 fills 1.5 waves of 132 SMs with 256-wide tiles; I <= 128 takes them too; the others 128-wide ones."""
-    from llavamod import kernels as Kk
-    H = 136
-    g = _gen(M + I)
-    dy, w_dn, h1 = _rnd(g, M, H, scale=0.2), _rnd(g, H, I, scale=0.1), _rnd(g, M, 2 * I)
-    with poisoned_uninitialised_memory():
-        dh1 = Kk.gemm_silu_bwd(dy, w_dn, h1)
-        want = Kk.silu_mul_bwd(Kk.gemm(dy, w_dn, b_mn=True), h1)
-    _bits_equal("dh1", dh1, want)
-    assert bool(torch.isfinite(dh1).all())
-    print(f"\nGEMMEXACT silu_bwd M={M} I={I}: BN={pick_bn(-(-M // 128), I)}")
-
-
-def test_fused_silu_bwd_covers_both_widths():
-    assert {pick_bn(-(-M // 128), I) for M, I in [(300, 384), (129, 136), (257, 128), (3 * 128 * 67, 256)]} == {128, 256}
 
 
 QKV = [(300, 200, 4, 2, 64), (300, 200, 2, 1, 128), (2560, 136, 16, 16, 64), (2560, 136, 8, 8, 128), (129, 64, 3, 1, 64)]
@@ -423,60 +400,31 @@ def test_fused_qkv_rope_tails(M, H, nh, nkv, hd):
     pos[::3] = 0
     pos[1::3] = max_pos - 1
     cos, sin = rope_tables(hd, max_pos, 1e6, BF16, "cuda")
-    saved = Kk.FUSE_ROPE
-    Kk.FUSE_ROPE = "1"
-    try:
-        with torch.no_grad(), poisoned_uninitialised_memory():
-            fused = Kk.qkv_rope(x, w, b, cos, sin, pos, nh, nkv, hd)
-            two = Kk.rope_(Kk.gemm(x, w, bias=b), cos, sin, pos, nh, nkv, hd)
-    finally:
-        Kk.FUSE_ROPE = saved
+    with torch.no_grad(), poisoned_uninitialised_memory():
+        fused = Kk.qkv_rope(x, w, b, cos, sin, pos, nh, nkv, hd)
+        two = Kk.rope_(Kk.gemm(x, w, bias=b), cos, sin, pos, nh, nkv, hd)
     _bits_equal("qkv", fused, two)
     assert bool(torch.isfinite(fused).all())
     print(f"\nGEMMEXACT qkv_rope M={M} N={N} hd={hd}: BN={pick_bn(-(-M // 128), N)}")
 
 
-@pytest.mark.parametrize("M,N,K", [(1, 264, 200), (129, 520, 136), (300, 136, 48)])
-def test_fused_residual_in_place_tails(M, N, K):
-    from llavamod import kernels as Kk
-    g = _gen(M + N + K)
-    x, w, b, res = _rnd(g, M, K), _rnd(g, N, K, scale=0.1), _rnd(g, N), _rnd(g, M, N)
-    with poisoned_uninitialised_memory():
-        y = Kk.gemm(x, w, bias=b)
-        want = torch.empty_like(res)
-        Kk.call("lmod_add", Kk.ptr(res), Kk.ptr(y), res.numel(), Kk.ptr(want))
-        r2 = res.clone()
-        out = Kk.gemm_residual(x, w, b, r2, inplace=True)
-    assert out.data_ptr() == r2.data_ptr()
-    _bits_equal("residual", r2, want)
-
-
 @pytest.mark.parametrize("sizes,I", [([128, 0, 256], 128), ([0, 384], 256), ([128, 0, 128, 0, 0, 256, 128, 0], 128)])
 def test_fused_grouped_swiglu_forms(sizes, I):
-    """Grouped SwiGLU forward and backward on expert groups (empty first, middle, last): bit for bit against the grouped GEMM + element-wise
-    kernels on the rows below offsets[G].  The slab has rows past offsets[G] (NaN in A and dY, not read).  I = 128 runs the backward in
-    256-wide tiles of which only 128 columns exist, I = 256 in 128-wide ones."""
+    """Grouped SwiGLU forward on expert groups (empty first, middle, last): bit for bit against the grouped GEMM + silu_mul on the rows
+    below offsets[G].  The slab has rows past offsets[G] (NaN in A, not read)."""
     from llavamod import kernels as Kk
     G, H = len(sizes), 200
     offs = _offsets(sizes)
     R = offs[-1] + 128
     g = _gen(G + I + R)
-    xp, w_gu, w_dn = _rnd(g, R, H), _rnd(g, G, 2 * I, H, scale=0.1), _rnd(g, G, H, I, scale=0.1)
-    dy = _rnd(g, R, H, scale=0.2)
+    xp, w_gu = _rnd(g, R, H), _rnd(g, G, 2 * I, H, scale=0.1)
     xp[offs[-1]:] = NAN
-    dy[offs[-1]:] = NAN
     offsets = torch.tensor(offs, dtype=torch.int32, device="cuda")
     n = offs[-1]
     with poisoned_uninitialised_memory():
-        act, h1 = Kk.grouped_gemm_swiglu(xp, w_gu, offsets, R, True)
+        act = Kk.grouped_gemm_swiglu(xp, w_gu, offsets, R)
         h1_ref = torch.zeros(R, 2 * I, dtype=BF16, device="cuda")
         Kk.grouped_gemm(xp, w_gu, h1_ref, offsets, 0)
-        dh1 = Kk.grouped_gemm_silu_bwd(dy, w_dn, h1, offsets, R)
-        dact = torch.zeros(R, I, dtype=BF16, device="cuda")
-        Kk.grouped_gemm(dy, w_dn, dact, offsets, 1)
-    _bits_equal("h1", h1[:n], h1_ref[:n])
     _bits_equal("act", act[:n], Kk.silu_mul(h1_ref)[:n])
-    _bits_equal("dh1", dh1[:n], Kk.silu_mul_bwd(dact, h1_ref)[:n])
-    for name, t in (("act", act[:n]), ("h1", h1[:n]), ("dh1", dh1[:n])):
-        assert bool(torch.isfinite(t).all()), name
+    assert bool(torch.isfinite(act[:n]).all())
 

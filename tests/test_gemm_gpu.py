@@ -56,27 +56,20 @@ def test_gemm_two_cta_path(M, N, K, a_mn, b_mn):
 
 
 @pytest.mark.parametrize("M,H,I", [(2048, 512, 2816 + 128 * 10), (300, 256, 384), (2048, 1024, 2816)])
-def test_gemm_fused_swiglu_forward_and_backward(M, H, I):
+def test_gemm_fused_swiglu_forward(M, H, I):
     """One GEMM with the SwiGLU epilogue == GEMM then silu_mul kernel, bit for bit (same bf16 roundings), on the CTA-pair kernel (first
-    shape) and the 1-CTA kernel; the saved pre-activations equal the plain GEMM output; the dgrad GEMM with the silu-backward epilogue ==
-    dgrad GEMM then silu_mul_bwd kernel, bit for bit.  The weight is the fused gate|up matrix as the checkpoint stores it (no re-layout)."""
+    shape) and the 1-CTA kernel.  The weight is the fused gate|up matrix as the checkpoint stores it (no re-layout).  (The backward of the
+    MLP is GEMM + silu_mul_bwd: test_mlp_function_gradients_match_autograd.)"""
     from llavamod import kernels as Kk
     g = torch.Generator(device="cuda").manual_seed(9 + M)
     x = torch.randn(M, H, device="cuda", generator=g).to(torch.bfloat16)
     w = (torch.randn(2 * I, H, device="cuda", generator=g) * 0.05).to(torch.bfloat16)
-    w_dn = (torch.randn(H, I, device="cuda", generator=g) * 0.05).to(torch.bfloat16)
-    act, h1 = Kk.gemm_swiglu(x, w, True)
-    h1_ref = Kk.gemm(x, w)
-    assert torch.equal(h1, h1_ref)
-    assert torch.equal(act, Kk.silu_mul(h1_ref))
-    assert torch.equal(Kk.gemm_swiglu(x, w, False)[0], act)
+    act = Kk.gemm_swiglu(x, w)
+    assert torch.equal(act, Kk.silu_mul(Kk.gemm(x, w)))
     ref = torch.nn.functional.silu(x.float() @ w[:I].float().t()) * (x.float() @ w[I:].float().t())
     # vs the un-rounded fp32 formula: gate, up and silu(gate) are each rounded to bf16 on the way (as in the reference's bf16 modules)
     err = (act.float() - ref).abs()
     assert bool((err <= 2.0 ** -6 * ref.abs() + 0.05).all()), err.max().item()
-    dy = (torch.randn(M, H, device="cuda", generator=g) * 0.1).to(torch.bfloat16)
-    dh1 = Kk.gemm_silu_bwd(dy, w_dn, h1)
-    assert torch.equal(dh1, Kk.silu_mul_bwd(Kk.gemm(dy, w_dn, b_mn=True), h1))
 
 
 @pytest.mark.parametrize("M,H,nh,nkv,hd", [(2048, 1024, 16, 16, 64), (300, 256, 4, 2, 128), (2048, 4096, 32, 32, 128), (257, 128, 2, 1, 64)])
@@ -92,7 +85,6 @@ def test_qkv_projection_with_fused_rope(M, H, nh, nkv, hd):
     b = torch.randn(N, device="cuda", generator=g).to(torch.bfloat16)
     pos = torch.randint(0, 2048, (M,), device="cuda", generator=g)
     cos, sin = rope_tables(hd, 2048, 1e6, torch.bfloat16, "cuda")
-    Kk.FUSE_ROPE = "1"                                     # the model path fuses by reduction length; here the fused op itself is under test
     fused = Kk.qkv_rope(x, w, b, cos, sin, pos, nh, nkv, hd)
     two = Kk.rope_(Kk.gemm(x, w, bias=b), cos, sin, pos, nh, nkv, hd)
     assert torch.equal(fused, two)
@@ -108,33 +100,11 @@ def test_qkv_projection_with_fused_rope(M, H, nh, nkv, hd):
             res.append((xx.grad, wg, bg))
         for a, c in zip(res[0], res[1]):
             assert torch.equal(a, c)
-    Kk.FUSE_ROPE = "auto"
 
 
-@pytest.mark.parametrize("M,N,K,bias", [(2048, 4096, 4096, False), (2048, 4096, 11008, False), (2048, 1024, 1024, True), (577, 1024, 4096, True),
-                                        (300, 520, 200, True), (1154, 1024, 1024, True)])
-def test_gemm_with_residual_epilogue_is_gemm_plus_add(M, N, K, bias):
-    """o_proj / down_proj (modeling_qwen2.py:796,808) and CLIP out_proj / fc2 with the residual add in the GEMM epilogue: bit-identical to
-    GEMM (+bias, rounded to bf16) followed by the bf16 add kernel -- CTA-pair tiles (teacher shapes), 1-CTA tiles, ragged edges, in place."""
-    from llavamod import kernels as Kk
-    g = torch.Generator(device="cuda").manual_seed(M + N + K)
-    x = torch.randn(M, K, device="cuda", generator=g).to(torch.bfloat16)
-    w = (torch.randn(N, K, device="cuda", generator=g) * 0.03).to(torch.bfloat16)
-    b = torch.randn(N, device="cuda", generator=g).to(torch.bfloat16) if bias else None
-    res = torch.randn(M, N, device="cuda", generator=g).to(torch.bfloat16)
-    y = Kk.gemm(x, w, bias=b)
-    want = torch.empty_like(res)
-    Kk.call("lmod_add", Kk.ptr(res), Kk.ptr(y), res.numel(), Kk.ptr(want))
-    assert torch.equal(want, (res.float() + y.float()).to(torch.bfloat16))          # the add kernel is the reference's bf16 add
-    got = Kk.gemm_residual(x, w, b, res)
-    assert torch.equal(got, want)
-    r2 = res.clone()
-    out = Kk.gemm_residual(x, w, b, r2, inplace=True)
-    assert out.data_ptr() == r2.data_ptr() and torch.equal(r2, want)
-
-
-def test_grouped_swiglu_forward_and_backward():
-    """Expert form on ragged 128-aligned row groups (one empty group): fused == grouped GEMM + element-wise kernels, bit for bit."""
+def test_grouped_swiglu_forward():
+    """Expert form on ragged 128-aligned row groups (one empty group): fused == grouped GEMM + silu_mul, bit for bit.  (The experts'
+    backward is grouped GEMM + silu_mul_bwd: tests/test_moe_exact_gpu.py.)"""
     from llavamod import kernels as Kk
     E, H, I = 4, 256, 384
     offs = torch.tensor([0, 256, 256, 640, 768], dtype=torch.int32, device="cuda")
@@ -142,21 +112,16 @@ def test_grouped_swiglu_forward_and_backward():
     g = torch.Generator(device="cuda").manual_seed(5)
     xp = torch.randn(R, H, device="cuda", generator=g).to(torch.bfloat16)
     w_gu = (torch.randn(E, 2 * I, H, device="cuda", generator=g) * 0.05).to(torch.bfloat16)
-    w_dn = (torch.randn(E, H, I, device="cuda", generator=g) * 0.05).to(torch.bfloat16)
-    act, h1 = Kk.grouped_gemm_swiglu(xp, w_gu, offs, R, True)
+    act = Kk.grouped_gemm_swiglu(xp, w_gu, offs, R)
     h1_ref = torch.zeros(R, 2 * I, dtype=torch.bfloat16, device="cuda")
     Kk.grouped_gemm(xp, w_gu, h1_ref, offs, 0)
     n = int(offs[-1])
-    assert torch.equal(h1[:n], h1_ref[:n]) and torch.equal(act[:n], Kk.silu_mul(h1_ref)[:n])
-    dy = (torch.randn(R, H, device="cuda", generator=g) * 0.1).to(torch.bfloat16)
-    dh1 = Kk.grouped_gemm_silu_bwd(dy, w_dn, h1, offs, R)
-    dact = torch.zeros(R, I, dtype=torch.bfloat16, device="cuda")
-    Kk.grouped_gemm(dy, w_dn, dact, offs, 1)
-    assert torch.equal(dh1[:n], Kk.silu_mul_bwd(dact, h1_ref)[:n])
+    assert torch.equal(act[:n], Kk.silu_mul(h1_ref)[:n])
 
 
 def test_mlp_function_gradients_match_autograd():
-    """K.mlp (fused forward / backward) against fp32 autograd of the plain formula, incl. the in-place weight-gradient accumulation."""
+    """K.mlp's training path (GEMM + silu_mul forward, GEMM + silu_mul_bwd backward) against fp32 autograd of the plain formula, incl. the
+    in-place weight-gradient accumulation."""
     from llavamod import kernels as Kk
     M, H, I = 384, 256, 512
     g = torch.Generator(device="cuda").manual_seed(3)
@@ -165,7 +130,6 @@ def test_mlp_function_gradients_match_autograd():
     w_dn = (torch.randn(H, I, device="cuda", generator=g) * 0.05).to(torch.bfloat16)
     g_gu, g_dn = torch.zeros_like(w_gu), torch.zeros_like(w_dn)
     go = torch.randn(M, H, device="cuda", generator=g).to(torch.bfloat16)
-    Kk.FUSE_SWIGLU = "1"                                   # exercise MLPFn (the model path only fuses frozen MLPs with a long reduction)
     y = Kk.mlp(x, w_gu, w_dn, g_gu, g_dn)
     y.backward(go)
     xf = x.detach().float().requires_grad_(True)
@@ -176,7 +140,6 @@ def test_mlp_function_gradients_match_autograd():
     assert rel(y, yr) < 1e-2 and rel(x.grad, xf.grad) < 1.5e-2 and rel(g_gu, wg.grad) < 1.5e-2 and rel(g_dn, wd.grad) < 1.5e-2
     with torch.no_grad():
         assert torch.equal(Kk.mlp(x.detach(), w_gu, w_dn), y.detach())
-    Kk.FUSE_SWIGLU = "auto"
 
 
 def test_gemm_bias_beta_and_f32_accumulate():

@@ -272,7 +272,7 @@ def test_moe_layer_forward_backward_vs_oracle():
     # element by element: every stage against the float64 reference from the kernels' previous stage (tests/helpers.py), and MoEFn
     # gives the stage functions' bytes
     zeros = {k: torch.zeros_like(v) for k, v in grads.items()}
-    k = moe_run_stages(xd.detach(), rd.detach(), wg, w_gu, w_dn, noise.to(dev()), cf, 0, go.to(dev()), 0.37, zeros, False)
+    k = moe_run_stages(xd.detach(), rd.detach(), wg, w_gu, w_dn, noise.to(dev()), cf, 0, go.to(dev()), 0.37, zeros)
     assert torch.equal(out, k["out"]) and torch.equal(xd.grad, k["dx"])
     for name in ("wg", "w_gu", "w_dn"):
         assert torch.equal(grads[name], k["g_" + name]), name

@@ -60,60 +60,41 @@ def test_moe_block_stage_by_stage(case):
     name, S, H, I, E, cf, mc, n1, n2, specials, clamp_to, g_laux = case
     rows, pairs, x, wg, noise, w_gu, w_dn, res, dout, old = _inputs(S, H, I, E, cf, mc, n1, n2, specials, clamp_to, S + H + E)
     assert K.moe_capacity(S, E, cf, mc) == R.moe_capacity(S, E, cf, mc)
-    paths = [False, True] if I % 128 == 0 else [False]
-    runs = {}
     report = REPORT.setdefault(name, {})
-    for fused in paths:
-        k = Hh.moe_run_stages(x, res, wg, w_gu, w_dn, noise, cf, mc, dout, g_laux, old, fused)
-        ref = Hh.moe_reference_fp64(x, res, wg, w_gu, w_dn, noise, cf, mc, dout=dout, g_laux=g_laux, old=old, k=k, store=torch.float32)
-        assert torch.equal(ref["rec"]["idx"].cpu(), pairs)           # the planted routing is the oracle's
-        Hh.check_moe_stages(k, ref, E, old, report)
-        rec = ref["rec"]
-        for s, _, _, _, what in rows:
-            if what == "both dropped":
-                assert int(k["row"][s, 0]) == -1 and int(k["row"][s, 1]) == -1
-                Hh.check_moe("out (both dropped)", k["out"][s], res[s])
-            if what == "dropped first, clamped second":
-                assert int(k["row"][s, 0]) == -1 and int(k["row"][s, 1]) >= 0
-                assert float(k["gates"][s, rec["idx"][s, 1]]) < Hh.FLT_EPS
-        assert int((~rec["keep"][:, 0]).sum()) > 0 and int((~rec["keep"][:, 1]).sum()) > 0
-        del ref
-        # a second launch gives the same bytes (no float atomics on the path: integer shared-memory counters, fixed-order sums)
-        k2 = Hh.moe_run_stages(x, res, wg, w_gu, w_dn, noise, cf, mc, dout, g_laux, old, fused)
-        n = int(k["offsets"][-1])                                    # rows past offsets[E] are never written (uninitialised)
-        for key, v in k.items():
-            if isinstance(v, torch.Tensor):
-                v, v2 = (v[:n], k2[key][:n]) if v.shape[0] == k["max_rows"] else (v, k2[key])
-                assert torch.equal(v, v2), f"{key} differs between two launches"
-        del k2
-        runs[fused] = k
-    if len(paths) == 2:                                              # fused and unfused SwiGLU agree bit for bit
-        a, b = runs[False], runs[True]
-        n = int(a["offsets"][-1])
-        for key in ("out", "h1", "act", "y", "dy", "dw", "dh1", "dxp", "dlogits", "dx", "g_wg", "g_w_gu", "g_w_dn"):
-            va, vb = (a[key][:n], b[key][:n]) if a[key].shape[0] == a["max_rows"] else (a[key], b[key])
-            assert torch.equal(va, vb), f"{key}: fused and unfused SwiGLU differ"
-    # MoEFn (FUSE_SWIGLU auto, and "1") and the no-grad eval path give the stage functions' bytes
-    saved = K.FUSE_SWIGLU
-    try:
-        for mode in ("auto", "1") if I % 128 == 0 else ("auto",):
-            K.FUSE_SWIGLU = mode
-            fused = K.swiglu_fusable(I, H, training=True)
-            want = runs[fused]
-            grads = {kk: v.clone() for kk, v in old.items()}
-            xd, rd = x.clone().requires_grad_(True), res.clone().requires_grad_(True)
-            out, l_aux = K.MoEFn.apply(xd, rd, wg, w_gu, w_dn, noise, cf, mc, grads)
-            ((out.float() * dout.float()).sum() + g_laux * l_aux).backward()
-            assert torch.equal(out, want["out"]) and torch.equal(l_aux, want["meta"][0])
-            assert torch.equal(xd.grad, want["dx"]) and torch.equal(rd.grad, dout)
-            for gname in ("wg", "w_gu", "w_dn"):
-                assert torch.equal(grads[gname], want["g_" + gname]), gname
-        K.FUSE_SWIGLU = saved
-        with torch.no_grad():
-            out_ng, la_ng, _ = K.moe_forward_nograd(x, res, wg, w_gu, w_dn, noise, cf, mc)
-        assert torch.equal(out_ng, runs[False]["out"]) and torch.equal(la_ng, runs[False]["meta"][0])
-    finally:
-        K.FUSE_SWIGLU = saved
+    k = Hh.moe_run_stages(x, res, wg, w_gu, w_dn, noise, cf, mc, dout, g_laux, old)
+    ref = Hh.moe_reference_fp64(x, res, wg, w_gu, w_dn, noise, cf, mc, dout=dout, g_laux=g_laux, old=old, k=k, store=torch.float32)
+    assert torch.equal(ref["rec"]["idx"].cpu(), pairs)               # the planted routing is the oracle's
+    Hh.check_moe_stages(k, ref, E, old, report)
+    rec = ref["rec"]
+    for s, _, _, _, what in rows:
+        if what == "both dropped":
+            assert int(k["row"][s, 0]) == -1 and int(k["row"][s, 1]) == -1
+            Hh.check_moe("out (both dropped)", k["out"][s], res[s])
+        if what == "dropped first, clamped second":
+            assert int(k["row"][s, 0]) == -1 and int(k["row"][s, 1]) >= 0
+            assert float(k["gates"][s, rec["idx"][s, 1]]) < Hh.FLT_EPS
+    assert int((~rec["keep"][:, 0]).sum()) > 0 and int((~rec["keep"][:, 1]).sum()) > 0
+    del ref
+    # a second launch gives the same bytes (no float atomics on the path: integer shared-memory counters, fixed-order sums)
+    k2 = Hh.moe_run_stages(x, res, wg, w_gu, w_dn, noise, cf, mc, dout, g_laux, old)
+    n = int(k["offsets"][-1])                                        # rows past offsets[E] are never written (uninitialised)
+    for key, v in k.items():
+        if isinstance(v, torch.Tensor):
+            v, v2 = (v[:n], k2[key][:n]) if v.shape[0] == k["max_rows"] else (v, k2[key])
+            assert torch.equal(v, v2), f"{key} differs between two launches"
+    del k2
+    # MoEFn and the no-grad eval path (fused SwiGLU where swiglu_fusable allows) give the stage functions' bytes
+    grads = {kk: v.clone() for kk, v in old.items()}
+    xd, rd = x.clone().requires_grad_(True), res.clone().requires_grad_(True)
+    out, l_aux = K.MoEFn.apply(xd, rd, wg, w_gu, w_dn, noise, cf, mc, grads)
+    ((out.float() * dout.float()).sum() + g_laux * l_aux).backward()
+    assert torch.equal(out, k["out"]) and torch.equal(l_aux, k["meta"][0])
+    assert torch.equal(xd.grad, k["dx"]) and torch.equal(rd.grad, dout)
+    for gname in ("wg", "w_gu", "w_dn"):
+        assert torch.equal(grads[gname], k["g_" + gname]), gname
+    with torch.no_grad():
+        out_ng, la_ng, _ = K.moe_forward_nograd(x, res, wg, w_gu, w_dn, noise, cf, mc)
+    assert torch.equal(out_ng, k["out"]) and torch.equal(la_ng, k["meta"][0])
     print(f"\n{name}: max err/bound " + ", ".join(f"{k} {v:.3g}" for k, v in report.items() if v) +
           f"; peak allocated {torch.cuda.max_memory_allocated() / 2**30:.2f} GiB")
 

@@ -103,9 +103,8 @@ def test_mix_backward_against_float64(S, H):
 # ---------------------------------------------------------------------------------------------------------------------------------
 # the whole residual block at config 2, stage by stage
 # ---------------------------------------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("fused", [False, True], ids=["unfused", "fused"])
 @pytest.mark.parametrize("k", [2, 1])
-def test_residual_block_stage_by_stage(k, fused):
+def test_residual_block_stage_by_stage(k):
     from llavamod import kernels as K
     S, H, I, E, cf = 2048, 1024, 2816, 4, 0.8
     dev = "cuda"
@@ -132,10 +131,10 @@ def test_residual_block_stage_by_stage(k, fused):
                wc=(torch.randn(2, H, device=dev, generator=g) * 1e-2).to(bf), bc=(torch.randn(2, device=dev, generator=g) * 1e-2).to(bf))
     gl = torch.tensor(0.37, device=dev)
     grads = {n: v.clone() for n, v in old.items()}
-    st = K.moe_residual_forward_stages(x, res, wg, w_gu, w_dn, noise, cf, 0, r_gu, r_dn, wc, bc, fused, k)
+    st = K.moe_residual_forward_stages(x, res, wg, w_gu, w_dn, noise, cf, 0, r_gu, r_dn, wc, bc, k)
     bw = K.moe_residual_backward_stages(st, x, wg, w_gu, w_dn, r_gu, r_dn, wc, dout, gl, grads)
     # the routed part is the plain MoE path with no residual, bit for bit, forward and backward (dres as its extra addend)
-    plain = K.moe_forward_stages(x, None, wg, w_gu, w_dn, noise, cf, 0, fused, k)
+    plain = K.moe_forward_stages(x, None, wg, w_gu, w_dn, noise, cf, 0, k)
     assert torch.equal(plain["out"], st["moe"]) and torch.equal(plain["row"], st["row"])
     pg = {n: old[n].clone() for n in ("wg", "w_gu", "w_dn")}
     pb = K.moe_backward_stages(plain, x, wg, w_gu, w_dn, bw["mix"]["d_moe"], gl, pg, dres=bw["dres"])
@@ -185,15 +184,13 @@ def test_residual_block_stage_by_stage(k, fused):
         want = A.t() @ B + old[n].double()
         Hh.check_moe("g_" + n, grads[n], want, Hh._gemm_tol(want, A.abs().t() @ B.abs() + old[n].double().abs(), S))
     # ResidualMoEFn and the no-grad path give the stage functions' bytes
-    fused_train = K.swiglu_fusable(I, H, training=True)
-    if fused == fused_train:
-        g2 = {n: v.clone() for n, v in old.items()}
-        xg, rg = x.clone().requires_grad_(True), res.clone().requires_grad_(True)
-        out, l_aux = K.ResidualMoEFn.apply(xg, rg, wg, w_gu, w_dn, noise, cf, 0, r_gu, r_dn, wc, bc, g2, k)
-        ((out.float() * dout.float()).sum() + 0.37 * l_aux).backward()
-        assert torch.equal(out, st["out"]) and torch.equal(xg.grad, bw["dx"]) and torch.equal(rg.grad, dout)
-        for n in g2:
-            assert torch.equal(g2[n], grads[n]), n
+    g2 = {n: v.clone() for n, v in old.items()}
+    xg, rg = x.clone().requires_grad_(True), res.clone().requires_grad_(True)
+    out, l_aux = K.ResidualMoEFn.apply(xg, rg, wg, w_gu, w_dn, noise, cf, 0, r_gu, r_dn, wc, bc, g2, k)
+    ((out.float() * dout.float()).sum() + 0.37 * l_aux).backward()
+    assert torch.equal(out, st["out"]) and torch.equal(xg.grad, bw["dx"]) and torch.equal(rg.grad, dout)
+    for n in g2:
+        assert torch.equal(g2[n], grads[n]), n
     with torch.no_grad():
         out_ng, _, rec = K.moe_residual_forward_nograd(x, res, wg, w_gu, w_dn, noise, cf, 0, r_gu, r_dn, wc, bc, k)
     assert torch.equal(out_ng, st["out"]) and torch.equal(rec["coef"], st["coef"])

@@ -178,88 +178,79 @@ def test_moe_block_top1_stage_by_stage(case):
                w_gu=(torch.randn(E, 2 * I, H, device=dev, generator=g) * 1e-2).to(torch.bfloat16),
                w_dn=(torch.randn(E, H, I, device=dev, generator=g) * 1e-2).to(torch.bfloat16))
     g_laux = 0.37
-    runs = {}
-    for fused in ([False, True] if I % 128 == 0 else [False]):
-        grads = {k: v.clone() for k, v in old.items()}
-        st = K.moe_forward_stages(x, res, wg, w_gu, w_dn, u, cf, mc, fused, k=1)
-        bw = K.moe_backward_stages(st, x, wg, w_gu, w_dn, dout, torch.tensor(g_laux, device=dev), grads)
-        _, o = check_route(x, wg, u, cf, mc)
-        row, keep = st["row"][:, 0].long(), st["row"][:, 0] >= 0
-        idx = st["idx"][:, :1].long()
-        offs, used = st["offsets"].long().cpu(), torch.minimum(torch.bincount(idx[:, 0], minlength=E).cpu(), torch.tensor(st["capacity"]))
-        n = int(offs[-1])
-        # expert forward
-        want, tol = _per_expert(st["xp"][:n], lambda e: w_gu[e].double().t(), offs, used, 2 * I, H)
-        Hh.check_moe("h1", st["h1"][:n], want, tol)
-        h1 = st["h1"][:n].double()
-        gg, uu = h1[:, :I], h1[:, I:]
-        sg = torch.sigmoid(gg)
-        act = gg * sg * uu
-        Hh.check_moe("act", st["act"][:n], act, (2.0 ** -7 + 2.0 ** -16) * act.abs())
-        want, tol = _per_expert(st["act"][:n], lambda e: w_dn[e].double().t(), offs, used, H, I)
-        Hh.check_moe("y", st["y"][:n], want, tol)
-        # combine: bit exact from the kernel's y and w
-        wb = st["w"][:, :1].to(torch.bfloat16).float()
-        ysel = torch.where(keep[:, None], st["y"][row.clamp(min=0)].float(), torch.zeros(S, H, device=dev))
-        Hh.check_moe("out", st["out"], (res.float() + (wb * ysel).to(torch.bfloat16).float()).to(torch.bfloat16))
-        # combine backward
-        dy = torch.zeros(st["xp"].shape[0], H, dtype=torch.bfloat16, device=dev)
-        dy[row[keep]] = (wb[keep] * dout[keep].float()).to(torch.bfloat16)
-        Hh.check_moe("dy", bw["dy"], dy)
-        d64 = dout.double()
-        yr = st["y"][row.clamp(min=0)].double()
-        dw = torch.where(keep, (d64 * yr).sum(1), torch.zeros(S, dtype=torch.float64, device=dev))
-        lane_fmas = 8 * -(-H // 256)
-        dwt = (lane_fmas + 6) * u24 * (d64.abs() * yr.abs()).sum(1) * keep
-        Hh.check_moe("dw", bw["dw"][:, 0], dw, dwt)
-        assert bool((bw["dw"][:, 1] == 0).all())
-        # expert backward
-        dact, dact_tol = _per_expert(bw["dy"][:n], lambda e: w_dn[e].double(), offs, used, I, H)
-        if not fused:
-            Hh.check_moe("dact", bw["dact"][:n], dact, dact_tol)
-        cg, cu = uu * sg * (1 + gg * (1 - sg)), gg * sg
-        dh1 = torch.cat([dact * cg, dact * cu], 1)
-        derr = dact_tol + 2.0 ** -16 * dact.abs()
-        Hh.check_moe("dh1", bw["dh1"][:n], dh1, 2.0 ** -8 * dh1.abs() + (1 + 2.0 ** -8) * torch.cat([derr * cg.abs(), derr * cu.abs()], 1))
-        want, tol = _per_expert(bw["dh1"][:n], lambda e: w_gu[e].double(), offs, used, H, 2 * I)
-        Hh.check_moe("dxp", bw["dxp"][:n], want, tol)
-        for gname, a, b, M, N in (("w_dn", bw["dy"], st["act"], H, I), ("w_gu", bw["dh1"], st["xp"], 2 * I, H)):
-            for e in range(E):
-                r0, r1, r2 = int(offs[e]), int(offs[e]) + int(used[e]), int(offs[e + 1])
-                o_e = old[gname][e].double()
-                if r1 > r0:
-                    A, B = a[r0:r1].double(), b[r0:r1].double()
-                    ref = A.t() @ B + o_e
-                    Hh.check_moe("g_" + gname, grads[gname][e], ref, Hh._gemm_tol(ref, A.abs().t() @ B.abs(), r2 - r0) + 2.0 ** -23 * ref.abs())
-                else:
-                    Hh.check_moe("g_" + gname, grads[gname][e], o_e.to(grads[gname].dtype))
-        # gate backward: dgates[s, idx1] += dw (kept), the l_aux term, the softmax
-        gk = st["gates"].double()
-        dwk = bw["dw"][:, 0].double() * keep
-        lterm = (g_laux * E * o["exp_counts"].to(dev).double() / S / S)[None].expand(S, E)
-        rterm = torch.zeros(S, E, dtype=torch.float64, device=dev).scatter_add_(1, idx, dwk[:, None])
-        dg = lterm + rterm
-        D = lterm.abs() + rterm.abs()
-        dl = gk * (dg - (gk * dg).sum(1, keepdim=True))
-        dl_tol = gk * (16 * u24 * D + (gk * (16 * u24 * D + E * u24 * dg.abs())).sum(1, keepdim=True)) + 2 * u24 * dl.abs() + 2.0 ** -140
-        Hh.check_moe("dlogits", bw["dlogits"], dl, dl_tol)
-        dlk = bw["dlogits"].double()
-        wg64 = wg.double()
-        dx = dlk @ wg64
-        maj = dlk.abs() @ wg64.abs()
-        v = bw["dxp"][row.clamp(min=0)].double() * keep[:, None]
-        dx, maj = dx + v, maj + v.abs()
-        Hh.check_moe("dx", bw["dx"], dx, 2.0 ** -8 * dx.abs() + (1 + 2.0 ** -8) * (E + 2) * u24 * maj)
-        dwg = old["wg"].double() + dlk.t() @ x.double()
-        Hh.check_moe("g_wg", grads["wg"], dwg, (-(-S // 32) + 34) * u24 * (dlk.abs().t() @ x.double().abs() + old["wg"].double().abs()))
-        runs[fused] = (st, bw, grads)
-    if len(runs) == 2:
-        (a, ab, ag), (b, bb, bg) = runs[False], runs[True]
-        n = int(a["offsets"][-1])
-        assert torch.equal(a["out"], b["out"]) and torch.equal(ab["dx"], bb["dx"])
-        assert torch.equal(ab["dxp"][:n], bb["dxp"][:n]) and all(torch.equal(ag[k], bg[k]) for k in ag)
+    grads = {k: v.clone() for k, v in old.items()}
+    st = K.moe_forward_stages(x, res, wg, w_gu, w_dn, u, cf, mc, k=1)
+    bw = K.moe_backward_stages(st, x, wg, w_gu, w_dn, dout, torch.tensor(g_laux, device=dev), grads)
+    _, o = check_route(x, wg, u, cf, mc)
+    row, keep = st["row"][:, 0].long(), st["row"][:, 0] >= 0
+    idx = st["idx"][:, :1].long()
+    offs, used = st["offsets"].long().cpu(), torch.minimum(torch.bincount(idx[:, 0], minlength=E).cpu(), torch.tensor(st["capacity"]))
+    n = int(offs[-1])
+    # expert forward
+    want, tol = _per_expert(st["xp"][:n], lambda e: w_gu[e].double().t(), offs, used, 2 * I, H)
+    Hh.check_moe("h1", st["h1"][:n], want, tol)
+    h1 = st["h1"][:n].double()
+    gg, uu = h1[:, :I], h1[:, I:]
+    sg = torch.sigmoid(gg)
+    act = gg * sg * uu
+    Hh.check_moe("act", st["act"][:n], act, (2.0 ** -7 + 2.0 ** -16) * act.abs())
+    want, tol = _per_expert(st["act"][:n], lambda e: w_dn[e].double().t(), offs, used, H, I)
+    Hh.check_moe("y", st["y"][:n], want, tol)
+    # combine: bit exact from the kernel's y and w
+    wb = st["w"][:, :1].to(torch.bfloat16).float()
+    ysel = torch.where(keep[:, None], st["y"][row.clamp(min=0)].float(), torch.zeros(S, H, device=dev))
+    Hh.check_moe("out", st["out"], (res.float() + (wb * ysel).to(torch.bfloat16).float()).to(torch.bfloat16))
+    # combine backward
+    dy = torch.zeros(st["xp"].shape[0], H, dtype=torch.bfloat16, device=dev)
+    dy[row[keep]] = (wb[keep] * dout[keep].float()).to(torch.bfloat16)
+    Hh.check_moe("dy", bw["dy"], dy)
+    d64 = dout.double()
+    yr = st["y"][row.clamp(min=0)].double()
+    dw = torch.where(keep, (d64 * yr).sum(1), torch.zeros(S, dtype=torch.float64, device=dev))
+    lane_fmas = 8 * -(-H // 256)
+    dwt = (lane_fmas + 6) * u24 * (d64.abs() * yr.abs()).sum(1) * keep
+    Hh.check_moe("dw", bw["dw"][:, 0], dw, dwt)
+    assert bool((bw["dw"][:, 1] == 0).all())
+    # expert backward
+    dact, dact_tol = _per_expert(bw["dy"][:n], lambda e: w_dn[e].double(), offs, used, I, H)
+    Hh.check_moe("dact", bw["dact"][:n], dact, dact_tol)
+    cg, cu = uu * sg * (1 + gg * (1 - sg)), gg * sg
+    dh1 = torch.cat([dact * cg, dact * cu], 1)
+    derr = dact_tol + 2.0 ** -16 * dact.abs()
+    Hh.check_moe("dh1", bw["dh1"][:n], dh1, 2.0 ** -8 * dh1.abs() + (1 + 2.0 ** -8) * torch.cat([derr * cg.abs(), derr * cu.abs()], 1))
+    want, tol = _per_expert(bw["dh1"][:n], lambda e: w_gu[e].double(), offs, used, H, 2 * I)
+    Hh.check_moe("dxp", bw["dxp"][:n], want, tol)
+    for gname, a, b, M, N in (("w_dn", bw["dy"], st["act"], H, I), ("w_gu", bw["dh1"], st["xp"], 2 * I, H)):
+        for e in range(E):
+            r0, r1, r2 = int(offs[e]), int(offs[e]) + int(used[e]), int(offs[e + 1])
+            o_e = old[gname][e].double()
+            if r1 > r0:
+                A, B = a[r0:r1].double(), b[r0:r1].double()
+                ref = A.t() @ B + o_e
+                Hh.check_moe("g_" + gname, grads[gname][e], ref, Hh._gemm_tol(ref, A.abs().t() @ B.abs(), r2 - r0) + 2.0 ** -23 * ref.abs())
+            else:
+                Hh.check_moe("g_" + gname, grads[gname][e], o_e.to(grads[gname].dtype))
+    # gate backward: dgates[s, idx1] += dw (kept), the l_aux term, the softmax
+    gk = st["gates"].double()
+    dwk = bw["dw"][:, 0].double() * keep
+    lterm = (g_laux * E * o["exp_counts"].to(dev).double() / S / S)[None].expand(S, E)
+    rterm = torch.zeros(S, E, dtype=torch.float64, device=dev).scatter_add_(1, idx, dwk[:, None])
+    dg = lterm + rterm
+    D = lterm.abs() + rterm.abs()
+    dl = gk * (dg - (gk * dg).sum(1, keepdim=True))
+    dl_tol = gk * (16 * u24 * D + (gk * (16 * u24 * D + E * u24 * dg.abs())).sum(1, keepdim=True)) + 2 * u24 * dl.abs() + 2.0 ** -140
+    Hh.check_moe("dlogits", bw["dlogits"], dl, dl_tol)
+    dlk = bw["dlogits"].double()
+    wg64 = wg.double()
+    dx = dlk @ wg64
+    maj = dlk.abs() @ wg64.abs()
+    v = bw["dxp"][row.clamp(min=0)].double() * keep[:, None]
+    dx, maj = dx + v, maj + v.abs()
+    Hh.check_moe("dx", bw["dx"], dx, 2.0 ** -8 * dx.abs() + (1 + 2.0 ** -8) * (E + 2) * u24 * maj)
+    dwg = old["wg"].double() + dlk.t() @ x.double()
+    Hh.check_moe("g_wg", grads["wg"], dwg, (-(-S // 32) + 34) * u24 * (dlk.abs().t() @ x.double().abs() + old["wg"].double().abs()))
     # MoEFn and the no-grad path give the stage functions' bytes
-    st, bw, grads_want = runs[K.swiglu_fusable(I, H, training=True)]
+    grads_want = grads
     grads = {k: v.clone() for k, v in old.items()}
     xd, rd = x.clone().requires_grad_(True), res.clone().requires_grad_(True)
     out, l_aux = K.MoEFn.apply(xd, rd, wg, w_gu, w_dn, u, cf, mc, grads, 1)
@@ -269,7 +260,7 @@ def test_moe_block_top1_stage_by_stage(case):
         assert torch.equal(grads[k], grads_want[k]), k
     with torch.no_grad():
         out_ng, la_ng, _ = K.moe_forward_nograd(x, res, wg, w_gu, w_dn, u, cf, mc, 1)
-    assert torch.equal(out_ng, runs[False][0]["out"]) and torch.equal(la_ng, st["meta"][0])
+    assert torch.equal(out_ng, st["out"]) and torch.equal(la_ng, st["meta"][0])
 
 
 # ---------------------------------------------------------------------------------------------------------------------------------
