@@ -655,7 +655,7 @@ class RopeFn(Function):
 
 class QKVRopeFn(Function):
     """q|k|v projection + rotary embedding (modeling_qwen2.py:678-691): ONE GEMM whose epilogue adds the bias and rotates the q / k heads
-    (lmod_gemm_qkv_rope).  Backward: the transpose rotation in place on the incoming dqkv, then dgrad / wgrad / bias gradient as LinearFn."""
+    (lmod_gemm_qkv_rope).  Backward: the transpose rotation on a copy of the incoming dqkv, then dgrad / wgrad / bias gradient as LinearFn."""
 
     @staticmethod
     def forward(ctx, x, w, bias, cos, sin, pos, nh, nkv, hd, wgrad, bgrad):
@@ -675,7 +675,9 @@ class QKVRopeFn(Function):
         x2, w, cos, sin, pos = ctx.saved_tensors
         nh, nkv, hd = ctx.dims
         wgrad, bgrad = ctx.g
-        d = _c(d)                                         # the fused dq|dk|dv buffer of the attention backward: rotated back in place
+        # Rotated back in a copy, as RopeFn does: autograd may hand backward a gradient that is still read elsewhere (the caller's tensor
+        # in out.backward(grad), a tensor hook's argument), and rotating it in place would change what those see.
+        d = d.clone(memory_format=torch.contiguous_format)
         ld = d.shape[-1]
         call("lmod_rope", ptr(d), ld, nh, d.data_ptr() + nh * hd * 2, ld, nkv, hd, ptr(cos), ptr(sin), ptr(pos), d.numel() // ld, 1)
         dx = mm_nn(d, w).reshape(ctx.xshape) if ctx.needs_input_grad[0] else None
@@ -687,9 +689,10 @@ class QKVRopeFn(Function):
 
 
 def qkv_rope(x, w, bias, cos, sin, pos, nh, nkv, hd, wgrad=None, bgrad=None):
-    """Fused q|k|v projection + RoPE for the head dims the epilogue is built for; other head dims (tiny test shapes) take GEMM + lmod_rope."""
+    """Fused q|k|v projection + RoPE for the head dims the epilogue is built for; other head dims (tiny test shapes) take GEMM + lmod_rope.
+    Both return [rows, (nh + 2 nkv) hd]: the unfused path rotates the GEMM output in place, so it must not be a view LinearFn made."""
     if hd not in ATTN_HEAD_DIMS:
-        return rope_(linear(x, w, bias, wgrad, bgrad), cos, sin, pos, nh, nkv, hd)
+        return rope_(linear(_rows(x), w, bias, wgrad, bgrad), cos, sin, pos, nh, nkv, hd)
     if torch.is_grad_enabled() and (x.requires_grad or wgrad is not None):
         return QKVRopeFn.apply(x, w, bias, cos, sin, pos, nh, nkv, hd, wgrad, bgrad)
     x2 = _rows(x)

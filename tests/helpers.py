@@ -920,6 +920,53 @@ def accumulate_tol(old, S, e):
     return (BF16_U + FP32_U) * (old + S).abs() + (1 + 2 * BF16_U) * (BF16_U * S.abs() + (1 + BF16_U) * e) + ELEM_ABS_FLOOR
 
 
+def bias_grad_reference_fp64(dy, old):
+    """The bias gradient of kernels.LinearFn / QKVRopeFn:  bgrad = bf16(old + bf16(S')),  S' = dy.sum(0), torch's fp32 column sum of the
+    bf16 rows dy [M, N] rounded to bf16 once, then `bgrad.add_` (one fp32 add of two bf16 values, rounded to bf16).
+      torch's reduction kernel picks its own order (a chain per thread, then a tree over threads and blocks).  In any order each term goes
+      through at most M - 1 fp32 additions, so |S' - S| <= gamma_{M-1} sum_r |dy_r|, gamma_n = n 2^-24 / (1 - n 2^-24) <= M 2^-24 for
+      M <= 4096 (M (M - 1) <= 2^24).  accumulate_tol adds the two bf16 roundings.
+    Returns want = old + S and tol, float64 [N]."""
+    d = dy.double()
+    M = d.shape[0]
+    assert M <= 4096, "the first-order chain bound below holds for M <= 4096"
+    S = d.sum(0)
+    o = old.double()
+    return dict(want=o + S, tol=accumulate_tol(o, S, M * FP32_U * d.abs().sum(0)))
+
+
+def qkv_rope_reference_fp64(x, w, bias, cos, sin, pos, nh, nkv, hd, K_red):
+    """lmod_gemm_qkv_rope (and GEMM + lmod_rope, which it equals bit for bit) on x [M, K] bf16, w [N, K], bias [N] or None:
+    P = x W^T + b in float64; the q and k heads rotated, Y1 = P1 c - P2 s, Y2 = P2 c + P1 s (c, s the bf16 table rows of pos, P1 / P2 the
+    two halves of a head); the v heads Y = P.  The GEMM's bf16 p is within E = _gemm_tol(P, |x||W|^T + |b|, K_red) of P; the rotation is
+    y1 = bf16(bf16(p1 c) + bf16(-p2 s)) (y2 alike):
+      |p1 c - P1 c| <= |c| E1; rounding p1 c adds u |p1 c| <= u (|P1 c| + |c| E1), the same for p2 s, so before the last rounding the error
+      is E' = (1 + u)(|c| E1 + |s| E2) + u (|P1 c| + |P2 s|); the last rounding adds u (|Y1| + E'):
+        tol = u |Y| + (1 + u) E'.
+    Returns (want, tol), float64 [M, N]."""
+    x64, w64 = x.double(), w.double()
+    P = x64 @ w64.t()
+    maj = x64.abs() @ w64.abs().t()
+    if bias is not None:
+        P, maj = P + bias.double(), maj + bias.double().abs()
+    E = _gemm_tol(P, maj, K_red)
+    M = P.shape[0]
+    nr = nh + nkv
+    h = hd // 2
+    p = P[:, :nr * hd].view(M, nr, hd)
+    e = E[:, :nr * hd].view(M, nr, hd)
+    c, s = cos[pos].double()[:, None, :h], sin[pos].double()[:, None, :h]
+    p1, p2, e1, e2 = p[..., :h], p[..., h:], e[..., :h], e[..., h:]
+    Y = torch.cat([p1 * c - p2 * s, p2 * c + p1 * s], -1)
+    Ep = torch.cat([(1 + BF16_U) * (c.abs() * e1 + s.abs() * e2) + BF16_U * ((p1 * c).abs() + (p2 * s).abs()),
+                    (1 + BF16_U) * (c.abs() * e2 + s.abs() * e1) + BF16_U * ((p2 * c).abs() + (p1 * s).abs())], -1)
+    tol = BF16_U * Y.abs() + (1 + BF16_U) * Ep + ELEM_ABS_FLOOR
+    want, tl = P.clone(), E.clone()
+    want[:, :nr * hd] = Y.reshape(M, -1)
+    tl[:, :nr * hd] = tol.reshape(M, -1)
+    return want, tl
+
+
 def rmsnorm_wgrad_reference_fp64(dy, s, rstd_k, old):
     """lmod_rmsnorm_wgrad:  wgrad = bf16(old + bf16(sum_r t_r)),  t_r = bf16(dy_r * bf16(s_r * rstd_r)) (autograd of `w * h.to(bf16)`).
     The terms are bit exact in fp32 from the kernel's rstd; the kernel sums them in fp32: a warp walks 32 of a 256-row chunk, 8 warps are
