@@ -1160,9 +1160,10 @@ class DistillHeadFn(Function):
     def backward(ctx, g, _a, _c2):
         dlogits, w_head, h2, perm, count = ctx.saved_tensors
         # the kernel produced d(total)/d(logits); the upstream scalar g multiplies the two SMALL operands instead of the [N,V] / [V,H] results:
-        # dH = g * (dlogits @ W),  dW += dlogits^T @ (g * h)
-        gs = g.to(h2.dtype)
-        dh = mm_nn(dlogits, w_head, m_dev=count) * gs
+        # dH = g * (dlogits @ W),  dW += dlogits^T @ (g * h).  g is applied in fp32 and each product rounded to bf16 once: a g rounded to bf16
+        # first would scale both gradients by bf16(g) / g (up to 2^-9 off 1, the same sign on every element).  At g = 1 both are exact.
+        g = g.float()
+        dh = (mm_nn(dlogits, w_head, m_dev=count).float() * g).to(h2.dtype)
         if perm is not None:
             n = 1
             for d in ctx.hshape[:-1]:
@@ -1170,7 +1171,7 @@ class DistillHeadFn(Function):
             dh = scatter_rows(dh, perm, count, n)
         dh = dh.reshape(ctx.hshape)
         if ctx.head_grad is not None:
-            mm_tn_acc(dlogits, h2 * gs, ctx.head_grad, k_dev=count)
+            mm_tn_acc(dlogits, (h2.float() * g).to(h2.dtype), ctx.head_grad, k_dev=count)
         return dh, None, None, None, None, None, None, None, None, None, None, None
 
 

@@ -1340,3 +1340,164 @@ def poisoned_uninitialised_memory():
     finally:
         det.fill_uninitialized_memory = was_fill
         torch.use_deterministic_algorithms(was_det, warn_only=was_warn)
+
+
+# ---------------------------------------------------------------------------------------------------
+# gradient views for the exact autograd tests: one arena of sentinels, and the run-twice byte comparison
+# ---------------------------------------------------------------------------------------------------
+DEV = "cuda"
+SENT = -12345.0                                   # bf16 -12352
+
+
+def randn(*shape, seed, scale=1.0):
+    """Seeded bf16 normal values on the GPU."""
+    g = torch.Generator(device=DEV).manual_seed(seed)
+    return (torch.randn(*shape, generator=g, device=DEV) * scale).to(torch.bfloat16)
+
+
+class Arena:
+    """The gradient views of one case, carved out of one flat bf16 buffer as train/engine.py _pack lays the arena out, with one ALIGN unit
+    of guard in front and behind.  The views hold seeded values (what earlier micro-batches left); every other element holds SENT."""
+
+    def __init__(self, shapes, seed, scale=0.5):
+        from llavamod.train.engine import ALIGN
+        offs, off = [], ALIGN
+        for s in shapes:
+            offs.append(off)
+            off += -(-math.prod(s) // ALIGN) * ALIGN
+        self.buf = torch.full((off + ALIGN,), SENT, dtype=torch.bfloat16, device=DEV)
+        self.owned = torch.zeros(off + ALIGN, dtype=torch.bool, device=DEV)
+        self.views = []
+        for i, (o, s) in enumerate(zip(offs, shapes)):
+            n = math.prod(s)
+            v = self.buf[o:o + n].view(s)
+            v.copy_(randn(*s, seed=seed + i, scale=scale))
+            self.owned[o:o + n] = True
+            self.views.append(v)
+        self.fresh = self.buf.clone()
+
+    def snapshot(self):
+        return [v.clone() for v in self.views]
+
+    def check_sentinels(self, tag):
+        bad = (self.buf.view(torch.int16) != self.fresh.view(torch.int16)) & ~self.owned
+        n = int(bad.sum())
+        assert n == 0, f"{tag}: {n} arena elements outside the views changed; first at flat index {int(torch.nonzero(bad)[0])}"
+
+
+def no_nan(tag, **ts):
+    for name, t in ts.items():
+        if t is not None:
+            assert not bool(torch.isnan(t).any()), f"{tag}: NaN in {name}"
+
+
+def same_bytes(tag, a, b):
+    assert len(a) == len(b)
+    for i, (x, y) in enumerate(zip(a, b)):
+        iv = torch.int16 if x.element_size() == 2 else torch.int32
+        assert x.shape == y.shape and torch.equal(x.view(iv), y.view(iv)), f"{tag}: output {i} differs between two identical runs"
+
+
+def twice(tag, run, label="AUTOGRAD"):
+    """run(report) -> list of output tensors; run(None), which checks nothing, must give the same bytes."""
+    report = {}
+    first = run(report)
+    same_bytes(tag, first, run(None))
+    worst = max(report, key=report.get)
+    print(f"\n{label} {tag}: worst err/bound {report[worst]:.3g} ({worst}; {len(report)} checks)")
+
+
+# ---------------------------------------------------------------------------------------------------
+# kernels.DistillHeadFn (lm_head GEMM + fused KL/CE + the lm_head backward): float64 stage references
+# ---------------------------------------------------------------------------------------------------
+def distill_head_reference_fp64(h, W, t, labels, T, vocab, w_kd, w_ce, distill_all, g, rows=None, logits=None, dlogits=None, old=None,
+                                store=torch.float64, block_rows=256, block_cols=16384):
+    """Float64 restatement of kernels.DistillHeadFn, stage by stage, with the bounds of tests/helpers.py for each stage.
+
+    h [N, H] the hidden rows, W [V_s, H] the lm_head, labels [N] flat (B = N / T sequences), g the upstream scalar of `total`, old [V_s, H]
+    the lm_head gradient view before the call (zeros when None).  rows = (perm, count) as kernels.active_rows gives them: then t, logits and
+    dlogits hold row perm[j] of the batch in their row j < count (the compact layout); without rows they hold every row in order.
+    t [., >= vocab] are the teacher logits.  logits / dlogits [., V_s] are the kernel's stages: each stage takes its input from them when
+    given, else from this reference's own previous stage (float64, unrounded).  Works on h's device in blocks.
+
+    Returns a dict (`store` is the dtype of the [n, V_s] and [V_s, H] results):
+      act          [n] the original index of every active row (KD or CE mask), ascending
+      logits, logits_tol [n, V_s]   h[act] W^T and _gemm_tol(K = H)
+      kl           kl_reference_fp64 of the logits (placed on their original rows) against t, over the first vocab columns
+      align, ce, total              total = w_kd align + w_ce ce (w_ce = 0 drops ce, NaN included, as the Function does)
+      dh, dh_tol   [N, H]  g (d W) over the first vocab columns of d = the d logits of the active rows, zero on the other rows.  The bound is
+                   |g| _gemm_tol(d W, |d| |W|, K = V_s) for the GEMM (stored in bf16), then one fp32 product with g and one bf16 rounding
+      dW, dW_tol   [V_s, H]  old + d^T (g h[act]) (rows vocab and above: old, exact), with _gemm_tol(K = n) + 2^-23 |ref| for the fp32 add to the
+                   old value and, when g is not a power of two, 2^-8 |d|^T |g h| for the bf16 operand g h"""
+    f64 = torch.float64
+    dev = h.device
+    N, H = h.shape
+    Vs = W.shape[0]
+    gs = float(g)
+    labels = labels.reshape(-1).to(dev)
+    m_kd, m_ce, _ = kl_row_masks(labels, T, distill_all)
+    act = torch.nonzero(m_kd | m_ce)[:, 0]
+    n = act.numel()
+    if rows is not None:
+        perm, count = rows
+        assert int(count) == n and torch.equal(perm[:n].long().to(dev), act), "rows do not list the active rows"
+        src = torch.arange(n, device=dev)                              # row of the compact tensors that holds act[i]
+    else:
+        src = act
+    W64 = W.to(f64)
+    W64a = W64.abs()
+    h_act = h[act].to(f64)
+    out = dict(act=act)
+
+    lg = torch.zeros(n, Vs, dtype=store, device=dev)
+    lt = torch.zeros_like(lg)
+    for r0 in range(0, n, block_rows):
+        a = h_act[r0:r0 + block_rows]
+        ref = a @ W64.t()
+        lg[r0:r0 + block_rows] = ref.to(store)
+        lt[r0:r0 + block_rows] = _gemm_tol(ref, a.abs() @ W64a.t(), H).to(store)
+        del ref
+    out["logits"], out["logits_tol"] = lg, lt
+
+    def placed(x, idx):                                                # rows idx of x on the original rows act, zero elsewhere
+        full = torch.zeros(N, vocab, dtype=x.dtype, device=dev)
+        full[act] = x[idx, :vocab]
+        return full
+
+    s_full = placed(logits, src) if logits is not None else placed(lg, torch.arange(n, device=dev))
+    kl = kl_reference_fp64(s_full, placed(t, src), labels, T, vocab, w_kd, w_ce, distill_all, g_dtype=store)
+    del s_full
+    out["kl"], out["align"], out["ce"] = kl, kl["align"], kl["ce"]
+    out["total"] = w_kd * kl["align"] + (w_ce * kl["ce"] if w_ce != 0.0 else 0.0)
+
+    d = dlogits[src, :vocab] if dlogits is not None else kl["g"][act]  # [n, vocab]
+    Wv, Wva = W64[:vocab], W64a[:vocab]
+    dh = torch.zeros(N, H, dtype=f64, device=dev)
+    dh_tol = torch.zeros_like(dh)
+    for r0 in range(0, n, block_rows):
+        db = d[r0:r0 + block_rows].to(f64)
+        ref0 = db @ Wv
+        r = act[r0:r0 + block_rows]
+        dh[r] = gs * ref0
+        dh_tol[r] = (1 + BF16_U) * abs(gs) * _gemm_tol(ref0, db.abs() @ Wva, Vs) + (BF16_U + FP32_U) * (gs * ref0).abs()
+        del db, ref0
+    out["dh"], out["dh_tol"] = dh, dh_tol
+
+    gh = gs * h_act
+    exact_scale = gs != 0.0 and math.frexp(gs)[0] == 0.5                # g h is exact in bf16
+    dW = (old.to(store) if old is not None else torch.zeros(Vs, H, dtype=store, device=dev)).clone()
+    dW_tol = torch.zeros_like(dW)
+    for v0 in range(0, vocab, block_cols):
+        v1 = min(vocab, v0 + block_cols)
+        db = d[:, v0:v1].to(f64)
+        o = dW[v0:v1].to(f64)
+        c = db.t() @ gh
+        cm = db.abs().t() @ gh.abs()
+        ref = o + c
+        tol = _gemm_tol(ref, o.abs() + cm, n) + 2.0 ** -23 * ref.abs()
+        if not exact_scale:
+            tol = tol + BF16_U * cm
+        dW[v0:v1], dW_tol[v0:v1] = ref.to(store), tol.to(store)
+        del db, o, c, cm, ref, tol
+    out["dW"], out["dW_tol"] = dW, dW_tol
+    return out

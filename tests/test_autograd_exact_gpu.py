@@ -11,25 +11,23 @@ Every case
     references of tests/helpers.py for the rest;
   - checks every accumulated view from the value the kernels left in it after the micro-batch before: g <- bf16(g + contribution), so a
     lost, doubled or overwritten micro-batch fails at the step where it happens;
-  - runs twice and requires the same bytes from both runs.  No shape here reaches the split-K dgrad of mm_nn (the lm_head's); the one
+  - runs twice and requires the same bytes from both runs.  No shape here reaches the split-K dgrad of mm_nn (the lm_head's: see
+    test_distill_head_exact_gpu.py); the one
     fp32-atomic path that is reached, lmod_rmsnorm_wgrad from 257 rows on, is left out of the byte comparison (see test_rmsnorm_fn);
   - prints its worst err / bound."""
-import math
 import types
 
 import pytest
 import torch
 
-from tests.helpers import (BF16_U, _gemm_tol, bias_act_reference_fp64, bias_grad_reference_fp64, check_bound,  # noqa: E402
-                           embed_grad_reference_fp64, gelu_bwd_reference_fp64, poisoned_uninitialised_memory, qkv_rope_reference_fp64,
-                           rmsnorm_bwd_reference_fp64, rmsnorm_reference_fp64, rmsnorm_wgrad_reference_fp64, rope_bwd_reference_fp64,
-                           silu_mul_reference_fp64, splice_bwd_reference, splice_reference)
+from tests.helpers import (BF16_U, DEV, Arena, _gemm_tol, bias_act_reference_fp64, bias_grad_reference_fp64, check_bound,  # noqa: E402
+                           embed_grad_reference_fp64, gelu_bwd_reference_fp64, no_nan, poisoned_uninitialised_memory,
+                           qkv_rope_reference_fp64, randn, rmsnorm_bwd_reference_fp64, rmsnorm_reference_fp64, rmsnorm_wgrad_reference_fp64,
+                           rope_bwd_reference_fp64, silu_mul_reference_fp64, splice_bwd_reference, splice_reference, twice)
 
 pytestmark = pytest.mark.gpu
 
 bf16 = torch.bfloat16
-DEV = "cuda"
-SENT = -12345.0                                   # bf16 -12352
 MICRO_BATCHES = 3
 # (B, T) of the 3-D inputs: row counts 1, 127, 129, 333 and 2047 leave a tail tile in every GEMM and wgrad, 2048 is the step's T'
 ROWS = [(1, 1), (1, 127), (3, 43), (3, 111), (23, 89), (2, 1024)]
@@ -39,63 +37,6 @@ ROW_IDS = [f"rows{b * t}" for b, t in ROWS]
 def K():
     from llavamod import kernels
     return kernels
-
-
-def randn(*shape, seed, scale=1.0):
-    g = torch.Generator(device=DEV).manual_seed(seed)
-    return (torch.randn(*shape, generator=g, device=DEV) * scale).to(bf16)
-
-
-class Arena:
-    """The gradient views of one case, carved out of one flat bf16 buffer as train/engine.py _pack lays the arena out, with one ALIGN unit
-    of guard in front and behind.  The views hold seeded values (what earlier micro-batches left); every other element holds SENT."""
-
-    def __init__(self, shapes, seed, scale=0.5):
-        from llavamod.train.engine import ALIGN
-        offs, off = [], ALIGN
-        for s in shapes:
-            offs.append(off)
-            off += -(-math.prod(s) // ALIGN) * ALIGN
-        self.buf = torch.full((off + ALIGN,), SENT, dtype=bf16, device=DEV)
-        self.owned = torch.zeros(off + ALIGN, dtype=torch.bool, device=DEV)
-        self.views = []
-        for i, (o, s) in enumerate(zip(offs, shapes)):
-            n = math.prod(s)
-            v = self.buf[o:o + n].view(s)
-            v.copy_(randn(*s, seed=seed + i, scale=scale))
-            self.owned[o:o + n] = True
-            self.views.append(v)
-        self.fresh = self.buf.clone()
-
-    def snapshot(self):
-        return [v.clone() for v in self.views]
-
-    def check_sentinels(self, tag):
-        bad = (self.buf.view(torch.int16) != self.fresh.view(torch.int16)) & ~self.owned
-        n = int(bad.sum())
-        assert n == 0, f"{tag}: {n} arena elements outside the views changed; first at flat index {int(torch.nonzero(bad)[0])}"
-
-
-def no_nan(tag, **ts):
-    for name, t in ts.items():
-        if t is not None:
-            assert not bool(torch.isnan(t).any()), f"{tag}: NaN in {name}"
-
-
-def same_bytes(tag, a, b):
-    assert len(a) == len(b)
-    for i, (x, y) in enumerate(zip(a, b)):
-        iv = torch.int16 if x.element_size() == 2 else torch.int32
-        assert x.shape == y.shape and torch.equal(x.view(iv), y.view(iv)), f"{tag}: output {i} differs between two identical runs"
-
-
-def twice(tag, run):
-    """run(report) -> list of output tensors; run(None), which checks nothing, must give the same bytes."""
-    report = {}
-    first = run(report)
-    same_bytes(tag, first, run(None))
-    worst = max(report, key=report.get)
-    print(f"\nAUTOGRAD {tag}: worst err/bound {report[worst]:.3g} ({worst}; {len(report)} checks)")
 
 
 def gemm_check(name, got, A, B, k_red, report, bias=None, old=None):
