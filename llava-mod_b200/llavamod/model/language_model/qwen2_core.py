@@ -320,7 +320,6 @@ class Qwen2Model(nn.Module):
         Returns (final-normed hidden [B,T,H], [l_aux per MoE layer], routing records)."""
         if cache is not None and cache.length > 0:
             return self._decode_step(inputs_embeds, moe_noise, training_moe, cache)
-        cfg = self.config
         B, T, H = inputs_embeds.shape
         dev = inputs_embeds.device
         padded = attention_mask is not None and not bool(attention_mask.all())      # MaskInfo answers on the host (no sync)
@@ -349,62 +348,21 @@ class Qwen2Model(nn.Module):
             position_ids = torch.arange(T, device=dev, dtype=torch.int64).unsqueeze(0).expand(B, T)
         pos = position_ids.reshape(-1).to(torch.int64).contiguous()
         cos, sin = self.rope(T, dev, inputs_embeds.dtype)
-
-        stream = inputs_embeds.reshape(B * T, H)
-        branch = None                                   # pending residual-branch output (added inside the next norm)
-        l_auxes, records = [], []
-        moe_i = 0
         if moe_noise is None:
             # DeepSpeed draws fresh Gumbel noise (top-2) or uniforms (top-1's token selection) in every MoE layer; one draw for all layers
             # of this forward is the same distribution with 5 launches instead of 5 per layer
             moes = [l.mlp for l in self.layers if isinstance(l.mlp, MoE)]
             if moes and len({(m.num_experts, m.k) for m in moes}) == 1:
                 moe_noise = moe_draw((len(moes), B * T, moes[0].num_experts), moes[0].k, dev).unbind(0)
-        for li, layer in enumerate(self.layers):
-            at = layer.self_attn
-            nh, nkv, hd = at.num_heads, at.num_key_value_heads, at.head_dim
-            fp8 = isinstance(at.qkv_weight, K.Fp8Rows)      # a layer of quantize_fp8_: the norms hand e4m3 rows to e4m3 projections
-            if fp8:
-                x, stream = K.rmsnorm_quant(stream if branch is None else branch, layer.input_layernorm.weight, cfg.rms_norm_eps,
-                                            res=None if branch is None else stream)
-                qkv = K.qkv_rope_fp8(x, at.qkv_weight, at.qkv_bias, cos, sin, pos, nh, nkv, hd)
-            else:
-                if branch is None:
-                    x, stream = K.rmsnorm(stream, layer.input_layernorm.weight, cfg.rms_norm_eps, wgrad=self.gview(layer.input_layernorm.weight))
-                else:
-                    x, stream = K.rmsnorm(branch, layer.input_layernorm.weight, cfg.rms_norm_eps, res=stream, wgrad=self.gview(layer.input_layernorm.weight))
-                qkv = K.qkv_rope(x, at.qkv_weight, at.qkv_bias, cos, sin, pos, nh, nkv, hd, self.gview(at.qkv_weight), self.gview(at.qkv_bias))
+
+        def attend(li, qkv, nh, nkv, hd):
             if ragged:
                 K.kv_append_rows(qkv, B, T, nh, nkv, hd, cache.k[li], cache.v[li], pad[0], pad[1], cache.len)
             elif cache is not None:
                 K.kv_append(qkv, B, T, nh, nkv, hd, cache.k[li], cache.v[li], cache.len)
-            attn = K.attention(qkv, B, T, nh, nkv, hd, True, None, pad)
-            if fp8:
-                branch = K.linear_fp8(attn, at.o_fp8)
-                x, stream = K.rmsnorm_quant(branch, layer.post_attention_layernorm.weight, cfg.rms_norm_eps, res=stream)
-            else:
-                branch = K.linear(attn, at.o_proj.weight, None, self.gview(at.o_proj.weight), None)
-                x, stream = K.rmsnorm(branch, layer.post_attention_layernorm.weight, cfg.rms_norm_eps, res=stream,
-                                      wgrad=self.gview(layer.post_attention_layernorm.weight))
-            mlp = layer.mlp
-            if isinstance(mlp, MoE):
-                E = mlp.num_experts
-                noise = moe_noise[moe_i] if moe_noise is not None else moe_draw((B * T, E), mlp.k, dev)
-                moe_i += 1
-                cf = mlp.capacity_factor if training_moe else mlp.eval_capacity_factor
-                stream, l_aux, rec = mlp.run(x, stream, noise, cf, self.gview)
-                if rec is not None:
-                    records.append(rec)
-                l_auxes.append(l_aux)
-                branch = None
-            elif fp8:
-                branch = K.mlp_fp8(x, mlp.gu_weight, mlp.down_fp8)
-            else:
-                branch = K.mlp(x, mlp.gu_weight, mlp.down_proj.weight, self.gview(mlp.gu_weight), self.gview(mlp.down_proj.weight))
-        if branch is None:
-            out, _ = K.rmsnorm(stream, self.norm.weight, cfg.rms_norm_eps, wgrad=self.gview(self.norm.weight))
-        else:
-            out, _ = K.rmsnorm(branch, self.norm.weight, cfg.rms_norm_eps, res=stream, wgrad=self.gview(self.norm.weight))
+            return K.attention(qkv, B, T, nh, nkv, hd, True, None, pad)
+
+        out, l_auxes, records = self._layers(inputs_embeds.reshape(B * T, H), cos, sin, pos, attend, moe_noise, training_moe)
         if ragged:
             cache.len.add_(pad[1] - pad[0])
             cache.advance(lengths)
@@ -413,6 +371,7 @@ class Qwen2Model(nn.Module):
             cache.advance(T)
         return out.view(B, T, H), l_auxes, records
 
+    @torch.no_grad()
     def _decode_step(self, inputs_embeds, moe_noise, training_moe, cache):
         """One cached step: each sequence's new token sits at position len[b] (the reference's rule for a cached step,
         llava_arch.py:162-172, on unpadded prompts; for a padded prompt len[b] = n_b + s counts its real rows only), its k / v are appended
@@ -424,10 +383,8 @@ class Qwen2Model(nn.Module):
         Everything the step reads about the position is on the device, so the step can be captured once and replayed.  MoE layers route
         the B new tokens alone (top2gating / top1gating with S = B, as MoEQwen1_5Model_forward does with a cache,
         llava_qwen1_5_moe.py:223-236).
-        The layer body is forward's no-grad layer body with the attention swapped for append + decode attention: the same norm
-        choices, the same MoE call and final norm.  A change to one loop must be made to the other;
-        tests/test_decode_gpu.py checks that the two give the same K / V, bit for bit."""
-        cfg = self.config
+        The step builds no autograd graph, whatever the caller's grad mode: decode attention has no backward, and the cached path is for
+        decoding (it takes no labels)."""
         B, T, H = inputs_embeds.shape
         if T != 1 and any(isinstance(l.mlp, MoE) for l in self.layers):
             raise NotImplementedError("a cached step of the sparse model decodes one token per sequence (got %d): a step of T tokens would "
@@ -443,52 +400,62 @@ class Qwen2Model(nn.Module):
         else:
             pos = (cache.len.to(torch.int64)[:, None] + torch.arange(T, device=dev, dtype=torch.int64)[None, :]).reshape(B * T)
             ws = cache.chunk_workspace(T)
-        stream = inputs_embeds.reshape(B * T, H)
-        branch = None
+
+        def attend(li, qkv, nh, nkv, hd):
+            K.kv_append(qkv, B, T, nh, nkv, hd, cache.k[li], cache.v[li], cache.len)
+            if T == 1:
+                return K.attn_decode(qkv, nh, nkv, hd, cache.k[li], cache.v[li], cache.end, cache.ws)[0]
+            return K.attn_decode_chunk(qkv, B, T, nh, nkv, hd, cache.k[li], cache.v[li], cache.end, ws)[0]
+
+        out, l_auxes, records = self._layers(inputs_embeds.reshape(B * T, H), cos, sin, pos, attend, moe_noise, training_moe)
+        cache.len.copy_(cache.end)
+        cache.advance(T)
+        return out.view(B, T, H), l_auxes, records
+
+    def _layers(self, stream, cos, sin, pos, attend, moe_noise, training_moe):
+        """The decoder layers and the final norm on the residual stream [S,H]: -> (final-normed hidden [S,H], [l_aux per MoE layer],
+        routing records).  attend(li, qkv, nh, nkv, hd) -> attn is layer li's attention on its RoPE'd q|k|v rows, the one part in which
+        forward and the cached step differ.  moe_noise: one tensor per MoE layer, or None to draw each layer's noise for its S tokens."""
+        eps = self.config.rms_norm_eps
+        branch = None                                   # pending residual-branch output (added inside the next norm)
         l_auxes, records = [], []
         moe_i = 0
         for li, layer in enumerate(self.layers):
             at = layer.self_attn
             nh, nkv, hd = at.num_heads, at.num_key_value_heads, at.head_dim
-            fp8 = isinstance(at.qkv_weight, K.Fp8Rows)
-            norm = K.rmsnorm_quant if fp8 else K.rmsnorm
-            if branch is None:
-                x, stream = norm(stream, layer.input_layernorm.weight, cfg.rms_norm_eps)
+            fp8 = isinstance(at.qkv_weight, K.Fp8Rows)      # a layer of quantize_fp8_: the norms hand e4m3 rows to e4m3 projections
+            x, res = (stream, None) if branch is None else (branch, stream)
+            if fp8:
+                x, stream = K.rmsnorm_quant(x, layer.input_layernorm.weight, eps, res=res)
+                qkv = K.qkv_rope_fp8(x, at.qkv_weight, at.qkv_bias, cos, sin, pos, nh, nkv, hd)
             else:
-                x, stream = norm(branch, layer.input_layernorm.weight, cfg.rms_norm_eps, res=stream)
-            qkv = (K.qkv_rope_fp8 if fp8 else K.qkv_rope)(x, at.qkv_weight, at.qkv_bias, cos, sin, pos, nh, nkv, hd)
-            K.kv_append(qkv, B, T, nh, nkv, hd, cache.k[li], cache.v[li], cache.len)
-            if T == 1:
-                attn, _ = K.attn_decode(qkv, nh, nkv, hd, cache.k[li], cache.v[li], cache.end, cache.ws)
-            else:
-                attn, _ = K.attn_decode_chunk(qkv, B, T, nh, nkv, hd, cache.k[li], cache.v[li], cache.end, ws)
+                x, stream = K.rmsnorm(x, layer.input_layernorm.weight, eps, res=res, wgrad=self.gview(layer.input_layernorm.weight))
+                qkv = K.qkv_rope(x, at.qkv_weight, at.qkv_bias, cos, sin, pos, nh, nkv, hd, self.gview(at.qkv_weight), self.gview(at.qkv_bias))
+            attn = attend(li, qkv, nh, nkv, hd)
             if fp8:
                 branch = K.linear_fp8(attn, at.o_fp8)
-                x, stream = K.rmsnorm_quant(branch, layer.post_attention_layernorm.weight, cfg.rms_norm_eps, res=stream)
+                x, stream = K.rmsnorm_quant(branch, layer.post_attention_layernorm.weight, eps, res=stream)
             else:
-                branch = K.linear(attn, at.o_proj.weight)
-                x, stream = K.rmsnorm(branch, layer.post_attention_layernorm.weight, cfg.rms_norm_eps, res=stream)
+                branch = K.linear(attn, at.o_proj.weight, None, self.gview(at.o_proj.weight), None)
+                x, stream = K.rmsnorm(branch, layer.post_attention_layernorm.weight, eps, res=stream,
+                                      wgrad=self.gview(layer.post_attention_layernorm.weight))
             mlp = layer.mlp
             if isinstance(mlp, MoE):
-                noise = moe_noise[moe_i] if moe_noise is not None else moe_draw((B, mlp.num_experts), mlp.k, dev)
+                noise = moe_noise[moe_i] if moe_noise is not None else moe_draw((stream.shape[0], mlp.num_experts), mlp.k, stream.device)
                 moe_i += 1
                 cf = mlp.capacity_factor if training_moe else mlp.eval_capacity_factor
-                with torch.no_grad():
-                    stream, l_aux, rec = mlp.run(x, stream, noise, cf, self.gview)
-                records.append(rec)
+                stream, l_aux, rec = mlp.run(x, stream, noise, cf, self.gview)
+                if rec is not None:
+                    records.append(rec)
                 l_auxes.append(l_aux)
                 branch = None
             elif fp8:
                 branch = K.mlp_fp8(x, mlp.gu_weight, mlp.down_fp8)
             else:
-                branch = K.mlp(x, mlp.gu_weight, mlp.down_proj.weight)
-        if branch is None:
-            out, _ = K.rmsnorm(stream, self.norm.weight, cfg.rms_norm_eps)
-        else:
-            out, _ = K.rmsnorm(branch, self.norm.weight, cfg.rms_norm_eps, res=stream)
-        cache.len.copy_(cache.end)
-        cache.advance(T)
-        return out.view(B, T, H), l_auxes, records
+                branch = K.mlp(x, mlp.gu_weight, mlp.down_proj.weight, self.gview(mlp.gu_weight), self.gview(mlp.down_proj.weight))
+        x, res = (stream, None) if branch is None else (branch, stream)
+        out, _ = K.rmsnorm(x, self.norm.weight, eps, res=res, wgrad=self.gview(self.norm.weight))
+        return out, l_auxes, records
 
 
 class KVCache:

@@ -83,6 +83,29 @@ def test_prefill_and_decode_cache_bit_identical_to_recompute(monkeypatch, heads,
         next_token_logits(model, toks[:, :1], cache=full)         # one position past max_len: refused before anything is written
 
 
+@pytest.mark.parametrize("T", [1, 3])                                  # the one-token step and the verify step of assisted decoding
+def test_cached_step_builds_no_graph_with_grad_enabled(T):
+    """A cached step of a model whose embedding trains, called with grad enabled, returns a hidden state that needs no grad (decode
+    attention has no backward), with the bytes of the same step under no_grad and the same K / V."""
+    model = _teacher(seed=27)
+    model.model.embed_tokens.weight.requires_grad_(True)
+    batch, _ = Hh.tiny_batch(model, B=2, Tt=24, seed=28)
+    ids, images = batch["input_ids"].cuda(), batch["images"]
+    toks = torch.randint(0, model.config.vocab_size, (2, T), generator=torch.Generator().manual_seed(29)).cuda()
+    caches = [model.new_kv_cache(2, 64) for _ in range(2)]
+    with torch.no_grad():
+        for c in caches:
+            model.forward_hidden(input_ids=ids, images=images, cache=c)
+        ref = model.forward_hidden(input_ids=toks, cache=caches[0])["hidden"]
+    with torch.enable_grad():
+        got = model.forward_hidden(input_ids=toks, cache=caches[1])["hidden"]
+    assert not got.requires_grad and got.grad_fn is None
+    assert torch.equal(got, ref)
+    assert caches[0].len.tolist() == caches[1].len.tolist() == [caches[0].length] * 2
+    for i in range(model.config.num_hidden_layers):
+        assert torch.equal(caches[0][i][0], caches[1][i][0]) and torch.equal(caches[0][i][1], caches[1][i][1]), i
+
+
 @pytest.mark.parametrize("name", ["decode_mha_hd32", "decode_gqa_4_2", "decode_hd64_kv1", "decode_text_only"])
 def test_cached_forward_matches_reference_golden(name, golden_dir):
     """The reference's own cached decoding (tests/golden/make_decode_golden.py: prefill + teacher-forced cached steps) against
