@@ -224,6 +224,14 @@ int lmod_sumsq(const void* g_bf16_or_f32, int is_f32, int64_t count, float* out_
 int lmod_adamw(float* master, float* m, float* v, const void* grad, int grad_is_f32, void* model_bf16,
                int64_t count, float lr, float beta1, float beta2, float eps, float wd, int64_t step,
                const float* gnorm_sq /* optional */, float max_norm, float grad_scale, void* stream);
+/* The same step with 8-bit block-wise moments: the reference's --optim adamw_bnb_8bit / adamw_8bit, which HF's
+ * Trainer.get_optimizer_cls_and_kwargs maps to bitsandbytes' 8-bit AdamW (align_trainer.py:409-429).  m8 / v8 [count] uint8 codes of
+ * bitsandbytes' signed / unsigned dynamic maps; absmax_m / absmax_v [ceil(count / 2048)] fp32 scales, one per 2048-element block from
+ * the start of the buffer.  grad and model are bf16 (model optional).  master, m8, v8, grad, model 16B aligned; count % 8 == 0; step >= 1.
+ * Semantics (block rule, rounding, NaN): DESIGN.md section 5. */
+int lmod_adamw_8bit(float* master, uint8_t* m8, uint8_t* v8, float* absmax_m, float* absmax_v, const void* grad_bf16,
+                    void* model_bf16, int64_t count, float lr, float beta1, float beta2, float eps, float wd, int64_t step,
+                    const float* gnorm_sq /* optional */, float max_norm, float grad_scale, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * K5/K8/K9/K12/K14: hand-written wgmma + TMA GEMM  D[M,N] (+)= A[M,K] * B[N,K]^T, bf16 in, fp32 register accumulate.

@@ -97,6 +97,13 @@ __device__ __forceinline__ float block_max(float v, float* red) {
   return r;
 }
 
+// max that returns NaN when an operand is NaN (PTX max.NaN, sm_80+; fmaxf returns the non-NaN operand)
+__device__ __forceinline__ float max_nan(float a, float b) {
+  float r;
+  asm("max.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+  return r;
+}
+
 __device__ __forceinline__ uint4 ldg_nc_v4(const void* p) {
   uint4 r;
   asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];"

@@ -9,8 +9,8 @@
 // kept (no flush to zero); an all-zero row gets scale 1 and zero bytes.  x ~= scale * q.
 // Non-finite rows: a row holding a NaN gets scale NaN and NaN bytes; a row holding an inf gets scale inf, NaN bytes at its infinite
 // elements and +-0 elsewhere.  Either way every column of that row of an e4m3 GEMM is NaN, as in the bf16 teacher, and no other row
-// changes.  (fmaxf / fminf return the non-NaN operand, which would turn such a row into finite -448's: hence max_nan / clamp448 below,
-// kept local to this file.)
+// changes.  (fmaxf / fminf return the non-NaN operand, which would turn such a row into finite -448's: hence max_nan (common.cuh) and
+// clamp448 below.)
 // tests/fp8_oracle.py restates exactly this; lmod_quant_rows_e4m3 and lmod_rmsnorm_quant_e4m3 are bit-equal to it.
 //
 // One CTA of 128 threads per row.  The row is read from global memory once (16-byte loads), parked in shared memory while the block
@@ -32,12 +32,7 @@ __device__ __forceinline__ uint4 pack8(const float* f) {
   o.x = pack_bf16x2(f[0], f[1]); o.y = pack_bf16x2(f[2], f[3]); o.z = pack_bf16x2(f[4], f[5]); o.w = pack_bf16x2(f[6], f[7]);
   return o;
 }
-// max and clamp that return NaN when an operand is NaN (PTX max.NaN / min.NaN, sm_80+)
-__device__ __forceinline__ float max_nan(float a, float b) {
-  float r;
-  asm("max.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
-  return r;
-}
+// clamp that returns NaN when the operand is NaN (PTX max.NaN / min.NaN, sm_80+; max_nan is in common.cuh)
 __device__ __forceinline__ float clamp448(float v) {
   float r;
   asm("max.NaN.f32 %0, %1, 0fC3E00000;\n\tmin.NaN.f32 %0, %0, 0f43E00000;" : "=f"(r) : "f"(v));     // -448, 448

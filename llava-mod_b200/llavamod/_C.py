@@ -60,6 +60,7 @@ SIGNATURES = {
     "lmod_splice_embed_bwd": [_P, _P, _P, _L, _L, _L, _P, _P],
     "lmod_sumsq": [_P, _I, _L, _P, _P],
     "lmod_adamw": [_P, _P, _P, _P, _I, _P, _L, _F, _F, _F, _F, _F, _L, _P, _F, _F, _P],
+    "lmod_adamw_8bit": [_P, _P, _P, _P, _P, _P, _P, _L, _F, _F, _F, _F, _F, _L, _P, _F, _F, _P],
     "lmod_gemm_bf16": [_P, _L, _I, _P, _L, _I, _P, _L, _L, _L, _L, _P, _I, _P, _P],
     "lmod_gemm_bf16_dyn": [_P, _L, _I, _P, _L, _I, _P, _L, _L, _L, _L, _P, _I, _P, _P, _P, _P],
     "lmod_gemm_qkv_rope": [_P, _L, _P, _L, _P, _P, _L, _L, _L, _I, _I, _I, _P, _P, _P, _P],

@@ -1252,6 +1252,9 @@ def align_loss_dense(logp, probs, labels, distill_all=False):
 # ---------------------------------------------------------------------------------------------------
 # optimizer
 # ---------------------------------------------------------------------------------------------------
+ADAMW8_BLOCK = 2048          # elements per absmax of the 8-bit state (A8_BLOCK in csrc/optim.cu)
+
+
 def sumsq_(buf, out):
     call("lmod_sumsq", ptr(buf), 1 if buf.dtype == torch.float32 else 0, buf.numel(), ptr(out))
 
@@ -1260,3 +1263,21 @@ def adamw_(master, m, v, grad, model, lr, beta1, beta2, eps, wd, step, gnorm_sq=
     call("lmod_adamw", ptr(master), ptr(m), ptr(v), ptr(grad), 1 if grad.dtype == torch.float32 else 0,
          ptr(model) if model is not None else None, master.numel(), float(lr), float(beta1), float(beta2), float(eps), float(wd),
          int(step), ptr(gnorm_sq) if gnorm_sq is not None else None, float(max_norm), float(grad_scale))
+
+
+def adamw_8bit_(master, m8, v8, absmax_m, absmax_v, grad, model, lr, beta1, beta2, eps, wd, step, gnorm_sq=None, max_norm=0.0,
+                grad_scale=1.0):
+    """adamw_ with 8-bit block-wise moments (``--optim adamw_bnb_8bit``): codes ``m8`` / ``v8`` [n] uint8, scales ``absmax_m`` /
+    ``absmax_v`` [ceil(n / 2048)] fp32, ``grad`` bf16."""
+    _need_cuda(master, m8, v8, absmax_m, absmax_v, grad, model)
+    if grad.dtype != BF16 or m8.dtype != torch.uint8 or v8.dtype != torch.uint8 or absmax_m.dtype != torch.float32 \
+            or absmax_v.dtype != torch.float32:
+        raise _C.LmodError("adamw_8bit_: bf16 gradient, uint8 codes and fp32 scales expected")
+    n = master.numel()
+    nb = (n + ADAMW8_BLOCK - 1) // ADAMW8_BLOCK
+    if not (m8.numel() == v8.numel() == grad.numel() == n and absmax_m.numel() == absmax_v.numel() == nb
+            and (model is None or model.numel() == n)):
+        raise _C.LmodError("adamw_8bit_: %d elements need %d codes per moment and %d scales per moment" % (n, n, nb))
+    call("lmod_adamw_8bit", ptr(master), ptr(m8), ptr(v8), ptr(absmax_m), ptr(absmax_v), ptr(grad), ptr(model) if model is not None else None,
+         n, float(lr), float(beta1), float(beta2), float(eps), float(wd), int(step), ptr(gnorm_sq) if gnorm_sq is not None else None,
+         float(max_norm), float(grad_scale))

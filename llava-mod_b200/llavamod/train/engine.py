@@ -22,6 +22,28 @@ from ..model.language_model.qwen2_core import Experts, Qwen2Attention, Qwen2MLP
 
 ALIGN = 128  # elements
 
+# --optim values that select 8-bit block-wise AdamW state (HF's names for bitsandbytes' 8-bit AdamW, align_trainer.py:409-429); every other
+# value keeps the fp32 moments
+OPTIM_8BIT = ("adamw_bnb_8bit", "adamw_8bit")
+
+
+def optim_bits_of(optim):
+    """Bits of optimizer state a ``--optim`` value selects: 8 for the bitsandbytes 8-bit AdamW names, 32 otherwise."""
+    return 8 if optim in OPTIM_8BIT else 32
+
+
+def state_bytes(slice_lengths16, n16, n32, optim_bits=32):
+    """Bytes of optimizer state (fp32 master + moments, not the bf16 weights / gradients) for a bf16 arena of ``n16`` elements cut into
+    optimizer-group slices of ``slice_lengths16`` and an fp32 arena of ``n32``.  32 bits: fp32 master, m, v (12 B per bf16 element).
+    8 bits: fp32 master, uint8 m and v codes (6 B per element) + two fp32 scales per started 2048-element block of every slice.
+    The fp32 arena keeps fp32 moments either way (the fp32 weights are the master there)."""
+    if optim_bits == 8:
+        blocks = sum((L + K.ADAMW8_BLOCK - 1) // K.ADAMW8_BLOCK for L in slice_lengths16)
+        b16 = 6 * n16 + 8 * blocks
+    else:
+        b16 = 12 * n16
+    return b16 + 8 * n32
+
 
 def _units(model):
     """Yields (storage_tensor, [member Parameters]) -- fused buffers first, then every remaining parameter."""
@@ -61,8 +83,11 @@ def param_group_of(name, in_layernorm, projector_lr_set):
 
 class TrainState:
     def __init__(self, model, lr=2e-5, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, max_grad_norm=1.0,
-                 process_group=None, mm_projector_lr=None):
+                 process_group=None, mm_projector_lr=None, optim_bits=32):
+        if optim_bits not in (8, 32):
+            raise ValueError("optim_bits must be 32 or 8, got %r" % (optim_bits,))
         self.model = model
+        self.optim_bits = optim_bits
         self.lr, self.betas, self.eps, self.wd, self.max_grad_norm = lr, betas, eps, weight_decay, max_grad_norm
         self.mm_projector_lr = mm_projector_lr
         self.pg = process_group
@@ -97,8 +122,21 @@ class TrainState:
         self.n16 = self._pack(u16, torch.bfloat16, dev, "16")
         self.n32 = self._pack(u32, torch.float32, dev, "32")
         self.master = self.w16.float() if self.n16 else None
-        self.m16 = torch.zeros_like(self.master) if self.n16 else None
-        self.v16 = torch.zeros_like(self.master) if self.n16 else None
+        self.m16 = self.v16 = self.m8 = self.v8 = self.absmax = None
+        if self.n16 and optim_bits == 32:
+            self.m16 = torch.zeros_like(self.master)
+            self.v16 = torch.zeros_like(self.master)
+        elif self.n16:
+            # 8-bit state: codes per element, and per group slice [absmax_m | absmax_v] over its 2048-element blocks (the first block at the
+            # slice start, the last one partial).  All-zero scales dequantise every code to 0: the fresh state.
+            self.m8 = torch.zeros(self.master.numel(), dtype=torch.uint8, device=dev)
+            self.v8 = torch.zeros(self.master.numel(), dtype=torch.uint8, device=dev)
+            self.scale_slices, off = [], 0
+            for _, a, b in self.segments["16"]:
+                nb = (b - a + K.ADAMW8_BLOCK - 1) // K.ADAMW8_BLOCK
+                self.scale_slices.append((off, nb))
+                off += 2 * nb
+            self.absmax = torch.zeros(off, dtype=torch.float32, device=dev)
         self.m32 = torch.zeros_like(self.w32) if self.n32 else None
         self.v32 = torch.zeros_like(self.w32) if self.n32 else None
         self.gnorm_sq = torch.zeros(1, dtype=torch.float32, device=dev)
@@ -152,6 +190,10 @@ class TrainState:
         setattr(self, "g" + tag, g)
         return off
 
+    def state_bytes(self):
+        """Bytes of the optimizer state this TrainState holds, counted by ``state_bytes`` from its layout."""
+        return state_bytes([b - a for _, a, b in self.segments["16"]], self.n16, self.n32, self.optim_bits)
+
     # ---------------------------------------------------------------------------------------------
     def zero_grad(self):
         self.grads_reduced = False
@@ -193,8 +235,14 @@ class TrainState:
         # one fused AdamW launch per optimizer group (a contiguous slice of the arenas); the clip coefficient is global (one norm over
         # every group, as torch.nn.utils.clip_grad_norm_ over all parameters), the projector group follows the same schedule scaled to its
         # own base LR (HF schedulers multiply each group's initial lr by the same lambda)
-        for (is_proj, no_decay), a, b in (self.segments["16"] if self.n16 else []):
+        for i, ((is_proj, no_decay), a, b) in enumerate(self.segments["16"] if self.n16 else []):
             g_lr = lr * (self.mm_projector_lr / self.lr) if (is_proj and self.lr) else lr
+            if self.optim_bits == 8:
+                so, nb = self.scale_slices[i]
+                K.adamw_8bit_(self.master[a:b], self.m8[a:b], self.v8[a:b], self.absmax[so:so + nb], self.absmax[so + nb:so + 2 * nb],
+                              self.g16[a:b], self.w16[a:b], g_lr, self.betas[0], self.betas[1], self.eps, 0.0 if no_decay else self.wd,
+                              self.step_count, gn, mx, grad_scale)
+                continue
             K.adamw_(self.master[a:b], self.m16[a:b], self.v16[a:b], self.g16[a:b], self.w16[a:b], g_lr, self.betas[0], self.betas[1], self.eps,
                      0.0 if no_decay else self.wd, self.step_count, gn, mx, grad_scale)
         for (is_proj, no_decay), a, b in (self.segments["32"] if self.n32 else []):

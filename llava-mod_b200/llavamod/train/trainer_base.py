@@ -15,7 +15,7 @@ from collections import defaultdict
 import torch
 import torch.distributed as dist
 
-from .engine import TrainState, cosine_lr, warmup_steps_of
+from .engine import TrainState, cosine_lr, optim_bits_of, warmup_steps_of
 
 
 def _with_lookahead(iterable):
@@ -75,12 +75,15 @@ class BaseTrainer:
     def create_optimizer(self):
         """Fused AdamW over the flat arenas with the reference's parameter groups (align_trainer.py:326-434): decay / no-decay (names
         containing "bias", nn.LayerNorm parameters) and, with --mm_projector_lr, the projector's own LR groups -- each a contiguous slice
-        of the arenas (engine.TrainState).  DeepSpeed's split into MoE expert groups changes no hyper-parameter and is not mirrored."""
+        of the arenas (engine.TrainState).  DeepSpeed's split into MoE expert groups changes no hyper-parameter and is not mirrored.
+        ``--optim adamw_bnb_8bit`` / ``adamw_8bit`` (HF's bitsandbytes 8-bit AdamW, align_trainer.py:409-429) keep the moments of the bf16
+        arena as 8-bit block-wise codes; every other value keeps fp32 moments."""
         if self.optimizer is None:
             a = self.args
             self.optimizer = TrainState(self.model, lr=a.learning_rate, betas=(a.adam_beta1, a.adam_beta2), eps=a.adam_epsilon,
                                         weight_decay=a.weight_decay, max_grad_norm=a.max_grad_norm,
-                                        mm_projector_lr=getattr(a, "mm_projector_lr", None))
+                                        mm_projector_lr=getattr(a, "mm_projector_lr", None),
+                                        optim_bits=optim_bits_of(getattr(a, "optim", "adamw_torch")))
         return self.optimizer
 
     def current_lr(self):
@@ -322,7 +325,11 @@ class BaseTrainer:
         if self.rank == 0:
             self.model.save_pretrained(d)
             opt = self.optimizer
-            if opt is not None:
+            if opt is not None and opt.optim_bits == 8:
+                torch.save({"optim": "adamw_8bit", "master": opt.master, "m8": opt.m8, "v8": opt.v8, "absmax": opt.absmax,
+                            "w32": getattr(opt, "w32", None), "m32": opt.m32, "v32": opt.v32, "step_count": opt.step_count},
+                           os.path.join(d, "optimizer.pt"))
+            elif opt is not None:
                 torch.save({"master": opt.master, "m16": opt.m16, "v16": opt.v16, "w32": getattr(opt, "w32", None), "m32": opt.m32,
                             "v32": opt.v32, "step_count": opt.step_count}, os.path.join(d, "optimizer.pt"))
             with open(os.path.join(d, "trainer_state.json"), "w") as f:
@@ -369,7 +376,13 @@ class BaseTrainer:
         op = os.path.join(d, "optimizer.pt")
         if os.path.exists(op):
             st = torch.load(op, map_location=self.model.device, weights_only=True)
-            for k in ("master", "m16", "v16", "m32", "v32"):
+            saved_bits = 8 if st.get("optim") == "adamw_8bit" else 32          # checkpoints without the key hold fp32 moments
+            if saved_bits != opt.optim_bits:
+                raise ValueError("%s holds %d-bit AdamW state (%s) but this run has --optim %s (%d-bit state); resume with the --optim the "
+                                 "checkpoint was saved with -- the state is not converted" % (
+                                     op, saved_bits, "--optim adamw_bnb_8bit / adamw_8bit" if saved_bits == 8 else "--optim adamw_torch",
+                                     self.args.optim, opt.optim_bits))
+            for k in ("master", "m16", "v16", "m8", "v8", "absmax", "m32", "v32"):
                 if st.get(k) is not None and getattr(opt, k) is not None:
                     getattr(opt, k).copy_(st[k])
             opt.step_count = st["step_count"]
