@@ -32,7 +32,7 @@ def nvtx(name):
 
 
 def _c(t):
-    return t if t.is_contiguous() else t.contiguous()
+    return t if t is None or t.is_contiguous() else t.contiguous()
 
 
 def _need_cuda(*ts):
@@ -102,7 +102,7 @@ def gather_rows(x2, perm, count, out=None):
     n, h = x2.shape
     if out is None:
         out = torch.empty((n + ROW_PAD - 1) // ROW_PAD * ROW_PAD, h, dtype=x2.dtype, device=x2.device)
-    call("lmod_gather_rows", ptr(x2), x2.stride(0), ptr(perm) if perm is not None else None, ptr(count), out.shape[0], h, ROW_PAD,
+    call("lmod_gather_rows", ptr(x2), x2.stride(0), ptr(perm), ptr(count), out.shape[0], h, ROW_PAD,
          ptr(out), out.stride(0))
     return out
 
@@ -120,16 +120,14 @@ def gemm(a, b, a_mn=False, b_mn=False, bias=None, out=None, accumulate=False, ou
     _need_cuda(a, b)
     M, K = (a.shape[1], a.shape[0]) if a_mn else (a.shape[0], a.shape[1])
     N = b.shape[1] if b_mn else b.shape[0]
-    dyn = (ptr(m_dev) if m_dev is not None else None, ptr(k_dev) if k_dev is not None else None)
-    if out_f32 is not None:
-        call("lmod_gemm_bf16_dyn", ptr(a), a.stride(0), int(a_mn), ptr(b), b.stride(0), int(b_mn), None, out_f32.stride(0), M, N, K, None,
-             (int(split_k) << 8) if split_k > 1 else 0, ptr(out_f32), *dyn)
-        return out_f32
-    if out is None:
-        out = torch.empty(M, N, dtype=a.dtype, device=a.device)
-    call("lmod_gemm_bf16_dyn", ptr(a), a.stride(0), int(a_mn), ptr(b), b.stride(0), int(b_mn), ptr(out), out.stride(0), M, N, K,
-         ptr(bias) if bias is not None else None, 1 if accumulate else 0, None, *dyn)
-    return out
+    if out_f32 is not None:                 # fp32 D32 += acc, split-K in epilogue bits 8..; no bf16 D, no bias
+        D, ldd, bias, epilogue = None, out_f32.stride(0), None, (int(split_k) << 8) if split_k > 1 else 0
+    else:
+        D = out if out is not None else torch.empty(M, N, dtype=a.dtype, device=a.device)
+        ldd, epilogue = D.stride(0), 1 if accumulate else 0
+    call("lmod_gemm_bf16_dyn", ptr(a), a.stride(0), int(a_mn), ptr(b), b.stride(0), int(b_mn), ptr(D), ldd, M, N, K, ptr(bias), epilogue,
+         ptr(out_f32), ptr(m_dev), ptr(k_dev))
+    return out_f32 if out_f32 is not None else D
 
 
 # The fused SwiGLU forward pays off only when the GEMM's main loop is long enough to hide its epilogue: it is used from a reduction
@@ -181,15 +179,12 @@ def grouped_gemm(a, b, out, offsets, mode, max_rows=None, accumulate=False):
     G = offsets.numel() - 1
     R = a.shape[0] if max_rows is None else max_rows
     if mode == 0:
-        N, K = b.shape[1], b.shape[2]
-        call("lmod_grouped_gemm_bf16", ptr(a), a.stride(0), ptr(b), b.stride(1), ptr(out), out.stride(0), ptr(offsets), G, R, 0, N, K, 0, 0)
+        ldb, ldd, M, N, K, mode, acc = b.stride(1), out.stride(0), 0, b.shape[1], b.shape[2], 0, 0
     elif mode == 1:
-        K, N = b.shape[1], b.shape[2]
-        call("lmod_grouped_gemm_bf16", ptr(a), a.stride(0), ptr(b), b.stride(1), ptr(out), out.stride(0), ptr(offsets), G, R, 0, N, K, 1, 0)
+        ldb, ldd, M, N, K, mode, acc = b.stride(1), out.stride(0), 0, b.shape[2], b.shape[1], 1, 0
     else:
-        M, N = a.shape[1], b.shape[1]
-        call("lmod_grouped_gemm_bf16", ptr(a), a.stride(0), ptr(b), b.stride(0), ptr(out), out.stride(1), ptr(offsets), G, R, M, N, 0, 2,
-             1 if accumulate else 0)
+        ldb, ldd, M, N, K, mode, acc = b.stride(0), out.stride(1), a.shape[1], b.shape[1], 0, 2, 1 if accumulate else 0
+    call("lmod_grouped_gemm_bf16", ptr(a), a.stride(0), ptr(b), ldb, ptr(out), ldd, ptr(offsets), G, R, M, N, K, mode, acc)
     return out
 
 
@@ -264,7 +259,7 @@ def rmsnorm_quant(x, w, eps, res=None):
     rows = x.numel() // H
     out = Fp8Rows(torch.empty(rows, H, dtype=torch.uint8, device=x.device), torch.empty(rows, dtype=torch.float32, device=x.device))
     s = torch.empty_like(x) if res is not None else None
-    call("lmod_rmsnorm_quant_e4m3", ptr(x), ptr(_c(res)) if res is not None else None, ptr(w), rows, H, eps, ptr(out.q), ptr(out.scale), ptr(s))
+    call("lmod_rmsnorm_quant_e4m3", ptr(x), ptr(_c(res)), ptr(w), rows, H, eps, ptr(out.q), ptr(out.scale), ptr(s))
     return out, (s if res is not None else x)
 
 
@@ -272,7 +267,7 @@ def gemm_fp8(a, w, bias=None):
     """bf16 [M,N] = a (Fp8Rows [M,K]) x w (Fp8Rows [N,K])^T (+bias) on the e4m3 wgmma GEMM (lmod_gemm_e4m3)."""
     M, Kd = a.shape
     out = torch.empty(M, w.shape[0], dtype=BF16, device=a.q.device)
-    call("lmod_gemm_e4m3", ptr(a.q), a.q.stride(0), ptr(a.scale), ptr(w.q), w.q.stride(0), ptr(w.scale), ptr(bias) if bias is not None else None,
+    call("lmod_gemm_e4m3", ptr(a.q), a.q.stride(0), ptr(a.scale), ptr(w.q), w.q.stride(0), ptr(w.scale), ptr(bias),
          ptr(out), out.stride(0), M, w.shape[0], Kd)
     return out
 
@@ -283,7 +278,7 @@ def qkv_rope_fp8(a, w, bias, cos, sin, pos, nh, nkv, hd):
         return rope_(gemm_fp8(a, w, bias), cos, sin, pos, nh, nkv, hd)
     M, Kd = a.shape
     out = torch.empty(M, w.shape[0], dtype=BF16, device=a.q.device)
-    call("lmod_gemm_e4m3_qkv_rope", ptr(a.q), a.q.stride(0), ptr(a.scale), ptr(w.q), w.q.stride(0), ptr(w.scale), ptr(bias) if bias is not None else None,
+    call("lmod_gemm_e4m3_qkv_rope", ptr(a.q), a.q.stride(0), ptr(a.scale), ptr(w.q), w.q.stride(0), ptr(w.scale), ptr(bias),
          ptr(out), out.stride(0), M, Kd, nh, nkv, hd, ptr(cos), ptr(sin), ptr(pos))
     return out
 
@@ -330,7 +325,7 @@ def attention_fwd(qkv, B, T, nh, nkv, hd, causal, scale=None, need_lse=False, pa
     lse = torch.empty(B, nh, T, dtype=torch.float32, device=qkv.device) if need_lse else None
     lo, hi = pad if pad is not None else (None, None)
     call("lmod_attn_fwd", ptr(qkv), qkv.stride(0), B, T, nh, nkv, hd, 1 if causal else 0, float(scale if scale is not None else hd ** -0.5),
-         ptr(out), out.stride(0), ptr(lse) if lse is not None else None, ptr(lo), ptr(hi))
+         ptr(out), out.stride(0), ptr(lse), ptr(lo), ptr(hi))
     return out, lse
 
 
@@ -374,13 +369,10 @@ def attention(qkv, B, T, nh, nkv, hd, causal=True, scale=None, pad=None):
     the TRUE head dim); the pad / slice are plain tensor ops, so autograd carries the gradient back to the unpadded buffer."""
     scale = float(scale if scale is not None else hd ** -0.5)
     _check_pad(causal, pad)
-    if hd not in ATTN_HEAD_DIMS:
-        hp = 64 if hd < 64 else 128
-        if hd > 128:
-            raise _C.LmodError("head_dim %d > 128 is not built" % hd)
-        q3 = torch.nn.functional.pad(qkv.view(B * T, nh + 2 * nkv, hd), (0, hp - hd)).view(B * T, (nh + 2 * nkv) * hp)
-        o = attention(q3, B, T, nh, nkv, hp, causal, scale, pad)
-        return o.view(B * T, nh, hp)[:, :, :hd].reshape(B * T, nh * hd)
+    hp = attn_head_dim(hd)
+    if hp != hd:
+        o = attention(_pad_heads(qkv, nh + 2 * nkv, hd, hp), B, T, nh, nkv, hp, causal, scale, pad)
+        return _unpad_heads(o, nh, hd)
     lo, hi = pad if pad is not None else (None, None)
     if torch.is_grad_enabled() and qkv.requires_grad:
         return AttnFn.apply(qkv, B, T, nh, nkv, hd, causal, scale, lo, hi)
@@ -399,6 +391,12 @@ def _pad_heads(x, heads, hd, hp):
     return torch.nn.functional.pad(x.view(x.shape[0], heads, hd), (0, hp - hd)).view(x.shape[0], heads * hp)
 
 
+def _unpad_heads(x, heads, hd):
+    """Inverse of _pad_heads: [rows, heads*hp] -> [rows, heads*hd], the first hd columns of every head (x itself when hp == hd)."""
+    hp = x.shape[1] // heads
+    return x if hp == hd else x.view(x.shape[0], heads, hp)[:, :, :hd].reshape(x.shape[0], heads * hd)
+
+
 def _check_cache(k_cache, v_cache, B, nkv, hd):
     """The kernels index the cache as dense bf16 [B, nkv, max_len, attn_head_dim(hd)]."""
     want = (B, nkv, k_cache.shape[2] if k_cache.dim() == 4 else -1, attn_head_dim(hd))
@@ -413,65 +411,67 @@ def _check_i32(t, B, name):
         raise _C.LmodError("%s must be a contiguous int32 tensor of %d elements, got %s %s" % (name, B, t.dtype, tuple(t.shape)))
 
 
+def _cache_qkv(name, qkv, B, n, nh, nkv, hd, k_cache, v_cache, **i32):
+    """Checks shared by the cache appends -> the QKV rows [B*n, (nh+2nkv)*hd] with every head padded to the cache's width hp.
+    i32: the int32 [B] device arrays of the call, by name."""
+    _need_cuda(qkv, k_cache, v_cache, *i32.values())
+    _check_cache(k_cache, v_cache, B, nkv, hd)
+    for key, t in i32.items():
+        _check_i32(t, B, key)
+    if qkv.dim() != 2 or qkv.shape[0] != B * n or qkv.shape[1] != (nh + 2 * nkv) * hd or qkv.stride(1) != 1:
+        raise _C.LmodError("%s: qkv must be [B*%d, (nh+2nkv)*hd] with unit column stride, got %s" % (name, n, tuple(qkv.shape)))
+    hp = k_cache.shape[-1]
+    return qkv if hp == hd else _pad_heads(qkv, nh + 2 * nkv, hd, hp)
+
+
 def kv_append(qkv, B, n_new, nh, nkv, hd, k_cache, v_cache, offsets):
     """DynamicCache.update: the k / v heads of the fused, RoPE'd QKV rows [B*n_new, (nh+2nkv)*hd] -> cache rows offsets[b] + [0, n_new)
     of k_cache / v_cache [B, nkv, max_len, hp] (hp = attn_head_dim(hd); padded heads get zero columns).  offsets: int32 [B] on the device."""
-    _need_cuda(qkv, k_cache, v_cache, offsets)
-    _check_cache(k_cache, v_cache, B, nkv, hd)
-    _check_i32(offsets, B, "offsets")
-    if qkv.dim() != 2 or qkv.shape[0] != B * n_new or qkv.shape[1] != (nh + 2 * nkv) * hd or qkv.stride(1) != 1:
-        raise _C.LmodError("kv_append: qkv must be [B*n_new, (nh+2nkv)*hd] with unit column stride, got %s" % (tuple(qkv.shape),))
-    hp = k_cache.shape[-1]
-    if hp != hd:
-        qkv = _pad_heads(qkv, nh + 2 * nkv, hd, hp)
-    call("lmod_kv_append", ptr(qkv), qkv.stride(0), B, n_new, nh, nkv, hp, ptr(offsets), ptr(k_cache), ptr(v_cache), k_cache.shape[2])
+    qkv = _cache_qkv("kv_append", qkv, B, n_new, nh, nkv, hd, k_cache, v_cache, offsets=offsets)
+    call("lmod_kv_append", ptr(qkv), qkv.stride(0), B, n_new, nh, nkv, k_cache.shape[3], ptr(offsets), ptr(k_cache), ptr(v_cache),
+         k_cache.shape[2])
 
 
 def kv_append_rows(qkv, B, T, nh, nkv, hd, k_cache, v_cache, src_lo, src_hi, offsets):
     """The prefill of a padded batch into the cache: rows [src_lo[b], src_hi[b]) of sequence b's T rows of the fused, RoPE'd QKV buffer
     [B*T, (nh+2nkv)*hd] -> cache rows offsets[b] + (r - src_lo[b]), so every sequence's real rows are packed from offsets[b].  src_lo /
     src_hi / offsets: int32 [B] on the device (pad_ranges gives the ranges); no other cache row is written."""
-    _need_cuda(qkv, k_cache, v_cache, src_lo, src_hi, offsets)
-    _check_cache(k_cache, v_cache, B, nkv, hd)
-    for t, name in ((src_lo, "src_lo"), (src_hi, "src_hi"), (offsets, "offsets")):
-        _check_i32(t, B, name)
-    if qkv.dim() != 2 or qkv.shape[0] != B * T or qkv.shape[1] != (nh + 2 * nkv) * hd or qkv.stride(1) != 1:
-        raise _C.LmodError("kv_append_rows: qkv must be [B*T, (nh+2nkv)*hd] with unit column stride, got %s" % (tuple(qkv.shape),))
-    hp = k_cache.shape[-1]
-    if hp != hd:
-        qkv = _pad_heads(qkv, nh + 2 * nkv, hd, hp)
-    call("lmod_kv_append_rows", ptr(qkv), qkv.stride(0), B, T, nh, nkv, hp, ptr(src_lo), ptr(src_hi), ptr(offsets), ptr(k_cache),
-         ptr(v_cache), k_cache.shape[2])
+    qkv = _cache_qkv("kv_append_rows", qkv, B, T, nh, nkv, hd, k_cache, v_cache, src_lo=src_lo, src_hi=src_hi, offsets=offsets)
+    call("lmod_kv_append_rows", ptr(qkv), qkv.stride(0), B, T, nh, nkv, k_cache.shape[3], ptr(src_lo), ptr(src_hi), ptr(offsets),
+         ptr(k_cache), ptr(v_cache), k_cache.shape[2])
 
 
 def attn_decode_ws_elems(B, nh, nkv, hd, max_len):
     return int(_C.lib().lmod_attn_decode_ws_elems(B, nh, nkv, attn_head_dim(hd), max_len))
 
 
+def _decode_io(name, q, B, T, nh, nkv, hd, k_cache, v_cache, lens, ws, need_lse):
+    """Checks shared by the decode-attention forms -> (q with every head padded to the cache's width hp, out [B*T, nh*hp] bf16,
+    lse [B*T, nh] fp32 or None)."""
+    _need_cuda(q, k_cache, v_cache, lens, ws)
+    _check_cache(k_cache, v_cache, B, nkv, hd)
+    _check_i32(lens, B, "lens")
+    if T < 1 or q.dim() != 2 or q.shape[0] != B * T or q.shape[1] < nh * hd or q.stride(1) != 1 or q.dtype != BF16:
+        raise _C.LmodError("%s: q must be bf16 [B*%d, >= nh*hd] with unit column stride, got %s %s" % (name, T, q.dtype, tuple(q.shape)))
+    if ws.dtype != torch.float32 or not ws.is_contiguous():
+        raise _C.LmodError("%s: ws must be a contiguous fp32 tensor" % name)
+    hp = k_cache.shape[3]
+    if hp != hd:
+        q = _pad_heads(q[:, :nh * hd], nh, hd, hp)
+    out = torch.empty(B * T, nh * hp, dtype=q.dtype, device=q.device)
+    lse = torch.empty(B * T, nh, dtype=torch.float32, device=q.device) if need_lse else None
+    return q, out, lse
+
+
 def attn_decode(q, nh, nkv, hd, k_cache, v_cache, lens, ws, scale=None, need_lse=False):
     """Single-query attention of every sequence over its cached keys [0, lens[b]) (split-KV, lmod_attn_decode).  q: [B, >= nh*hd] rows
     whose first nh*hd columns are the query heads (the fused QKV rows of a decode step); k_cache / v_cache [B, nkv, max_len, hp];
     lens int32 [B] on the device; ws fp32 of at least attn_decode_ws_elems(...).  -> (out [B, nh*hd] bf16, lse [B, nh] fp32 or None)."""
-    _need_cuda(q, k_cache, v_cache, lens, ws)
     B = q.shape[0]
-    _check_cache(k_cache, v_cache, B, nkv, hd)
-    _check_i32(lens, B, "lens")
-    if q.dim() != 2 or q.shape[1] < nh * hd or q.stride(1) != 1 or q.dtype != BF16:
-        raise _C.LmodError("attn_decode: q must be bf16 [B, >= nh*hd] with unit column stride, got %s %s" % (q.dtype, tuple(q.shape)))
-    if ws.dtype != torch.float32 or not ws.is_contiguous():
-        raise _C.LmodError("attn_decode: ws must be a contiguous fp32 tensor")
-    hp, max_len = k_cache.shape[-1], k_cache.shape[2]
-    scale = float(scale if scale is not None else hd ** -0.5)
-    if hp != hd:
-        q = _pad_heads(q[:, :nh * hd], nh, hd, hp)
-    out = torch.empty(B, nh * hp, dtype=q.dtype, device=q.device)
-    lse = torch.empty(B, nh, dtype=torch.float32, device=q.device) if need_lse else None
-    call("lmod_attn_decode", ptr(q), q.stride(0), ptr(k_cache), ptr(v_cache), ptr(lens), B, nh, nkv, hp, max_len, scale, ptr(out), out.stride(0),
-         ptr(lse), ptr(ws), ws.numel())
-    if hp != hd:
-        out = out.view(B, nh, hp)[:, :, :hd].reshape(B, nh * hd)
-    return out, lse
-
+    q, out, lse = _decode_io("attn_decode", q, B, 1, nh, nkv, hd, k_cache, v_cache, lens, ws, need_lse)
+    call("lmod_attn_decode", ptr(q), q.stride(0), ptr(k_cache), ptr(v_cache), ptr(lens), B, nh, nkv, k_cache.shape[3], k_cache.shape[2],
+         float(scale if scale is not None else hd ** -0.5), ptr(out), out.stride(0), ptr(lse), ptr(ws), ws.numel())
+    return _unpad_heads(out, nh, hd), lse
 
 
 def attn_decode_chunk_ws_elems(B, T, nh, nkv, hd, max_len):
@@ -483,24 +483,10 @@ def attn_decode_chunk(q, B, T, nh, nkv, hd, k_cache, v_cache, lens, ws, scale=No
     [0, lens[b] - T + t + 1), where lens is the length after the T rows' k / v were appended.  q: [B*T, >= nh*hd] rows (row b*T + t);
     k_cache / v_cache [B, nkv, max_len, hp]; lens int32 [B] on the device; ws fp32 of at least attn_decode_chunk_ws_elems(...).
     Row t gives the bytes attn_decode gives for that row alone at lens[b] - T + t + 1.  -> (out [B*T, nh*hd] bf16, lse [B*T, nh] or None)."""
-    _need_cuda(q, k_cache, v_cache, lens, ws)
-    _check_cache(k_cache, v_cache, B, nkv, hd)
-    _check_i32(lens, B, "lens")
-    if T < 1 or q.dim() != 2 or q.shape[0] != B * T or q.shape[1] < nh * hd or q.stride(1) != 1 or q.dtype != BF16:
-        raise _C.LmodError("attn_decode_chunk: q must be bf16 [B*T, >= nh*hd] with unit column stride, got %s %s" % (q.dtype, tuple(q.shape)))
-    if ws.dtype != torch.float32 or not ws.is_contiguous():
-        raise _C.LmodError("attn_decode_chunk: ws must be a contiguous fp32 tensor")
-    hp, max_len = k_cache.shape[-1], k_cache.shape[2]
-    scale = float(scale if scale is not None else hd ** -0.5)
-    if hp != hd:
-        q = _pad_heads(q[:, :nh * hd], nh, hd, hp)
-    out = torch.empty(B * T, nh * hp, dtype=q.dtype, device=q.device)
-    lse = torch.empty(B * T, nh, dtype=torch.float32, device=q.device) if need_lse else None
-    call("lmod_attn_decode_chunk", ptr(q), q.stride(0), ptr(k_cache), ptr(v_cache), ptr(lens), B, T, nh, nkv, hp, max_len, scale, ptr(out),
-         out.stride(0), ptr(lse), ptr(ws), ws.numel())
-    if hp != hd:
-        out = out.view(B * T, nh, hp)[:, :, :hd].reshape(B * T, nh * hd)
-    return out, lse
+    q, out, lse = _decode_io("attn_decode_chunk", q, B, T, nh, nkv, hd, k_cache, v_cache, lens, ws, need_lse)
+    call("lmod_attn_decode_chunk", ptr(q), q.stride(0), ptr(k_cache), ptr(v_cache), ptr(lens), B, T, nh, nkv, k_cache.shape[3],
+         k_cache.shape[2], float(scale if scale is not None else hd ** -0.5), ptr(out), out.stride(0), ptr(lse), ptr(ws), ws.numel())
+    return _unpad_heads(out, nh, hd), lse
 
 
 def spec_accept(target_logits, draft_tokens, draft_logits=None, u=None, len_target=None, len_draft=None):
@@ -557,17 +543,8 @@ class RMSNormFn(Function):
     def forward(ctx, x, res, w, eps, wgrad=None):
         _need_cuda(x, w)
         x = _c(x)
-        H = x.shape[-1]
-        rows = x.numel() // H
-        y = torch.empty_like(x)
-        rstd = torch.empty(rows, dtype=torch.float32, device=x.device)
-        if res is not None:
-            res = _c(res)
-            s = torch.empty_like(x)
-            call("lmod_rmsnorm_fwd", ptr(x), ptr(res), ptr(w), rows, H, eps, ptr(y), ptr(s), ptr(rstd))
-        else:
-            s = x
-            call("lmod_rmsnorm_fwd", ptr(x), None, ptr(w), rows, H, eps, ptr(y), None, ptr(rstd))
+        rstd = torch.empty(x.numel() // x.shape[-1], dtype=torch.float32, device=x.device)
+        y, s = _rmsnorm_fwd(x, res, w, eps, rstd)
         ctx.save_for_backward(s, w, rstd)
         ctx.had_res = res is not None
         ctx.wgrad = wgrad                                   # view of the flat gradient buffer when the norm weight trains
@@ -602,21 +579,22 @@ def _zero_ws(device, n):
     return ws
 
 
+def _rmsnorm_fwd(x, res, w, eps, rstd=None):
+    """lmod_rmsnorm_fwd -> (y, stream): stream = x + res, or x itself without res.  rstd: fp32 [rows] output, or None."""
+    x = _c(x)
+    H = x.shape[-1]
+    y = torch.empty_like(x)
+    s = torch.empty_like(x) if res is not None else None
+    call("lmod_rmsnorm_fwd", ptr(x), ptr(_c(res)), ptr(w), x.numel() // H, H, eps, ptr(y), ptr(s), ptr(rstd))
+    return y, (s if s is not None else x)
+
+
 def rmsnorm(x, w, eps, res=None, wgrad=None):
     """-> (y, stream) where stream = x + res (or x).  Without autograd the kernel is called directly."""
     if torch.is_grad_enabled() and (x.requires_grad or (res is not None and res.requires_grad) or wgrad is not None):
         y, s = RMSNormFn.apply(x, res, w, eps, wgrad)
         return y, (s if res is not None else x)
-    x = _c(x)
-    H = x.shape[-1]
-    rows = x.numel() // H
-    y = torch.empty_like(x)
-    if res is not None:
-        s = torch.empty_like(x)
-        call("lmod_rmsnorm_fwd", ptr(x), ptr(_c(res)), ptr(w), rows, H, eps, ptr(y), ptr(s), None)
-        return y, s
-    call("lmod_rmsnorm_fwd", ptr(x), None, ptr(w), rows, H, eps, ptr(y), None, None)
-    return y, x
+    return _rmsnorm_fwd(x, res, w, eps)
 
 
 def layernorm(x, w, b, eps):
@@ -628,15 +606,27 @@ def layernorm(x, w, b, eps):
     return y
 
 
+def _rope(buf, cos, sin, pos, nh, nkv, hd, inverse):
+    """lmod_rope in place on the q and k heads of the fused QKV rows buf [rows, (nh + 2*nkv)*hd]; inverse: the transpose rotation."""
+    ld = buf.shape[-1]
+    call("lmod_rope", ptr(buf), ld, nh, buf.data_ptr() + nh * hd * 2, ld, nkv, hd, ptr(cos), ptr(sin), ptr(pos), buf.numel() // ld,
+         1 if inverse else 0)
+    return buf
+
+
+def _rope_grad(d, cos, sin, pos, nh, nkv, hd):
+    # Rotated back in a copy: autograd may hand backward a gradient that is still read elsewhere (the caller's tensor in
+    # out.backward(grad), a tensor hook's argument), and rotating it in place would change what those see.
+    return _rope(d.clone(memory_format=torch.contiguous_format), cos, sin, pos, nh, nkv, hd, True)
+
+
 class RopeFn(Function):
     """apply_rotary_pos_emb (modeling_qwen2.py:159-184) in place on the fused QKV projection output
     [rows, (nh + 2*nkv)*hd]: q heads first, then k heads, then v."""
 
     @staticmethod
     def forward(ctx, qkv, cos, sin, pos, nh, nkv, hd):
-        rows = qkv.numel() // qkv.shape[-1]
-        ld = qkv.shape[-1]
-        call("lmod_rope", ptr(qkv), ld, nh, qkv.data_ptr() + nh * hd * 2, ld, nkv, hd, ptr(cos), ptr(sin), ptr(pos), rows, 0)
+        _rope(qkv, cos, sin, pos, nh, nkv, hd, False)
         ctx.mark_dirty(qkv)
         ctx.save_for_backward(cos, sin, pos)
         ctx.dims = (nh, nkv, hd)
@@ -645,12 +635,15 @@ class RopeFn(Function):
     @staticmethod
     def backward(ctx, d):
         cos, sin, pos = ctx.saved_tensors
-        nh, nkv, hd = ctx.dims
-        d = d.contiguous().clone()
-        rows = d.numel() // d.shape[-1]
-        ld = d.shape[-1]
-        call("lmod_rope", ptr(d), ld, nh, d.data_ptr() + nh * hd * 2, ld, nkv, hd, ptr(cos), ptr(sin), ptr(pos), rows, 1)
-        return d, None, None, None, None, None, None
+        return (_rope_grad(d, cos, sin, pos, *ctx.dims),) + (None,) * 6
+
+
+def _gemm_qkv_rope(x2, w, bias, cos, sin, pos, nh, nkv, hd):
+    """lmod_gemm_qkv_rope: [rows, (nh + 2*nkv)*hd] = x2 @ w^T + bias with the q and k heads rotated."""
+    out = torch.empty(x2.shape[0], w.shape[0], dtype=x2.dtype, device=x2.device)
+    call("lmod_gemm_qkv_rope", ptr(x2), x2.stride(0), ptr(w), w.stride(0), ptr(bias), ptr(out), out.stride(0), x2.shape[0], x2.shape[1],
+         nh, nkv, hd, ptr(cos), ptr(sin), ptr(pos))
+    return out
 
 
 class QKVRopeFn(Function):
@@ -660,10 +653,7 @@ class QKVRopeFn(Function):
     @staticmethod
     def forward(ctx, x, w, bias, cos, sin, pos, nh, nkv, hd, wgrad, bgrad):
         x2 = _rows(x)
-        M, Kd = x2.shape
-        out = torch.empty(M, w.shape[0], dtype=x.dtype, device=x.device)
-        call("lmod_gemm_qkv_rope", ptr(x2), x2.stride(0), ptr(w), w.stride(0), ptr(bias) if bias is not None else None, ptr(out), out.stride(0), M, Kd,
-             nh, nkv, hd, ptr(cos), ptr(sin), ptr(pos))
+        out = _gemm_qkv_rope(x2, w, bias, cos, sin, pos, nh, nkv, hd)
         ctx.save_for_backward(x2, w, cos, sin, pos)
         ctx.dims = (nh, nkv, hd)
         ctx.g = (wgrad, bgrad)
@@ -673,13 +663,8 @@ class QKVRopeFn(Function):
     @staticmethod
     def backward(ctx, d):
         x2, w, cos, sin, pos = ctx.saved_tensors
-        nh, nkv, hd = ctx.dims
         wgrad, bgrad = ctx.g
-        # Rotated back in a copy, as RopeFn does: autograd may hand backward a gradient that is still read elsewhere (the caller's tensor
-        # in out.backward(grad), a tensor hook's argument), and rotating it in place would change what those see.
-        d = d.clone(memory_format=torch.contiguous_format)
-        ld = d.shape[-1]
-        call("lmod_rope", ptr(d), ld, nh, d.data_ptr() + nh * hd * 2, ld, nkv, hd, ptr(cos), ptr(sin), ptr(pos), d.numel() // ld, 1)
+        d = _rope_grad(d, cos, sin, pos, *ctx.dims)
         dx = mm_nn(d, w).reshape(ctx.xshape) if ctx.needs_input_grad[0] else None
         if wgrad is not None:
             mm_tn_acc(d, x2, wgrad)
@@ -695,20 +680,21 @@ def qkv_rope(x, w, bias, cos, sin, pos, nh, nkv, hd, wgrad=None, bgrad=None):
         return rope_(linear(_rows(x), w, bias, wgrad, bgrad), cos, sin, pos, nh, nkv, hd)
     if torch.is_grad_enabled() and (x.requires_grad or wgrad is not None):
         return QKVRopeFn.apply(x, w, bias, cos, sin, pos, nh, nkv, hd, wgrad, bgrad)
-    x2 = _rows(x)
-    out = torch.empty(x2.shape[0], w.shape[0], dtype=x.dtype, device=x.device)
-    call("lmod_gemm_qkv_rope", ptr(x2), x2.stride(0), ptr(w), w.stride(0), ptr(bias) if bias is not None else None, ptr(out), out.stride(0), x2.shape[0],
-         x2.shape[1], nh, nkv, hd, ptr(cos), ptr(sin), ptr(pos))
-    return out
+    return _gemm_qkv_rope(_rows(x), w, bias, cos, sin, pos, nh, nkv, hd)
 
 
 def rope_(qkv, cos, sin, pos, nh, nkv, hd):
     if torch.is_grad_enabled() and qkv.requires_grad:
         return RopeFn.apply(qkv, cos, sin, pos, nh, nkv, hd)
-    rows = qkv.numel() // qkv.shape[-1]
-    ld = qkv.shape[-1]
-    call("lmod_rope", ptr(qkv), ld, nh, qkv.data_ptr() + nh * hd * 2, ld, nkv, hd, ptr(cos), ptr(sin), ptr(pos), rows, 0)
-    return qkv
+    return _rope(qkv, cos, sin, pos, nh, nkv, hd, False)
+
+
+def _silu_mul(gu):
+    """lmod_silu_mul_fwd on the contiguous fused gate|up rows gu [..., 2I] -> [..., I]."""
+    I = gu.shape[-1] // 2
+    out = torch.empty(gu.shape[:-1] + (I,), dtype=gu.dtype, device=gu.device)
+    call("lmod_silu_mul_fwd", ptr(gu), 2 * I, gu.numel() // gu.shape[-1], I, ptr(out))
+    return out
 
 
 class SiluMulFn(Function):
@@ -717,31 +703,19 @@ class SiluMulFn(Function):
     @staticmethod
     def forward(ctx, gu):
         gu = _c(gu)
-        I = gu.shape[-1] // 2
-        rows = gu.numel() // gu.shape[-1]
-        out = torch.empty(gu.shape[:-1] + (I,), dtype=gu.dtype, device=gu.device)
-        call("lmod_silu_mul_fwd", ptr(gu), 2 * I, rows, I, ptr(out))
         ctx.save_for_backward(gu)
-        return out
+        return _silu_mul(gu)
 
     @staticmethod
     def backward(ctx, d):
         (gu,) = ctx.saved_tensors
-        I = gu.shape[-1] // 2
-        rows = gu.numel() // gu.shape[-1]
-        dgu = torch.empty_like(gu)
-        call("lmod_silu_mul_bwd", ptr(_c(d)), ptr(gu), 2 * I, rows, I, ptr(dgu))
-        return dgu
+        return silu_mul_bwd(d, gu)
 
 
 def silu_mul(gu):
     if torch.is_grad_enabled() and gu.requires_grad:
         return SiluMulFn.apply(gu)
-    gu = _c(gu)
-    I = gu.shape[-1] // 2
-    out = torch.empty(gu.shape[:-1] + (I,), dtype=gu.dtype, device=gu.device)
-    call("lmod_silu_mul_fwd", ptr(gu), 2 * I, gu.numel() // gu.shape[-1], I, ptr(out))
-    return out
+    return _silu_mul(_c(gu))
 
 
 def silu_mul_bwd(d, gu):
@@ -760,6 +734,12 @@ def bias_act(x, bias, act):
     y = torch.empty_like(x)
     call("lmod_bias_act_fwd", ptr(x), ptr(bias), x.numel() // n, n, act, ptr(y))
     return y
+
+
+def add_(a, b):
+    """a += b in place, element by element in bf16 (lmod_add); a and b contiguous with the same number of elements."""
+    call("lmod_add", ptr(a), ptr(b), a.numel(), ptr(a))
+    return a
 
 
 class GeluFn(Function):
@@ -789,14 +769,19 @@ def gelu(x):
 # multimodal splice (llava_arch.py:228-320): the integer plan is built on the host (see llava_arch.py in this
 # package); the device part is one gather kernel and, backwards, one scatter into the projector output grads.
 # ---------------------------------------------------------------------------------------------------
+def _splice_embed(feats, embed_w, src, img_index, n_patches):
+    """lmod_splice_embed -> [B, T, H]: embedding rows of the tokens of src [B, T], image feature rows where it points at them."""
+    B, T = src.shape
+    H = embed_w.shape[1]
+    out = torch.empty(B, T, H, dtype=embed_w.dtype, device=embed_w.device)
+    call("lmod_splice_embed", ptr(embed_w), ptr(feats), ptr(src), ptr(img_index), B * T, H, n_patches, ptr(out))
+    return out
+
+
 class SpliceFn(Function):
     @staticmethod
     def forward(ctx, feats, embed_w, src, img_index, n_patches, embed_grad=None, order=None):
-        B, T = src.shape
-        H = embed_w.shape[1]
-        out = torch.empty(B, T, H, dtype=embed_w.dtype, device=embed_w.device)
-        call("lmod_splice_embed", ptr(embed_w), ptr(feats) if feats is not None else None, ptr(src), ptr(img_index),
-             B * T, H, n_patches, ptr(out))
+        out = _splice_embed(feats, embed_w, src, img_index, n_patches)
         ctx.save_for_backward(src, img_index, order)
         ctx.fshape = feats.shape
         ctx.n_patches = n_patches
@@ -811,7 +796,7 @@ class SpliceFn(Function):
         d = _c(d)
         call("lmod_splice_embed_bwd", ptr(d), ptr(src), ptr(img_index), B * T, d.shape[-1], ctx.n_patches, ptr(dfeats))
         if ctx.embed_grad is not None:
-            call("lmod_embed_grad", ptr(d), ptr(src), ptr(order), B * T, d.shape[-1], ptr(ctx.embed_grad))
+            embed_grad_(d, src, order, ctx.embed_grad)
         return dfeats, None, None, None, None, None, None
 
 
@@ -829,11 +814,7 @@ def splice_embed(feats, embed_w, src, img_index, n_patches, embed_grad=None, ord
         raise ValueError("splice_embed: the embedding gradient needs the plan's row order (llava_arch.embed_grad_order)")
     if torch.is_grad_enabled() and (feats.requires_grad or embed_grad is not None):
         return SpliceFn.apply(feats, embed_w, src, img_index, n_patches, embed_grad, order)
-    B, T = src.shape
-    H = embed_w.shape[1]
-    out = torch.empty(B, T, H, dtype=embed_w.dtype, device=embed_w.device)
-    call("lmod_splice_embed", ptr(embed_w), ptr(feats), ptr(src), ptr(img_index), B * T, H, n_patches, ptr(out))
-    return out
+    return _splice_embed(feats, embed_w, src, img_index, n_patches)
 
 
 # ---------------------------------------------------------------------------------------------------
@@ -894,7 +875,7 @@ def moe_gather_combine(y, row, w, residual=None):
     S = row.shape[0]
     H = y.shape[-1]
     out = torch.empty(S, H, dtype=y.dtype, device=y.device)
-    call("lmod_moe_gather_combine", ptr(y), ptr(row), ptr(w), ptr(residual) if residual is not None else None, S, H, ptr(out))
+    call("lmod_moe_gather_combine", ptr(y), ptr(row), ptr(w), ptr(residual), S, H, ptr(out))
     return out
 
 
@@ -943,7 +924,7 @@ def moe_backward_stages(st, x, wg, w_gu, w_dn, dout, dlaux, grads, dres=None):
     if dlaux is not None:
         gl = dlaux.to(torch.float32).reshape(1).contiguous()
     call("lmod_moe_gate_bwd_top1" if st.get("k", 2) == 1 else "lmod_moe_gate_bwd", ptr(gates), ptr(idx), ptr(row), ptr(dw), ptr(meta),
-         ptr(gl) if gl is not None else None, S, E, ptr(dlogits))
+         ptr(gl), S, E, ptr(dlogits))
     dx = torch.empty_like(x)
     call("lmod_moe_scatter_bwd", ptr(dxp), ptr(row), ptr(dlogits), ptr(wg), ptr(dres), S, H, E, ptr(dx))
     if g is not None and g.get("wg") is not None:
@@ -991,7 +972,7 @@ def moe_forward_nograd(x, res, wg, w_gu, w_dn, noise, cf, min_cap, k=2):
         act = silu_mul(h1)
     y = torch.empty(R, H, dtype=x.dtype, device=x.device)
     grouped_gemm(act, w_dn, y, r["offsets"], 0)
-    return moe_gather_combine(y, r["row"], r["w"], _c(res) if res is not None else None), r["meta"][0].clone(), r
+    return moe_gather_combine(y, r["row"], r["w"], _c(res)), r["meta"][0].clone(), r
 
 
 # ---- Residual-MoE (DeepSpeed MoE(use_residual=True), SURVEY.md Appendix A "Residual"): the routed output and the dense MLP on every token,
@@ -1121,12 +1102,12 @@ def kl_fused(s_logits, t_logits, labels, seq_len, vocab, w_kd, w_ce, distill_all
     row_out = torch.empty(N, 4, dtype=torch.float32, device=dev)
     out4 = torch.empty(4, dtype=torch.float32, device=dev)
     da = 1 if distill_all else 0
+    perm, count = rows if rows is not None else (None, None)
     call("lmod_kl_counts", ptr(labels), N, seq_len, da, ptr(counts))
     with _Timed("kl_fwd_bwd"):
         call("lmod_kl_fwd_bwd_rows", ptr(s_logits), s_logits.stride(0), ptr(t_logits), t_logits.stride(0), ptr(labels), N, seq_len, vocab, da,
-             float(w_kd), float(w_ce), ptr(counts), ptr(row_out), ptr(dlogits) if dlogits is not None else None,
-             dlogits.stride(0) if dlogits is not None else 0, ptr(rows[0]) if rows is not None else None,
-             ptr(rows[1]) if rows is not None else None)
+             float(w_kd), float(w_ce), ptr(counts), ptr(row_out), ptr(dlogits), dlogits.stride(0) if dlogits is not None else 0,
+             ptr(perm), ptr(count))
     call("lmod_kl_finalize", ptr(row_out), ptr(labels), N, seq_len, da, ptr(out4))
     return out4, row_out
 
@@ -1197,6 +1178,13 @@ def logp_gather(logits, labels, average=False):
     return seq, tok, lse
 
 
+def logp_gather_bwd(logits, labels, lse, g_seq, out):
+    """d seq_logp / d logits of logp_gather for the upstream gradient g_seq [B] fp32, written to out [B,T,V] (out may be logits)."""
+    B, T, V = logits.shape
+    call("lmod_logp_gather_bwd", ptr(logits), logits.stride(1), ptr(labels), B, T, V, ptr(lse), ptr(g_seq), 0, ptr(out), out.stride(1))
+    return out
+
+
 class LogpHeadFn(Function):
     """lm_head GEMM + DPOTrainer.get_logp; backward writes d logits in place and returns d hidden."""
 
@@ -1216,7 +1204,7 @@ class LogpHeadFn(Function):
         B, T, V = logits.shape
         g = _c(g.to(torch.float32))
         with _Timed("logp_bwd"):
-            call("lmod_logp_gather_bwd", ptr(logits), logits.stride(1), ptr(labels), B, T, V, ptr(lse), ptr(g), 0, ptr(logits), logits.stride(1))
+            logp_gather_bwd(logits, labels, lse, g, logits)
         d2 = logits.view(B * T, V)
         dh = mm_nn(d2, w_head).view(hidden.shape)
         if ctx.head_grad is not None:
@@ -1261,8 +1249,8 @@ def sumsq_(buf, out):
 
 def adamw_(master, m, v, grad, model, lr, beta1, beta2, eps, wd, step, gnorm_sq=None, max_norm=0.0, grad_scale=1.0):
     call("lmod_adamw", ptr(master), ptr(m), ptr(v), ptr(grad), 1 if grad.dtype == torch.float32 else 0,
-         ptr(model) if model is not None else None, master.numel(), float(lr), float(beta1), float(beta2), float(eps), float(wd),
-         int(step), ptr(gnorm_sq) if gnorm_sq is not None else None, float(max_norm), float(grad_scale))
+         ptr(model), master.numel(), float(lr), float(beta1), float(beta2), float(eps), float(wd),
+         int(step), ptr(gnorm_sq), float(max_norm), float(grad_scale))
 
 
 def adamw_8bit_(master, m8, v8, absmax_m, absmax_v, grad, model, lr, beta1, beta2, eps, wd, step, gnorm_sq=None, max_norm=0.0,
@@ -1278,6 +1266,6 @@ def adamw_8bit_(master, m8, v8, absmax_m, absmax_v, grad, model, lr, beta1, beta
     if not (m8.numel() == v8.numel() == grad.numel() == n and absmax_m.numel() == absmax_v.numel() == nb
             and (model is None or model.numel() == n)):
         raise _C.LmodError("adamw_8bit_: %d elements need %d codes per moment and %d scales per moment" % (n, n, nb))
-    call("lmod_adamw_8bit", ptr(master), ptr(m8), ptr(v8), ptr(absmax_m), ptr(absmax_v), ptr(grad), ptr(model) if model is not None else None,
-         n, float(lr), float(beta1), float(beta2), float(eps), float(wd), int(step), ptr(gnorm_sq) if gnorm_sq is not None else None,
+    call("lmod_adamw_8bit", ptr(master), ptr(m8), ptr(v8), ptr(absmax_m), ptr(absmax_v), ptr(grad), ptr(model),
+         n, float(lr), float(beta1), float(beta2), float(eps), float(wd), int(step), ptr(gnorm_sq),
          float(max_norm), float(grad_scale))

@@ -44,11 +44,8 @@ class ShiftedCEFn(Function):
     @staticmethod
     def backward(ctx, g):
         logits, labels, lse, cnt = ctx.saved_tensors
-        B, T, V = logits.shape
-        gseq = (-g.to(torch.float32) / cnt).expand(B).contiguous()
-        d = torch.empty_like(logits)
-        K.call("lmod_logp_gather_bwd", K.ptr(logits), logits.stride(1), K.ptr(labels), B, T, V, K.ptr(lse), K.ptr(gseq), 0, K.ptr(d), d.stride(1))
-        return d, None
+        gseq = (-g.to(torch.float32) / cnt).expand(logits.shape[0]).contiguous()
+        return K.logp_gather_bwd(logits, labels, lse, gseq, torch.empty_like(logits)), None
 
 
 class LlavaQwenForCausalLMBase(nn.Module, LlavaMetaForCausalLM):

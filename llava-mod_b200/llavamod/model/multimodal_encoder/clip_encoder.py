@@ -158,7 +158,7 @@ class CLIPVisionModel(nn.Module):
         seq[:, 0] = vm.embeddings.class_embedding
         seq[:, 1:] = pe
         pos = vm.embeddings.position_embedding.weight[None].expand(n, T, H).contiguous()
-        K.call("lmod_add", K.ptr(seq), K.ptr(pos), seq.numel(), K.ptr(seq))
+        K.add_(seq, pos)
         h = K.layernorm(seq.view(n * T, H), vm.pre_layrnorm.weight, vm.pre_layrnorm.bias, c.layer_norm_eps)
         n_run = c.num_hidden_layers + 1 + select_layer if select_layer < 0 else select_layer
         hd = H // nh
@@ -168,12 +168,12 @@ class CLIPVisionModel(nn.Module):
             qkv = K.mm_nt(y, a.qkv_weight, a.qkv_bias)
             o = K.attention(qkv, n, T, nh, nh, hd, causal=False, scale=hd ** -0.5)
             o = K.mm_nt(o, a.out_proj.weight, a.out_proj.bias)
-            K.call("lmod_add", K.ptr(h), K.ptr(o), h.numel(), K.ptr(h))
+            K.add_(h, o)
             y = K.layernorm(h, layer.layer_norm2.weight, layer.layer_norm2.bias, c.layer_norm_eps)
             f = K.mm_nt(y, layer.mlp.fc1.weight)
             f = K.bias_act(f, layer.mlp.fc1.bias, K.ACT_QUICK_GELU)
             f = K.mm_nt(f, layer.mlp.fc2.weight, layer.mlp.fc2.bias)
-            K.call("lmod_add", K.ptr(h), K.ptr(f), h.numel(), K.ptr(h))
+            K.add_(h, f)
         return h.view(n, T, H)
 
 

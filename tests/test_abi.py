@@ -1,17 +1,17 @@
 """CPU-side checks of the drop-in boundary: the C-ABI library loads and exports every symbol include/lmod.h declares,
-and the ctypes table covers them (no compute calls -- there is no GPU here)."""
+and the ctypes types taken from that header are the right ones (no compute calls -- there is no GPU here)."""
 import ctypes
 import os
-import re
+
+import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def declared_symbols():
-    src = open(os.path.join(ROOT, "include", "lmod.h")).read()
-    src = re.sub(r"/\*LMOD_PLANNED_BEGIN.*?LMOD_PLANNED_END\*/", "", src, flags=re.S)   # planned, not yet exported
-    src = re.sub(r"/\*.*?\*/", "", src, flags=re.S)
-    return sorted(set(re.findall(r"\b(lmod_[a-z0-9_]+)\s*\(", src)))
+    from llavamod import _C
+    with open(os.path.join(ROOT, "include", "lmod.h")) as f:
+        return sorted(_C.parse_header(f.read()))
 
 
 def test_library_exports_every_declared_symbol():
@@ -24,43 +24,76 @@ def test_library_exports_every_declared_symbol():
     assert not missing, missing
 
 
-def test_ctypes_table_matches_header():
+def test_every_declared_symbol_is_typed_on_load():
+    """lib() gives every prototype of include/lmod.h its ctypes argument and return types; none is left to ctypes' int default."""
     from llavamod import _C
-    syms = set(declared_symbols())
-    table = set(_C.SIGNATURES) | {"lmod_last_error", "lmod_launch_count"}
-    assert syms <= table, sorted(syms - table)
-    assert _C.lib().lmod_version() >= 100
-    assert _C.lib().lmod_last_error() is not None
+    L = _C.lib()
+    untyped = [s for s in declared_symbols() if getattr(L, s).argtypes is None]
+    assert not untyped, untyped
+    assert L.lmod_version() >= 100
+    assert L.lmod_last_error() is not None
 
 
-def test_ctypes_signatures_have_the_arity_of_the_header_prototypes():
-    """An argument ctypes has no declared type for is passed as a 32-bit int -- a truncated pointer (e.g. the stream) that crashes on the GPU
-    box only.  Every ctypes signature must list exactly as many parameters as the prototype in include/lmod.h."""
+def test_header_parser():
+    """The parser behind the ctypes types: multi-line prototypes, inline comments, const pointers, (void), every return type, and a
+    type it does not know refused rather than guessed (ctypes would pass an untyped argument as a 32-bit int)."""
     from llavamod import _C
-    src = open(os.path.join(ROOT, "include", "lmod.h")).read()
-    src = re.sub(r"/\*.*?\*/", "", src, flags=re.S)
-    seen = 0
-    for m in re.finditer(r"\b(?:int|int64_t|const char\*|void)\s+(lmod_\w+)\s*\(([^;]*?)\)\s*;", src, flags=re.S):
-        name, params = m.group(1), m.group(2).strip()
-        if name not in _C.SIGNATURES:
-            continue
-        n = 0 if params in ("", "void") else params.count(",") + 1
-        assert len(_C.SIGNATURES[name]) == n, (name, len(_C.SIGNATURES[name]), n)
-        seen += 1
-    assert seen >= 40
+    P, I, L, F, D = ctypes.c_void_p, ctypes.c_int, ctypes.c_int64, ctypes.c_float, ctypes.c_double
+    src = """
+    #include <stdint.h>
+    /* lmod_commented_out(int x); */
+    typedef enum { LMOD_OK = 0, LMOD_ERR_ARG = -1 } lmod_status;
+    const char* lmod_name(void);
+    void lmod_reset(void);
+    int64_t lmod_elems(int64_t n, int k /* heads */, double cf);
+    int lmod_op(const void* x, int64_t ld /* row stride */, const int32_t *perm,
+                float eps, uint8_t* codes,
+                void* stream);
+    float lmod_scale(float* out);
+    double lmod_ratio(const char* tag, double d);
+    """
+    got = _C.parse_header(src)
+    assert got == {
+        "lmod_name": ([], ctypes.c_char_p),
+        "lmod_reset": ([], None),
+        "lmod_elems": ([L, I, D], L),
+        "lmod_op": ([P, L, P, F, P, P], I),
+        "lmod_scale": ([P], F),
+        "lmod_ratio": ([ctypes.c_char_p, D], D),
+    }
+    for bad in ("int lmod_bad(size_t n, void* stream);", "unsigned lmod_bad(void* stream);", "int lmod_bad(long long n);"):
+        with pytest.raises(_C.LmodError, match="lmod_bad"):
+            _C.parse_header(bad)
+
+
+def test_loaded_library_types():
+    from llavamod import _C
+    L = _C.lib()
+    assert len(declared_symbols()) >= 60
+    assert L.lmod_moe_capacity.argtypes == [ctypes.c_int64, ctypes.c_int, ctypes.c_double, ctypes.c_int64]
+    assert L.lmod_moe_capacity.restype is ctypes.c_int
+    assert L.lmod_attn_decode_ws_elems.restype is ctypes.c_int64
+    assert L.lmod_last_error.argtypes == [] and L.lmod_last_error.restype is ctypes.c_char_p
+    assert L.lmod_launch_count_reset.argtypes == [] and L.lmod_launch_count_reset.restype is None
+
+
+def test_missing_header_fails_loudly(monkeypatch):
+    from llavamod import _C
+    monkeypatch.setattr(_C, "_lib", None)
+    monkeypatch.setattr(_C, "HEADER_PATH", "/nonexistent/lmod.h")
+    with pytest.raises(_C.LmodError, match="lmod.h"):
+        _C.lib()
 
 
 def test_missing_library_fails_loudly(monkeypatch):
     from llavamod import _C
     monkeypatch.setattr(_C, "_lib", None)
     monkeypatch.setattr(_C, "LIB_PATH", "/nonexistent/liblmod_b200.so")
-    import pytest
     with pytest.raises(_C.LmodError):
         _C.lib()
 
 
 def test_cpu_tensor_is_rejected_not_silently_computed():
-    import pytest
     import torch
     from llavamod import _C, kernels as K
     with pytest.raises(_C.LmodError):
