@@ -63,15 +63,17 @@ class _Embeddings(nn.Module):
         self._wcache = None
 
     def patch_weight_2d(self):
-        """[hidden, Kpad] view of the conv kernel, K = C*p*p padded to a multiple of 8 (16-byte rows for the GEMM)."""
-        w = self.patch_embedding.weight
-        if self._wcache is None or self._wcache[0] != w._version:
+        """[hidden, Kpad] copy of the conv kernel, K = C*p*p zero-padded on the right to a multiple of 8 (16-byte rows for the GEMM).
+        Kept until the weight changes.  The version counter alone only sees writes in place: a weight loaded with assign=True, a new
+        Parameter or `.data =` brings its own counter, which can equal the old one.  So the key is the storage too (address, device,
+        dtype, shape, strides), and the cache holds the tensor it was made from, so that its address cannot be handed to a new weight."""
+        w = self.patch_embedding.weight.detach()
+        key = (w.data_ptr(), w._version, w.device, w.dtype, w.shape, w.stride())
+        if self._wcache is None or self._wcache[0] != key:
             k = w[0].numel()
             kp = (k + 7) // 8 * 8
-            w2 = torch.zeros(w.shape[0], kp, device=w.device, dtype=w.dtype)
-            w2[:, :k] = w.detach().reshape(w.shape[0], k)
-            self._wcache = (w._version, w2, kp)
-        return self._wcache[1], self._wcache[2]
+            self._wcache = (key, w, torch.nn.functional.pad(w.reshape(w.shape[0], k), (0, kp - k)), kp)
+        return self._wcache[2], self._wcache[3]
 
 
 class _Attn(nn.Module):
@@ -142,6 +144,9 @@ class CLIPVisionModel(nn.Module):
     @torch.no_grad()
     def hidden_state(self, images, select_layer=-2):
         c = self.config
+        n_run = c.num_hidden_layers + 1 + select_layer if select_layer < 0 else select_layer
+        if not 0 <= n_run <= c.num_hidden_layers:      # hidden_states has num_hidden_layers + 1 entries; a slice would clamp silently
+            raise IndexError("select_layer %d out of range for a tower with hidden states 0..%d" % (select_layer, c.num_hidden_layers))
         vm = self.vision_model
         n = images.shape[0]
         p, g = c.patch_size, c.image_size // c.patch_size
@@ -160,7 +165,6 @@ class CLIPVisionModel(nn.Module):
         pos = vm.embeddings.position_embedding.weight[None].expand(n, T, H).contiguous()
         K.add_(seq, pos)
         h = K.layernorm(seq.view(n * T, H), vm.pre_layrnorm.weight, vm.pre_layrnorm.bias, c.layer_norm_eps)
-        n_run = c.num_hidden_layers + 1 + select_layer if select_layer < 0 else select_layer
         hd = H // nh
         for layer in vm.encoder.layers[:n_run]:
             a = layer.self_attn
