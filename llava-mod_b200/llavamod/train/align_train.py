@@ -54,6 +54,15 @@ def _arch_from_name(name):
     raise FileNotFoundError(name)
 
 
+def init_process(seed):
+    """One process per GPU (torchrun-style env): joins the NCCL group when WORLD_SIZE > 1, seeds torch; -> this rank's device."""
+    if "RANK" in os.environ and int(os.environ.get("WORLD_SIZE", "1")) > 1 and not dist.is_initialized():
+        torch.cuda.set_device(int(os.environ.get("LOCAL_RANK", "0")))
+        dist.init_process_group("nccl")
+    torch.manual_seed(seed)
+    return torch.device("cuda", int(os.environ.get("LOCAL_RANK", "0")))
+
+
 def create_model_tokenizer(model_args, data_args, training_args, name_or_path, model_type, pretrain_adapter=None, device="cuda"):
     sparse = model_type == "sparse"
     if sparse:
@@ -159,11 +168,7 @@ def make_supervised_data_module(data_args, training_args, model, tokenizer=None)
 def train(argv=None):
     model_args, data_args, training_args, align_args = parse_args_into_dataclasses(
         (ModelArguments, DataArguments, TrainingArguments, AlignArguments), argv)
-    if "RANK" in os.environ and int(os.environ.get("WORLD_SIZE", "1")) > 1 and not dist.is_initialized():
-        torch.cuda.set_device(int(os.environ.get("LOCAL_RANK", "0")))
-        dist.init_process_group("nccl")
-    device = torch.device("cuda", int(os.environ.get("LOCAL_RANK", "0")))
-    torch.manual_seed(training_args.seed)
+    device = init_process(training_args.seed)
     if training_args.deepspeed:
         rank0_print("note: --deepspeed %s accepted and ignored (plain data parallelism, resident optimizer state)" % training_args.deepspeed)
     model, _ = create_model_tokenizer(model_args, data_args, training_args, align_args.policy_model_name_or_path,

@@ -10,86 +10,35 @@ lm_head GEMM output goes straight into ONE fused kernel that produces the mimic 
 sweep (no fp32 [N,V] probability tensors -- the reference materialises five of them); when teacher and student hold the
 same frozen CLIP tower it runs once per micro-batch instead of twice.
 """
-from collections import defaultdict
-from typing import Any, Dict, Literal, Optional, Tuple, Union
+import os
+from typing import Any, Dict, Union
 
 import torch
-import torch.nn as nn
 
 from .. import kernels as K
-from ..constants import IGNORE_INDEX, KD_VOCAB_SIZE
-from ..model.utils import create_reference_model, disable_dropout_in_model
-from .trainer_base import BaseTrainer
+from ..constants import KD_VOCAB_SIZE
+from .trainer_base import AdapterCheckpointMixin, BaseTrainer, image_count_shape
+from .trainer_base import quantize_ref_fp8  # noqa: F401  (--ref_fp8's switch, still importable from the trainer that takes it)
 
 
-class _Wrapped:
-    """Gives a bare module the ``.module`` attribute the reference dereferences on the DeepSpeed-wrapped teacher
-    (align_trainer.py:305,309); the build accepts wrapped and bare teachers (SURVEY.md Appendix B)."""
-
-    def __init__(self, module):
-        self.module = module
-
-    def __call__(self, *a, **kw):
-        return self.module(*a, **kw)
-
-    def __getattr__(self, k):
-        return getattr(self.module, k)
-
-
-def same_frozen_tower(a, b):
-    ta, tb = a.get_image_tower(), b.get_image_tower()
-    if ta is None or tb is None or not (ta.is_loaded and tb.is_loaded):
-        return False
-    sa, sb = ta.state_dict(), tb.state_dict()
-    if sa.keys() != sb.keys() or any(p.requires_grad for p in ta.parameters()) or any(p.requires_grad for p in tb.parameters()):
-        return False
-    return ta.select_layer == tb.select_layer and all(torch.equal(sa[k], sb[k]) for k in sa)
-
-
-def quantize_ref_fp8(ref, ref_fp8):
-    """--ref_fp8 / LLAVAMOD_REF_FP8=1: the frozen teacher's decoder linears run in FP8 (e4m3) from here on (quantize_fp8_ of the dense
-    causal-LM classes).  Opt-in: it changes the teacher's logits.  The quantisers and the e4m3 GEMM are plain stream-ordered launches, so
-    the teacher keeps its side stream, its one-micro-batch lead and its place in the captured step."""
-    import os
-    if (ref_fp8 or bool(int(os.environ.get("LLAVAMOD_REF_FP8", "0")))) and not ref.is_fp8:
-        ref.quantize_fp8_()
-
-
-class AlignTrainer(BaseTrainer):
+class AlignTrainer(AdapterCheckpointMixin, BaseTrainer):
     def __init__(self, model=None, ref_model=None, args=None, data_collator=None, train_dataset=None, eval_dataset=None,
                  tokenizer=None, label_pad_token_id: int = -100, padding_value: int = 0, beta: float = 0.1,
                  label_smoothing: float = 0, loss_type: str = "sigmoid", moe_loss_enable: bool = False,
                  disable_dropout: bool = True, model_init=None, compute_metrics=None, callbacks=None,
                  optimizers=(None, None), preprocess_logits_for_metrics=None, ref_fp8: bool = False):
-        if ref_model:
-            self.ref_model = ref_model
-        else:
-            self.ref_model = create_reference_model(model)
-        if disable_dropout:
-            disable_dropout_in_model(model)
-            disable_dropout_in_model(self.ref_model.module if hasattr(self.ref_model, "module") else self.ref_model)
         self.label_pad_token_id = label_pad_token_id
         self.padding_value = padding_value
         self.beta = beta
         self.label_smoothing = label_smoothing
         self.loss_type = loss_type
         self.moe_loss_enable = moe_loss_enable
-        self._stored_metrics = defaultdict(lambda: defaultdict(list))
         super().__init__(model=model, args=args, data_collator=data_collator, train_dataset=train_dataset,
                          eval_dataset=eval_dataset, tokenizer=tokenizer, model_init=model_init,
                          compute_metrics=compute_metrics, callbacks=callbacks, optimizers=optimizers,
                          preprocess_logits_for_metrics=preprocess_logits_for_metrics)
-        if not hasattr(self.ref_model, "module"):
-            self.ref_model = _Wrapped(self.ref_model)
-        self.ref_model.module.eval()
-        for p in self.ref_model.module.parameters():
-            p.requires_grad = False
-        self.share_tower = same_frozen_tower(self.model, self.ref_model.module)
+        self._init_teacher(ref_model, disable_dropout, ref_fp8)
         self.kd_vocab = KD_VOCAB_SIZE
-        import os
-        quantize_ref_fp8(self.ref_model.module, ref_fp8)
-        self.overlap_teacher = bool(int(os.environ.get("LLAVAMOD_OVERLAP_TEACHER", "1"))) and next(model.parameters()).is_cuda
-        self._teacher_stream = torch.cuda.Stream() if self.overlap_teacher else None
         self.pipeline_teacher = bool(int(os.environ.get("LLAVAMOD_PIPELINE_TEACHER", "1")))
         # loss head on the batch's supervised rows only (csrc/rows.cu): both lm_head GEMMs, the fused KL+CE kernel and the lm_head
         # backward skip the positions the reference multiplies by zero
@@ -131,6 +80,11 @@ class AlignTrainer(BaseTrainer):
         dev = model.device
         return torch.stack([im.to(dev, non_blocking=True) for im in images]) if not torch.is_tensor(images) else images.to(dev)
 
+    @staticmethod
+    def _forward_args(inputs, images):
+        """Keyword arguments of ``forward_hidden`` for the batch ``inputs`` with ``images`` (host list, device tensor or static buffer)."""
+        return dict(input_ids=inputs["input_ids"], labels=inputs["labels"], attention_mask=inputs.get("attention_mask"), images=images)
+
     def _teacher_forward(self, fwd, tower_feats, plan):
         """Frozen teacher -> bf16 logits (get_p's forward, align_trainer.py:458-461; its softmax lives in the fused kernel).
         -> (logits, (B, T'), rows): with the compact head `rows` = (perm, count) of the supervised rows of the post-splice labels and
@@ -150,7 +104,7 @@ class AlignTrainer(BaseTrainer):
         assert self.ref_model is not None, "ref model can not be none!"
         ref = self.ref_model.module
         images = inputs.get("images", None)
-        fwd = dict(input_ids=inputs["input_ids"], labels=inputs["labels"], attention_mask=inputs.get("attention_mask"), images=images)
+        fwd = self._forward_args(inputs, images)
         pipe = inputs.get("_pipeline")          # software pipeline across micro-batches (see _graph_static_inputs): teacher logits and tower
         tower_feats = None                      # features of THIS batch were produced during the previous micro-batch
         with torch.no_grad():
@@ -168,28 +122,19 @@ class AlignTrainer(BaseTrainer):
         # kernels (H=1024: launch/tail bound) fill the gaps of the teacher's machine-filling GEMMs (a fork/join inside the CUDA graph).
         # Pipelined form: the side stream computes the teacher for the NEXT micro-batch while the main stream runs the student's
         # forward, the loss and the backward of THIS one against teacher logits produced one micro-batch earlier.
-        main = torch.cuda.current_stream()
-        side = self._teacher_stream if self.overlap_teacher else None
-        if side is not None:
-            side.wait_stream(main)
-        with torch.no_grad(), torch.cuda.stream(side if side is not None else main):
+        with self._teacher_side():
             if pipe is not None:
                 nxt = pipe["next"]
                 tower_next = model.get_image_tower()(nxt["images"].to(model.dtype))
-                t_next, _, rows_next = self._teacher_forward(dict(input_ids=nxt["input_ids"], labels=nxt["labels"],
-                                                                  attention_mask=nxt.get("attention_mask"), images=nxt["images"]),
-                                                             tower_next, nxt["splice_plan"])
+                t_next, _, rows_next = self._teacher_forward(self._forward_args(nxt, nxt["images"]), tower_next, nxt["splice_plan"])
                 t_logits, t_shape, rows = pipe["t_cur"], pipe["t_shape"], pipe["rows_cur"]
             else:
                 with K.nvtx("teacher_forward"):
                     t_logits, t_shape, rows = self._teacher_forward(fwd, tower_feats, plan)
         with K.nvtx("student_forward"):
             s = model.forward_hidden(**fwd, tower_features=tower_feats, moe_noise=inputs.get("moe_noise"), plan=plan)
-        if side is not None and pipe is None:
-            main.wait_stream(side)
-            t_logits.record_stream(main)
-            for r in (rows or ()):
-                r.record_stream(main)
+        if pipe is None:
+            self._join_teacher(t_logits, *(rows or ()))
         labels = s["labels"]
         if s["hidden"].shape[:2] != labels.shape or tuple(t_shape) != tuple(labels.shape):
             raise ValueError("Logits (batch and sequence length dim) and labels must have the same shape.")
@@ -219,12 +164,6 @@ class AlignTrainer(BaseTrainer):
             return losses.mean(), outputs
         return losses.mean()
 
-    def store_metrics(self, metrics: Dict[str, float], train_eval: Literal["train", "eval"] = "train") -> None:
-        if self._suppress_store:          # graph capture: the static output tensors are cloned after every replay instead
-            return
-        for key, value in metrics.items():
-            self._stored_metrics[train_eval][key].append(value)
-
     # ---- CUDA-graph plumbing (see BaseTrainer._graphed_micro_batch) -------------------------------------------------
     def _graph_signature(self, inputs, next_inputs=None):
         images = inputs.get("images")
@@ -238,8 +177,7 @@ class AlignTrainer(BaseTrainer):
             inputs["splice_plan"] = plan
         if not self.share_tower or not plan["all_true"]:
             return None                   # padded batches take the masked-attention path eagerly
-        n_img = len(images) if not torch.is_tensor(images) else images.shape[0]
-        ish = tuple(images[0].shape) if not torch.is_tensor(images) else tuple(images.shape[1:])
+        n_img, ish = image_count_shape(images)
         sig = ("align", tuple(ids.shape), tuple(plan["src"].shape), n_img, ish, plan["has_mask"], plan["has_labels"], self.loss_type,
                tuple(tuple(t.shape) for t in noise) if noise is not None else None)
         if next_inputs is not None and self.overlap_teacher and self.pipeline_teacher:
@@ -257,9 +195,7 @@ class AlignTrainer(BaseTrainer):
                 with torch.no_grad():
                     self._fill_static(nxt, inputs)
                     tower = self.model.get_image_tower()(nxt["images"].to(self.model.dtype))
-                    t_cur, t_shape, rows_cur = self._teacher_forward(dict(input_ids=inputs["input_ids"], labels=inputs["labels"],
-                                                                          attention_mask=inputs.get("attention_mask"), images=nxt["images"]),
-                                                                     tower, nxt["splice_plan"])
+                    t_cur, t_shape, rows_cur = self._teacher_forward(self._forward_args(inputs, nxt["images"]), tower, nxt["splice_plan"])
                 static["_pipeline"] = dict(next=nxt, t_cur=t_cur.clone(), tower_cur=tower.clone(), t_shape=tuple(t_shape), holds=inputs,
                                            rows_cur=tuple(r.clone() for r in rows_cur) if rows_cur is not None else None)
         self._fill_static(static, inputs)
@@ -268,9 +204,7 @@ class AlignTrainer(BaseTrainer):
             if pipe["holds"] is not inputs:       # the "current" buffers do not belong to this batch (first call / caller skipped ahead)
                 with torch.no_grad():
                     tower = self.model.get_image_tower()(static["images"].to(self.model.dtype))
-                    t_cur, _, rows_cur = self._teacher_forward(dict(input_ids=inputs["input_ids"], labels=inputs["labels"],
-                                                                    attention_mask=inputs.get("attention_mask"), images=static["images"]),
-                                                               tower, static["splice_plan"])
+                    t_cur, _, rows_cur = self._teacher_forward(self._forward_args(inputs, static["images"]), tower, static["splice_plan"])
                     pipe["t_cur"].copy_(t_cur)
                     if rows_cur is not None:
                         for dst, src in zip(pipe["rows_cur"], rows_cur):
@@ -294,28 +228,3 @@ class AlignTrainer(BaseTrainer):
             else:
                 pipe["t_cur"].copy_(pipe["t_next"])
             pipe["tower_cur"].copy_(pipe["tower_next"])
-
-    def log(self, logs: Dict[str, float]) -> None:
-        train_eval = "train" if "loss" in logs else "eval"
-        for key, metrics in self._stored_metrics[train_eval].items():
-            logs[key] = torch.stack([torch.as_tensor(m, dtype=torch.float32).detach().cpu() for m in metrics]).mean().item()
-        del self._stored_metrics[train_eval]
-        return super().log(logs)
-
-    def _save_checkpoint(self, model, trial, metrics=None):
-        if getattr(self.args, "tune_mm_mlp_adapter", False):        # adaptor-only checkpoints (align_trainer.py:616-633)
-            import os
-            d = os.path.join(self._get_output_dir(trial), f"checkpoint-{self.state.global_step}")
-            if self.rank == 0:
-                os.makedirs(d, exist_ok=True)
-                self.model.config.save_pretrained(d)
-                w = {k: v.detach().cpu() for k, v in self.model.state_dict().items() if "mm_projector" in k}
-                torch.save(w, os.path.join(d, "mm_projector.bin"))
-        else:
-            super()._save_checkpoint(model, trial, metrics)
-
-    def _save(self, output_dir: Optional[str] = None, state_dict=None):
-        if getattr(self.args, "tune_mm_mlp_adapter", False):
-            pass
-        else:
-            super()._save(output_dir, state_dict)

@@ -9,7 +9,7 @@ import torch.distributed as dist
 
 from ..config.args import DataArguments, DPOArguments, ModelArguments, TrainingArguments, parse_args_into_dataclasses
 from ..constants import IGNORE_INDEX
-from .align_train import SyntheticMimicDataset, create_model_tokenizer, rank0_print
+from .align_train import SyntheticMimicDataset, create_model_tokenizer, init_process
 from .dpo_trainer import DPOTrainer
 
 
@@ -42,11 +42,7 @@ def collate_dpo(instances, pad_id=0):
 def train(argv=None):
     model_args, data_args, training_args, dpo_args = parse_args_into_dataclasses(
         (ModelArguments, DataArguments, TrainingArguments, DPOArguments), argv)
-    if "RANK" in os.environ and int(os.environ.get("WORLD_SIZE", "1")) > 1 and not dist.is_initialized():
-        torch.cuda.set_device(int(os.environ.get("LOCAL_RANK", "0")))
-        dist.init_process_group("nccl")
-    device = torch.device("cuda", int(os.environ.get("LOCAL_RANK", "0")))
-    torch.manual_seed(training_args.seed)
+    device = init_process(training_args.seed)
     model, _ = create_model_tokenizer(model_args, data_args, training_args, dpo_args.policy_model_name_or_path, dpo_args.policy_model_type, None, device)
     ref_model, _ = create_model_tokenizer(types.SimpleNamespace(**vars(model_args)), data_args, training_args, dpo_args.ref_model_name_or_path,
                                           dpo_args.ref_model_type, None, device)

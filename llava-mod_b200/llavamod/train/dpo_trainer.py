@@ -8,16 +8,13 @@ Hot loop: two frozen-teacher forwards (no grad) and two student forwards; each l
 log-softmax+gather kernel (online LSE + pick, 2*V bytes/token) instead of materialising log_softmax over [B,T,V]; the DPO
 scalar math runs on [B] device tensors; backward re-reads the bf16 logits once and writes d(logits) in place.
 """
-from collections import defaultdict
-from typing import Any, Dict, Literal, Tuple, Union
+from typing import Any, Dict, Tuple, Union
 
 import torch
 import torch.nn.functional as F
 
 from .. import kernels as K
-from ..model.utils import create_reference_model, disable_dropout_in_model
-from .align_trainer import _Wrapped, quantize_ref_fp8, same_frozen_tower
-from .trainer_base import BaseTrainer
+from .trainer_base import BaseTrainer, image_count_shape
 
 
 class DPOTrainer(BaseTrainer):
@@ -26,30 +23,17 @@ class DPOTrainer(BaseTrainer):
                  label_smoothing: float = 0, loss_type: str = "sigmoid", moe_loss_enable: bool = False,
                  disable_dropout: bool = True, model_init=None, compute_metrics=None, callbacks=None,
                  optimizers=(None, None), preprocess_logits_for_metrics=None, ref_fp8: bool = False):
-        self.ref_model = ref_model if ref_model else create_reference_model(model)
-        if disable_dropout:
-            disable_dropout_in_model(model)
         self.label_pad_token_id = label_pad_token_id
         self.padding_value = padding_value
         self.beta = beta
         self.label_smoothing = label_smoothing
         self.loss_type = loss_type
         self.moe_loss_enable = moe_loss_enable
-        self._stored_metrics = defaultdict(lambda: defaultdict(list))
         super().__init__(model=model, args=args, data_collator=data_collator, train_dataset=train_dataset,
                          eval_dataset=eval_dataset, tokenizer=tokenizer, model_init=model_init,
                          compute_metrics=compute_metrics, callbacks=callbacks, optimizers=optimizers,
                          preprocess_logits_for_metrics=preprocess_logits_for_metrics)
-        if not hasattr(self.ref_model, "module"):
-            self.ref_model = _Wrapped(self.ref_model)
-        self.ref_model.module.eval()
-        for p in self.ref_model.module.parameters():
-            p.requires_grad = False
-        self.share_tower = same_frozen_tower(self.model, self.ref_model.module)
-        quantize_ref_fp8(self.ref_model.module, ref_fp8)
-        import os
-        self.overlap_teacher = bool(int(os.environ.get("LLAVAMOD_OVERLAP_TEACHER", "1"))) and next(model.parameters()).is_cuda
-        self._teacher_stream = torch.cuda.Stream() if self.overlap_teacher else None
+        self._init_teacher(ref_model, disable_dropout, ref_fp8)
 
     def _seq_logp(self, model, fwd, tower_feats, noise=None, grad=True, plan=None):
         r = model.forward_hidden(**fwd, tower_features=tower_feats, moe_noise=noise, plan=plan)
@@ -119,20 +103,13 @@ class DPOTrainer(BaseTrainer):
             plan_r = model.make_splice_plan(rj["input_ids"], rj["attention_mask"], rj["labels"])
         # the two frozen reference forwards are independent of the policy until dpo_loss: they run on a side stream so the 0.5B policy's
         # small kernels fill the gaps of the 7B reference's machine-filling GEMMs (a fork/join inside the CUDA graph), as in AlignTrainer
-        main = torch.cuda.current_stream()
-        side = self._teacher_stream if self.overlap_teacher else None
-        if side is not None:
-            side.wait_stream(main)
-        with torch.no_grad(), torch.cuda.stream(side if side is not None else main):
+        with self._teacher_side():
             reference_chosen_logps, _ = self._seq_logp(ref, ch, tower_feats, grad=False, plan=plan_c)
             reference_rejected_logps, _ = self._seq_logp(ref, rj, tower_feats, grad=False, plan=plan_r)
         noise = inputs.get("moe_noise") or (None, None)
         policy_chosen_logps, rc = self._seq_logp(model, ch, tower_feats, noise[0], plan=plan_c)
         policy_rejected_logps, rr = self._seq_logp(model, rj, tower_feats, noise[1], plan=plan_r)
-        if side is not None:
-            main.wait_stream(side)
-            reference_chosen_logps.record_stream(main)
-            reference_rejected_logps.record_stream(main)
+        self._join_teacher(reference_chosen_logps, reference_rejected_logps)
         reward_losses, chosen_rewards, rejected_rewards = self.dpo_loss(policy_chosen_logps, policy_rejected_logps,
                                                                         reference_chosen_logps, reference_rejected_logps)
         enabled = getattr(self.args, "moe_enable", False) and self.moe_loss_enable and getattr(model, "is_moe", False)
@@ -160,14 +137,12 @@ class DPOTrainer(BaseTrainer):
             return losses.mean(), outputs
         return losses.mean()
 
-    def store_metrics(self, metrics: Dict[str, float], train_eval: Literal["train", "eval"] = "train") -> None:
-        if self._suppress_store:          # graph capture: the static output tensors are cloned after every replay instead
-            return
-        for key, value in metrics.items():
-            self._stored_metrics[train_eval][key].append(value)
-
     # ---- CUDA-graph plumbing (see BaseTrainer._graphed_micro_batch): the four forwards + two backwards of a pair are captured once per
     # input signature; static inputs = the image tensor and the two splice plans ------------------------------------------------------
+    _static_keys = ("chosen_input_ids", "chosen_labels", "chosen_attention_mask", "rejected_input_ids", "rejected_labels",
+                    "rejected_attention_mask")
+    _static_plans = ("splice_plan_chosen", "splice_plan_rejected")
+
     def _graph_signature(self, inputs, next_inputs=None):
         images = inputs.get("images")
         if images is None or inputs.get("moe_noise") is not None or not self.share_tower:
@@ -179,35 +154,5 @@ class DPOTrainer(BaseTrainer):
         pc, pr = inputs["splice_plan_chosen"], inputs["splice_plan_rejected"]
         if not (pc["all_true"] and pr["all_true"]):
             return None                   # padded pairs run eagerly
-        n_img = len(images) if not torch.is_tensor(images) else images.shape[0]
-        ish = tuple(images[0].shape) if not torch.is_tensor(images) else tuple(images.shape[1:])
+        n_img, ish = image_count_shape(images)
         return ("dpo", tuple(pc["src"].shape), tuple(pr["src"].shape), n_img, ish, pc["has_mask"], pr["has_mask"], self.loss_type)
-
-    def _graph_static_inputs(self, inputs, static):
-        images = inputs["images"]
-        if static is None:
-            dev = self.model.device
-            n = len(images) if not torch.is_tensor(images) else images.shape[0]
-            ish = tuple(images[0].shape) if not torch.is_tensor(images) else tuple(images.shape[1:])
-            static = {k: inputs[k] for k in ("chosen_input_ids", "chosen_labels", "chosen_attention_mask", "rejected_input_ids",
-                                             "rejected_labels", "rejected_attention_mask")}
-            static["images"] = torch.empty((n,) + ish, dtype=self.model.dtype, device=dev)
-            for side in ("chosen", "rejected"):
-                static["splice_plan_" + side] = {k: (torch.empty_like(v) if torch.is_tensor(v) else v) for k, v in inputs["splice_plan_" + side].items()}
-        if torch.is_tensor(images):
-            static["images"].copy_(images, non_blocking=True)
-        else:
-            for i, im in enumerate(images):
-                static["images"][i].copy_(im, non_blocking=True)
-        for side in ("chosen", "rejected"):
-            for k, v in inputs["splice_plan_" + side].items():
-                if torch.is_tensor(v):
-                    static["splice_plan_" + side][k].copy_(v, non_blocking=True)
-        return static
-
-    def log(self, logs: Dict[str, float]) -> None:
-        train_eval = "train" if "loss" in logs else "eval"
-        for key, metrics in self._stored_metrics[train_eval].items():
-            logs[key] = torch.stack([torch.as_tensor(m, dtype=torch.float32).detach().cpu() for m in metrics]).mean().item()
-        del self._stored_metrics[train_eval]
-        return super().log(logs)

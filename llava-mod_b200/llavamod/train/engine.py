@@ -140,7 +140,7 @@ class TrainState:
         self.m32 = torch.zeros_like(self.w32) if self.n32 else None
         self.v32 = torch.zeros_like(self.w32) if self.n32 else None
         self.gnorm_sq = torch.zeros(1, dtype=torch.float32, device=dev)
-        self.grads_reduced = False           # set by the trainer when the all-reduce already ran inside the last micro-batch's CUDA graph
+        self.grads_reduced = False           # True: the next step() skips the all-reduce (scripts/bench_optim_8bit.py times the step alone)
         gv = {}
         for storage, g in self._views:
             gv[id(storage)] = g

@@ -5,38 +5,12 @@ Reference: llavamod/train/llava_trainer.py:135-281 -- an HF `Trainer` whose loss
 the sparse classes), with the length-grouped sampler (:137-150; ours lives in BaseTrainer.get_train_dataloader), the decay / no-decay /
 projector-LR optimizer groups (:152-247; see BaseTrainer.create_optimizer for what the shells actually use) and adaptor-only
 checkpoints (:249-281).  Every kernel is the distillation path's; the teacher, the KL head and the side stream drop out."""
-import os
-from collections import defaultdict
-from typing import Optional
-
 import torch
 
-from .trainer_base import BaseTrainer
-
-
-class AdapterCheckpointMixin:
-    """`--tune_mm_mlp_adapter`: checkpoints hold config.json + mm_projector.bin only (llava_trainer.py:249-281, align_trainer.py:616-643)."""
-
-    def _save_checkpoint(self, model, trial, metrics=None):
-        if not getattr(self.args, "tune_mm_mlp_adapter", False):
-            return super()._save_checkpoint(model, trial, metrics)
-        d = os.path.join(self._get_output_dir(trial), f"checkpoint-{self.state.global_step}")
-        if self.rank == 0:
-            os.makedirs(d, exist_ok=True)
-            self.model.config.save_pretrained(d)
-            torch.save({k: v.detach().cpu() for k, v in self.model.state_dict().items() if "mm_projector" in k}, os.path.join(d, "mm_projector.bin"))
-
-    def _save(self, output_dir: Optional[str] = None, state_dict=None):
-        if not getattr(self.args, "tune_mm_mlp_adapter", False):
-            super()._save(output_dir, state_dict)
+from .trainer_base import AdapterCheckpointMixin, BaseTrainer, image_count_shape
 
 
 class LLaVATrainer(AdapterCheckpointMixin, BaseTrainer):
-    def __init__(self, model=None, args=None, data_collator=None, train_dataset=None, eval_dataset=None, tokenizer=None, **kw):
-        super().__init__(model=model, args=args, data_collator=data_collator, train_dataset=train_dataset, eval_dataset=eval_dataset,
-                         tokenizer=tokenizer, **kw)
-        self._stored_metrics = defaultdict(lambda: defaultdict(list))
-
     # ---- loss ------------------------------------------------------------------------------------------------------------------
     def compute_loss(self, model, inputs, return_outputs=False):
         images = inputs.get("images")
@@ -44,24 +18,11 @@ class LLaVATrainer(AdapterCheckpointMixin, BaseTrainer):
             images = [im.to(model.device, non_blocking=True) for im in images]
         loss, ce, moe = model.forward_train_loss(input_ids=inputs["input_ids"], attention_mask=inputs.get("attention_mask"), labels=inputs["labels"],
                                                  images=images, moe_noise=inputs.get("moe_noise"), plan=inputs.get("splice_plan"))
-        outputs = {"loss": loss.detach(), "loss/lm": ce}
+        outputs = {"loss/lm": ce}                        # no stored "loss": the logged loss is the train loop's average of the float losses
         if moe is not None:
             outputs["loss/moe_balance"] = moe.detach()
         self.store_metrics(outputs)
         return (loss, outputs) if return_outputs else loss
-
-    def store_metrics(self, metrics, train_eval="train"):
-        if self._suppress_store:
-            return
-        for k, v in metrics.items():
-            self._stored_metrics[train_eval][k].append(v)
-
-    def log(self, logs):
-        for key, vals in self._stored_metrics["train"].items():
-            if key != "loss":
-                logs[key] = torch.stack([torch.as_tensor(v, dtype=torch.float32).detach().cpu() for v in vals]).mean().item()
-        self._stored_metrics["train"].clear()
-        return super().log(logs)
 
     # ---- CUDA-graph plumbing (BaseTrainer._graphed_micro_batch): un-padded batches with explicit router noise absent -----------
     def _graph_signature(self, inputs, next_inputs=None):
@@ -73,12 +34,5 @@ class LLaVATrainer(AdapterCheckpointMixin, BaseTrainer):
             plan = inputs["splice_plan"] = self.model.make_splice_plan(inputs["input_ids"], inputs.get("attention_mask"), inputs["labels"])
         if not plan["all_true"]:
             return None                                  # padded batches take the masked-attention path eagerly
-        n = len(images) if not torch.is_tensor(images) else images.shape[0]
-        ish = tuple(images[0].shape) if not torch.is_tensor(images) else tuple(images.shape[1:])
+        n, ish = image_count_shape(images)
         return ("sft", tuple(inputs["input_ids"].shape), tuple(plan["src"].shape), n, ish, plan["has_mask"], plan["has_labels"])
-
-    def _graph_static_inputs(self, inputs, static, next_inputs=None, pipelined=False):
-        if static is None:
-            static = self._new_static(inputs)
-        self._fill_static(static, inputs)
-        return static

@@ -16,7 +16,7 @@ import torch
 import torch.distributed as dist
 
 from ..config.args import DataArguments, ModelArguments, TrainingArguments, parse_args_into_dataclasses
-from .align_train import create_model_tokenizer, load_tokenizer, make_supervised_data_module, rank0_print
+from .align_train import create_model_tokenizer, init_process, load_tokenizer, make_supervised_data_module
 from .llava_trainer import LLaVATrainer
 from .train_utils import safe_save_model_for_hf_trainer
 
@@ -43,11 +43,7 @@ def train(argv=None):
         raise NotImplementedError("LoRA / 4-8-bit training is outside the Qwen distillation path")
     if model_args.mm_use_im_start_end:
         raise NotImplementedError("--mm_use_im_start_end adds tokens and resizes the embeddings (initialize_vision_tokenizer); the Qwen shells keep it off")
-    if "RANK" in os.environ and int(os.environ.get("WORLD_SIZE", "1")) > 1 and not dist.is_initialized():
-        torch.cuda.set_device(int(os.environ.get("LOCAL_RANK", "0")))
-        dist.init_process_group("nccl")
-    device = torch.device("cuda", int(os.environ.get("LOCAL_RANK", "0")))
-    torch.manual_seed(training_args.seed)
+    device = init_process(training_args.seed)
     model, _ = create_model_tokenizer(model_args, data_args, training_args, model_args.model_name_or_path,
                                       "sparse" if model_args.moe_enable else "dense", model_args.pretrain_mm_mlp_adapter, device)
     training_args.moe_enable = model_args.moe_enable

@@ -5,16 +5,19 @@ The reference subclasses ``transformers.Trainer`` and runs under accelerate + De
 (llavamod/train/align_trainer.py:180-309).  Here one process drives one GPU; gradient accumulation is local, the
 optimizer is the fused AdamW of ``engine.TrainState`` and the only collective is the student-gradient all-reduce.
 """
+import contextlib
 import glob
 import json
 import os
 import re
 import time
 from collections import defaultdict
+from typing import Dict, Literal, Optional
 
 import torch
 import torch.distributed as dist
 
+from ..model.utils import create_reference_model, disable_dropout_in_model
 from .engine import TrainState, cosine_lr, optim_bits_of, warmup_steps_of
 
 
@@ -29,6 +32,45 @@ def _with_lookahead(iterable):
         yield cur, nxt
         cur = nxt
     yield cur, None
+
+
+class _Wrapped:
+    """Gives a bare module the ``.module`` attribute the reference dereferences on the DeepSpeed-wrapped teacher
+    (align_trainer.py:305,309); the build accepts wrapped and bare teachers (SURVEY.md Appendix B)."""
+
+    def __init__(self, module):
+        self.module = module
+
+    def __call__(self, *a, **kw):
+        return self.module(*a, **kw)
+
+    def __getattr__(self, k):
+        return getattr(self.module, k)
+
+
+def same_frozen_tower(a, b):
+    ta, tb = a.get_image_tower(), b.get_image_tower()
+    if ta is None or tb is None or not (ta.is_loaded and tb.is_loaded):
+        return False
+    sa, sb = ta.state_dict(), tb.state_dict()
+    if sa.keys() != sb.keys() or any(p.requires_grad for p in ta.parameters()) or any(p.requires_grad for p in tb.parameters()):
+        return False
+    return ta.select_layer == tb.select_layer and all(torch.equal(sa[k], sb[k]) for k in sa)
+
+
+def quantize_ref_fp8(ref, ref_fp8):
+    """--ref_fp8 / LLAVAMOD_REF_FP8=1: the frozen teacher's decoder linears run in FP8 (e4m3) from here on (quantize_fp8_ of the dense
+    causal-LM classes).  Opt-in: it changes the teacher's logits.  The quantisers and the e4m3 GEMM are plain stream-ordered launches, so
+    the teacher keeps its side stream, its one-micro-batch lead and its place in the captured step."""
+    if (ref_fp8 or bool(int(os.environ.get("LLAVAMOD_REF_FP8", "0")))) and not ref.is_fp8:
+        ref.quantize_fp8_()
+
+
+def image_count_shape(images):
+    """(number of images, shape of one image) of a batch's images: one tensor [n, ...] or a list of n tensors."""
+    if torch.is_tensor(images):
+        return images.shape[0], tuple(images.shape[1:])
+    return len(images), tuple(images[0].shape)
 
 
 class TrainerState:
@@ -63,13 +105,46 @@ class BaseTrainer:
         # pins its activations, so the cache is bounded (least-recently-used graph dropped) and all graphs share ONE memory pool
         self.max_graphs = int(os.environ.get("LLAVAMOD_MAX_GRAPHS", "6"))
         self._graph_pool = None
-        self._statics = {}                   # base signature -> static input buffers shared by the graphs of that signature
-        # data parallel experiment (LLAVAMOD_GRAPH_ALLREDUCE=1, OFF by default): capture the gradient all-reduce INSIDE the graph of the step's
-        # last micro-batch, behind the student's backward and ahead of the join with the teacher stream.  NCCL's CTAs then compete with the
-        # teacher's persistent GEMMs instead of hiding behind them, and c10d aborts at shutdown with captured NCCL work outstanding.
-        self.graph_allreduce = bool(int(os.environ.get("LLAVAMOD_GRAPH_ALLREDUCE", "0")))
         self._suppress_store = False
         self.graph_replayed_launches = 0     # liblmod kernels executed through graph replays (not seen by the host-side counter)
+        self._stored_metrics = defaultdict(lambda: defaultdict(list))
+
+    # ---- frozen teacher (AlignTrainer, DPOTrainer) ---------------------------------------------------------------
+    def _init_teacher(self, ref_model, disable_dropout, ref_fp8):
+        """Builds (a deep copy of the student) or takes the reference model, wraps a bare module in ``_Wrapped``, puts it in eval mode
+        and freezes it; then --ref_fp8, whether the two models share one frozen CLIP tower, and the teacher's side stream."""
+        ref = ref_model if ref_model else create_reference_model(self.model)
+        self.ref_model = ref if hasattr(ref, "module") else _Wrapped(ref)
+        if disable_dropout:
+            disable_dropout_in_model(self.model)
+            disable_dropout_in_model(self.ref_model.module)
+        self.ref_model.module.eval()
+        for p in self.ref_model.module.parameters():
+            p.requires_grad = False
+        self.share_tower = same_frozen_tower(self.model, self.ref_model.module)
+        quantize_ref_fp8(self.ref_model.module, ref_fp8)
+        self.overlap_teacher = bool(int(os.environ.get("LLAVAMOD_OVERLAP_TEACHER", "1"))) and next(self.model.parameters()).is_cuda
+        self._teacher_stream = torch.cuda.Stream() if self.overlap_teacher else None
+
+    @contextlib.contextmanager
+    def _teacher_side(self):
+        """Runs the block without grad on the teacher's side stream, after the work already queued on the main stream (on the main
+        stream when the overlap is off).  The main stream waits for it in ``_join_teacher``."""
+        main = torch.cuda.current_stream()
+        side = self._teacher_stream if self.overlap_teacher else None
+        if side is not None:
+            side.wait_stream(main)
+        with torch.no_grad(), torch.cuda.stream(side if side is not None else main):
+            yield
+
+    def _join_teacher(self, *tensors):
+        """With the overlap on, the main stream waits for the side stream and ``tensors``, allocated there, are marked as used by the
+        main stream."""
+        if self.overlap_teacher:
+            main = torch.cuda.current_stream()
+            main.wait_stream(self._teacher_stream)
+            for t in tensors:
+                t.record_stream(main)
 
     # ---- optimizer ---------------------------------------------------------------------------------------
     def create_optimizer(self):
@@ -135,20 +210,12 @@ class BaseTrainer:
     # ---- CUDA-graph replay of one micro-batch ----------------------------------------------------------------------
     def _graphed_micro_batch(self, model, inputs, next_inputs=None):
         """Returns the loss tensor (detached, static buffer clone) or None when this batch must run eagerly.
-        Subclasses provide ``_graph_signature(inputs)`` (hashable, or None = not capturable) and
-        ``_graph_static_inputs(inputs, static=None)`` (allocate / refill the static device inputs)."""
-        import torch
-        try:
-            sig = self._graph_signature(inputs, next_inputs)
-        except TypeError:
-            sig = self._graph_signature(inputs)
+        Subclasses provide ``_graph_signature(inputs, next_inputs)`` (hashable, or None = not capturable) and may override
+        ``_graph_static_inputs``."""
+        sig = self._graph_signature(inputs, next_inputs)
         if sig is None:
             return None
-        pipelined = isinstance(sig, tuple) and sig[-1] == "pipelined"
-        closing = (self.graph_allreduce and self.world_size > 1 and self._accum + 1 == self.args.gradient_accumulation_steps)
-        base_sig = sig
-        if closing:
-            sig = ("closing",) + tuple(sig)                 # its own graph: the same micro-batch + the captured gradient all-reduce
+        pipelined = sig[-1] == "pipelined"
         ent = self._graphs.pop(sig, None)                # re-inserted below: dict order = recency
         if ent is None:
             ent = {"warm": 0}
@@ -162,21 +229,8 @@ class BaseTrainer:
                 return None
             captured = [k for k, v in self._graphs.items() if "graph" in v]
             while len(captured) >= max(1, self.max_graphs):      # drop the least recently used graph with its static buffers
-                old = self._graphs.pop(captured.pop(0))
-                old_base = old.get("base")
-                old.clear()
-                if not any(v.get("base") == old_base for v in self._graphs.values()):
-                    self._statics.pop(old_base, None)
-            # the plain and the step-closing graph of one signature are captured against the SAME static buffers: they take turns on one
-            # stream of micro-batches, and the teacher's look-ahead state (logits / tower features of the next batch) must carry over
-            static = self._statics.get(base_sig)
-            if static is None:
-                static = self._graph_static_inputs(inputs, None, next_inputs, pipelined) if pipelined else self._graph_static_inputs(inputs, None)
-                self._statics[base_sig] = static
-            elif pipelined:
-                self._graph_static_inputs(inputs, static, next_inputs, True)
-            else:
-                self._graph_static_inputs(inputs, static)
+                self._graphs.pop(captured.pop(0)).clear()
+            static = self._graph_static_inputs(inputs, None, next_inputs, pipelined)
             torch.cuda.synchronize()
             from .. import _C
             g = torch.cuda.CUDAGraph()
@@ -188,52 +242,56 @@ class BaseTrainer:
                 with torch.cuda.graph(g, pool=self._graph_pool):
                     loss, outputs = self.compute_loss(model, static, return_outputs=True)
                     loss.backward()
-                    if closing:
-                        self.optimizer.allreduce_grads()          # NCCL nodes in the graph, ahead of the join with the teacher stream
                     if hasattr(self, "_graph_epilogue"):
                         self._graph_epilogue(static)
             finally:
                 self._suppress_store = False
-            ent.update(graph=g, static=static, base=base_sig, loss=loss.detach(), outputs={k: v for k, v in outputs.items()},
+            ent.update(graph=g, static=static, loss=loss.detach(), outputs={k: v for k, v in outputs.items()},
                        launches=_C.launch_count() - n0)
             # the capture pass does not execute: fall through to a replay for this very batch
-        if pipelined:
-            self._graph_static_inputs(inputs, ent["static"], next_inputs, True)
-        else:
-            self._graph_static_inputs(inputs, ent["static"])
+        self._graph_static_inputs(inputs, ent["static"], next_inputs, pipelined)
         ent["graph"].replay()
-        if closing:
-            self.optimizer.grads_reduced = True              # TrainState.step() must not reduce again
         self.graph_replayed_launches += ent["launches"]
         self.store_metrics({k: (v.clone() if hasattr(v, "clone") else v) for k, v in ent["outputs"].items()}, train_eval="train")
         return ent["loss"].clone()
 
-    # static device inputs of a captured micro-batch: images + the precomputed splice plan (ids / labels / masks stay host-side: the
-    # plan already encodes them)
+    # static device inputs of a captured micro-batch: images + the precomputed splice plans (ids / labels / masks stay host-side: the
+    # plans already encode them).  _static_keys are carried as they are, _static_plans are the splice plans' keys.
+    _static_keys = ("input_ids", "labels", "attention_mask")
+    _static_plans = ("splice_plan",)
+
+    def _graph_static_inputs(self, inputs, static, next_inputs=None, pipelined=False):
+        """Allocates (static None) and refills the static inputs of a captured micro-batch."""
+        if static is None:
+            static = self._new_static(inputs)
+        self._fill_static(static, inputs)
+        return static
+
     def _fill_static(self, static, inputs):
-        images, plan = inputs["images"], inputs["splice_plan"]
+        images = inputs["images"]
         if torch.is_tensor(images):
             static["images"].copy_(images, non_blocking=True)
         else:
             for i, im in enumerate(images):
                 static["images"][i].copy_(im, non_blocking=True)
-        for k, v in plan.items():
-            if torch.is_tensor(v):
-                static["splice_plan"][k].copy_(v, non_blocking=True)
+        for name in self._static_plans:
+            for k, v in inputs[name].items():
+                if torch.is_tensor(v):
+                    static[name][k].copy_(v, non_blocking=True)
         if static.get("moe_noise") is not None:           # explicit router noise (parity runs): static buffers like every other device input
             for dst, src in zip(static["moe_noise"], inputs["moe_noise"]):
                 dst.copy_(src, non_blocking=True)
 
     def _new_static(self, inputs):
         dev = self.model.device
-        images, plan = inputs["images"], inputs["splice_plan"]
-        n = len(images) if not torch.is_tensor(images) else images.shape[0]
-        ish = tuple(images[0].shape) if not torch.is_tensor(images) else tuple(images.shape[1:])
+        n, ish = image_count_shape(inputs["images"])
         noise = inputs.get("moe_noise")
-        return dict(input_ids=inputs["input_ids"], labels=inputs["labels"], attention_mask=inputs.get("attention_mask"),
-                    moe_noise=[torch.empty(tuple(t.shape), dtype=torch.float32, device=dev) for t in noise] if noise is not None else None,
-                    images=torch.empty((n,) + ish, dtype=self.model.dtype, device=dev),
-                    splice_plan={k: (torch.empty_like(v) if torch.is_tensor(v) else v) for k, v in plan.items()})
+        static = {k: inputs.get(k) for k in self._static_keys}
+        static["moe_noise"] = [torch.empty(tuple(t.shape), dtype=torch.float32, device=dev) for t in noise] if noise is not None else None
+        static["images"] = torch.empty((n,) + ish, dtype=self.model.dtype, device=dev)
+        for name in self._static_plans:
+            static[name] = {k: (torch.empty_like(v) if torch.is_tensor(v) else v) for k, v in inputs[name].items()}
+        return static
 
     # ---- loop ------------------------------------------------------------------------------------------------
     def get_train_dataloader(self):
@@ -298,7 +356,18 @@ class BaseTrainer:
         return {"train_runtime": time.time() - t0, "global_step": self.state.global_step}
 
     # ---- logging / saving --------------------------------------------------------------------------------------
-    def log(self, logs):
+    def store_metrics(self, metrics: Dict[str, float], train_eval: Literal["train", "eval"] = "train") -> None:
+        if self._suppress_store:          # graph capture: the static output tensors are cloned after every replay instead
+            return
+        for key, value in metrics.items():
+            self._stored_metrics[train_eval][key].append(value)
+
+    def log(self, logs: Dict[str, float]) -> None:
+        """store_metrics/log of the reference (align_trainer.py:596-614): the means of the stored metrics join the logged values."""
+        train_eval = "train" if "loss" in logs else "eval"
+        for key, metrics in self._stored_metrics[train_eval].items():
+            logs[key] = torch.stack([torch.as_tensor(m, dtype=torch.float32).detach().cpu() for m in metrics]).mean().item()
+        del self._stored_metrics[train_eval]
         logs = dict(logs)
         logs["step"] = self.state.global_step
         self.state.log_history.append(logs)
@@ -397,3 +466,20 @@ class BaseTrainer:
             self.state.global_step = int(m[-1])
         rp = os.path.join(d, "rng_state.pth")
         return torch.load(rp, map_location="cpu", weights_only=True) if os.path.exists(rp) else None
+
+
+class AdapterCheckpointMixin:
+    """`--tune_mm_mlp_adapter`: checkpoints hold config.json + mm_projector.bin only (llava_trainer.py:249-281, align_trainer.py:616-643)."""
+
+    def _save_checkpoint(self, model, trial, metrics=None):
+        if not getattr(self.args, "tune_mm_mlp_adapter", False):
+            return super()._save_checkpoint(model, trial, metrics)
+        d = os.path.join(self._get_output_dir(trial), f"checkpoint-{self.state.global_step}")
+        if self.rank == 0:
+            os.makedirs(d, exist_ok=True)
+            self.model.config.save_pretrained(d)
+            torch.save({k: v.detach().cpu() for k, v in self.model.state_dict().items() if "mm_projector" in k}, os.path.join(d, "mm_projector.bin"))
+
+    def _save(self, output_dir: Optional[str] = None, state_dict=None):
+        if not getattr(self.args, "tune_mm_mlp_adapter", False):
+            super()._save(output_dir, state_dict)

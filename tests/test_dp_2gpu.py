@@ -48,7 +48,7 @@ def _run_inner(rank, world, port, q, loss_kind, graphs=False):
     accum = GLOBAL // world
     kind = "dpo" if loss_kind == "sigmoid" else "align"
     tr = Hh.make_trainer(student, teacher, loss_kind, accum=accum, lr=1e-3, max_steps=STEPS, kind=kind)
-    tr.use_cuda_graphs = graphs             # graphs on: the last micro-batch of a step replays the variant that holds the NCCL all-reduce
+    tr.use_cuda_graphs = graphs             # graphs on: micro-batches replay their graphs; the NCCL all-reduce runs eagerly in the optimizer step
     assert tr.world_size == world
     losses, gnorms = [], []
     for step in range(STEPS):

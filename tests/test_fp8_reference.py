@@ -163,7 +163,7 @@ def test_quantize_fp8_refuses_trainable_decoder_weights_and_sparse_models():
 
 def test_trainers_take_ref_fp8_and_the_environment_switch(monkeypatch):
     import inspect
-    from llavamod.train import align_trainer as A
+    from llavamod.train import align_trainer as A, trainer_base as B
     from llavamod.train.dpo_trainer import DPOTrainer
     assert inspect.signature(A.AlignTrainer.__init__).parameters["ref_fp8"].default is False
     assert inspect.signature(DPOTrainer.__init__).parameters["ref_fp8"].default is False
@@ -177,9 +177,9 @@ def test_trainers_take_ref_fp8_and_the_environment_switch(monkeypatch):
 
     r = Ref()
     monkeypatch.delenv("LLAVAMOD_REF_FP8", raising=False)
-    A.quantize_ref_fp8(r, False)
+    B.quantize_ref_fp8(r, False)
     assert r.calls == 0
     monkeypatch.setenv("LLAVAMOD_REF_FP8", "1")
-    A.quantize_ref_fp8(r, False)
-    A.quantize_ref_fp8(r, True)                                 # already quantised: not again
+    B.quantize_ref_fp8(r, False)
+    B.quantize_ref_fp8(r, True)                                 # already quantised: not again
     assert r.calls == 1

@@ -359,6 +359,37 @@ def test_dpo_trainer_matches_oracle():
                 assert abs(got - want) < 1e-2 * abs(want) + (2e-2 if (k.startswith("rewards") or lt == "ipo") else 5e-3), (lt, k, got, want)
 
 
+def test_dpo_graph_replay_matches_eager():
+    """Un-padded pairs without explicit router noise are captured into a CUDA graph after two eager warm-ups; the replayed losses and
+    all ten logged metrics equal the eager ones (dense policy, whose forward draws no router noise; lr = 0)."""
+    from llavamod.model import synthetic as S
+    teacher = S.make_teacher(dict(S.ARCH["tiny"]), "tiny", seed=0)
+    student = S.make_teacher(dict(S.ARCH["tiny"]), "tiny", seed=9).train()
+    student.get_image_tower().load_state_dict(teacher.get_image_tower().state_dict())
+    for n, p in student.named_parameters():
+        p.requires_grad = "image_tower" not in n
+    pairs = []
+    for i in range(3):
+        inputs = _dpo_inputs(student, seeds=(60 + 2 * i, 61 + 2 * i))[-1]
+        del inputs["moe_noise"]                                    # the dense policy draws none
+        pairs.append(inputs)
+    tr = Hh.make_trainer(student, teacher, "sigmoid", lr=0.0, kind="dpo")
+    tr.use_cuda_graphs = False
+    eager = [float(tr.training_step(student, dict(pairs[i % 3]))) for i in range(6)]
+    tr2 = Hh.make_trainer(student, teacher, "sigmoid", lr=0.0, kind="dpo")
+    tr2.optimizer = tr.optimizer
+    got = [float(tr2.training_step(student, dict(pairs[i % 3]))) for i in range(6)]
+    assert tr2._graphs and any("graph" in e for e in tr2._graphs.values())
+    for a, b in zip(eager, got):
+        assert abs(a - b) < 1e-5 * abs(a) + 1e-6, (eager, got)
+    for k in DPO_METRICS:
+        want = [float(v) for v in tr._stored_metrics["train"][k]]
+        have = [float(v) for v in tr2._stored_metrics["train"][k]]
+        assert len(want) == len(have) == 6, k
+        for a, b in zip(want, have):
+            assert abs(a - b) < 1e-5 * abs(a) + 1e-6, (k, want, have)
+
+
 @pytest.mark.parametrize("loss_type", ["sigmoid", "ipo"])
 def test_dpo_gradients_match_oracle_autograd(loss_type):
     """Backward of the preference step through the fused log-prob head (lmod_logp_gather_bwd), two student forwards sharing one set of
