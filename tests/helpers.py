@@ -949,7 +949,12 @@ def qkv_rope_reference_fp64(x, w, bias, cos, sin, pos, nh, nkv, hd, K_red):
     maj = x64.abs() @ w64.abs().t()
     if bias is not None:
         P, maj = P + bias.double(), maj + bias.double().abs()
-    E = _gemm_tol(P, maj, K_red)
+    return rope_of_product_fp64(P, _gemm_tol(P, maj, K_red), cos, sin, pos, nh, nkv, hd)
+
+
+def rope_of_product_fp64(P, E, cos, sin, pos, nh, nkv, hd):
+    """The rotation of qkv_rope_reference_fp64 on a given float64 product P [M, N] whose bf16 kernel value is within E of it (the bf16 GEMM
+    there, the e4m3 GEMM of lmod_gemm_e4m3_qkv_rope in tests/decoder_oracle.py).  Returns (want, tol), float64 [M, N]."""
     M = P.shape[0]
     nr = nh + nkv
     h = hd // 2
@@ -1290,8 +1295,9 @@ def moe_run_stages(x, res, wg, w_gu, w_dn, noise, cf, mc, dout, g_laux, old):
     return k
 
 
-def check_moe_stages(k, ref, E, old, report=None):
-    """Every stage of moe_run_stages against moe_reference_fp64(..., k=k): the routing record bit for bit, then each stage's bound."""
+def check_moe_stages(k, ref, E, old, report=None, backward=True):
+    """Every stage of moe_run_stages against moe_reference_fp64(..., k=k): the routing record bit for bit, then each stage's bound.
+    backward=False: the forward stages only (k from kernels.moe_forward_stages, ref without dout)."""
     rec = ref["rec"]
     n_rows = int(rec["offsets"][-1])
     assert torch.equal(k["idx"].long(), rec["idx"]), "routing record (first / second expert)"
@@ -1301,17 +1307,19 @@ def check_moe_stages(k, ref, E, old, report=None):
     assert torch.equal(k["meta"][4:4 + E].long(), rec["counts"])
     routed = rec["tok"] >= 0
     pad = ~routed
-    for name in ("logits", "gates", "dw", "dlogits", "dx"):
+    for name in ("logits", "gates") + (("dw", "dlogits", "dx") if backward else ()):
         check_moe(name, k[name], *ref[name], report=report)
     check_moe("w", k["w"], ref["w"][0], None, report)
     la_want, la_tol = ref["l_aux"]
     assert abs(float(k["meta"][0]) - float(la_want)) <= float(la_tol), ("l_aux", float(k["meta"][0]), float(la_want))
     check_moe("xp", k["xp"][:n_rows], ref["xp"][0], None, report)
-    for name in ("h1", "act", "y", "dh1", "dxp", "dact"):
+    for name in ("h1", "act", "y") + (("dh1", "dxp", "dact") if backward else ()):
         check_moe(name, k[name][:n_rows], *ref[name], report=report, rows=routed)
         if name in ("h1", "act", "y"):                           # padding rows below offsets[E] are exact zeros
             assert int(k[name][:n_rows][pad].ne(0).sum()) == 0, f"{name}: non-zero padding row"
     check_moe("out", k["out"], ref["out"][0], None, report)
+    if not backward:
+        return
     check_moe("dy", k["dy"][:n_rows], ref["dy"][0], None, report)
     assert int(k["dy"][n_rows:].ne(0).sum()) == 0
     check_moe("g_wg", k["g_wg"], *ref["g_wg"], report=report)
