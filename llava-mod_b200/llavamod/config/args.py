@@ -6,6 +6,7 @@ DeepSpeed are not on this path); unknown HF flags are accepted and ignored with 
 command lines keep working (``--deepspeed <json>`` is accepted and ignored: plain data parallelism replaces ZeRO-2)."""
 import argparse
 import dataclasses
+import json
 import sys
 import warnings
 from dataclasses import dataclass, field
@@ -86,6 +87,7 @@ class TrainingArguments:
     fp16: bool = False
     tf32: Optional[bool] = None
     gradient_checkpointing: bool = False
+    gradient_checkpointing_kwargs: Optional[dict] = None       # HF's; accepted, no effect (one checkpoint implementation)
     dataloader_num_workers: int = 0
     report_to: Optional[str] = "none"
     deepspeed: Optional[str] = None
@@ -165,6 +167,8 @@ def parse_args_into_dataclasses(dataclass_types, argv=None):
             kw = {}
             if "bool" in tp:
                 kw = dict(type=_str2bool, nargs="?", const=True)
+            elif "dict" in tp:
+                kw = dict(type=json.loads)              # HfArgumentParser takes a dict field as a JSON string
             elif "List[int]" in tp:
                 kw = dict(type=int, nargs="+")
             elif "List[str]" in tp:

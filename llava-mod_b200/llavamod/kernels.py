@@ -1069,6 +1069,49 @@ def moe_residual_forward_nograd(x, res, wg, w_gu, w_dn, noise, cf, min_cap, r_gu
 
 
 # ---------------------------------------------------------------------------------------------------
+# activation checkpointing of one decoder layer (HF gradient checkpointing, modeling_qwen2.py:1062-1072)
+# ---------------------------------------------------------------------------------------------------
+_ANCHOR = torch.empty(0, requires_grad=True)
+
+
+class CheckpointFn(Function):
+    """One decoder layer as a checkpointed segment.  run(*inputs) -> tuple of output tensors runs the layer on the Functions above; it
+    must draw no random numbers (the caller draws the router noise before the segment and binds it into run).
+    Forward: run under autograd on detached copies of the inputs, so the very kernels of the un-checkpointed layer run (grad forms
+    included), then drop that graph: only the inputs are kept.  Backward: run again -- the same kernels on the same bytes give the same
+    bytes -- and back-propagate the incoming gradients through it; parameter gradients accumulate into their arena views as in the plain
+    layer.  anchor: a tensor that requires grad, so the segment of a trainable layer whose inputs do not require grad still gets a
+    backward (what enable_input_require_grads works around in the reference)."""
+
+    @staticmethod
+    def forward(ctx, run, anchor, *inputs):
+        ctx.run = run
+        ctx.save_for_backward(*inputs)
+        with torch.enable_grad():
+            outs = run(*_ckpt_inputs(inputs, ctx.needs_input_grad[2:]))
+        return tuple(o.detach() for o in outs)
+
+    @staticmethod
+    def backward(ctx, *grads):
+        xs = _ckpt_inputs(ctx.saved_tensors, ctx.needs_input_grad[2:])
+        with torch.enable_grad():
+            outs = ctx.run(*xs)
+        pairs = [(o, g) for o, g in zip(outs, grads) if o.requires_grad and g is not None]
+        if pairs:
+            torch.autograd.backward([o for o, _ in pairs], [g for _, g in pairs])
+        return (None, None) + tuple(x.grad if x.requires_grad else None for x in xs)
+
+
+def _ckpt_inputs(inputs, needs):
+    return [t.detach().requires_grad_(n) for t, n in zip(inputs, needs)]
+
+
+def checkpoint(run, *inputs):
+    """CheckpointFn on the segment inputs -> run's outputs, none of run's intermediates kept."""
+    return CheckpointFn.apply(run, _ANCHOR, *inputs)
+
+
+# ---------------------------------------------------------------------------------------------------
 # fused lm_head + mimic-KL (+ shifted CE) loss head
 # ---------------------------------------------------------------------------------------------------
 # optional per-kernel device timing (bench.py roofline): name -> list of (start_event, end_event) on the launching stream

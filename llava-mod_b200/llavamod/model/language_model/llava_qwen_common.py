@@ -7,6 +7,7 @@ The Qwen-1.5 and Qwen-2 files of the reference differ only in names, so the conc
 ``llava_qwen1_5*.py`` / ``llava_qwen2*.py`` just bind names to this implementation.
 """
 import os
+import warnings
 from typing import List, Optional
 
 import torch
@@ -82,6 +83,32 @@ class LlavaQwenForCausalLMBase(nn.Module, LlavaMetaForCausalLM):
 
     def get_input_embeddings(self):
         return self.model.embed_tokens
+
+    # ---- gradient checkpointing (HF PreTrainedModel surface) -----------------------------------------
+    supports_gradient_checkpointing = True
+    _input_require_grads = False
+
+    def gradient_checkpointing_enable(self, gradient_checkpointing_kwargs=None):
+        """From now on every decoder layer of the language model that has something to differentiate runs as one checkpointed segment
+        while the model trains with autograd recording: its activations are recomputed in the backward instead of kept (Qwen2Model._layers,
+        kernels.CheckpointFn).  Loss, routing and gradients are those of the run without it.  gradient_checkpointing_kwargs (e.g.
+        use_reentrant) is accepted for HF compatibility and has no effect: there is one implementation."""
+        self.model.gradient_checkpointing = True
+
+    def gradient_checkpointing_disable(self):
+        self.model.gradient_checkpointing = False
+
+    @property
+    def is_gradient_checkpointing(self):
+        return self.model.gradient_checkpointing
+
+    def enable_input_require_grads(self):
+        """The embeddings the decoder receives require grad while autograd records (HF registers a forward hook on the input embeddings
+        for this).  A checkpointed layer delivers its parameter gradients without it; the reference's trainers call it with checkpointing."""
+        self._input_require_grads = True
+
+    def disable_input_require_grads(self):
+        self._input_require_grads = False
 
     def state_dict_reference_layout(self):
         """state_dict with tied lm_head de-duplicated the way HF saves it."""
@@ -187,6 +214,8 @@ class LlavaQwenForCausalLMBase(nn.Module, LlavaMetaForCausalLM):
                     attention_mask = attention_mask.to(self.device)
                 if labels is not None:
                     labels = labels.to(self.device)
+        if self._input_require_grads and torch.is_grad_enabled() and not inputs_embeds.requires_grad:
+            inputs_embeds = inputs_embeds.detach().requires_grad_(True)
         hidden, l_auxes, records = self.model(inputs_embeds, attention_mask, position_ids, moe_noise=moe_noise,
                                               training_moe=self.training, cache=cache)
         if hasattr(attention_mask, "mask"):
@@ -217,6 +246,9 @@ class LlavaQwenForCausalLMBase(nn.Module, LlavaMetaForCausalLM):
         cache = None
         if self.is_fp8 and labels is not None:
             raise RuntimeError("an e4m3-quantised model is forward-only: call it without labels")
+        if use_cache and self.model.gradient_checkpointing and self.training and torch.is_grad_enabled():
+            warnings.warn("`use_cache=True` is incompatible with gradient checkpointing. Setting `use_cache=False`...")     # modeling_qwen2.py:993-998
+            use_cache = False
         if past_key_values is not None or use_cache:
             # KV-cache path (modeling_qwen2.py:1110-1217 with past_key_values; llava_arch.py:162-172 for the cached multimodal step).
             # Without a cache one is allocated for the prompt plus CACHE_ROOM positions; pass new_kv_cache(B, max_len) for longer runs.

@@ -362,7 +362,8 @@ class Qwen2Model(nn.Module):
                 K.kv_append(qkv, B, T, nh, nkv, hd, cache.k[li], cache.v[li], cache.len)
             return K.attention(qkv, B, T, nh, nkv, hd, True, None, pad)
 
-        out, l_auxes, records = self._layers(inputs_embeds.reshape(B * T, H), cos, sin, pos, attend, moe_noise, training_moe)
+        checkpoint = cache is None and self.gradient_checkpointing and self.training and torch.is_grad_enabled()
+        out, l_auxes, records = self._layers(inputs_embeds.reshape(B * T, H), cos, sin, pos, attend, moe_noise, training_moe, checkpoint)
         if ragged:
             cache.len.add_(pad[1] - pad[0])
             cache.advance(lengths)
@@ -412,50 +413,71 @@ class Qwen2Model(nn.Module):
         cache.advance(T)
         return out.view(B, T, H), l_auxes, records
 
-    def _layers(self, stream, cos, sin, pos, attend, moe_noise, training_moe):
+    def _layers(self, stream, cos, sin, pos, attend, moe_noise, training_moe, checkpoint=False):
         """The decoder layers and the final norm on the residual stream [S,H]: -> (final-normed hidden [S,H], [l_aux per MoE layer],
         routing records).  attend(li, qkv, nh, nkv, hd) -> attn is layer li's attention on its RoPE'd q|k|v rows, the one part in which
-        forward and the cached step differ.  moe_noise: one tensor per MoE layer, or None to draw each layer's noise for its S tokens."""
+        forward and the cached step differ.  moe_noise: one tensor per MoE layer, or None to draw each layer's noise for its S tokens.
+        checkpoint: every layer with something to differentiate runs as one checkpointed segment (K.checkpoint): its activations are
+        recomputed in the backward instead of kept."""
         eps = self.config.rms_norm_eps
         branch = None                                   # pending residual-branch output (added inside the next norm)
         l_auxes, records = [], []
         moe_i = 0
         for li, layer in enumerate(self.layers):
-            at = layer.self_attn
-            nh, nkv, hd = at.num_heads, at.num_key_value_heads, at.head_dim
-            fp8 = isinstance(at.qkv_weight, K.Fp8Rows)      # a layer of quantize_fp8_: the norms hand e4m3 rows to e4m3 projections
-            x, res = (stream, None) if branch is None else (branch, stream)
-            if fp8:
-                x, stream = K.rmsnorm_quant(x, layer.input_layernorm.weight, eps, res=res)
-                qkv = K.qkv_rope_fp8(x, at.qkv_weight, at.qkv_bias, cos, sin, pos, nh, nkv, hd)
-            else:
-                x, stream = K.rmsnorm(x, layer.input_layernorm.weight, eps, res=res, wgrad=self.gview(layer.input_layernorm.weight))
-                qkv = K.qkv_rope(x, at.qkv_weight, at.qkv_bias, cos, sin, pos, nh, nkv, hd, self.gview(at.qkv_weight), self.gview(at.qkv_bias))
-            attn = attend(li, qkv, nh, nkv, hd)
-            if fp8:
-                branch = K.linear_fp8(attn, at.o_fp8)
-                x, stream = K.rmsnorm_quant(branch, layer.post_attention_layernorm.weight, eps, res=stream)
-            else:
-                branch = K.linear(attn, at.o_proj.weight, None, self.gview(at.o_proj.weight), None)
-                x, stream = K.rmsnorm(branch, layer.post_attention_layernorm.weight, eps, res=stream,
-                                      wgrad=self.gview(layer.post_attention_layernorm.weight))
             mlp = layer.mlp
+            noise = None
             if isinstance(mlp, MoE):
+                # drawn before the layer runs, so a checkpointed layer's recompute routes with the noise of its first forward
                 noise = moe_noise[moe_i] if moe_noise is not None else moe_draw((stream.shape[0], mlp.num_experts), mlp.k, stream.device)
                 moe_i += 1
-                cf = mlp.capacity_factor if training_moe else mlp.eval_capacity_factor
-                stream, l_aux, rec = mlp.run(x, stream, noise, cf, self.gview)
+            inputs = (stream,) if branch is None else (branch, stream)
+            if checkpoint and (any(t.requires_grad for t in inputs) or any(p.requires_grad for p in layer.parameters())):
+                def run(*xs, li=li, layer=layer, noise=noise):
+                    return self._layer(li, layer, xs, cos, sin, pos, attend, noise, training_moe)[:2]
+                branch_or_stream, out = K.checkpoint(run, *inputs)
+                rec = None
+            else:
+                branch_or_stream, out, rec = self._layer(li, layer, inputs, cos, sin, pos, attend, noise, training_moe)
+            if not isinstance(mlp, MoE):
+                branch, stream = branch_or_stream, out
+            else:
+                branch, stream = None, branch_or_stream
+                l_auxes.append(out)
                 if rec is not None:
                     records.append(rec)
-                l_auxes.append(l_aux)
-                branch = None
-            elif fp8:
-                branch = K.mlp_fp8(x, mlp.gu_weight, mlp.down_fp8)
-            else:
-                branch = K.mlp(x, mlp.gu_weight, mlp.down_proj.weight, self.gview(mlp.gu_weight), self.gview(mlp.down_proj.weight))
         x, res = (stream, None) if branch is None else (branch, stream)
         out, _ = K.rmsnorm(x, self.norm.weight, eps, res=res, wgrad=self.gview(self.norm.weight))
         return out, l_auxes, records
+
+    def _layer(self, li, layer, inputs, cos, sin, pos, attend, noise, training_moe):
+        """Decoder layer li on its inputs: (stream,) or (pending branch, stream) -> (branch, stream, None) for a dense layer, (stream, l_aux,
+        routing record or None) for an MoE layer.  noise: the MoE layer's router noise."""
+        eps = self.config.rms_norm_eps
+        at = layer.self_attn
+        nh, nkv, hd = at.num_heads, at.num_key_value_heads, at.head_dim
+        fp8 = isinstance(at.qkv_weight, K.Fp8Rows)      # a layer of quantize_fp8_: the norms hand e4m3 rows to e4m3 projections
+        x, res = inputs if len(inputs) == 2 else (inputs[0], None)
+        if fp8:
+            x, stream = K.rmsnorm_quant(x, layer.input_layernorm.weight, eps, res=res)
+            qkv = K.qkv_rope_fp8(x, at.qkv_weight, at.qkv_bias, cos, sin, pos, nh, nkv, hd)
+        else:
+            x, stream = K.rmsnorm(x, layer.input_layernorm.weight, eps, res=res, wgrad=self.gview(layer.input_layernorm.weight))
+            qkv = K.qkv_rope(x, at.qkv_weight, at.qkv_bias, cos, sin, pos, nh, nkv, hd, self.gview(at.qkv_weight), self.gview(at.qkv_bias))
+        attn = attend(li, qkv, nh, nkv, hd)
+        if fp8:
+            branch = K.linear_fp8(attn, at.o_fp8)
+            x, stream = K.rmsnorm_quant(branch, layer.post_attention_layernorm.weight, eps, res=stream)
+        else:
+            branch = K.linear(attn, at.o_proj.weight, None, self.gview(at.o_proj.weight), None)
+            x, stream = K.rmsnorm(branch, layer.post_attention_layernorm.weight, eps, res=stream,
+                                  wgrad=self.gview(layer.post_attention_layernorm.weight))
+        mlp = layer.mlp
+        if isinstance(mlp, MoE):
+            cf = mlp.capacity_factor if training_moe else mlp.eval_capacity_factor
+            return mlp.run(x, stream, noise, cf, self.gview)
+        if fp8:
+            return K.mlp_fp8(x, mlp.gu_weight, mlp.down_fp8), stream, None
+        return K.mlp(x, mlp.gu_weight, mlp.down_proj.weight, self.gview(mlp.gu_weight), self.gview(mlp.down_proj.weight)), stream, None
 
 
 class KVCache:

@@ -106,6 +106,17 @@ def create_model_tokenizer(model_args, data_args, training_args, name_or_path, m
     return model, None
 
 
+def prepare_gradient_checkpointing(model, training_args):
+    """--gradient_checkpointing on the model being trained (align_train.py:276-281, dpo_train.py:245-247, train.py:278-281); the frozen
+    teacher is never differentiated and is left alone.  The trainer switches the decoder's recompute on when training starts."""
+    if not training_args.gradient_checkpointing:
+        return
+    if model.config.use_cache:
+        rank0_print("`use_cache=True` is incompatible with gradient checkpointing: use_cache=False while training")
+        model.config.use_cache = False
+    model.enable_input_require_grads()
+
+
 class SyntheticMimicDataset(torch.utils.data.Dataset):
     """Seeded samples of the named shape (SURVEY section 8d): one <image>, 40 % instruction mask."""
 
@@ -173,6 +184,7 @@ def train(argv=None):
         rank0_print("note: --deepspeed %s accepted and ignored (plain data parallelism, resident optimizer state)" % training_args.deepspeed)
     model, _ = create_model_tokenizer(model_args, data_args, training_args, align_args.policy_model_name_or_path,
                                       align_args.policy_model_type, align_args.policy_pretrain_mm_mlp_adapter, device)
+    prepare_gradient_checkpointing(model, training_args)
     ref_args = types.SimpleNamespace(**vars(model_args))
     ref_model, _ = create_model_tokenizer(ref_args, data_args, training_args, align_args.ref_model_name_or_path,
                                           align_args.ref_model_type, align_args.ref_pretrain_mm_mlp_adapter, device)

@@ -179,7 +179,7 @@ class AlignTrainer(AdapterCheckpointMixin, BaseTrainer):
             return None                   # padded batches take the masked-attention path eagerly
         n_img, ish = image_count_shape(images)
         sig = ("align", tuple(ids.shape), tuple(plan["src"].shape), n_img, ish, plan["has_mask"], plan["has_labels"], self.loss_type,
-               tuple(tuple(t.shape) for t in noise) if noise is not None else None)
+               tuple(tuple(t.shape) for t in noise) if noise is not None else None, self._grad_ckpt_key())
         if next_inputs is not None and self.overlap_teacher and self.pipeline_teacher:
             nsig = self._graph_signature(next_inputs)
             if nsig == sig:

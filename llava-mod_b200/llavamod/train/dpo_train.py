@@ -9,7 +9,7 @@ import torch.distributed as dist
 
 from ..config.args import DataArguments, DPOArguments, ModelArguments, TrainingArguments, parse_args_into_dataclasses
 from ..constants import IGNORE_INDEX
-from .align_train import SyntheticMimicDataset, create_model_tokenizer, init_process
+from .align_train import SyntheticMimicDataset, create_model_tokenizer, init_process, prepare_gradient_checkpointing
 from .dpo_trainer import DPOTrainer
 
 
@@ -44,6 +44,7 @@ def train(argv=None):
         (ModelArguments, DataArguments, TrainingArguments, DPOArguments), argv)
     device = init_process(training_args.seed)
     model, _ = create_model_tokenizer(model_args, data_args, training_args, dpo_args.policy_model_name_or_path, dpo_args.policy_model_type, None, device)
+    prepare_gradient_checkpointing(model, training_args)
     ref_model, _ = create_model_tokenizer(types.SimpleNamespace(**vars(model_args)), data_args, training_args, dpo_args.ref_model_name_or_path,
                                           dpo_args.ref_model_type, None, device)
     training_args.moe_enable = model_args.moe_enable

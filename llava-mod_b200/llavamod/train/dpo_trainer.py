@@ -155,4 +155,5 @@ class DPOTrainer(BaseTrainer):
         if not (pc["all_true"] and pr["all_true"]):
             return None                   # padded pairs run eagerly
         n_img, ish = image_count_shape(images)
-        return ("dpo", tuple(pc["src"].shape), tuple(pr["src"].shape), n_img, ish, pc["has_mask"], pr["has_mask"], self.loss_type)
+        return ("dpo", tuple(pc["src"].shape), tuple(pr["src"].shape), n_img, ish, pc["has_mask"], pr["has_mask"], self.loss_type,
+                self._grad_ckpt_key())

@@ -35,4 +35,5 @@ class LLaVATrainer(AdapterCheckpointMixin, BaseTrainer):
         if not plan["all_true"]:
             return None                                  # padded batches take the masked-attention path eagerly
         n, ish = image_count_shape(images)
-        return ("sft", tuple(inputs["input_ids"].shape), tuple(plan["src"].shape), n, ish, plan["has_mask"], plan["has_labels"])
+        return ("sft", tuple(inputs["input_ids"].shape), tuple(plan["src"].shape), n, ish, plan["has_mask"], plan["has_labels"],
+                self._grad_ckpt_key())

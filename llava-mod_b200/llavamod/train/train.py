@@ -16,7 +16,8 @@ import torch
 import torch.distributed as dist
 
 from ..config.args import DataArguments, ModelArguments, TrainingArguments, parse_args_into_dataclasses
-from .align_train import create_model_tokenizer, init_process, load_tokenizer, make_supervised_data_module
+from .align_train import (create_model_tokenizer, init_process, load_tokenizer, make_supervised_data_module,
+                          prepare_gradient_checkpointing)
 from .llava_trainer import LLaVATrainer
 from .train_utils import safe_save_model_for_hf_trainer
 
@@ -49,6 +50,7 @@ def train(argv=None):
     training_args.moe_enable = model_args.moe_enable
     model.config.mm_use_im_start_end = data_args.mm_use_im_start_end = model_args.mm_use_im_start_end      # train.py (reference): same assignment
     select_trainable(model, model_args, training_args)
+    prepare_gradient_checkpointing(model, training_args)
     path = (data_args.data_path or ["synthetic"])[0]
     tokenizer = None
     if not str(path).startswith("synthetic"):

@@ -108,6 +108,8 @@ class BaseTrainer:
         self._suppress_store = False
         self.graph_replayed_launches = 0     # liblmod kernels executed through graph replays (not seen by the host-side counter)
         self._stored_metrics = defaultdict(lambda: defaultdict(list))
+        if getattr(args, "gradient_checkpointing", False) and hasattr(model, "enable_input_require_grads"):
+            model.enable_input_require_grads()         # align_trainer.py:243-246, dpo_trainer.py:243-246
 
     # ---- frozen teacher (AlignTrainer, DPOTrainer) ---------------------------------------------------------------
     def _init_teacher(self, ref_model, disable_dropout, ref_fp8):
@@ -313,8 +315,14 @@ class BaseTrainer:
         return DataLoader(self.train_dataset, batch_size=self.args.per_device_train_batch_size, sampler=sampler,
                           collate_fn=self.data_collator, num_workers=self.args.dataloader_num_workers, pin_memory=True, drop_last=True)
 
+    def _grad_ckpt_key(self):
+        """Part of every _graph_signature: a graph captured with checkpointing on holds the recompute, one captured with it off does not."""
+        return ("grad_ckpt", bool(getattr(self.model, "is_gradient_checkpointing", False)))
+
     def train(self, resume_from_checkpoint=None):
         a = self.args
+        if getattr(a, "gradient_checkpointing", False):  # transformers Trainer._inner_training_loop
+            self.model.gradient_checkpointing_enable(gradient_checkpointing_kwargs=getattr(a, "gradient_checkpointing_kwargs", None))
         dl = self.get_train_dataloader()
         steps_per_epoch = max(1, len(dl) // a.gradient_accumulation_steps)
         self._total_steps = a.max_steps if a.max_steps > 0 else int(steps_per_epoch * a.num_train_epochs)
