@@ -356,6 +356,20 @@ int64_t lmod_attn_decode_chunk_ws_elems(int64_t batch, int64_t T, int nh, int nk
 int lmod_attn_decode_chunk(const void* q, int64_t ld_q, const void* k_cache, const void* v_cache, const int32_t* len, int64_t batch,
                            int64_t T, int nh, int nkv, int hd, int64_t max_len, float softmax_scale, void* out, int64_t ld_o, float* lse,
                            float* ws, int64_t ws_elems, void* stream);
+/* lmod_attn_decode_shared: one new query for each of n sequences per prompt that share the prompt's K / V (num_return_sequences): q
+ *   [batch*n, ld_q] (row b*n + j: copy j of prompt b).  Prompt b's keys [0, prefix_len[b]) are rows of the prefix buffers
+ *   [batch, nkv, p_max, hd]; copy j's keys from prefix_len[b] on are rows of its suffix buffers [batch*n, nkv, s_max, hd] (key i at suffix
+ *   row i - prefix_len[b]).  len int32 [batch*n] total keys per sequence, prefix_len int32 [batch], both on the device; len - prefix_len
+ *   <= s_max.  A 64-key block wholly inside the prefix is read once for all copies a CTA serves (min(n, 8 / (nh/nkv)) of them).  max_len:
+ *   the length the expanded per-sequence cache would have; the splits are lmod_attn_decode's at that max_len, so every row's out and lse
+ *   are the bytes lmod_attn_decode gives on that row's materialised cache (its prefix rows, then its suffix rows).  out [batch*n, nh*hd]
+ *   (row stride ld_o), lse [batch*n, nh] or NULL.  hd in {64,128}, nh/nkv <= 8, any n >= 1.  ws: fp32 workspace of at least
+ *   lmod_attn_decode_shared_ws_elems(...). */
+int64_t lmod_attn_decode_shared_ws_elems(int64_t batch, int64_t n, int nh, int nkv, int hd, int64_t max_len);
+int lmod_attn_decode_shared(const void* q, int64_t ld_q, const void* k_prefix, const void* v_prefix, const int32_t* prefix_len, int64_t p_max,
+                            const void* k_suffix, const void* v_suffix, int64_t s_max, const int32_t* len, int64_t batch, int64_t n, int nh,
+                            int nkv, int hd, int64_t max_len, float softmax_scale, void* out, int64_t ld_o, float* lse, float* ws,
+                            int64_t ws_elems, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Assisted decoding (csrc/spec.cu).

@@ -22,6 +22,17 @@
 // each virtual head has its own key limit.  A key at or past the limit scores -inf and is skipped by P.V, and a split wholly past a row's
 // limit leaves (m, l) = (-inf, 0), so row t runs the single-query kernel's arithmetic at len = len[b] - T + t + 1 operation for operation:
 // the same splits, 64-key blocks, lane-to-key mapping and merge.  Its out and lse are the bytes lmod_attn_decode gives for that row alone.
+//
+// lmod_attn_decode_shared: n sequences per prompt (num_return_sequences) that share the prompt's K / V.  Prompt b's rows
+// [0, prefix_len[b]) live once in a prefix buffer [B, nkv, P_max, hd]; copy j's rows from prefix_len[b] on in its own suffix buffer
+// [B*n, nkv, S_max, hd] (suffix row i - prefix_len[b] holds key i).  The same kernel body with SHARED: a CTA serves the virtual heads
+// (copy j, query head g) of one KV head, min(n, 8 / G) copies per CTA, each with its own key limit len[b*n + j].  Its key range is walked
+// as a list of items: a 64-key block wholly inside the prefix is one item, loaded once and scored for every virtual head of the CTA (the
+// bandwidth saving); a block that reaches past the prefix is one item per copy, loaded from the prefix and the copy's suffix rows and
+// applied to that copy's heads only.
+// Each copy's heads see every block of its key range once, with the lmod_attn_decode splits of the max_len passed in (the bucketed length
+// the expanded cache would have), the same lane-to-key mapping, per-head limits as in the chunk kernel, and the same merge, so sequence
+// b*n + j's out and lse are the bytes lmod_attn_decode gives on its materialised cache (prefix rows then suffix rows) at that max_len.
 #include "sm90.cuh"
 
 namespace {
@@ -30,6 +41,7 @@ constexpr int DEC_THREADS = 128;
 constexpr int DEC_BK = 64;            // keys per ring stage
 constexpr int DEC_MIN_BLOCKS = 4;     // a split covers at least this many key blocks
 constexpr int DEC_MAX_G = 8;          // query heads per KV head
+enum DecMode { DEC_SINGLE, DEC_CHUNK, DEC_SHARED };
 
 template <int HD> struct DecCfg {
   static constexpr int NST = HD == 128 ? 3 : 4;
@@ -51,7 +63,12 @@ struct DecParams {
   float* ws_ml;             // [B, nh, nsplit, 2]  (running max in log2 units, sum of exp2)
   int nh, nkv, max_len, nsplit, split_blocks;
   float scale_log2;
-  int T, g, rows;           // chunk only: query rows per sequence (q / ws rows are b*T + t), query heads per KV head, rows per CTA
+  int T, g, rows;           // chunk: query rows per sequence (q / ws rows are b*T + t), query heads per KV head, rows per CTA
+                            // shared: T = n copies per prompt (q / ws / len rows are b*n + j), g as chunk, rows = copies per CTA
+  const __nv_bfloat16* ks;  // shared only: suffix buffers [B*n, nkv, s_max, HD]; k / v above are the prefix buffers [B, nkv, max_len, HD]
+  const __nv_bfloat16* vs;
+  const int32_t* plen;      // shared only: [B] prefix rows per prompt (device)
+  int p_max, s_max;
 };
 
 template <int HD>
@@ -66,12 +83,62 @@ __device__ __forceinline__ void dec_issue(uint8_t* sK, uint8_t* sV, uint64_t* fu
   bulk_g2s(sV + s * C::KV_BYTES, vg + (size_t)k0 * HD, bytes, &full[s]);
 }
 
-// CHUNK = false: G query heads of one row per CTA.  CHUNK = true: G virtual heads v = (row t0 + v / p.g, head v % p.g), the rows of
-// blockIdx.y / nkv's row group; virtual heads past row T - 1 have limit 0 and write nothing.
-template <int HD, int G, bool CHUNK = false>
+// shared: item i of a CTA's key range -> (block j, copy c of the CTA, or -1 for a block wholly in the prefix, which is the first jp blocks)
+__device__ __forceinline__ void dec_item(int i, int jp, int ncopy, int& j, int& c) {
+  if (i < jp) { j = i; c = -1; }
+  else { j = jp + (i - jp) / ncopy; c = (i - jp) % ncopy; }
+}
+
+// shared: the keys copy c0 + c of prompt b may see, clamped so no row outside the prefix or suffix buffer is ever addressed
+__device__ __forceinline__ int dec_shared_lim(const DecParams& p, int b, int c, int plen) {
+  return c < p.T ? max(0, min(min(p.len[b * p.T + c], p.max_len), plen + p.s_max)) : 0;
+}
+
+// shared: stage the rows of item i.  A prefix block comes from the prefix buffer; a copy's block from the prefix rows below plen and its
+// own suffix rows from plen on, only rows below the copy's limit (an item with none still arrives on the stage's barrier).
+template <int HD>
+__device__ __forceinline__ void dec_issue_shared(uint8_t* sK, uint8_t* sV, uint64_t* full, const DecParams& p, int b, int hk, int c0,
+                                                 int plen, int kbeg, int kend, int jp, int ncopy, int i) {
+  using C = DecCfg<HD>;
+  const int s = i % C::NST;
+  int j, c;
+  dec_item(i, jp, ncopy, j, c);
+  const int k0 = kbeg + j * DEC_BK;
+  const int kn = min(DEC_BK, kend - k0);
+  const size_t pre = ((size_t)b * p.nkv + hk) * p.p_max;
+  uint8_t* dk = sK + s * C::KV_BYTES;
+  uint8_t* dv = sV + s * C::KV_BYTES;
+  if (c < 0) {
+    const uint32_t bytes = (uint32_t)kn * HD * 2;
+    mbar_expect_tx(&full[s], 2 * bytes);
+    bulk_g2s(dk, p.k + (pre + k0) * HD, bytes, &full[s]);
+    bulk_g2s(dv, p.v + (pre + k0) * HD, bytes, &full[s]);
+    return;
+  }
+  const int e = min(k0 + kn, dec_shared_lim(p, b, c0 + c, plen));      // this copy's keys of the block: [k0, e)
+  const int np = max(0, min(e, plen) - k0);                            // from the prefix: [k0, k0 + np)
+  const int k1 = max(k0, plen);
+  const int ns = max(0, e - k1);                                       // from the suffix: [k1, k1 + ns)
+  mbar_expect_tx(&full[s], 2u * (uint32_t)(np + ns) * HD * 2);
+  if (np > 0) {
+    bulk_g2s(dk, p.k + (pre + k0) * HD, (uint32_t)np * HD * 2, &full[s]);
+    bulk_g2s(dv, p.v + (pre + k0) * HD, (uint32_t)np * HD * 2, &full[s]);
+  }
+  if (ns > 0) {
+    const size_t suf = (((size_t)b * p.T + c0 + c) * p.nkv + hk) * p.s_max + (k1 - plen);
+    bulk_g2s(dk + (size_t)(k1 - k0) * HD * 2, p.ks + suf * HD, (uint32_t)ns * HD * 2, &full[s]);
+    bulk_g2s(dv + (size_t)(k1 - k0) * HD * 2, p.vs + suf * HD, (uint32_t)ns * HD * 2, &full[s]);
+  }
+}
+
+// SINGLE: G query heads of one row per CTA.  CHUNK: G virtual heads v = (row t0 + v / p.g, head v % p.g), the rows of blockIdx.y / nkv's
+// row group; virtual heads past row T - 1 have limit 0 and write nothing.  SHARED: as CHUNK with copies for rows (t0 = the CTA's first copy,
+// b = the prompt), each virtual head limited by its copy's len, the key range walked as items (dec_item).
+template <int HD, int G, int MODE = DEC_SINGLE>
 __global__ void __launch_bounds__(DEC_THREADS) attn_decode_kernel(const DecParams p) {
   using C = DecCfg<HD>;
   constexpr int NST = C::NST, LANES = C::LANES, GROUPS = C::GROUPS, PAIRS = C::PAIRS, KSUB = C::KSUB;
+  constexpr bool VIRT = MODE != DEC_SINGLE, SHARED = MODE == DEC_SHARED;
   extern __shared__ __align__(128) uint8_t dec_smem[];
   __shared__ __align__(8) uint64_t full[NST];
   __shared__ __align__(16) float s_p[DEC_BK][DEC_MAX_G];       // scores, then probabilities: [key][head]
@@ -80,12 +147,13 @@ __global__ void __launch_bounds__(DEC_THREADS) attn_decode_kernel(const DecParam
   uint8_t* sK = dec_smem;
   uint8_t* sV = dec_smem + NST * C::KV_BYTES;
 
-  const int split = blockIdx.x, hk = CHUNK ? blockIdx.y % p.nkv : blockIdx.y, b = blockIdx.z;
+  const int split = blockIdx.x, hk = VIRT ? blockIdx.y % p.nkv : blockIdx.y, b = blockIdx.z;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  int len = min(p.len[b], p.max_len);
-  int lim[G];                                           // chunk: key limit of each virtual head
-  const int t0 = CHUNK ? (int)(blockIdx.y / p.nkv) * p.rows : 0;
-  if constexpr (CHUNK) {
+  int len = SHARED ? 0 : min(p.len[b], p.max_len);
+  int lim[G];                                           // chunk / shared: key limit of each virtual head
+  const int t0 = VIRT ? (int)(blockIdx.y / p.nkv) * p.rows : 0;
+  const int plen = SHARED ? max(0, min(p.plen[b], p.p_max)) : 0;
+  if constexpr (MODE == DEC_CHUNK) {
     const int base = p.len[b] - p.T;                    // cached rows before this step's T
 #pragma unroll
     for (int g = 0; g < G; ++g) {
@@ -94,9 +162,20 @@ __global__ void __launch_bounds__(DEC_THREADS) attn_decode_kernel(const DecParam
     }
     len = max(0, min(base + min(t0 + p.rows, p.T), p.max_len));     // the row group's largest limit
   }
+  if constexpr (SHARED) {
+#pragma unroll
+    for (int g = 0; g < G; ++g) {
+      lim[g] = dec_shared_lim(p, b, t0 + g / p.g, plen);
+      len = max(len, lim[g]);
+    }
+  }
   const int kbeg = split * p.split_blocks * DEC_BK;
   const int kend = min(len, kbeg + p.split_blocks * DEC_BK);
   const int nblk = kend > kbeg ? (kend - kbeg + DEC_BK - 1) / DEC_BK : 0;     // a split at or past len[b] contributes nothing
+  // shared: the first jp blocks lie wholly in the prefix (one item each), every later block is one item per copy of the CTA
+  const int ncopy = SHARED ? max(1, min(p.rows, p.T - t0)) : 1;
+  const int jp = !SHARED || kend <= plen ? nblk : min(nblk, max(0, plen - kbeg) / DEC_BK);
+  const int nitem = jp + (nblk - jp) * ncopy;
   const size_t head_row = ((size_t)b * p.nkv + hk) * p.max_len;
   const __nv_bfloat16* kg = p.k + head_row * HD;
   const __nv_bfloat16* vg = p.v + head_row * HD;
@@ -108,7 +187,10 @@ __global__ void __launch_bounds__(DEC_THREADS) attn_decode_kernel(const DecParam
   if (tid < G) { s_m[tid] = -INFINITY; s_l[tid] = 0.f; }
   __syncthreads();
   if (tid == 0)
-    for (int j = 0; j < min(NST, nblk); ++j) dec_issue<HD>(sK, sV, full, kg, vg, kbeg, kend, j);
+    for (int i = 0; i < min(NST, nitem); ++i) {
+      if constexpr (SHARED) dec_issue_shared<HD>(sK, sV, full, p, b, hk, t0, plen, kbeg, kend, jp, ncopy, i);
+      else dec_issue<HD>(sK, sV, full, kg, vg, kbeg, kend, i);
+    }
 
   // this lane's 8 columns of every query head of the group
   const int li = tid % LANES, grp = tid / LANES;
@@ -116,7 +198,7 @@ __global__ void __launch_bounds__(DEC_THREADS) attn_decode_kernel(const DecParam
 #pragma unroll
   for (int g = 0; g < G; ++g) {
     uint4 w;
-    if constexpr (CHUNK) {
+    if constexpr (VIRT) {
       const int t = t0 + g / p.g;
       w = t < p.T ? *reinterpret_cast<const uint4*>(p.q + ((int64_t)b * p.T + t) * p.ld_q + (int64_t)(hk * p.g + g % p.g) * HD + li * 8)
                   : make_uint4(0u, 0u, 0u, 0u);
@@ -131,16 +213,18 @@ __global__ void __launch_bounds__(DEC_THREADS) attn_decode_kernel(const DecParam
 #pragma unroll
   for (int g = 0; g < G; ++g) o[g][0] = o[g][1] = 0.f;
 
-  for (int j = 0; j < nblk; ++j) {
-    const int s = j % NST;
+  for (int i = 0; i < nitem; ++i) {
+    const int s = i % NST;
+    int j = i, c = -1;                                   // c >= 0: an item of copy t0 + c only (shared), whose heads alone it updates
+    if constexpr (SHARED) dec_item(i, jp, ncopy, j, c);
     const int kb = kbeg + j * DEC_BK;
     const int n = min(DEC_BK, kend - kb);
-    mbar_wait_bounded(&full[s], (j / NST) & 1);
+    mbar_wait_bounded(&full[s], (i / NST) & 1);
     // ---- scores: every lane group runs the same trip count (the shuffles need the whole warp); rows >= n are discarded ----
     const uint8_t* Ks = sK + s * C::KV_BYTES;
 #pragma unroll
-    for (int t0 = 0; t0 < DEC_BK; t0 += GROUPS) {
-      const int t = t0 + grp;
+    for (int r0 = 0; r0 < DEC_BK; r0 += GROUPS) {
+      const int t = r0 + grp;
       const uint4 w = *reinterpret_cast<const uint4*>(Ks + (t * HD + li * 8) * 2);
       const float kf[8] = {bf16lo(w.x), bf16hi(w.x), bf16lo(w.y), bf16hi(w.y), bf16lo(w.z), bf16hi(w.z), bf16lo(w.w), bf16hi(w.w)};
       float sc[G];
@@ -157,17 +241,18 @@ __global__ void __launch_bounds__(DEC_THREADS) attn_decode_kernel(const DecParam
         for (int g = 0; g < G; ++g) sc[g] += __shfl_xor_sync(0xffffffffu, sc[g], off);
       if (li == 0)
 #pragma unroll
-        for (int g = 0; g < G; ++g) s_p[t][g] = t < n && (!CHUNK || kb + t < lim[g]) ? sc[g] * p.scale_log2 : -INFINITY;
+        for (int g = 0; g < G; ++g) s_p[t][g] = t < n && (!VIRT || kb + t < lim[g]) ? sc[g] * p.scale_log2 : -INFINITY;
     }
     __syncthreads();
     // ---- online softmax, one warp per head (key 0 of the block is always valid, so the block max is finite; in a chunk a virtual head
     //      may have seen no valid key yet: m stays -inf, and exponents are taken against 0 so p = alpha = l = 0 instead of NaN) ----
     for (int g = warp; g < G; g += DEC_THREADS / 32) {
-      const float a = s_p[lane][g], c = s_p[lane + 32][g];
+      if (SHARED && c >= 0 && g / p.g != c) continue;   // another copy's head: its rows are not in this stage
+      const float a = s_p[lane][g], cc = s_p[lane + 32][g];
       const float m_old = s_m[g];
-      const float m_new = fmaxf(m_old, warp_max(fmaxf(a, c)));
-      const float m_ref = CHUNK && m_new == -INFINITY ? 0.f : m_new;
-      const float pa = ex2f(a - m_ref), pc = ex2f(c - m_ref);
+      const float m_new = fmaxf(m_old, warp_max(fmaxf(a, cc)));
+      const float m_ref = VIRT && m_new == -INFINITY ? 0.f : m_new;
+      const float pa = ex2f(a - m_ref), pc = ex2f(cc - m_ref);
       s_p[lane][g] = pa;
       s_p[lane + 32][g] = pc;
       const float sum = warp_sum(pa + pc);
@@ -181,21 +266,28 @@ __global__ void __launch_bounds__(DEC_THREADS) attn_decode_kernel(const DecParam
     __syncthreads();
     // ---- O = alpha * O + P V over the valid rows only ----
 #pragma unroll
-    for (int g = 0; g < G; ++g) { o[g][0] *= s_alpha[g]; o[g][1] *= s_alpha[g]; }
+    for (int g = 0; g < G; ++g) {
+      if (SHARED && c >= 0 && g / p.g != c) continue;
+      o[g][0] *= s_alpha[g]; o[g][1] *= s_alpha[g];
+    }
     const uint8_t* Vs = sV + s * C::KV_BYTES;
     for (int t = ks; t < n; t += KSUB) {
       const uint32_t w = *reinterpret_cast<const uint32_t*>(Vs + (t * HD + 2 * pair) * 2);
       const float v0 = bf16lo(w), v1 = bf16hi(w);
 #pragma unroll
       for (int g = 0; g < G; ++g) {
-        if (CHUNK && kb + t >= lim[g]) continue;        // past this row's limit: not visited, as the single-query kernel does not
+        if (VIRT && kb + t >= lim[g]) continue;         // past this row's limit: not visited, as the single-query kernel does not
+        if (SHARED && c >= 0 && g / p.g != c) continue;
         const float pg = s_p[t][g];
         o[g][0] = fmaf(pg, v0, o[g][0]);
         o[g][1] = fmaf(pg, v1, o[g][1]);
       }
     }
     __syncthreads();                                     // stage s and s_p are free again
-    if (tid == 0 && j + NST < nblk) dec_issue<HD>(sK, sV, full, kg, vg, kbeg, kend, j + NST);
+    if (tid == 0 && i + NST < nitem) {
+      if constexpr (SHARED) dec_issue_shared<HD>(sK, sV, full, p, b, hk, t0, plen, kbeg, kend, jp, ncopy, i + NST);
+      else dec_issue<HD>(sK, sV, full, kg, vg, kbeg, kend, i + NST);
+    }
   }
 
   // ---- reduce the key subsets, write this split's partial ----
@@ -207,7 +299,7 @@ __global__ void __launch_bounds__(DEC_THREADS) attn_decode_kernel(const DecParam
     float a = 0.f;
 #pragma unroll
     for (int q = 0; q < KSUB; ++q) a += s_red[q][g][d];
-    if constexpr (CHUNK) {
+    if constexpr (VIRT) {
       const int t = t0 + g / p.g;
       if (t < p.T) p.ws_o[((((size_t)b * p.T + t) * p.nh + hk * p.g + g % p.g) * p.nsplit + split) * HD + d] = a;
     } else {
@@ -217,7 +309,7 @@ __global__ void __launch_bounds__(DEC_THREADS) attn_decode_kernel(const DecParam
   }
   if (tid < G) {
     float* ml;
-    if constexpr (CHUNK) {
+    if constexpr (VIRT) {
       const int t = t0 + tid / p.g;
       if (t >= p.T) return;
       ml = p.ws_ml + ((((size_t)b * p.T + t) * p.nh + hk * p.g + tid % p.g) * p.nsplit + split) * 2;
@@ -332,32 +424,32 @@ int launch_decode_g(const DecParams& p, int64_t batch, int G, cudaStream_t st) {
   }
 }
 
-// chunk: G = virtual heads per CTA (rows per CTA * query heads per KV head); grid y = KV head + nkv * row group
-template <int HD, int G>
-int launch_decode_chunk(const DecParams& p, int64_t batch, cudaStream_t st) {
+// chunk / shared: G = virtual heads per CTA (rows or copies per CTA * query heads per KV head); grid y = KV head + nkv * row group
+template <int HD, int G, int MODE>
+int launch_decode_virt(const DecParams& p, int64_t batch, cudaStream_t st) {
   constexpr int SMEM = DecCfg<HD>::SMEM;
   static bool attr = false;
   if (!attr) {
-    LMOD_CUDA_OK(cudaFuncSetAttribute(attn_decode_kernel<HD, G, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
+    LMOD_CUDA_OK(cudaFuncSetAttribute(attn_decode_kernel<HD, G, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
     attr = true;
   }
   const unsigned groups = (unsigned)((p.T + p.rows - 1) / p.rows);
-  attn_decode_kernel<HD, G, true><<<dim3(p.nsplit, p.nkv * groups, (unsigned)batch), DEC_THREADS, SMEM, st>>>(p);
+  attn_decode_kernel<HD, G, MODE><<<dim3(p.nsplit, p.nkv * groups, (unsigned)batch), DEC_THREADS, SMEM, st>>>(p);
   LMOD_LAUNCH_OK();
   return LMOD_OK;
 }
 
-template <int HD>
-int launch_decode_chunk_g(const DecParams& p, int64_t batch, int VG, cudaStream_t st) {
+template <int HD, int MODE>
+int launch_decode_virt_g(const DecParams& p, int64_t batch, int VG, cudaStream_t st) {
   switch (VG) {
-    case 1: return launch_decode_chunk<HD, 1>(p, batch, st);
-    case 2: return launch_decode_chunk<HD, 2>(p, batch, st);
-    case 3: return launch_decode_chunk<HD, 3>(p, batch, st);
-    case 4: return launch_decode_chunk<HD, 4>(p, batch, st);
-    case 5: return launch_decode_chunk<HD, 5>(p, batch, st);
-    case 6: return launch_decode_chunk<HD, 6>(p, batch, st);
-    case 7: return launch_decode_chunk<HD, 7>(p, batch, st);
-    default: return launch_decode_chunk<HD, 8>(p, batch, st);
+    case 1: return launch_decode_virt<HD, 1, MODE>(p, batch, st);
+    case 2: return launch_decode_virt<HD, 2, MODE>(p, batch, st);
+    case 3: return launch_decode_virt<HD, 3, MODE>(p, batch, st);
+    case 4: return launch_decode_virt<HD, 4, MODE>(p, batch, st);
+    case 5: return launch_decode_virt<HD, 5, MODE>(p, batch, st);
+    case 6: return launch_decode_virt<HD, 6, MODE>(p, batch, st);
+    case 7: return launch_decode_virt<HD, 7, MODE>(p, batch, st);
+    default: return launch_decode_virt<HD, 8, MODE>(p, batch, st);
   }
 }
 
@@ -457,10 +549,52 @@ extern "C" int lmod_attn_decode_chunk(const void* q, int64_t ld_q, const void* k
   p.rows = (int)std::min<int64_t>(T, DEC_MAX_G / p.g);
   cudaStream_t st = (cudaStream_t)stream;
   const int VG = p.rows * p.g;
-  int rc = hd == 128 ? launch_decode_chunk_g<128>(p, batch, VG, st) : launch_decode_chunk_g<64>(p, batch, VG, st);
+  int rc = hd == 128 ? launch_decode_virt_g<128, DEC_CHUNK>(p, batch, VG, st) : launch_decode_virt_g<64, DEC_CHUNK>(p, batch, VG, st);
   if (rc) return rc;
   // the merge is lmod_attn_decode's, over batch * T rows
   const dim3 grid(nh, (unsigned)(batch * T));
+  if (hd == 128) attn_decode_merge_kernel<128><<<grid, 128, 0, st>>>(p.ws_o, p.ws_ml, nh, p.nsplit, (__nv_bfloat16*)out, ld_o, lse);
+  else attn_decode_merge_kernel<64><<<grid, 64, 0, st>>>(p.ws_o, p.ws_ml, nh, p.nsplit, (__nv_bfloat16*)out, ld_o, lse);
+  LMOD_LAUNCH_OK();
+  return LMOD_OK;
+}
+
+extern "C" int64_t lmod_attn_decode_shared_ws_elems(int64_t batch, int64_t n, int nh, int nkv, int hd, int64_t max_len) {
+  if (n <= 0) return 0;
+  return lmod_attn_decode_ws_elems(batch * n, nh, nkv, hd, max_len);
+}
+
+extern "C" int lmod_attn_decode_shared(const void* q, int64_t ld_q, const void* k_prefix, const void* v_prefix, const int32_t* prefix_len,
+                                       int64_t p_max, const void* k_suffix, const void* v_suffix, int64_t s_max, const int32_t* len,
+                                       int64_t batch, int64_t n, int nh, int nkv, int hd, int64_t max_len, float softmax_scale, void* out,
+                                       int64_t ld_o, float* lse, float* ws, int64_t ws_elems, void* stream) {
+  LMOD_CHECK_ARG(q && k_prefix && v_prefix && prefix_len && k_suffix && v_suffix && len && out && ws && batch > 0 && n > 0 && n <= 4096 &&
+                 nh > 0 && nkv > 0 && nh % nkv == 0 && p_max > 0 && s_max > 0 && max_len > 0 && max_len < (1 << 30) &&
+                 p_max < (1 << 30) && s_max < (1 << 30), "lmod_attn_decode_shared: bad arguments");
+  LMOD_CHECK_ARG(hd == 64 || hd == 128, "lmod_attn_decode_shared: head_dim %d not built (64 and 128 are)", hd);
+  LMOD_CHECK_ARG(nh / nkv <= DEC_MAX_G, "lmod_attn_decode_shared: %d query heads per KV head (at most %d are built)", nh / nkv, DEC_MAX_G);
+  LMOD_CHECK_ARG(ld_q % 8 == 0 && (uintptr_t)q % 16 == 0 && (uintptr_t)k_prefix % 16 == 0 && (uintptr_t)v_prefix % 16 == 0 &&
+                 (uintptr_t)k_suffix % 16 == 0 && (uintptr_t)v_suffix % 16 == 0, "lmod_attn_decode_shared: alignment");
+  LMOD_CHECK_ARG(ws_elems >= lmod_attn_decode_shared_ws_elems(batch, n, nh, nkv, hd, max_len), "lmod_attn_decode_shared: workspace too small");
+  DecParams p;
+  p.q = (const __nv_bfloat16*)q; p.ld_q = ld_q;
+  p.k = (const __nv_bfloat16*)k_prefix; p.v = (const __nv_bfloat16*)v_prefix; p.len = len;
+  p.ks = (const __nv_bfloat16*)k_suffix; p.vs = (const __nv_bfloat16*)v_suffix; p.plen = prefix_len;
+  p.p_max = (int)p_max; p.s_max = (int)s_max;
+  p.nh = nh; p.nkv = nkv; p.max_len = (int)max_len;
+  p.nsplit = decode_splits(max_len, nkv, &p.split_blocks);      // lmod_attn_decode's splits at the expanded cache's max_len
+  p.ws_o = ws;
+  p.ws_ml = ws + batch * n * nh * (int64_t)p.nsplit * hd;
+  p.scale_log2 = softmax_scale * LOG2E_F;
+  p.T = (int)n;
+  p.g = nh / nkv;
+  p.rows = (int)std::min<int64_t>(n, DEC_MAX_G / p.g);
+  cudaStream_t st = (cudaStream_t)stream;
+  const int VG = p.rows * p.g;
+  int rc = hd == 128 ? launch_decode_virt_g<128, DEC_SHARED>(p, batch, VG, st) : launch_decode_virt_g<64, DEC_SHARED>(p, batch, VG, st);
+  if (rc) return rc;
+  // the merge is lmod_attn_decode's, over batch * n rows
+  const dim3 grid(nh, (unsigned)(batch * n));
   if (hd == 128) attn_decode_merge_kernel<128><<<grid, 128, 0, st>>>(p.ws_o, p.ws_ml, nh, p.nsplit, (__nv_bfloat16*)out, ld_o, lse);
   else attn_decode_merge_kernel<64><<<grid, 64, 0, st>>>(p.ws_o, p.ws_ml, nh, p.nsplit, (__nv_bfloat16*)out, ld_o, lse);
   LMOD_LAUNCH_OK();

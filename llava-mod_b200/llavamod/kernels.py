@@ -489,6 +489,28 @@ def attn_decode_chunk(q, B, T, nh, nkv, hd, k_cache, v_cache, lens, ws, scale=No
     return _unpad_heads(out, nh, hd), lse
 
 
+def attn_decode_shared_ws_elems(B, n, nh, nkv, hd, max_len):
+    return int(_C.lib().lmod_attn_decode_shared_ws_elems(B, n, nh, nkv, attn_head_dim(hd), max_len))
+
+
+def attn_decode_shared(q, n, nh, nkv, hd, k_prefix, v_prefix, prefix_len, k_suffix, v_suffix, lens, max_len, ws, scale=None,
+                       need_lse=False):
+    """Single-query attention of n sequences per prompt that share the prompt's cached rows (lmod_attn_decode_shared).  q: [B*n, >= nh*hd]
+    rows, row b*n + j copy j of prompt b; k_prefix / v_prefix [B, nkv, P, hp] hold prompt b's keys [0, prefix_len[b]); k_suffix / v_suffix
+    [B*n, nkv, S, hp] hold each copy's keys from prefix_len[b] on (key i at row i - prefix_len[b]); lens int32 [B*n] total keys,
+    prefix_len int32 [B], both on the device; max_len: the length of the equivalent per-sequence cache, which sets the splits.  Row b*n + j
+    gives the bytes attn_decode gives on its materialised cache of max_len rows.  -> (out [B*n, nh*hd] bf16, lse [B*n, nh] or None)."""
+    B = k_prefix.shape[0]
+    _need_cuda(k_prefix, v_prefix, prefix_len)
+    _check_cache(k_prefix, v_prefix, B, nkv, hd)
+    _check_i32(prefix_len, B, "prefix_len")
+    q, out, lse = _decode_io("attn_decode_shared", q, B * n, 1, nh, nkv, hd, k_suffix, v_suffix, lens, ws, need_lse)
+    call("lmod_attn_decode_shared", ptr(q), q.stride(0), ptr(k_prefix), ptr(v_prefix), ptr(prefix_len), k_prefix.shape[2], ptr(k_suffix),
+         ptr(v_suffix), k_suffix.shape[2], ptr(lens), B, n, nh, nkv, k_prefix.shape[3], max_len,
+         float(scale if scale is not None else hd ** -0.5), ptr(out), out.stride(0), ptr(lse), ptr(ws), ws.numel())
+    return _unpad_heads(out, nh, hd), lse
+
+
 def spec_accept(target_logits, draft_tokens, draft_logits=None, u=None, len_target=None, len_draft=None):
     """Acceptance of one assisted-decoding round (lmod_spec_accept).  target_logits fp32 [B, k+1, V_t]: row j scores draft token j+1 (row k
     the bonus token); draft_tokens int64 [B, k].  Greedy (u None): accept while the draft equals the target's argmax.  Sampling: u fp32

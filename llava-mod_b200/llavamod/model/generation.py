@@ -35,8 +35,17 @@ target's distribution.  Both models prefill the prompt with their own tower; pad
 sequences accept different counts.  EOS and max_new_tokens are applied to each round's tokens and stopping_criteria is called once per
 round, as HF does.  The per-call counts are kept in `last_assisted_stats`.
 
-Supported: greedy, temperature / top-p sampling, num_beams == 1, EOS and `stopping_criteria` callables, padded or unpadded batches,
-assisted decoding with a dense target."""
+num_return_sequences = n (sampling only, as in transformers 4.37): n sampled answers per prompt, returned as [B*n, T_in + new] with row
+b*n + j copy j of prompt b, and EOS, padding, max_new_tokens and stopping_criteria applied per row, as for the expanded batch.  A dense
+model with use_cache=True runs the tower, projector and prefill once per prompt into a shared KVCache (the prompt's K / V held once,
+each copy's new rows apart, lmod_attn_decode_shared reading the prompt's rows once for several copies), repeats the B prefill logits to
+B*n rows before the logits processors and the draw, and then decodes B*n rows per cached step.  Every kernel of that path gives each row
+the bytes it has in the expanded call, so the tokens are exactly those of generate on the inputs expanded with repeat_interleave(n, 0) and
+a generator in the same state.  The sparse student (whose router draws fresh noise for every row, so the copies' K / V differ after its
+first MoE layer) and use_cache=False run that expanded call itself.
+
+Supported: greedy, temperature / top-p sampling, num_beams == 1, num_return_sequences with sampling, EOS and `stopping_criteria`
+callables, padded or unpadded batches, assisted decoding with a dense target."""
 import collections
 import os
 import weakref
@@ -46,7 +55,8 @@ import torch
 from .. import kernels as K
 
 CACHE_BUCKET = 512
-_STEP_GRAPHS = collections.OrderedDict()     # (model id, B, max_len, T, weight pointers) -> dict(model, cache, graph, ids, logits)
+SUFFIX_BUCKET = 64                           # rows per copy past its prompt in a shared cache, rounded up to this
+_STEP_GRAPHS = collections.OrderedDict()     # (model id, B, max_len, T, weight pointers[, share]) -> dict(model, cache, graph, ids, logits)
 _GRAPH_POOL = None
 last_assisted_stats = None                   # counts of the last assisted generate call: rounds, drafted and accepted per sequence
 
@@ -81,14 +91,16 @@ def _graphs_enabled():
     return bool(int(os.environ.get("LLAVAMOD_CUDA_GRAPHS", "1")))
 
 
-def _decoder_entry(model, B, max_len, T=1):
+def _decoder_entry(model, B, max_len, T=1, share=1, suffix=None):
     """(cache, graph slot) for B sequences of up to max_len positions and steps of T tokens per sequence, reused across calls while graphs
     are on (T > 1: the verify step of assisted decoding; a model that is its own assistant gets one entry per width).  A captured step holds
     the addresses of the cache buffers and of the weights, and the host decisions made while it was captured: the MoE capacity rule of
     every sparse layer and the epilogue-fusion switches.  All of them are part of the key; the e4m3 buffers of a quantize_fp8_ model are not
-    Parameters, so they are listed beside them (a step captured before the quantisation is never replayed after it)."""
+    Parameters, so they are listed beside them (a step captured before the quantisation is never replayed after it).
+    share = n > 1: a shared cache of B prompts with n sequences each and `suffix` rows per sequence past its prompt (num_return_sequences);
+    n and suffix are part of the key, which is unchanged for n = 1."""
     if not _graphs_enabled():
-        return dict(cache=model.new_kv_cache(B, max_len), graph=None)
+        return dict(cache=model.new_kv_cache(B, max_len, share=share, suffix=suffix), graph=None)
     for k in [k for k, v in _STEP_GRAPHS.items() if v["model"]() is None]:       # the model is gone: free its cache and graph
         del _STEP_GRAPHS[k]
     moe = tuple((l.mlp.num_experts, l.mlp.k, l.mlp.use_residual, l.mlp.capacity_factor, l.mlp.eval_capacity_factor, l.mlp.min_capacity)
@@ -96,9 +108,11 @@ def _decoder_entry(model, B, max_len, T=1):
     fp8 = tuple(t.data_ptr() for l in model.model.layers if isinstance(l.self_attn.qkv_weight, K.Fp8Rows)
                 for w in (l.self_attn.qkv_weight, l.self_attn.o_fp8, l.mlp.gu_weight, l.mlp.down_fp8) for t in (w.q, w.scale))
     key = (id(model), B, max_len, T, model.training, moe, tuple(p.data_ptr() for p in model.parameters()), fp8)
+    if share > 1:
+        key += (("share", share, suffix),)
     ent = _STEP_GRAPHS.pop(key, None)
     if ent is None or ent["model"]() is not model:
-        ent = dict(model=weakref.ref(model), cache=model.new_kv_cache(B, max_len), graph=None)
+        ent = dict(model=weakref.ref(model), cache=model.new_kv_cache(B, max_len, share=share, suffix=suffix), graph=None)
     _STEP_GRAPHS[key] = ent
     while len(_STEP_GRAPHS) > max(1, int(os.environ.get("LLAVAMOD_MAX_GRAPHS", "6"))):
         _STEP_GRAPHS.popitem(last=False)
@@ -161,12 +175,21 @@ def _pick(logits, do_sample, generator):
 @torch.no_grad()
 def generate(model, inputs=None, images=None, attention_mask=None, max_new_tokens=20, do_sample=False, temperature=1.0, top_p=None,
              num_beams=1, use_cache=False, stopping_criteria=None, eos_token_id=None, pad_token_id=None, generator=None,
-             assistant_model=None, num_assistant_tokens=5, **unused):
-    """-> [B, T_in + n_new] int64: the prompt ids (image placeholders -200 included, pads included, as HF returns them) followed by the
-    new tokens.  assistant_model: a draft model for assisted decoding (use_cache=True, dense target), num_assistant_tokens = k drafted
-    tokens per round."""
+             assistant_model=None, num_assistant_tokens=5, num_return_sequences=1, **unused):
+    """-> [B*n, T_in + n_new] int64 (n = num_return_sequences): the prompt ids (image placeholders -200 included, pads included, as HF
+    returns them) followed by the new tokens; row b*n + j is copy j of prompt b.  assistant_model: a draft model for assisted decoding
+    (use_cache=True, dense target), num_assistant_tokens = k drafted tokens per round.  num_return_sequences: n sampled sequences per
+    prompt (do_sample=True); a dense model with use_cache=True prefills each prompt once into a shared cache, the sparse student and
+    use_cache=False decode the inputs expanded with repeat_interleave(n, 0) (module docstring)."""
     if num_beams != 1:
         raise NotImplementedError("beam search is not built (the reference's eval shells run num_beams=1)")
+    n_ret = int(num_return_sequences) if num_return_sequences is not None else 1
+    if n_ret < 1:
+        raise ValueError("generate: num_return_sequences must be >= 1, got %r" % (num_return_sequences,))
+    if n_ret > 1 and not do_sample:
+        raise ValueError("num_return_sequences has to be 1 when doing greedy search, but is %d." % n_ret)
+    if n_ret > 1 and assistant_model is not None:
+        raise ValueError("num_return_sequences has to be 1 when doing assisted generate, but is %d." % n_ret)
     if assistant_model is not None:
         if not use_cache:
             raise ValueError("generate: assisted decoding needs use_cache=True (the draft and the verify step decode against KV caches)")
@@ -176,6 +199,10 @@ def generate(model, inputs=None, images=None, attention_mask=None, max_new_token
         if int(num_assistant_tokens) < 1:
             raise ValueError("generate: num_assistant_tokens must be >= 1, got %r" % (num_assistant_tokens,))
     dev = model.device
+    share = n_ret > 1 and use_cache and int(max_new_tokens) > 0 and not getattr(model, "is_moe", False)
+    if n_ret > 1 and not share:                 # the sparse student, use_cache=False: the expanded call itself
+        inputs, attention_mask, images = _expand(n_ret, inputs, attention_mask, images)
+        n_ret = 1
     ids = inputs.to(dev)
     mask = None
     if attention_mask is not None:
@@ -211,9 +238,19 @@ def generate(model, inputs=None, images=None, attention_mask=None, max_new_token
         return ids
     if use_cache and int(max_new_tokens) > 0:
         need = max(model.spliced_length(ids, images, mask)) + int(max_new_tokens)
-        ent = _decoder_entry(model, B, (need + CACHE_BUCKET - 1) // CACHE_BUCKET * CACHE_BUCKET)
+        max_len = (need + CACHE_BUCKET - 1) // CACHE_BUCKET * CACHE_BUCKET
+        if n_ret > 1:          # each copy appends at most max_new_tokens - 1 rows past its prompt
+            suffix = (int(max_new_tokens) + SUFFIX_BUCKET - 1) // SUFFIX_BUCKET * SUFFIX_BUCKET
+            ent = _decoder_entry(model, B, max_len, share=n_ret, suffix=suffix)
+        else:
+            ent = _decoder_entry(model, B, max_len)
         logits = next_token_logits(model, ids, images=images, tower_features=feats, attention_mask=mask.to(dev) if ragged else None,
                                    cache=ent["cache"], ragged=ragged)
+        if n_ret > 1:          # from here on B*n rows, the expanded call's layout; the draws see the expanded call's logits
+            logits = logits.repeat_interleave(n_ret, 0)
+            ids = ids.repeat_interleave(n_ret, 0)
+            B = B * n_ret
+            done = torch.zeros(B, dtype=torch.bool, device=dev)
     elif ragged:
         # the no-cache loop re-reads every prompt with its new tokens appended: each row holds its real tokens first, then the new ones,
         # then padding, so a row stays one run of real tokens and the unspliced text rows sit at positions 0 .. n_b - 1
@@ -245,6 +282,15 @@ def generate(model, inputs=None, images=None, attention_mask=None, max_new_token
     if was_training:
         model.train()
     return ids
+
+
+def _expand(n, inputs, attention_mask, images):
+    """HF's _expand_inputs_for_generation: input_ids, attention_mask and images repeated n times along the batch (repeat_interleave)."""
+    if attention_mask is not None:
+        attention_mask = attention_mask.repeat_interleave(n, 0)
+    if images is not None:
+        images = images.repeat_interleave(n, 0) if torch.is_tensor(images) else [im for im in images for _ in range(n)]
+    return inputs.repeat_interleave(n, 0), attention_mask, images
 
 
 def _bucket(n):

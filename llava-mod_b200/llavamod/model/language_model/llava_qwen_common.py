@@ -191,9 +191,10 @@ class LlavaQwenForCausalLMBase(nn.Module, LlavaMetaForCausalLM):
         return self.model.embed_tokens
 
     # ---- forward -------------------------------------------------------------------------------------
-    def new_kv_cache(self, batch, max_len):
-        """A KVCache for `batch` sequences of up to max_len spliced positions each (prompt incl. image patches + new tokens)."""
-        return KVCache(self.model, batch, max_len)
+    def new_kv_cache(self, batch, max_len, share=1, suffix=None):
+        """A KVCache for `batch` sequences of up to max_len spliced positions each (prompt incl. image patches + new tokens).  share = n > 1:
+        the shared form generate uses for num_return_sequences, `batch` prompts of n sequences each (see KVCache)."""
+        return KVCache(self.model, batch, max_len, share=share, suffix=suffix)
 
     def forward_hidden(self, input_ids=None, attention_mask=None, position_ids=None, inputs_embeds=None, labels=None,
                        images=None, moe_noise=None, tower_features=None, plan=None, cache=None):
@@ -255,6 +256,8 @@ class LlavaQwenForCausalLMBase(nn.Module, LlavaMetaForCausalLM):
             # A padded prompt batch prefills each sequence's real rows; the step's attention_mask is not read (the cache's lengths decide).
             if past_key_values is not None and not isinstance(past_key_values, KVCache):
                 raise NotImplementedError("past_key_values must be the KVCache this model returned (or new_kv_cache made)")
+            if past_key_values is not None and past_key_values.shared:
+                raise NotImplementedError("past_key_values must be a plain KVCache; the shared form is internal to generate")
             if labels is not None:
                 raise NotImplementedError("labels with a KV cache: the cached path is for decoding")
             cache = past_key_values

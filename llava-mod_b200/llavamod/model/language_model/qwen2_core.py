@@ -357,19 +357,17 @@ class Qwen2Model(nn.Module):
 
         def attend(li, qkv, nh, nkv, hd):
             if ragged:
-                K.kv_append_rows(qkv, B, T, nh, nkv, hd, cache.k[li], cache.v[li], pad[0], pad[1], cache.len)
+                K.kv_append_rows(qkv, B, T, nh, nkv, hd, cache.k[li], cache.v[li], pad[0], pad[1], cache.prefix_len)
             elif cache is not None:
-                K.kv_append(qkv, B, T, nh, nkv, hd, cache.k[li], cache.v[li], cache.len)
+                K.kv_append(qkv, B, T, nh, nkv, hd, cache.k[li], cache.v[li], cache.prefix_len)
             return K.attention(qkv, B, T, nh, nkv, hd, True, None, pad)
 
         checkpoint = cache is None and self.gradient_checkpointing and self.training and torch.is_grad_enabled()
         out, l_auxes, records = self._layers(inputs_embeds.reshape(B * T, H), cos, sin, pos, attend, moe_noise, training_moe, checkpoint)
         if ragged:
-            cache.len.add_(pad[1] - pad[0])
-            cache.advance(lengths)
+            cache.prefilled(pad[1] - pad[0], lengths)
         elif cache is not None:
-            cache.len.add_(T)
-            cache.advance(T)
+            cache.prefilled(T, T)
         return out.view(B, T, H), l_auxes, records
 
     @torch.no_grad()
@@ -391,10 +389,14 @@ class Qwen2Model(nn.Module):
             raise NotImplementedError("a cached step of the sparse model decodes one token per sequence (got %d): a step of T tokens would "
                                       "route its B*T tokens together (top2gating with S = B*T), which is not what T one-token steps "
                                       "compute" % T)
+        if T != 1 and cache.shared:
+            raise NotImplementedError("a shared KVCache decodes one token per sequence (got %d)" % T)
         cache.check(B, T)
         dev = inputs_embeds.device
         cos, sin = cache.rope
         torch.add(cache.len, T, out=cache.end)
+        if cache.shared:
+            torch.sub(cache.len, cache.prefix_rows, out=cache.suffix_len)
         if T == 1:
             pos = cache.pos
             pos.copy_(cache.len)
@@ -403,6 +405,10 @@ class Qwen2Model(nn.Module):
             ws = cache.chunk_workspace(T)
 
         def attend(li, qkv, nh, nkv, hd):
+            if cache.shared:                            # the new row goes to the copy's suffix; the prompt's rows are read once per CTA
+                K.kv_append(qkv, B, 1, nh, nkv, hd, cache.ks[li], cache.vs[li], cache.suffix_len)
+                return K.attn_decode_shared(qkv, cache.share, nh, nkv, hd, cache.k[li], cache.v[li], cache.prefix_len, cache.ks[li],
+                                            cache.vs[li], cache.end, cache.max_len, cache.ws)[0]
             K.kv_append(qkv, B, T, nh, nkv, hd, cache.k[li], cache.v[li], cache.len)
             if T == 1:
                 return K.attn_decode(qkv, nh, nkv, hd, cache.k[li], cache.v[li], cache.end, cache.ws)[0]
@@ -489,41 +495,98 @@ class KVCache:
     the host always knows how many rows a forward adds, so every append is bounds-checked without a sync.  Sequence b holds its rows
     packed at [0, lengths[b]), whatever padding its prompt had.  ``cache[i]`` gives layer i's (k, v) views [B, nkv, length, hd], the legacy
     tuple layout llava_arch.py:165 indexes; rows at or past a sequence's own length are unspecified.  The RoPE tables cover max_len at
-    allocation, so nothing is rebuilt inside a captured step."""
+    allocation, so nothing is rebuilt inside a captured step.
 
-    def __init__(self, model, batch, max_len):
+    Shared form (share = n > 1, generate's num_return_sequences on a dense model): `batch` prompts, each decoded as n sequences (row b*n + j
+    is copy j of prompt b; ``batch``, ``len`` and ``lengths`` count the B*n rows).  The prefill writes each prompt's rows once into ``k`` / ``v``
+    [B, nkv, max_len, hp] (``prefix_len`` int32 [B] on the device, ``prefixes`` its host mirror); each copy's later rows go to its own
+    ``ks`` / ``vs`` [B*n, nkv, suffix, hp], suffix row i - prefix_len[b] for key i, and the cached step attends with
+    lmod_attn_decode_shared.  max_len bounds every row's total length and sets the attention splits, so each row's attention has the bytes
+    of a plain cache of max_len rows.  It has no legacy tuple view: ``cache[i]`` raises, and forward(past_key_values=...) takes the plain
+    form only."""
+
+    def __init__(self, model, batch, max_len, share=1, suffix=None):
         cfg = model.config
         w = model.embed_tokens.weight
         dev, dt = w.device, w.dtype
         nh, nkv = cfg.num_attention_heads, cfg.num_key_value_heads
         self.head_dim = cfg.hidden_size // nh
         hp = K.attn_head_dim(self.head_dim)
-        self.batch, self.max_len = int(batch), int(max_len)
+        self.share, self.prompts = int(share), int(batch)
+        if self.share < 1:
+            raise ValueError("KVCache: share must be >= 1, got %r" % (share,))
+        self.batch, self.max_len = int(batch) * self.share, int(max_len)
         self.k = [torch.empty(batch, nkv, max_len, hp, device=dev, dtype=dt) for _ in model.layers]
         self.v = [torch.empty(batch, nkv, max_len, hp, device=dev, dtype=dt) for _ in model.layers]
-        self.len = torch.zeros(batch, dtype=torch.int32, device=dev)
-        self.end = torch.zeros(batch, dtype=torch.int32, device=dev)          # len + 1 during a decode step
-        self.pos = torch.zeros(batch, dtype=torch.int64, device=dev)          # RoPE positions of a decode step
-        self.ws = torch.empty(max(1, K.attn_decode_ws_elems(batch, nh, nkv, self.head_dim, max_len)), dtype=torch.float32, device=dev)
+        self.len = torch.zeros(self.batch, dtype=torch.int32, device=dev)
+        self.end = torch.zeros(self.batch, dtype=torch.int32, device=dev)     # len + 1 during a decode step
+        self.pos = torch.zeros(self.batch, dtype=torch.int64, device=dev)     # RoPE positions of a decode step
+        if self.share > 1:
+            self.suffix = int(suffix) if suffix is not None else self.max_len
+            self.ks = [torch.empty(self.batch, nkv, self.suffix, hp, device=dev, dtype=dt) for _ in model.layers]
+            self.vs = [torch.empty(self.batch, nkv, self.suffix, hp, device=dev, dtype=dt) for _ in model.layers]
+            self.prefix_len = torch.zeros(batch, dtype=torch.int32, device=dev)
+            self.prefix_rows = torch.zeros(self.batch, dtype=torch.int32, device=dev)     # prefix_len of every row
+            self.suffix_len = torch.zeros(self.batch, dtype=torch.int32, device=dev)      # len - prefix_len: a step's suffix append row
+            self.ws = torch.empty(max(1, K.attn_decode_shared_ws_elems(batch, self.share, nh, nkv, self.head_dim, max_len)),
+                                  dtype=torch.float32, device=dev)
+        else:
+            self.prefix_len = self.len                                        # the prefill appends at len
+            self.ws = torch.empty(max(1, K.attn_decode_ws_elems(batch, nh, nkv, self.head_dim, max_len)), dtype=torch.float32, device=dev)
         self._chunk_ws = {}                                                   # T -> workspace of a T-token step
         self._shape = (nh, nkv)
         self.rope = model.rope(max_len, dev, dt)
         self.lengths = [0] * self.batch
+        self.prefixes = [0] * self.prompts
+
+    @property
+    def shared(self):
+        return self.share > 1
 
     @property
     def length(self):
         return max(self.lengths)
 
-    def _per_seq(self, n_new):
-        return [int(n) for n in n_new] if isinstance(n_new, (list, tuple)) else [int(n_new)] * self.batch
+    @property
+    def nbytes(self):
+        """Bytes of the K / V buffers."""
+        bufs = self.k + self.v + (self.ks + self.vs if self.shared else [])
+        return sum(t.numel() * t.element_size() for t in bufs)
+
+    def _per_seq(self, n_new, rows=None):
+        rows = self.batch if rows is None else rows
+        return [int(n) for n in n_new] if isinstance(n_new, (list, tuple)) else [int(n_new)] * rows
 
     def check(self, batch, n_new):
-        """n_new: positions each sequence adds (an int for all, or one per sequence)."""
+        """n_new: positions each sequence adds (an int for all, or one per sequence).  The prefill of a shared cache (empty) takes one row
+        per prompt."""
+        if self.shared and self.length == 0:
+            if batch != self.prompts:
+                raise ValueError("shared KVCache holds %d prompts, got a prefill of %d" % (self.prompts, batch))
+            for b, a in enumerate(self._per_seq(n_new, self.prompts)):
+                if a > self.max_len:
+                    raise ValueError("KVCache is full: prompt %d has %d positions > max_len %d" % (b, a, self.max_len))
+            return
         if batch != self.batch:
             raise ValueError("KVCache holds %d sequences, got a batch of %d" % (self.batch, batch))
         for b, (n, a) in enumerate(zip(self.lengths, self._per_seq(n_new))):
             if n + a > self.max_len:
                 raise ValueError("KVCache is full: sequence %d has %d cached + %d new positions > max_len %d" % (b, n, a, self.max_len))
+            if self.shared and n + a - self.prefixes[b // self.share] > self.suffix:
+                raise ValueError("shared KVCache is full: sequence %d has %d rows past its prompt + %d new > suffix %d"
+                                 % (b, n - self.prefixes[b // self.share], a, self.suffix))
+
+    def prefilled(self, n_dev, n_new):
+        """After the prefill appended n_dev (int32 [prompts] on the device, or an int) rows per prompt at prefix_len; n_new: the same on the
+        host (an int for all, or one per prompt).  A shared cache hands every copy its prompt's length."""
+        self.prefix_len.add_(n_dev)
+        if not self.shared:
+            self.advance(n_new)
+            return
+        self.prefixes = self._per_seq(n_new, self.prompts)
+        self.prefix_rows.copy_(self.prefix_len.repeat_interleave(self.share))
+        self.len.copy_(self.prefix_rows)
+        self.advance([n for n in self.prefixes for _ in range(self.share)])
 
     def advance(self, n_new):
         self.lengths = [n + a for n, a in zip(self.lengths, self._per_seq(n_new))]
@@ -531,10 +594,15 @@ class KVCache:
     def reset(self):
         self.len.zero_()
         self.lengths = [0] * self.batch
+        if self.shared:
+            self.prefix_len.zero_()
+            self.prefixes = [0] * self.prompts
 
     def rollback(self, n_drop):
         """Forget the last n_drop[b] rows of every sequence (an int for all, or one per sequence) in the host mirror ``lengths``; the caller
         has applied the same rollback to the device ``len`` (lmod_spec_accept does it on the device)."""
+        if self.shared:
+            raise NotImplementedError("a shared KVCache is not rolled back (assisted decoding takes num_return_sequences = 1)")
         drop = self._per_seq(n_drop)
         if any(d < 0 or d > n for d, n in zip(drop, self.lengths)):
             raise ValueError("KVCache.rollback: cannot drop %s rows from lengths %s" % (drop, self.lengths))
@@ -556,6 +624,8 @@ class KVCache:
         return len(self.k)
 
     def __getitem__(self, i):
+        if self.shared:
+            raise TypeError("a shared KVCache has no [B, nkv, length, hd] view: its copies keep their prompt's rows once")
         n, hd = self.length, self.head_dim
         return self.k[i][:, :, :n, :hd], self.v[i][:, :, :n, :hd]
 

@@ -1,7 +1,8 @@
 """Decoding benchmark: tokens/s of `generate` with and without the KV cache, decode-attention bandwidth, and the device time per
 kernel family of one cached decode step.
 
-    python scripts/bench_decode.py [--models student,teacher] [--new 128,512] [--batch 1,8] [--profile] [--ragged] [--assisted] [--out DIR]
+    python scripts/bench_decode.py [--models student,teacher] [--new 128,512] [--batch 1,8] [--profile] [--ragged] [--assisted]
+                                   [--num-return 4,8] [--out DIR]
 
 * generate: the 0.5B-4E student and the 7B teacher (random weights, CLIP-L/336) on a prompt that splices to T' = 650 positions, greedy,
   use_cache False / True, CUDA graphs on / off (LLAVAMOD_CUDA_GRAPHS).  Tokens/s = B * new tokens / wall time of the call, which ends in
@@ -19,6 +20,13 @@ kernel family of one cached decode step.
   time (CUDA events over 20 graph replays / launches) of one draft step, one verify step of k + 1 tokens, one teacher step and one accept
   launch, with the per-token acceptance alpha at which a round breaks even with the teacher alone.  alpha of a trained pair is not
   measured here (random weights).
+* --num-return N[,N...]: sampled generate with num_return_sequences = n, the 7B teacher and the 0.5B-4E student (random weights, graphs on,
+  the first --new value of new tokens), B from --batch at T' = 650 and B = 1 at T' = 8175 (a 7600-token prompt with one image), against
+  the explicitly expanded call (inputs repeat_interleave'd to B*n, n = 1): tokens/s (B*n*new over the call), time to the first token
+  (a call with max_new_tokens = 1: tower, prefill and one draw), the K / V bytes of the decode cache each allocates, and the decode
+  attention of one layer at the middle step of the run: lmod_attn_decode_shared on the shared cache against lmod_attn_decode on the
+  expanded one, CUDA events over 50 launches each, alternated, with the bytes each must read (K / V rows, q, out).  The sparse student
+  runs the expanded call in both rows (its copies cannot share the cache), so its rows differ only by noise.
 The card's name and power limit are read in the same process and printed with the results (one JSON line per measurement)."""
 import argparse
 import json
@@ -198,6 +206,108 @@ def bench_assisted(teacher, student, batches, new, out, info, repeat):
         torch.cuda.empty_cache()
 
 
+def long_prompt(B, n_text=7600, seed=3):
+    """B prompts of n_text tokens with one image: T' = n_text - 1 + 576."""
+    g = torch.Generator().manual_seed(seed)
+    ids = torch.randint(0, 150000, (B, n_text), generator=g)
+    ids[:, 3] = -200
+    imgs = [torch.randn(3, 336, 336, generator=g).to(torch.bfloat16) for _ in range(B)]
+    return ids, imgs
+
+
+def _kv_bytes(model, rows, length):
+    cfg = model.config
+    from llavamod import kernels as K
+    hp = K.attn_head_dim(cfg.hidden_size // cfg.num_attention_heads)
+    return cfg.num_hidden_layers * 2 * rows * cfg.num_key_value_heads * length * hp * 2
+
+
+def _attn_shared_vs_expanded(model, B, n, P, S, max_len, suffix_cap):
+    """us per launch and bytes of lmod_attn_decode_shared and lmod_attn_decode at one layer's shapes, every copy at P + S keys."""
+    from llavamod import kernels as K
+    cfg = model.config
+    nh, nkv = cfg.num_attention_heads, cfg.num_key_value_heads
+    hd = cfg.hidden_size // nh
+    hp = K.attn_head_dim(hd)
+    g = torch.Generator(device="cuda").manual_seed(0)
+    rnd = lambda *s: torch.randn(*s, device="cuda", generator=g).to(torch.bfloat16)  # noqa: E731
+    q = rnd(B * n, nh * hd)
+    kp, vp = rnd(B, nkv, max_len, hp), rnd(B, nkv, max_len, hp)
+    ks, vs = rnd(B * n, nkv, suffix_cap, hp), rnd(B * n, nkv, suffix_cap, hp)
+    km, vm = kp.repeat_interleave(n, 0), vp.repeat_interleave(n, 0)
+    km[:, :, P:P + S], vm[:, :, P:P + S] = ks[:, :, :S], vs[:, :, :S]
+    plen = torch.full((B,), P, dtype=torch.int32, device="cuda")
+    lens = torch.full((B * n,), P + S, dtype=torch.int32, device="cuda")
+    ws1 = torch.empty(K.attn_decode_ws_elems(B * n, nh, nkv, hd, max_len), dtype=torch.float32, device="cuda")
+    ws2 = torch.empty(K.attn_decode_shared_ws_elems(B, n, nh, nkv, hd, max_len), dtype=torch.float32, device="cuda")
+    runs = {"expanded": lambda: K.attn_decode(q, nh, nkv, hd, km, vm, lens, ws1),
+            "shared": lambda: K.attn_decode_shared(q, n, nh, nkv, hd, kp, vp, plen, ks, vs, lens, max_len, ws2)}
+    a, b = runs["expanded"]()[0], runs["shared"]()[0]
+    same = bool(torch.equal(a.view(torch.int16), b.view(torch.int16)))
+    ms = {k: [] for k in runs}
+    for _ in range(3):                                                     # alternated rounds of 50 launches
+        for k, fn in runs.items():
+            ms[k].append(_replay_ms(fn, 50))
+    row = nkv * hp * 2 * 2                                                 # K and V bytes of one key of one sequence
+    rows_per_cta = min(n, 8 // (nh // nkv))
+    qo = B * n * nh * hd * 2 * 2
+    nbytes = {"expanded": B * n * (P + S) * row + qo,
+              "shared": B * -(-n // rows_per_cta) * P * row + B * n * S * row + qo}
+    res = {}
+    for k in runs:
+        t = sorted(ms[k])[1] * 1e-3
+        res[k] = dict(us=round(t * 1e6, 2), us_spread=[round(x * 1e3, 2) for x in sorted(ms[k])], MB=round(nbytes[k] / 1e6, 2),
+                      TBps=round(nbytes[k] / t / 1e12, 3))
+    return res, same
+
+
+def bench_num_return(models, ns, batches, new, out, info, repeat):
+    from llavamod.model import generation as Gm
+    from llavamod.model import synthetic as S
+    os.environ["LLAVAMOD_CUDA_GRAPHS"] = "1"
+    for name in models:
+        model = (S.make_student("qwen1.5-0.5b", "clip-l-336", seed=1) if name == "student" else
+                 S.make_teacher("qwen1.5-7b", "clip-l-336", seed=0)).eval()
+        shapes = [(B, prompt(B), 650) for B in batches] + [(1, long_prompt(1), 7600 - 1 + 576)]
+        for B, (ids, imgs), P in shapes:
+            for n in ns:
+                e_ids, e_imgs = ids.repeat_interleave(n, 0), [im for im in imgs for _ in range(n)]
+                kw = dict(use_cache=True, do_sample=True, eos_token_id=-1)
+                calls = {"expanded": lambda m: model.generate(e_ids, images=e_imgs, max_new_tokens=m, **kw),
+                         "shared": lambda m: model.generate(ids, images=imgs, max_new_tokens=m, num_return_sequences=n, **kw)}
+                rec = dict(kind="num_return", model=name, B=B, n=n, prompt_len=P, new=new, runs=repeat, card=info)
+                for row, fn in calls.items():
+                    Gm._STEP_GRAPHS.clear()
+                    torch.cuda.empty_cache()
+                    try:
+                        secs = _timed_generate(lambda: fn(new), repeat)
+                    except torch.OutOfMemoryError:
+                        rec[row] = dict(out_of_memory=True)
+                        Gm._STEP_GRAPHS.clear()
+                        torch.cuda.empty_cache()
+                        continue
+                    ents = list(Gm._STEP_GRAPHS.values())
+                    cache = ents[-1]["cache"]
+                    ttft = _timed_generate(lambda: fn(1), repeat)
+                    rec[row] = dict(tokens_per_s=round(B * n * new / secs[len(secs) // 2], 1), min=round(B * n * new / secs[-1], 1),
+                                    max=round(B * n * new / secs[0], 1), ttft_ms=round(ttft[len(ttft) // 2] * 1e3, 2),
+                                    ttft_spread_ms=[round(ttft[0] * 1e3, 2), round(ttft[-1] * 1e3, 2)],
+                                    cache_MB=round(cache.nbytes / 1e6, 1), shared_cache=cache.shared)
+                    del ents, cache
+                Gm._STEP_GRAPHS.clear()
+                torch.cuda.empty_cache()
+                max_len = Gm._bucket(P + new)
+                suffix = -(-new // Gm.SUFFIX_BUCKET) * Gm.SUFFIX_BUCKET
+                attn, same = _attn_shared_vs_expanded(model, B, n, P, new // 2, max_len, suffix)
+                if all("tokens_per_s" in rec[row] for row in calls):
+                    rec.update(speedup=round(rec["shared"]["tokens_per_s"] / rec["expanded"]["tokens_per_s"], 3))
+                rec.update(attn_layer_step=dict(attn, same_bytes=same, keys=P + new // 2))
+                emit(out, rec)
+                torch.cuda.empty_cache()
+        del model
+        torch.cuda.empty_cache()
+
+
 def bench_attention(out, info):
     from llavamod import kernels as K
     for hd, nh, nkv in [(64, 16, 16), (64, 14, 2), (128, 28, 4), (128, 32, 32)]:
@@ -272,6 +382,7 @@ def main():
     ap.add_argument("--skip-attention", action="store_true")
     ap.add_argument("--ragged", action="store_true", help="padded batches of prompts of different lengths (see the module docstring)")
     ap.add_argument("--assisted", action="store_true", help="assisted decoding, teacher with the student as draft (module docstring)")
+    ap.add_argument("--num-return", default=None, help="num_return_sequences values: shared against expanded (module docstring)")
     ap.add_argument("--repeat", type=int, default=3, help="timed generate calls per setting (median, min and max are reported)")
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
@@ -280,6 +391,10 @@ def main():
         os.makedirs(a.out, exist_ok=True)
     info = card()
     from llavamod.model import synthetic as S
+    if a.num_return:
+        bench_num_return(a.models.split(","), [int(x) for x in a.num_return.split(",")], [int(x) for x in a.batch.split(",")],
+                         int(a.new.split(",")[0]), a.out, info, a.repeat)
+        return
     if a.assisted:
         teacher = S.make_teacher("qwen1.5-7b", "clip-l-336", seed=0).eval()
         student = S.make_student("qwen1.5-0.5b", "clip-l-336", seed=1, share_tower_with=teacher).eval()
