@@ -370,6 +370,15 @@ int lmod_attn_decode_shared(const void* q, int64_t ld_q, const void* k_prefix, c
                             const void* k_suffix, const void* v_suffix, int64_t s_max, const int32_t* len, int64_t batch, int64_t n, int nh,
                             int nkv, int hd, int64_t max_len, float softmax_scale, void* out, int64_t ld_o, float* lse, float* ws,
                             int64_t ws_elems, void* stream);
+/* lmod_kv_beam_reorder: beam search's cache reorder (HF _reorder_cache / index_select over the beams), in place.  bufs: device array of
+ *   n_bufs pointers to bf16 buffers [prompts*n, nkv, cap, hp] (every layer's K and V in one launch); rows int32 [prompts], parent int32
+ *   [prompts*n] with values in [0, n), both on the device.  For every buffer, prompt b, beam j, KV head h and row r < rows[b]:
+ *   new[b*n + j, h, r, :hd] = old[b*n + parent[b*n + j], h, r, :hd], byte for byte.  Rows at or past rows[b] (clamped to cap) and columns
+ *   [hd, hp) are not written; any map works in place (cycles, many beams from one), and a prompt whose map is the identity moves nothing.
+ *   Everything read is on the device, so the launch can be captured.  hd %% 8 == 0, hd <= hp <= 128, n <= 128; n == 1 launches nothing.
+ *   Callers check the ranges (a parent outside [0, n) leaves its beam unwritten). */
+int lmod_kv_beam_reorder(void* const* bufs, int n_bufs, int64_t prompts, int64_t n, int nkv, int64_t cap, int hd, int hp, const int32_t* rows,
+                         const int32_t* parent, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Assisted decoding (csrc/spec.cu).

@@ -33,6 +33,9 @@
 // Each copy's heads see every block of its key range once, with the lmod_attn_decode splits of the max_len passed in (the bucketed length
 // the expanded cache would have), the same lane-to-key mapping, per-head limits as in the chunk kernel, and the same merge, so sequence
 // b*n + j's out and lse are the bytes lmod_attn_decode gives on its materialised cache (prefix rows then suffix rows) at that max_len.
+//
+// lmod_kv_beam_reorder: beam search's cache reorder (HF _reorder_cache), in place and for every layer's K and V in one launch.  On the
+// shared cache only the beams' suffix rows move (the prompt's rows are common to all beams); on a plain cache every row below len.
 #include "sm90.cuh"
 
 namespace {
@@ -386,6 +389,69 @@ __global__ void kv_append_rows_kernel(const __nv_bfloat16* qkv, int64_t ld, int 
   *reinterpret_cast<uint4*>(dst) = *reinterpret_cast<const uint4*>(src);
 }
 
+constexpr int BEAM_THREADS = 256;
+constexpr int BEAM_CHUNK = 512;         // rows per CTA, walked in blocks of R rows
+constexpr int BEAM_STAGE = 32768;       // staged bytes per CTA: R = BEAM_STAGE / (n * hd * 2) rows of every beam fit
+constexpr int BEAM_MAX_N = 128;         // beams per prompt (R >= 1 at hd 128)
+
+// Beam reorder, in place: new[b*n + j, h, r] = old[b*n + parent[b*n + j], h, r] for r < rows[b], columns [0, hd) of each hp-wide row.
+// CTA = (buffer, prompt, KV head) x chunk of BEAM_CHUNK rows.  Thread 0 lists the beams that change (parent != self) and the beams some
+// changed beam reads (sources, each staged once); per row block every source tile is loaded to shared memory before any changed beam is
+// written, so cycles and many-from-one maps need no second buffer.  A prompt whose map is the identity moves nothing.
+__global__ void __launch_bounds__(BEAM_THREADS) kv_beam_reorder_kernel(__nv_bfloat16* const* bufs, int64_t prompts, int n, int nkv,
+                                                                      int64_t cap, int hd, int hp, int R, const int32_t* rows,
+                                                                      const int32_t* parent) {
+  extern __shared__ __align__(16) uint4 stage[];
+  __shared__ int par[BEAM_MAX_N], slot[BEAM_MAX_N], src[BEAM_MAX_N], dst[BEAM_MAX_N];
+  __shared__ int n_src, n_dst;
+  const int64_t t = blockIdx.x;
+  const int h = (int)(t % nkv);
+  const int64_t b = (t / nkv) % prompts;
+  const int64_t buf = t / nkv / prompts;
+  const int64_t r_lo = (int64_t)blockIdx.y * BEAM_CHUNK;
+  const int64_t r_end = min(min((int64_t)rows[b], cap), r_lo + BEAM_CHUNK);
+  if (r_lo >= r_end) return;
+  if (threadIdx.x == 0) {
+    int ns = 0, nd = 0;
+    for (int j = 0; j < n; ++j) {
+      par[j] = parent[b * n + j];
+      slot[j] = -1;
+    }
+    for (int j = 0; j < n; ++j) {
+      const int p = par[j];
+      if (p == j || p < 0 || p >= n) continue;          // the host checks the range; an out-of-range parent leaves its beam alone
+      dst[nd++] = j;
+      if (slot[p] < 0) {
+        slot[p] = ns;
+        src[ns++] = p;
+      }
+    }
+    n_src = ns;
+    n_dst = nd;
+  }
+  __syncthreads();
+  const int ns = n_src, nd = n_dst;
+  if (nd == 0) return;
+  const int cpr = hd / 8;                               // 16-byte chunks per row
+  __nv_bfloat16* base = bufs[buf];
+  const int64_t beam_stride = (int64_t)nkv * cap * hp;
+  __nv_bfloat16* head = base + (b * n * nkv + h) * cap * hp;   // beam 0 of prompt b, head h, row 0
+  for (int64_t r0 = r_lo; r0 < r_end; r0 += R) {
+    const int per = (int)min((int64_t)R, r_end - r0) * cpr;
+    for (int i = threadIdx.x; i < ns * per; i += BEAM_THREADS) {
+      const int s = i / per, w = i - s * per, r = w / cpr, c = w - r * cpr;
+      stage[(s * R + r) * cpr + c] = reinterpret_cast<const uint4*>(head + src[s] * beam_stride + (r0 + r) * hp)[c];
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i < nd * per; i += BEAM_THREADS) {
+      const int d = i / per, w = i - d * per, r = w / cpr, c = w - r * cpr;
+      const int j = dst[d];
+      reinterpret_cast<uint4*>(head + j * beam_stride + (r0 + r) * hp)[c] = stage[(slot[par[j]] * R + r) * cpr + c];
+    }
+    __syncthreads();
+  }
+}
+
 // split count and length (in key blocks) from max_len, nkv and the SM count: about two waves of CTAs at B = 1, at least
 // DEC_MIN_BLOCKS blocks per split
 int decode_splits(int64_t max_len, int nkv, int* split_blocks) {
@@ -481,6 +547,21 @@ extern "C" int lmod_kv_append_rows(const void* qkv, int64_t ld_qkv, int64_t batc
   kv_append_rows_kernel<<<(unsigned)((chunks + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
       (const __nv_bfloat16*)qkv, ld_qkv, (int)n_rows, nh, nkv, hd, src_lo, src_hi, offsets, (__nv_bfloat16*)k_cache,
       (__nv_bfloat16*)v_cache, (int)max_len, chunks);
+  LMOD_LAUNCH_OK();
+  return LMOD_OK;
+}
+
+extern "C" int lmod_kv_beam_reorder(void* const* bufs, int n_bufs, int64_t prompts, int64_t n, int nkv, int64_t cap, int hd, int hp,
+                                    const int32_t* rows, const int32_t* parent, void* stream) {
+  LMOD_CHECK_ARG(bufs && rows && parent && n_bufs > 0 && prompts > 0 && n >= 1 && nkv > 0 && cap > 0, "lmod_kv_beam_reorder: bad arguments");
+  LMOD_CHECK_ARG(n <= BEAM_MAX_N, "lmod_kv_beam_reorder: %lld beams per prompt (at most %d are built)", (long long)n, BEAM_MAX_N);
+  LMOD_CHECK_ARG(hd > 0 && hd % 8 == 0 && hp % 8 == 0 && hd <= hp && hp <= 128, "lmod_kv_beam_reorder: hd %d / hp %d", hd, hp);
+  const int64_t tiles = (int64_t)n_bufs * prompts * nkv, chunks = (cap + BEAM_CHUNK - 1) / BEAM_CHUNK;
+  LMOD_CHECK_ARG(tiles < (1ll << 31) && chunks < 65536, "lmod_kv_beam_reorder: grid too large");
+  if (n == 1) return LMOD_OK;                           // a single beam's map is the identity
+  const int R = (int)max(1ll, min((long long)BEAM_CHUNK, (long long)(BEAM_STAGE / (n * hd * 2))));
+  kv_beam_reorder_kernel<<<dim3((unsigned)tiles, (unsigned)chunks), BEAM_THREADS, (size_t)n * R * hd * 2, (cudaStream_t)stream>>>(
+      (__nv_bfloat16* const*)bufs, prompts, (int)n, nkv, cap, hd, hp, R, rows, parent);
   LMOD_LAUNCH_OK();
   return LMOD_OK;
 }

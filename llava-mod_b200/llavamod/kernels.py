@@ -3,6 +3,8 @@
 Each wrapper cites the reference call site it stands in for.  Tensors are bf16 CUDA, contiguous; fp32 only
 where the reference keeps fp32 (router gate, loss scalars, optimizer state).  No CPU fallback.
 """
+import collections
+
 import torch
 from torch.autograd import Function
 
@@ -509,6 +511,47 @@ def attn_decode_shared(q, n, nh, nkv, hd, k_prefix, v_prefix, prefix_len, k_suff
          ptr(v_suffix), k_suffix.shape[2], ptr(lens), B, n, nh, nkv, k_prefix.shape[3], max_len,
          float(scale if scale is not None else hd ** -0.5), ptr(out), out.stride(0), ptr(lse), ptr(ws), ws.numel())
     return _unpad_heads(out, nh, hd), lse
+
+
+_BEAM_TABLES = collections.OrderedDict()     # buffer pointers -> the device array of them lmod_kv_beam_reorder reads
+
+
+def kv_beam_reorder(bufs, n, hd, rows, parent):
+    """Beam search's cache reorder in place (lmod_kv_beam_reorder), every buffer in one launch: bufs are bf16 [P*n, nkv, cap, hp] (all
+    layers' K and V), rows host ints [P] and parent host ints [P*n] in [0, n).  Row r < rows[b] of beam j of prompt b, columns [0, hd), takes
+    the bytes of beam parent[b*n + j]'s row r; nothing else is written.  The operands are checked on the host and copied to the device in
+    one transfer, so the call reads nothing back."""
+    bufs = list(bufs)
+    if not bufs:
+        raise _C.LmodError("kv_beam_reorder: no buffers")
+    _need_cuda(*bufs)
+    shape = tuple(bufs[0].shape)
+    if len(shape) != 4 or shape[0] % max(1, n) or n < 1:
+        raise _C.LmodError("kv_beam_reorder: buffers must be [P*n, nkv, cap, hp] with n = %r, got %s" % (n, shape))
+    for t in bufs:
+        if t.dtype != BF16 or tuple(t.shape) != shape or not t.is_contiguous() or t.device != bufs[0].device:
+            raise _C.LmodError("kv_beam_reorder: every buffer must be contiguous bf16 %s on one device, got %s %s" % (shape, t.dtype,
+                                                                                                                     tuple(t.shape)))
+    P, cap, hp = shape[0] // n, shape[2], shape[3]
+    if not 0 < hd <= hp or hd % 8:
+        raise _C.LmodError("kv_beam_reorder: hd %r must be a multiple of 8 in (0, %d]" % (hd, hp))
+    rows, parent = [int(r) for r in rows], [int(p) for p in parent]
+    if len(rows) != P or len(parent) != P * n:
+        raise _C.LmodError("kv_beam_reorder: %d prompts of %d beams need %d rows and %d parents, got %d and %d"
+                           % (P, n, P, P * n, len(rows), len(parent)))
+    if any(not 0 <= r <= cap for r in rows):
+        raise _C.LmodError("kv_beam_reorder: rows %s outside [0, cap = %d]" % (rows, cap))
+    if any(not 0 <= p < n for p in parent):
+        raise _C.LmodError("kv_beam_reorder: parents %s outside [0, n = %d)" % (parent, n))
+    key = tuple(t.data_ptr() for t in bufs)
+    table = _BEAM_TABLES.pop(key, None)
+    if table is None:
+        table = torch.tensor(key, dtype=torch.int64).to(bufs[0].device)
+    _BEAM_TABLES[key] = table
+    while len(_BEAM_TABLES) > 16:
+        _BEAM_TABLES.popitem(last=False)
+    ops = torch.tensor(rows + parent, dtype=torch.int32).to(bufs[0].device)
+    call("lmod_kv_beam_reorder", ptr(table), len(bufs), P, n, shape[1], cap, hd, hp, ptr(ops), ptr(ops[P:]))
 
 
 def spec_accept(target_logits, draft_tokens, draft_logits=None, u=None, len_target=None, len_draft=None):

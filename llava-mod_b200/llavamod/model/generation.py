@@ -44,8 +44,17 @@ the bytes it has in the expanded call, so the tokens are exactly those of genera
 a generator in the same state.  The sparse student (whose router draws fresh noise for every row, so the copies' K / V differ after its
 first MoE layer) and use_cache=False run that expanded call itself.
 
-Supported: greedy, temperature / top-p sampling, num_beams == 1, num_return_sequences with sampling, EOS and `stopping_criteria`
-callables, padded or unpadded batches, assisted decoding with a dense target."""
+Beam search, num_beams = nb > 1 with do_sample=False (transformers 4.37 beam_search + BeamSearchScorer, length_penalty, early_stopping
+True / False / "never", num_return_sequences <= nb): each step's fp32 log-softmax over the active vocabulary plus the beam scores, the top
+max(2, 1 + n_eos) * nb candidates of [B, nb * V] read to the host once, 4.37's process / is_done / finalize in BeamScorer, output
+[B*n, T_in + new] with row b*n + j the j-th best hypothesis of prompt b.  A dense model with use_cache=True prefills each prompt once
+into the shared cache of num_return_sequences (same graph key as num_return_sequences = nb) and lmod_kv_beam_reorder moves only the
+beams' rows past the prompt after each step; the sparse student decodes the inputs expanded nb times in a plain cache whose every row the
+same kernel reorders (HF's whole-cache reorder); use_cache=False re-runs each beam's sequence and reorders the ids.  Beam search needs
+an EOS id (the call's eos_token_id or the model config's): without one it raises NotImplementedError.
+
+Supported: greedy, temperature / top-p sampling, beam search, num_return_sequences with sampling or beams, EOS and `stopping_criteria`
+callables, padded or unpadded batches, assisted decoding with a dense target.  Not built: beam-sample, beams with an assistant."""
 import collections
 import os
 import weakref
@@ -172,20 +181,36 @@ def _pick(logits, do_sample, generator):
     return logits.argmax(dim=-1)
 
 
+class BeamsWithAssistantError(ValueError, NotImplementedError):
+    """num_beams > 1 with an assistant model: a ValueError, as transformers raises, and a NotImplementedError, as beams with an assistant
+    are not built here (callers written against either keep working)."""
+
+
 @torch.no_grad()
 def generate(model, inputs=None, images=None, attention_mask=None, max_new_tokens=20, do_sample=False, temperature=1.0, top_p=None,
              num_beams=1, use_cache=False, stopping_criteria=None, eos_token_id=None, pad_token_id=None, generator=None,
-             assistant_model=None, num_assistant_tokens=5, num_return_sequences=1, **unused):
+             assistant_model=None, num_assistant_tokens=5, num_return_sequences=1, length_penalty=1.0, early_stopping=False, **unused):
     """-> [B*n, T_in + n_new] int64 (n = num_return_sequences): the prompt ids (image placeholders -200 included, pads included, as HF
     returns them) followed by the new tokens; row b*n + j is copy j of prompt b.  assistant_model: a draft model for assisted decoding
     (use_cache=True, dense target), num_assistant_tokens = k drafted tokens per round.  num_return_sequences: n sampled sequences per
     prompt (do_sample=True); a dense model with use_cache=True prefills each prompt once into a shared cache, the sparse student and
     use_cache=False decode the inputs expanded with repeat_interleave(n, 0) (module docstring)."""
-    if num_beams != 1:
-        raise NotImplementedError("beam search is not built (the reference's eval shells run num_beams=1)")
     n_ret = int(num_return_sequences) if num_return_sequences is not None else 1
     if n_ret < 1:
         raise ValueError("generate: num_return_sequences must be >= 1, got %r" % (num_return_sequences,))
+    nb = int(num_beams) if num_beams is not None else 1
+    if nb < 1:
+        raise ValueError("generate: num_beams must be >= 1, got %r" % (num_beams,))
+    if nb > 1:
+        if do_sample:
+            raise NotImplementedError("beam-sample (num_beams > 1 with do_sample=True) is not built; beam search runs with do_sample=False")
+        if assistant_model is not None:
+            raise BeamsWithAssistantError("assisted generate is only supported with num_beams = 1, got num_beams = %d" % nb)
+        if n_ret > nb:
+            raise ValueError("num_return_sequences (%d) has to be smaller or equal to num_beams (%d)" % (n_ret, nb))
+        return _beam_search(model, inputs, images=images, attention_mask=attention_mask, max_new_tokens=max_new_tokens, num_beams=nb,
+                            num_return_sequences=n_ret, length_penalty=length_penalty, early_stopping=early_stopping, use_cache=use_cache,
+                            stopping_criteria=stopping_criteria, eos_token_id=eos_token_id, pad_token_id=pad_token_id)
     if n_ret > 1 and not do_sample:
         raise ValueError("num_return_sequences has to be 1 when doing greedy search, but is %d." % n_ret)
     if n_ret > 1 and assistant_model is not None:
@@ -203,29 +228,7 @@ def generate(model, inputs=None, images=None, attention_mask=None, max_new_token
     if n_ret > 1 and not share:                 # the sparse student, use_cache=False: the expanded call itself
         inputs, attention_mask, images = _expand(n_ret, inputs, attention_mask, images)
         n_ret = 1
-    ids = inputs.to(dev)
-    mask = None
-    if attention_mask is not None:
-        m = attention_mask.cpu().bool()
-        if not bool(m.all()):
-            n_real = m.sum(1)
-            if bool((n_real == 0).any()):
-                raise ValueError("generate: prompt %d has no real token" % int((n_real == 0).nonzero()[0]))
-            first = m.int().argmax(1)
-            if not bool((m.int().cumsum(1).gather(1, (first + n_real - 1)[:, None]).squeeze(1) == n_real).all()):
-                raise ValueError("generate: every prompt's real tokens must be contiguous (left or right padding)")
-            mask = m
-    was_training = model.training
-    model.eval()
-    eos = eos_token_id if eos_token_id is not None else getattr(model.config, "eos_token_id", None)
-    eos = [eos] if isinstance(eos, int) else (list(eos) if eos is not None else [])
-    pad = pad_token_id if pad_token_id is not None else (eos[0] if eos else 0)
-    n_vocab = getattr(model, "_active_vocab", None)                     # resize_token_embeddings(len(tokenizer)) narrows the usable vocabulary
-    feats = None
-    if images is not None and model.get_image_tower() is not None:       # tower + projector once; the splice still runs every step
-        imgs = torch.stack([im.to(dev) for im in images]) if not torch.is_tensor(images) else images.to(dev)
-        feats = model.get_image_tower()(imgs.to(model.dtype))
-        images = imgs
+    ids, mask, images, feats, eos, pad, n_vocab, was_training = _prepare(model, inputs, images, attention_mask, eos_token_id, pad_token_id)
     B = ids.shape[0]
     done = torch.zeros(B, dtype=torch.bool, device=dev)
     ent = None
@@ -282,6 +285,37 @@ def generate(model, inputs=None, images=None, attention_mask=None, max_new_token
     if was_training:
         model.train()
     return ids
+
+
+def _prepare(model, inputs, images, attention_mask, eos_token_id, pad_token_id):
+    """What every decoding loop starts from: the prompt ids on the device; the prompt mask (bool, host) when some prompt is padded, else None
+    (every prompt's real tokens must be one contiguous run); the images on the device with the tower + projector run once (the splice still
+    runs every step); the EOS ids, the pad id, the active vocabulary and whether the model was training (it is left in eval mode)."""
+    dev = model.device
+    ids = inputs.to(dev)
+    mask = None
+    if attention_mask is not None:
+        m = attention_mask.cpu().bool()
+        if not bool(m.all()):
+            n_real = m.sum(1)
+            if bool((n_real == 0).any()):
+                raise ValueError("generate: prompt %d has no real token" % int((n_real == 0).nonzero()[0]))
+            first = m.int().argmax(1)
+            if not bool((m.int().cumsum(1).gather(1, (first + n_real - 1)[:, None]).squeeze(1) == n_real).all()):
+                raise ValueError("generate: every prompt's real tokens must be contiguous (left or right padding)")
+            mask = m
+    was_training = model.training
+    model.eval()
+    eos = eos_token_id if eos_token_id is not None else getattr(model.config, "eos_token_id", None)
+    eos = [eos] if isinstance(eos, int) else (list(eos) if eos is not None else [])
+    pad = pad_token_id if pad_token_id is not None else (eos[0] if eos else 0)
+    n_vocab = getattr(model, "_active_vocab", None)                     # resize_token_embeddings(len(tokenizer)) narrows the usable vocabulary
+    feats = None
+    if images is not None and model.get_image_tower() is not None:
+        imgs = torch.stack([im.to(dev) for im in images]) if not torch.is_tensor(images) else images.to(dev)
+        feats = model.get_image_tower()(imgs.to(model.dtype))
+        images = imgs
+    return ids, mask, images, feats, eos, pad, n_vocab, was_training
 
 
 def _expand(n, inputs, attention_mask, images):
@@ -403,3 +437,180 @@ def _assemble(ids, out, pad, max_new):
         r = r[:W]
         new[b, :len(r)] = torch.tensor(r, dtype=torch.int64)
     return torch.cat([ids, new.to(ids.device)], dim=1)
+
+
+class BeamScorer:
+    """transformers 4.37 BeamSearchScorer with BeamHypotheses (one beam group), on host numbers.  Lengths count new tokens only (the
+    decoder prompt length is 0, as for HF's generate from inputs_embeds), so a hypothesis that ends in EOS at step s has length s + 1.
+    hyps[b]: at most num_beams (score, new tokens without the EOS) of prompt b; done[b]: 4.37's _done."""
+
+    def __init__(self, batch, num_beams, num_return_sequences, length_penalty, early_stopping, max_new_tokens, eos, pad):
+        if early_stopping not in (True, False, "never"):
+            raise ValueError("early_stopping must be True, False or 'never', got %r" % (early_stopping,))
+        self.nb, self.n_ret, self.lp, self.es = int(num_beams), int(num_return_sequences), float(length_penalty), early_stopping
+        self.max_new, self.eos, self.pad = int(max_new_tokens), list(eos), pad
+        self.hyps = [[] for _ in range(batch)]
+        self.worst = [1e9] * batch
+        self.done = [False] * batch
+
+    @property
+    def is_done(self):
+        return all(self.done)
+
+    def _add(self, b, tokens, sum_logprobs, generated_len):
+        """BeamHypotheses.add: keep the num_beams best by sum_logprobs / generated_len ** length_penalty."""
+        score = sum_logprobs / (generated_len ** self.lp)
+        hyps = self.hyps[b]
+        if len(hyps) < self.nb or score > self.worst[b]:
+            hyps.append((score, tokens))
+            if len(hyps) > self.nb:
+                ranked = sorted((s, i) for i, (s, _) in enumerate(hyps))
+                del hyps[ranked[0][1]]
+                self.worst[b] = ranked[1][0]
+            else:
+                self.worst[b] = min(score, self.worst[b])
+
+    def _is_done(self, b, best_sum_logprobs, cur_len):
+        """BeamHypotheses.is_done with the three early_stopping modes."""
+        if len(self.hyps[b]) < self.nb:
+            return False
+        if self.es is True:
+            return True
+        length = self.max_new if self.es == "never" and self.lp > 0.0 else cur_len
+        return self.worst[b] >= best_sum_logprobs / length ** self.lp
+
+    def process(self, cur_len, scores, tokens, beams, seqs):
+        """BeamSearchScorer.process for the step that makes the new sequences cur_len tokens long.  scores / tokens / beams: per prompt, the
+        top max(2, 1 + n_eos) * num_beams candidates, best first (summed log-prob, token, local beam); seqs: each running beam's new tokens.
+        -> (next beam scores, next tokens, next local parents), num_beams per prompt; a done prompt takes pad tokens from beam 0 at 0."""
+        nb = self.nb
+        out_s, out_t, out_p = [], [], []
+        for b in range(len(self.done)):
+            if self.done[b]:
+                out_s += [0.0] * nb
+                out_t += [self.pad] * nb
+                out_p += [0] * nb
+                continue
+            n = 0
+            for rank, (s, t, j) in enumerate(zip(scores[b], tokens[b], beams[b])):
+                if t in self.eos:
+                    if rank < nb:                   # an EOS ranked below num_beams is not a hypothesis
+                        self._add(b, seqs[b * nb + j], s, cur_len)
+                else:
+                    out_s.append(s)
+                    out_t.append(t)
+                    out_p.append(j)
+                    n += 1
+                if n == nb:
+                    break
+            if n < nb:
+                raise ValueError("beam search: prompt %d has %d non-EOS candidates for %d beams" % (b, n, nb))
+            self.done[b] = self.done[b] or self._is_done(b, max(scores[b]), cur_len)
+        return out_s, out_t, out_p
+
+    def finalize(self, seqs, scores):
+        """BeamSearchScorer.finalize: the running beams of every prompt not done become hypotheses; -> num_return_sequences rows of new
+        tokens per prompt, best first, as wide as the longest hypothesis + 1 (at most max_new_tokens); each row gets eos[0] after its tokens
+        where it fits (4.37 inserts the first EOS id, also after a beam that stopped without one) and pad after that."""
+        nb = self.nb
+        for b in range(len(self.done)):
+            if not self.done[b]:
+                for j in range(nb):
+                    self._add(b, seqs[b * nb + j], scores[b * nb + j], len(seqs[b * nb + j]))
+        best = []
+        for hyps in self.hyps:
+            ranked = sorted(hyps, key=lambda h: h[0])
+            best += [ranked.pop()[1] for _ in range(self.n_ret)]
+        width = min(max(len(r) for r in best) + 1, self.max_new)
+        rows = []
+        for r in best:
+            r = list(r) + ([self.eos[0]] if self.eos and len(r) < width else [])
+            rows.append(r + [self.pad] * (width - len(r)))
+        return rows
+
+
+@torch.no_grad()
+def _beam_search(model, inputs, images=None, attention_mask=None, max_new_tokens=20, num_beams=2, num_return_sequences=1, length_penalty=1.0,
+                 early_stopping=False, use_cache=False, stopping_criteria=None, eos_token_id=None, pad_token_id=None, expand=False,
+                 trace=None):
+    """Beam search (transformers 4.37 beam_search + BeamSearchScorer; module docstring) -> [B*n, T_in + new], row b*n + j the j-th best
+    hypothesis of prompt b.  Each step: fp32 log-softmax over the active vocabulary, plus each beam's score, the top max(2, 1 + n_eos) * nb
+    candidates of [B, nb * V] read to the host once, BeamScorer.process, then the running ids and the cache follow the chosen parents.
+    A dense model with use_cache=True prefills each prompt once into a shared cache and lmod_kv_beam_reorder moves the beams' rows past
+    the prompt; the sparse student, or expand=True, decodes the inputs expanded nb times in a plain cache whose every row is reordered.
+    trace: a list that receives every step's fp32 logits [B*nb, V] (the tests replay the scorer on them)."""
+    nb, n_ret, max_new = int(num_beams), int(num_return_sequences), int(max_new_tokens)
+    eos = eos_token_id if eos_token_id is not None else getattr(model.config, "eos_token_id", None)
+    if eos is None or (not isinstance(eos, int) and len(list(eos)) == 0):
+        # 4.37's scorer ends a hypothesis only at an EOS and its finalize writes eos_token_id[0] after every hypothesis shorter than the
+        # output; without one, a search a stopping criterion ends early has no defined output.  A model config or the call gives one.
+        raise NotImplementedError("beam search without an eos_token_id is not built: pass eos_token_id (the model config has none)")
+    ids, mask, images, feats, eos, pad, n_vocab, was_training = _prepare(model, inputs, images, attention_mask, eos_token_id, pad_token_id)
+    dev = model.device
+    B = ids.shape[0]
+    R = B * nb
+    ragged = mask is not None
+    if max_new <= 0:
+        return ids.repeat_interleave(n_ret, 0)
+    scorer = BeamScorer(B, nb, n_ret, length_penalty, early_stopping, max_new, eos, pad)
+    shared = use_cache and not expand and not getattr(model, "is_moe", False)
+    x_ids, x_mask, x_images = (ids, mask, images) if shared else _expand(nb, ids, mask, images)
+    x_feats = feats if shared or feats is None else feats.repeat_interleave(nb, 0)
+    ent = None
+    if use_cache:
+        max_len = _bucket(max(model.spliced_length(ids, images, mask)) + max_new)
+        if shared:
+            ent = _decoder_entry(model, B, max_len, share=nb, suffix=(max_new + SUFFIX_BUCKET - 1) // SUFFIX_BUCKET * SUFFIX_BUCKET)
+        else:
+            ent = _decoder_entry(model, R, max_len)
+        logits = next_token_logits(model, x_ids, images=x_images, tower_features=x_feats, attention_mask=x_mask.to(dev) if ragged else None,
+                                   cache=ent["cache"], ragged=ragged)
+        if shared:
+            logits = logits.repeat_interleave(nb, 0)
+    elif ragged:        # as in generate's no-cache loop: each row's real tokens first, then its new ones, then padding
+        work = x_ids.gather(1, torch.argsort((~x_mask).to(torch.int8), dim=1, stable=True).to(dev))
+        wlen = x_mask.sum(1).to(dev)
+    run = ids.repeat_interleave(nb, 0)                  # the running beams' ids, as stopping_criteria sees them
+    beam_scores = torch.zeros(B, nb, dtype=torch.float32, device=dev)
+    beam_scores[:, 1:] = -1e9
+    beam_scores = beam_scores.view(-1)
+    seqs = [[] for _ in range(R)]
+    top = max(2, 1 + len(eos)) * nb
+    for step in range(max_new):
+        if ent is not None and step > 0:
+            ent["cache"].reorder_beams(parents, nb)
+            eager = not _graphs_enabled() or (step == 1 and ent["graph"] is None)      # one eager step before the capture
+            logits = _decode_step(model, ent, tok, eager)
+        elif ent is None and ragged:
+            wmask = torch.arange(work.shape[1], device=dev)[None, :] < wlen[:, None]
+            logits = next_token_logits(model, work, images=x_images, tower_features=x_feats, attention_mask=wmask, ragged=True)
+        elif ent is None:
+            logits = next_token_logits(model, run, images=x_images, tower_features=x_feats)
+        if trace is not None:
+            trace.append(logits.clone())
+        V = n_vocab if n_vocab is not None and n_vocab < logits.shape[-1] else logits.shape[-1]
+        lp = torch.log_softmax(logits[:, :V], dim=-1) + beam_scores[:, None]
+        top_s, top_i = torch.topk(lp.view(B, nb * V), top, dim=1, largest=True, sorted=True)
+        host = torch.stack([top_s.double(), top_i.double()]).tolist()      # the step's one device-to-host read
+        idx = [[int(i) for i in row] for row in host[1]]
+        nxt_s, nxt_t, parents = scorer.process(step + 1, host[0], [[i % V for i in row] for row in idx],
+                                               [[i // V for i in row] for row in idx], seqs)
+        src = [b * nb + p for b in range(B) for p in parents[b * nb:(b + 1) * nb]]
+        seqs = [seqs[g] + [t] for g, t in zip(src, nxt_t)]
+        src_d = torch.tensor(src, dtype=torch.int64).to(dev)
+        tok = torch.tensor(nxt_t, dtype=torch.int64).to(dev)
+        beam_scores = torch.tensor(nxt_s, dtype=torch.float32).to(dev)
+        run = torch.cat([run.index_select(0, src_d), tok[:, None]], dim=1)
+        if ent is None and ragged:
+            work, wlen = work.index_select(0, src_d), wlen.index_select(0, src_d)
+            work = torch.cat([work, torch.full_like(tok[:, None], pad)], dim=1).scatter_(1, wlen[:, None], tok[:, None])
+            wlen = wlen + 1
+        stop = scorer.is_done
+        if not stop and stopping_criteria:
+            stop = any(bool(c(run, lp)) for c in stopping_criteria)        # transformers.StoppingCriteriaList.__call__: any criterion stops
+        if stop:
+            break
+    rows = scorer.finalize(seqs, nxt_s)
+    if was_training:
+        model.train()
+    return torch.cat([ids.repeat_interleave(n_ret, 0), torch.tensor(rows, dtype=torch.int64, device=dev)], dim=1)

@@ -608,6 +608,23 @@ class KVCache:
             raise ValueError("KVCache.rollback: cannot drop %s rows from lengths %s" % (drop, self.lengths))
         self.lengths = [n - d for n, d in zip(self.lengths, drop)]
 
+    def reorder_beams(self, parent, n):
+        """Beam search's cache reorder (HF _reorder_cache), in place by lmod_kv_beam_reorder: sequence b*n + j takes the rows of sequence
+        b*n + parent[b*n + j] (host ints in [0, n)).  The beams of a prompt advance together, so they hold the same number of rows.  A
+        shared cache (share == n) moves the rows past the prompt only; a plain cache of prompts*n sequences moves every row."""
+        if self.shared and n != self.share:
+            raise ValueError("KVCache.reorder_beams: a shared cache of %d sequences per prompt, got n = %d" % (self.share, n))
+        if self.batch % n:
+            raise ValueError("KVCache.reorder_beams: %d sequences are not prompts of %d beams" % (self.batch, n))
+        rows = []
+        for b in range(self.batch // n):
+            r = set(self.lengths[b * n:(b + 1) * n])
+            if len(r) != 1:
+                raise ValueError("KVCache.reorder_beams: the beams of prompt %d have lengths %s" % (b, self.lengths[b * n:(b + 1) * n]))
+            rows.append(r.pop() - (self.prefixes[b] if self.shared else 0))
+        if any(rows):
+            K.kv_beam_reorder(self.ks + self.vs if self.shared else self.k + self.v, n, self.head_dim, rows, parent)
+
     def chunk_workspace(self, T):
         """The decode-attention workspace of a step of T tokens per sequence (kept, so a captured step keeps its address)."""
         ws = self._chunk_ws.get(T)

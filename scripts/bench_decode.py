@@ -2,7 +2,7 @@
 kernel family of one cached decode step.
 
     python scripts/bench_decode.py [--models student,teacher] [--new 128,512] [--batch 1,8] [--profile] [--ragged] [--assisted]
-                                   [--num-return 4,8] [--out DIR]
+                                   [--num-return 4,8] [--num-beams 2,3,4] [--out DIR]
 
 * generate: the 0.5B-4E student and the 7B teacher (random weights, CLIP-L/336) on a prompt that splices to T' = 650 positions, greedy,
   use_cache False / True, CUDA graphs on / off (LLAVAMOD_CUDA_GRAPHS).  Tokens/s = B * new tokens / wall time of the call, which ends in
@@ -27,6 +27,13 @@ kernel family of one cached decode step.
   attention of one layer at the middle step of the run: lmod_attn_decode_shared on the shared cache against lmod_attn_decode on the
   expanded one, CUDA events over 50 launches each, alternated, with the bytes each must read (K / V rows, q, out).  The sparse student
   runs the expanded call in both rows (its copies cannot share the cache), so its rows differ only by noise.
+* --num-beams NB[,NB...]: beam search (num_beams = nb, eos_token_id -1 so every call runs all its steps), the 7B teacher and the
+  0.5B-4E student (random weights, graphs on), B from --batch, each --new value, T' = 650: prompts/s and steps/s of the shared-cache path
+  against the expanded form (generation._beam_search(expand=True)) for the dense teacher, the expanded form only for the sparse student,
+  and the K / V bytes each allocates.  Then lmod_kv_beam_reorder alone at each model's shapes, B and nb: the suffix reorder of the shared
+  cache at 128, 512 and 1024 rows past the prompt, and the whole-cache reorder of the expanded form (650 + those rows), each one launch
+  over every layer's K and V with a map that moves half the beams (the call's host checks and operand copy included); CUDA events over
+  20 calls, median of three alternated rounds, with the bytes it must move (sources read once, changed beams written) over 3.35 TB/s.
 The card's name and power limit are read in the same process and printed with the results (one JSON line per measurement)."""
 import argparse
 import json
@@ -308,6 +315,85 @@ def bench_num_return(models, ns, batches, new, out, info, repeat):
         torch.cuda.empty_cache()
 
 
+def _reorder_case(model, B, nb, rows, cap):
+    """(bufs, parent) for one reorder launch over every layer's K and V of B prompts of nb beams, and the bytes it moves: beams
+    1 .. nb//2 take beam 0's rows (the rest keep theirs), so one source is read and nb // 2 beams are written per prompt."""
+    from llavamod import kernels as K
+    cfg = model.config
+    hd = cfg.hidden_size // cfg.num_attention_heads
+    hp = K.attn_head_dim(hd)
+    bufs = [torch.empty(B * nb, cfg.num_key_value_heads, cap, hp, device="cuda", dtype=torch.bfloat16)
+            for _ in range(2 * cfg.num_hidden_layers)]
+    parent = [0 if 1 <= j <= nb // 2 else j for _ in range(B) for j in range(nb)]
+    nbytes = len(bufs) * B * (1 + nb // 2) * cfg.num_key_value_heads * rows * hd * 2
+    return bufs, parent, hd, nbytes
+
+
+def bench_num_beams(models, nbs, batches, news, out, info, repeat):
+    from llavamod import kernels as K
+    from llavamod.model import generation as Gm
+    from llavamod.model import synthetic as S
+    os.environ["LLAVAMOD_CUDA_GRAPHS"] = "1"
+    for name in models:
+        model = (S.make_student("qwen1.5-0.5b", "clip-l-336", seed=1) if name == "student" else
+                 S.make_teacher("qwen1.5-7b", "clip-l-336", seed=0)).eval()
+        for B in batches:
+            ids, imgs = prompt(B)
+            for new in news:
+                for nb in nbs:
+                    kw = dict(use_cache=True, eos_token_id=-1, num_beams=nb, max_new_tokens=new)
+                    calls = {"expanded": lambda: Gm._beam_search(model, ids, images=imgs, expand=True, **kw)}
+                    if not model.is_moe:
+                        calls["shared"] = lambda: model.generate(ids, images=imgs, **kw)
+                    rec = dict(kind="num_beams", model=name, B=B, nb=nb, prompt_len=650, new=new, runs=repeat, card=info)
+                    for row, fn in calls.items():
+                        Gm._STEP_GRAPHS.clear()
+                        torch.cuda.empty_cache()
+                        try:
+                            secs = _timed_generate(fn, repeat)
+                        except torch.OutOfMemoryError:
+                            rec[row] = dict(out_of_memory=True)
+                            continue
+                        cache = list(Gm._STEP_GRAPHS.values())[-1]["cache"]
+                        med = secs[len(secs) // 2]
+                        rec[row] = dict(prompts_per_s=round(B / med, 3), steps_per_s=round(new / med, 1),
+                                        spread_s=[round(secs[0], 3), round(secs[-1], 3)], cache_MB=round(cache.nbytes / 1e6, 1),
+                                        shared_cache=cache.shared)
+                        del cache
+                    Gm._STEP_GRAPHS.clear()
+                    torch.cuda.empty_cache()
+                    if all("steps_per_s" in rec.get(r, {}) for r in ("shared", "expanded")):
+                        rec.update(speedup=round(rec["shared"]["steps_per_s"] / rec["expanded"]["steps_per_s"], 3))
+                    emit(out, rec)
+        for B in batches:
+            for nb in nbs:
+                for rows in (128, 512, 1024):
+                    cases = {"suffix": (rows, -(-rows // Gm.SUFFIX_BUCKET) * Gm.SUFFIX_BUCKET),
+                             "whole": (650 + rows, Gm._bucket(650 + rows))}
+                    rec = dict(kind="beam_reorder", model=name, B=B, nb=nb, rows_past_prompt=rows, card=info)
+                    runs, ms, nbytes = {}, {}, {}
+                    try:
+                        for k, (r, cap) in cases.items():
+                            bufs, parent, hd, nbytes[k] = _reorder_case(model, B, nb, r, cap)
+                            runs[k] = (lambda bufs=bufs, parent=parent, hd=hd, r=r: K.kv_beam_reorder(bufs, nb, hd, [r] * B, parent))
+                            ms[k] = []
+                    except torch.OutOfMemoryError:
+                        rec["out_of_memory"] = True
+                    for _ in range(3):
+                        for k, fn in runs.items():
+                            ms[k].append(_replay_ms(fn, 20))
+                    for k in runs:
+                        t = sorted(ms[k])[1] * 1e-3
+                        rec[k] = dict(rows=cases[k][0], us=round(t * 1e6, 1), us_spread=[round(x * 1e3, 1) for x in sorted(ms[k])],
+                                      MB=round(nbytes[k] / 1e6, 1), TBps=round(nbytes[k] / t / 1e12, 3),
+                                      of_3_35TBps=round(nbytes[k] / t / 3.35e12, 3))
+                    emit(out, rec)
+                    runs.clear()
+                    torch.cuda.empty_cache()
+        del model
+        torch.cuda.empty_cache()
+
+
 def bench_attention(out, info):
     from llavamod import kernels as K
     for hd, nh, nkv in [(64, 16, 16), (64, 14, 2), (128, 28, 4), (128, 32, 32)]:
@@ -383,6 +469,7 @@ def main():
     ap.add_argument("--ragged", action="store_true", help="padded batches of prompts of different lengths (see the module docstring)")
     ap.add_argument("--assisted", action="store_true", help="assisted decoding, teacher with the student as draft (module docstring)")
     ap.add_argument("--num-return", default=None, help="num_return_sequences values: shared against expanded (module docstring)")
+    ap.add_argument("--num-beams", default=None, help="num_beams values: beam search shared against expanded (module docstring)")
     ap.add_argument("--repeat", type=int, default=3, help="timed generate calls per setting (median, min and max are reported)")
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
@@ -394,6 +481,10 @@ def main():
     if a.num_return:
         bench_num_return(a.models.split(","), [int(x) for x in a.num_return.split(",")], [int(x) for x in a.batch.split(",")],
                          int(a.new.split(",")[0]), a.out, info, a.repeat)
+        return
+    if a.num_beams:
+        bench_num_beams(a.models.split(","), [int(x) for x in a.num_beams.split(",")], [int(x) for x in a.batch.split(",")],
+                        [int(x) for x in a.new.split(",")], a.out, info, a.repeat)
         return
     if a.assisted:
         teacher = S.make_teacher("qwen1.5-7b", "clip-l-336", seed=0).eval()
